@@ -115,6 +115,37 @@ class Oracle:
         return int(self.lib.orc_host_threads())
 
 
+def to_radix(bits: np.ndarray, kind: str, descending: bool = False) -> np.ndarray:
+    """Unsigned key whose ascending order is the requested order of the typed value `bits` (uint32 or uint64 containers).
+    kind "u": unsigned, "i": two's-complement signed, "f": IEEE float in total order (-NaN < -inf < ... < -0.0 < +0.0 < ...
+    < +inf < +NaN, NaN payloads ordered by their bits).  Descending complements the key, so a stable sort on it keeps
+    equal keys in input order in both directions."""
+    nb = bits.dtype.itemsize * 8
+    u = bits.copy()
+    sign = np.array(1 << (nb - 1), dtype=bits.dtype)
+    if kind == "i":
+        u ^= sign
+    elif kind == "f":
+        neg = (u >> np.array(nb - 1, dtype=bits.dtype)).astype(bool)
+        u = np.where(neg, ~u, u | sign)
+    if descending:
+        u = ~u
+    return u
+
+
+def from_radix(keys: np.ndarray, kind: str, descending: bool = False) -> np.ndarray:
+    """Inverse of to_radix: the typed bits whose radix key is `keys` (lets a test build inputs digit by digit)."""
+    nb = keys.dtype.itemsize * 8
+    u = ~keys if descending else keys.copy()
+    sign = np.array(1 << (nb - 1), dtype=keys.dtype)
+    if kind == "i":
+        u ^= sign
+    elif kind == "f":
+        pos = (u >> np.array(nb - 1, dtype=keys.dtype)).astype(bool)
+        u = np.where(pos, u ^ sign, ~u)
+    return u
+
+
 def device_digest(t) -> int:
     """Order-sensitive 64-bit digest of a CUDA tensor's 32-bit words, computed on the device (the golden values of the
     2^30-element cases; an FNV pass over 4 GB on the host would take minutes).  Word i contributes

@@ -5,22 +5,9 @@ import numpy as np
 import pytest
 import torch
 
+from tests.oraclelib import to_radix
+
 pytestmark = pytest.mark.gpu
-
-
-def to_radix(bits: np.ndarray, kind: str, descending: bool) -> np.ndarray:
-    """unsigned key whose ascending order is the requested order of the typed value (reference transform)"""
-    nb = bits.dtype.itemsize * 8
-    u = bits.copy()
-    sign = np.array(1 << (nb - 1), dtype=bits.dtype)
-    if kind == "i":
-        u ^= sign
-    elif kind == "f":
-        neg = (u >> np.array(nb - 1, dtype=bits.dtype)).astype(bool)
-        u = np.where(neg, ~u, u | sign)
-    if descending:
-        u = ~u
-    return u
 
 
 CASES = [("u32", np.uint32, "u"), ("i32", np.uint32, "i"), ("f32", np.uint32, "f"),

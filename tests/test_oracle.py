@@ -86,6 +86,54 @@ def test_validate_counts_inversions(oracle):
     assert np.array_equal(std, np.sort(k))
 
 
+@pytest.mark.parametrize("ftype,utype", [(np.float32, np.uint32), (np.float64, np.uint64)])
+def test_to_radix_is_ieee_total_order(ftype, utype):
+    """The typed-key transform the GPU tests compare with, checked against numpy's float order and the IEEE 754 totalOrder
+    cases numpy cannot express (signed zeros, NaNs of both signs and several payloads)."""
+    from tests.oraclelib import from_radix, to_radix
+
+    rng = np.random.default_rng(11)
+    fi = np.finfo(ftype)
+    nb = np.dtype(utype).itemsize * 8
+    sign = 1 << (nb - 1)
+    # distinct magnitudes (numpy calls -0.0 == +0.0; total order does not), specials included
+    mags = np.concatenate([rng.standard_normal(3000) * 1e3, rng.standard_normal(500) * 1e-3,
+                           [fi.max, fi.tiny, fi.tiny * fi.eps, fi.tiny - fi.tiny * fi.eps, np.inf, 0.0, 1.0]]).astype(ftype)
+    mags = np.unique(np.abs(mags))
+    vals = mags * np.where(rng.random(mags.size) < 0.5, -1, 1).astype(ftype)
+    vals = vals[rng.permutation(vals.size)]
+    bits = vals.view(utype)
+    assert np.array_equal(np.argsort(to_radix(bits, "f"), kind="stable"), np.argsort(vals, kind="stable"))
+
+    u = lambda x: np.array([x], dtype=utype)  # noqa: E731
+    qnan, exp_all = 1 << (fi.nmant - 1), ((1 << (nb - 1 - fi.nmant)) - 1) << fi.nmant  # quiet bit, all-ones exponent
+    pinf, top = exp_all, (1 << fi.nmant) - 1
+    # ascending IEEE totalOrder of these bit patterns
+    chain = [sign | exp_all | top, sign | exp_all | qnan, sign | exp_all | 1, sign | pinf,   # -NaNs (payload large..small), -inf
+             sign | fi.max.view(utype).item(), sign | 1, sign, 0, 1, fi.max.view(utype).item(),  # -max, -min subnormal, -0, +0, ...
+             pinf, exp_all | 1, exp_all | qnan, exp_all | top]                                 # +inf, +NaNs (payload small..large)
+    keys = np.concatenate([to_radix(u(c), "f") for c in chain])
+    assert np.all(keys[1:] > keys[:-1])
+    shuffled = np.array(chain, dtype=utype)[rng.permutation(len(chain))]
+    assert np.array_equal(shuffled[np.argsort(to_radix(shuffled, "f"), kind="stable")], np.array(chain, dtype=utype))
+
+    # descending: the reverse order of the keys, equal keys (many ties here) keep their input order
+    for kind in ("u", "i", "f"):
+        b = rng.integers(0, 40, 2000).astype(np.int64) - 20
+        b = (b.astype(ftype) if kind == "f" else b.astype(np.int32 if nb == 32 else np.int64)).view(utype)
+        asc = to_radix(b, kind)
+        want = sorted(range(b.size), key=lambda i: -int(asc[i]))  # Python's sort is stable
+        assert np.array_equal(np.argsort(to_radix(b, kind, True), kind="stable"), want)
+        if kind != "u":
+            typed = b.view(ftype if kind == "f" else (np.int32 if nb == 32 else np.int64))
+            assert np.array_equal(np.argsort(to_radix(b, kind, True), kind="stable"), np.argsort(-typed, kind="stable"))
+        for desc in (False, True):
+            assert np.array_equal(from_radix(to_radix(b, kind, desc), kind, desc), b)
+    nans = np.array([c for c in chain if (c & exp_all) == exp_all and (c & top)], dtype=utype)
+    for desc in (False, True):
+        assert np.array_equal(from_radix(to_radix(nans, "f", desc), "f", desc), nans)
+
+
 @pytest.mark.skipif(not os.path.exists(GOLDEN), reason="golden fixture not generated yet")
 def test_oracle_reproduces_reference_golden_vectors(oracle):
     """Pins the oracle to the reference: inputs, sorted outputs, payloads and histograms produced by the
