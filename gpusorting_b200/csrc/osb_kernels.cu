@@ -838,6 +838,14 @@ struct PassParams {
     const SortPlan* plan;  // device plan or null
 };
 
+// Returns v unchanged, but the compiler can no longer prove the result equal to v: whatever is computed from the copy is
+// computed again rather than taken from earlier expressions in v that are still live.
+__device__ __forceinline__ uint32_t opaque_copy(uint32_t v)
+{
+    asm volatile("" : "+r"(v));
+    return v;
+}
+
 template <typename KeyT, bool PAIRS, int K, int WARPS>
 struct WideSmem {
     static constexpr int THREADS = WARPS * 32;
@@ -950,7 +958,8 @@ digit_binning_wide_kernel(KeyT* buf0, KeyT* buf1, uint32_t* val0, uint32_t* val1
     if (tile == 0xffffffffu) return;  // all keys share this digit: nothing to move (the plan accounts for the parity)
 #endif
     // plan_bits (direction, codec flags) is re-read from shared memory where it is needed instead of being carried in
-    // registers across the phases: the 64-register budget of this kernel is spent on the 32 keys and their counter addresses
+    // registers across the phases: the 64-register budget of this kernel is spent on the 32 keys (the rank phase recomputes
+    // their counter addresses, see opaque_copy below)
     const uint64_t tile_base = static_cast<uint64_t>(tile) * T;
     const bool full = tile_base + T <= n;
     const uint32_t valid = full ? T : static_cast<uint32_t>(n - tile_base);
@@ -1077,13 +1086,21 @@ digit_binning_wide_kernel(KeyT* buf0, KeyT* buf1, uint32_t* val0, uint32_t* val1
 #pragma unroll
     for (int i = 0; i < K; ++i) asm volatile("" ::"l"(static_cast<unsigned long long>(key[i])));  // keep the loads live
 #else
+    // The rank phase recomputes each key's digit and counter address from the key (two ALU ops) instead of reusing the count
+    // phase's: the compiler would otherwise keep the 32 addresses live across the barrier next to the 32 keys, which exceeds
+    // 64 registers and spills to local memory on sm_90a.  Opaque copies of shift and mask make the reuse impossible.  (Not of
+    // the histogram pointer: an opaque copy of it loses its shared-memory space, and the atomics become generic ones.  The
+    // ballot mode spills either way, and more with the copies; the HOT instantiation has 128 registers and does not spill.)
+    constexpr bool kRecompute = RANK_MODE == kRankAtomic && !HOT;
+    const uint32_t rshift = kRecompute ? opaque_copy(shift) : shift;
+    const uint32_t rmask = kRecompute ? opaque_copy(dmask) : dmask;
     uint32_t hot = kNoHotDigit;
     if constexpr (HOT && RANK_MODE == kRankAtomic) hot = hot_digit_of_tile(sm.wmax, T);
     if (HOT && hot != kNoHotDigit) {
         uint32_t hot_run = __shfl_sync(0xffffffffu, wh[hot], 0);  // this warp's next slot of the hot digit (warp-uniform)
 #pragma unroll
         for (int i = 0; i < K; ++i) {
-            const uint32_t d = digit_of(key[i], shift, dmask);
+            const uint32_t d = digit_of(key[i], rshift, rmask);
             const bool is_hot = d == hot;
             const uint32_t b = __ballot_sync(0xffffffffu, is_hot);
             uint32_t slot = hot_run + __popc(b & lt);
@@ -1095,7 +1112,7 @@ digit_binning_wide_kernel(KeyT* buf0, KeyT* buf1, uint32_t* val0, uint32_t* val1
     } else {
 #pragma unroll
         for (int i = 0; i < K; ++i) {
-            const uint32_t slot = warp_rank_and_count<RANK_MODE>(wh, digit_of(key[i], shift, dmask), lt);
+            const uint32_t slot = warp_rank_and_count<RANK_MODE>(wh, digit_of(key[i], rshift, rmask), lt);
             if constexpr (PAIRS) kv[slot] = make_uint2(static_cast<uint32_t>(key[i]), val[i]);
             else sm.sorted[slot] = key[i];
         }
@@ -1475,8 +1492,8 @@ struct RingSmem {
 #ifndef OSB_STEP
 #define OSB_STEP 8
 #endif
-#ifndef OSB_PAIRS_LOOK  // (key, payload) pairs, either kernel
-#define OSB_PAIRS_LOOK 16
+#ifndef OSB_PAIRS_LOOK  // (key, payload) pairs, either kernel; 8 beat 16 and 32 on the H100 with the default kernel's 8,192-pair tiles (DESIGN §4.2)
+#define OSB_PAIRS_LOOK 8
 #endif
 #ifndef OSB_U64_LOOK    // 64-bit keys: 8,192-key tiles, twice the tiles per byte
 #define OSB_U64_LOOK 32
@@ -1642,22 +1659,30 @@ static cudaError_t set_ring_attr()
 }
 
 // Geometry and lookback window: 16,384-key tiles on 2 x 512 threads per SM (~82 KB of shared memory per CTA, inside
-// H100's 227 KB per block and 228 KB per SM).  The geometry and the window were chosen with tools/sweep.sh on the GPU this
-// project was first written for (8,192-key tiles at 3 or 4 CTAs per SM, 31,744-key tiles on 1 x 1024 threads, 10,240-key
-// tiles on 3 x 320 threads and resident CTAs prefetching their next tile were slower or equal there: a geometry that avoids
-// spills is bound by the L1/shared-memory wavefronts per key, not by occupancy); they have not been re-swept on H100.
+// H100's 227 KB per block and 228 KB per SM).  Re-swept on the H100 with tools/sweep.sh (DESIGN §4.2): 8,192-key tiles on
+// 256 threads at 3 or 4 CTAs per SM are 11-18 % slower per sort -- twice the tiles double the chained scan's length, and the
+// lookback grows to half of a CTA's life -- and the u32 window of 32 tiles is within run-to-run noise of 16.
 template <typename KeyT, bool PAIRS> struct WideGeom;
 #ifndef OSB_WIDE_WARPS  // geometry of the u32 keys-only kernel, overridable for sweeps
 #define OSB_WIDE_WARPS 16
 #define OSB_WIDE_K 32
 #define OSB_WIDE_MINB 2
 #endif
-template <> struct WideGeom<uint32_t, false> { static constexpr int K = OSB_WIDE_K, WARPS = OSB_WIDE_WARPS, MINB = OSB_WIDE_MINB, LOOK = OSB_LOOK, STEP = OSB_STEP; };
-template <> struct WideGeom<uint32_t, true>  { static constexpr int K = 16, WARPS = 16, MINB = 2, LOOK = OSB_PAIRS_LOOK, STEP = OSB_STEP; };
+#ifndef OSB_PAIRS_WIDE_WARPS  // geometry of the u32 pairs kernel, overridable for sweeps
+#define OSB_PAIRS_WIDE_WARPS 16
+#define OSB_PAIRS_WIDE_K 16
+#define OSB_PAIRS_WIDE_MINB 2
+#endif
+#ifndef OSB_U64_WARPS  // geometry of the u64 keys kernel, overridable for sweeps
+#define OSB_U64_WARPS 16
+#define OSB_U64_MINB 2
+#endif
 #ifndef OSB_U64_K
 #define OSB_U64_K 16
 #endif
-template <> struct WideGeom<uint64_t, false> { static constexpr int K = OSB_U64_K, WARPS = 16, MINB = 2, LOOK = OSB_U64_LOOK, STEP = OSB_STEP; };
+template <> struct WideGeom<uint32_t, false> { static constexpr int K = OSB_WIDE_K, WARPS = OSB_WIDE_WARPS, MINB = OSB_WIDE_MINB, LOOK = OSB_LOOK, STEP = OSB_STEP; };
+template <> struct WideGeom<uint32_t, true>  { static constexpr int K = OSB_PAIRS_WIDE_K, WARPS = OSB_PAIRS_WIDE_WARPS, MINB = OSB_PAIRS_WIDE_MINB, LOOK = OSB_PAIRS_LOOK, STEP = OSB_STEP; };
+template <> struct WideGeom<uint64_t, false> { static constexpr int K = OSB_U64_K, WARPS = OSB_U64_WARPS, MINB = OSB_U64_MINB, LOOK = OSB_U64_LOOK, STEP = OSB_STEP; };
 
 template <typename KeyT, bool PAIRS, int RANK_MODE>
 static cudaError_t launch_wide_variant(const void* in, void* out, const uint32_t* in_val, uint32_t* out_val, uint64_t n,
