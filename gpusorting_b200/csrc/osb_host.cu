@@ -570,6 +570,11 @@ int osb200_set_option(osb200_handle h, const char* key, int64_t value)
         h->cfg.debug_stall_every = static_cast<uint32_t>(value);
         return OSB200_OK;
     }
+    if (!std::strcmp(key, "debug_max_ctas")) {  // test hook of the persistent pass's tile schedule (0 = off)
+        if (value < 0 || value > (1ll << 30)) return OSB200_ERR_INVALID_ARG;
+        h->cfg.debug_max_ctas = static_cast<uint32_t>(value);
+        return OSB200_OK;
+    }
     if (!std::strcmp(key, "variant")) {
         if (value < 0 || value >= osb::kNumVariants) return OSB200_ERR_INVALID_ARG;
         h->cfg.variant = static_cast<int>(value);

@@ -30,6 +30,7 @@ struct BinningConfig {
     uint32_t place = 0;               // index of this pass in the plan
     uint32_t spin_cap = 2048;         // lookback polls of one predecessor before the digit thread re-reduces that tile itself
     uint32_t debug_stall_every = 0;   // test hook: tiles with tile % N == N-1 never publish their reduction (0 = off)
+    uint32_t debug_max_ctas = 0;      // test hook: at most this many persistent CTAs per pass (0 = as many as can be resident)
     bool hot_passes = false;          // also enqueue the HOT instantiation (the plan decides which of the two runs the pass)
 };
 

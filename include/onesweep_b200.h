@@ -169,6 +169,8 @@ OSB200_API int osb200_init_random_u32(uint32_t* d_keys, uint32_t* d_payload, uin
  *   "spin_cap"       lookback polls of one predecessor tile before a digit thread stops waiting and re-reduces that
  *                    tile itself (forward-progress fallback, reference: Sort/EmulatedDeadlocking.cu:159-267)
  *   "debug_stall_every"  test hook for that fallback: N > 0 makes every N-th tile withhold its reduction
+ *   "debug_max_ctas" test hook of the persistent DigitBinningPass (uint32 keys, HOT passes): N > 0 runs it on at most N CTAs (the tiles after
+ *                    each CTA's first are handed out by an atomic ticket); 0 (default) = as many as can be resident
  *   "profile"        1 = record CUDA events between the kernels of a sort (osb200_get_profile)
  *   "small_path"     1 (default) = a sort of at most one tile (info "small_path_max_n": 16,384 keys, 8,192 for 64-bit keys)
  *                    is ONE launch of the single-block shared-memory sort (see osb200_segmented_sort_u32); 0 = always the

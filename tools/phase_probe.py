@@ -22,12 +22,15 @@ work.copy_(src)
 s.sort_keys(work)
 torch.cuda.synchronize()
 lib.osb200_debug_phases(out, 0)
-names = ["ticket+clear", "load", "count", "reduce/scan/bases", "rank", "lookback", "scatter", None, "barrier after lookback"]
-ctas = out[7]
+# a persistent CTA runs many tiles: every figure is per tile.  "tile start" holds each CTA's start-up (plan, histogram clear)
+# once; "wait for keys" is how long the tile's keys, loaded during the previous tile, still take to land
+names = ["tile start", "wait for keys", "count", "reduce/scan/bases", "rank + next loads", "lookback", "scatter", None,
+         "barrier after lookback"]
+tiles = out[7]
 tot = sum(out[i] for i in range(9) if i != 7)
-print(f"CTAs {ctas}; mean clocks per CTA-tile: total {tot / ctas:.0f}")
+print(f"tiles {tiles}; mean clocks per tile: total {tot / tiles:.0f}")
 for i, nm in enumerate(names):
     if nm is None:
         continue
-    print(f"  {nm:20s} {out[i] / ctas:9.0f} clk  {100.0 * out[i] / tot:5.1f}%")
-print(f"lookback windows per tile (digit 0): {out[9] / ctas:.2f}; stalled polls per tile: {out[10] / ctas:.2f}")
+    print(f"  {nm:22s} {out[i] / tiles:9.0f} clk  {100.0 * out[i] / tot:5.1f}%")
+print(f"lookback windows per tile (digit 0): {out[9] / tiles:.2f}; stalled polls per tile: {out[10] / tiles:.2f}")
