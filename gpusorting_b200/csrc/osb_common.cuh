@@ -17,7 +17,8 @@ constexpr int kRadixLog = 8;     // bits per digit                (reference: RA
 // The reference packs {value:30, flag:2} into 32 bits (OneSweep.cu:39-42), which caps n at 2^30 and
 // forces a memset of every descriptor before every sort (OneSweepDispatcher.cuh:301-309).  Here the value
 // field is 38 bits (n <= 2^38 per GPU) and the epoch field makes stale words from earlier passes / sorts
-// read as NOT_READY, so descriptors are never cleared between sorts.
+// read as NOT_READY, so descriptors are not cleared between eager sorts.  (A graph replays the epochs of its capture, so
+// a captured sort clears its descriptors before and after its passes: osb_host.cu, is_capturing.)
 constexpr uint64_t kFlagNotReady = 0;   // reference: FLAG_NOT_READY
 constexpr uint64_t kFlagReduction = 1;  // reference: FLAG_REDUCTION (tile-local digit count published)
 constexpr uint64_t kFlagInclusive = 2;  // reference: FLAG_INCLUSIVE (prefix over tiles 0..p published)

@@ -6,7 +6,8 @@
 // ping-ponging keys -> alt -> keys.  Differences, all deliberate (DESIGN.md):
 //   * no per-sort memset of the 64-bit inclusive descriptors (epoch-stamped); per sort there are two memsets: the 8.3 KB
 //     control block (global histogram + tile tickets) and the compact 16-bit reductions (512 B per tile and place:
-//     128 MiB at n = 2^30 u32, ~20 us) -- against the reference's 6 memsets over ~573 MB at n = 2^30;
+//     128 MiB at n = 2^30 u32, ~20 us) -- against the reference's 6 memsets over ~573 MB at n = 2^30.  A sort enqueued
+//     under stream capture also clears its descriptors before and after its passes (is_capturing);
 //   * passes whose digit is the same for every key are skipped, and passes with one dominant bin run in the HOT
 //     instantiation of the pass, both decided on the device (osb::SortPlan);
 //   * a sort of at most one tile is ONE launch of the single-CTA shared-memory sort (also the segmented sort);
@@ -62,7 +63,7 @@ struct osb200_sorter {
     void* alt_keys = nullptr;
     uint32_t* alt_vals = nullptr;
     unsigned char* control = nullptr;  // ControlLayout
-    uint64_t* desc = nullptr;          // [tiles][256] 64-bit descriptors (epoch-stamped, never cleared)
+    uint64_t* desc = nullptr;          // [tiles][256] 64-bit descriptors (epoch-stamped, cleared only by captured sorts)
     uint16_t* agg16 = nullptr;         // [places][tiles][256] compact reductions (zeroed once per sort)
     uint64_t desc_tiles = 0;
     uint32_t epoch = 0;
@@ -120,6 +121,21 @@ int next_epoch(osb200_sorter* s, cudaStream_t stream, uint32_t* out)
     return OSB200_OK;
 }
 
+// Under stream capture the epochs become launch arguments frozen into the graph: every replay runs with the epochs of the
+// capture.  Where the previous replay's last executed pass is the digit place of this replay's first (always for a single
+// pass; else when the plan skips passes), a tile would take the previous replay's inclusive prefixes for its own where no
+// other sort has overwritten them since.  So a captured sort clears the words of
+// its tiles before its first pass and after its last: the first clear hides words an eager sort left with the same epochs
+// (after a wrap-around), the second hides the replay's words from a later eager sort that reuses them.  Eager sorts never
+// clear.
+int is_capturing(cudaStream_t stream, bool* out)
+{
+    cudaStreamCaptureStatus st = cudaStreamCaptureStatusNone;
+    OSB_TRY(cudaStreamGetCaptureInfo(stream, &st));
+    *out = st == cudaStreamCaptureStatusActive;
+    return OSB200_OK;
+}
+
 int check_handle(const osb200_sorter* s) { return s ? OSB200_OK : OSB200_ERR_INVALID_ARG; }
 
 // The launch plan (reference: OneSweepDispatcher.cuh:311-363): GlobalHistogram, Scan, one DigitBinningPass per digit
@@ -155,9 +171,15 @@ int sort_impl(osb200_sorter* s, void* d_keys, uint32_t* d_vals, uint64_t n, cuda
         return OSB200_OK;
     }
 
+    bool capturing = false;
+    int st = is_capturing(stream, &capturing);
+    if (st != OSB200_OK) return st;
+    const uint32_t tile_keys = osb::binning_tile_keys(s->key_bytes, d_vals != nullptr, s->cfg);
+    const size_t desc_bytes = tiles_for(n, tile_keys) * osb::kRadix * sizeof(uint64_t);
+    if (capturing) OSB_TRY(cudaMemsetAsync(s->desc, 0, desc_bytes, stream));
     OSB_TRY(cudaMemsetAsync(s->control, 0, ControlLayout::zeroed_bytes, stream));
     const bool compact = s->cfg.variant != osb::kVariantTilePerCta;  // every other variant uses the compact reductions
-    const uint64_t agg_stride = agg_tiles_for(n, osb::binning_tile_keys(s->key_bytes, d_vals != nullptr, s->cfg)) * osb::kRadix;
+    const uint64_t agg_stride = agg_tiles_for(n, tile_keys) * osb::kRadix;
     // reductions carry no epoch (16-bit words): they are cleared per sort, 512 B per tile and place (128 MiB at n = 2^30)
     if (compact) OSB_TRY(cudaMemsetAsync(s->agg16, 0, agg_stride * places * sizeof(uint16_t), stream));
     int ne = 0;
@@ -187,7 +209,7 @@ int sort_impl(osb200_sorter* s, void* d_keys, uint32_t* d_vals, uint64_t n, cuda
     uint32_t* dv = d_vals ? s->alt_vals : nullptr;
     for (int p = 0; p < places; ++p) {
         uint32_t epoch = 0;
-        int st = next_epoch(s, stream, &epoch);
+        st = next_epoch(s, stream, &epoch);
         if (st != OSB200_OK) return st;
         osb::BinningConfig cfg = s->cfg;
         cfg.digit_bits = p == places - 1 ? last_bits : 8u;
@@ -213,6 +235,7 @@ int sort_impl(osb200_sorter* s, void* d_keys, uint32_t* d_vals, uint64_t n, cuda
     if (use_plan && (s->short_circuit || (places & 1)))
         OSB_TRY(osb::launch_copy_back(s->plan(), s->alt_keys, d_keys, d_vals ? s->alt_vals : nullptr, d_vals, n, s->key_bytes,
                                       s->sm_count, stream));
+    if (capturing) OSB_TRY(cudaMemsetAsync(s->desc, 0, desc_bytes, stream));
     s->ev_count = ne;
     return OSB200_OK;
 }
@@ -503,8 +526,14 @@ int osb200_digit_binning_pass(osb200_handle h, const void* d_in, void* d_out, co
     if ((d_in_values != nullptr) != (d_out_values != nullptr)) return OSB200_ERR_INVALID_ARG;
     if (d_in_values && (h->key_bytes != 4 || h->value_bytes != 4)) return OSB200_ERR_UNSUPPORTED;
     cudaStream_t q = static_cast<cudaStream_t>(stream);
+    bool capturing = false;
+    int st = is_capturing(q, &capturing);
+    if (st != OSB200_OK) return st;
+    const size_t desc_bytes = tiles_for(n, osb::binning_tile_keys(h->key_bytes, d_in_values != nullptr, h->cfg)) * osb::kRadix *
+                              sizeof(uint64_t);
+    if (capturing) OSB_TRY(cudaMemsetAsync(h->desc, 0, desc_bytes, q));
     // histogram of this digit only, then the pass (the reference's multiples of 8 and any other shift alike)
-    int st = osb_internal_digit_histogram(h, d_in, n, radix_shift, h->ghist(), q);
+    st = osb_internal_digit_histogram(h, d_in, n, radix_shift, h->ghist(), q);
     if (st != OSB200_OK) return st;
     OSB_TRY(cudaMemsetAsync(h->tickets(), 0, ControlLayout::ticket_bytes, q));
     OSB_TRY(osb::launch_scan(h->ghist(), h->gbase(), 1, q));
@@ -518,6 +547,7 @@ int osb200_digit_binning_pass(osb200_handle h, const void* d_in, void* d_out, co
     cfg.digit_bits = key_bits - radix_shift < 8u ? key_bits - radix_shift : 8u;
     OSB_TRY(osb::launch_digit_binning(d_in, d_out, d_in_values, d_out_values, n, h->key_bytes, radix_shift, h->gbase(), h->desc,
                                       h->agg16, h->tickets(), epoch, cfg, q));
+    if (capturing) OSB_TRY(cudaMemsetAsync(h->desc, 0, desc_bytes, q));
     return OSB200_OK;
 }
 
@@ -573,6 +603,11 @@ int osb200_set_option(osb200_handle h, const char* key, int64_t value)
     if (!std::strcmp(key, "debug_max_ctas")) {  // test hook of the persistent pass's tile schedule (0 = off)
         if (value < 0 || value > (1ll << 30)) return OSB200_ERR_INVALID_ARG;
         h->cfg.debug_max_ctas = static_cast<uint32_t>(value);
+        return OSB200_OK;
+    }
+    if (!std::strcmp(key, "debug_epoch")) {  // test hook: the epoch counter, to reach the wrap-around or reuse epochs
+        if (value < 0 || value > osb::kEpochMax) return OSB200_ERR_INVALID_ARG;
+        h->epoch = static_cast<uint32_t>(value);
         return OSB200_OK;
     }
     if (!std::strcmp(key, "variant")) {

@@ -67,7 +67,7 @@ cudaError_t launch_copy_back(const SortPlan* plan, const void* alt_keys, void* k
 
 // DigitBinningPass (reference: OneSweep::DigitBinningPassKeysOnly / Pairs, Sort/OneSweep.cu:164-600).
 //   gbase_place: [256] exclusive global digit bases for this digit place
-//   desc:        [tiles][256] 64-bit tile descriptors (never cleared; `epoch` distinguishes launches)
+//   desc:        [tiles][256] 64-bit tile descriptors (not cleared between eager launches; `epoch` distinguishes them)
 //   agg16:       [tiles][256] 16-bit tile reductions (flag:1|count:15) used by kVariantWide; zeroed per sort
 //   ticket:      one zeroed u32 (dynamic tile id counter, reference `index[]`)
 cudaError_t launch_digit_binning(const void* in, void* out, const uint32_t* in_val, uint32_t* out_val, uint64_t n,

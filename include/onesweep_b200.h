@@ -14,6 +14,11 @@
  *   - Calls are asynchronous on `stream` (a cudaStream_t passed as void*; NULL = default stream) and
  *     never synchronise the host, unlike the reference (cudaDeviceSynchronize inside the dispatch,
  *     OneSweepDispatcher.cuh:318).  One sort in flight per handle; distinct handles are independent.
+ *   - The single-GPU calls may be captured into a CUDA graph (cudaStreamBeginCapture, torch.cuda.graph) and the graph
+ *     replayed with new data in the same buffers.  The chained-scan descriptors carry a per-pass epoch that the host
+ *     passes at launch, so a replay reuses the epochs of the capture: a sort enqueued on a capturing stream therefore
+ *     also clears the descriptors of its tiles (2 KiB per tile) before its first pass and after its last.  Eager calls
+ *     do not.  The sharded sort (osb200_sharded_*) is not supported under capture.
  *   - Return value: 0 on success, a negative osb200_status otherwise.  Nothing aborts or prints (the
  *     reference ignores every CUDA error and printf()s on misuse, OneSweepDispatcher.cuh:195-199).
  *   - n == 0 or 1 is a successful no-op; n > max_n (from create) is OSB200_ERR_SIZE.
@@ -171,6 +176,9 @@ OSB200_API int osb200_init_random_u32(uint32_t* d_keys, uint32_t* d_payload, uin
  *   "debug_stall_every"  test hook for that fallback: N > 0 makes every N-th tile withhold its reduction
  *   "debug_max_ctas" test hook of the persistent DigitBinningPass (uint32 keys, HOT passes): N > 0 runs it on at most N CTAs (the tiles after
  *                    each CTA's first are handed out by an atomic ticket); 0 (default) = as many as can be resident
+ *   "debug_epoch"    test hook of the descriptor epochs: sets the handle's epoch counter (0 .. 2^24 - 1; info "epoch"), so
+ *                    that the next passes cross the wrap-around (which clears every descriptor) or reuse the epochs of a
+ *                    captured sort
  *   "profile"        1 = record CUDA events between the kernels of a sort (osb200_get_profile)
  *   "small_path"     1 (default) = a sort of at most one tile (info "small_path_max_n": 16,384 keys, 8,192 for 64-bit keys)
  *                    is ONE launch of the single-block shared-memory sort (see osb200_segmented_sort_u32); 0 = always the
