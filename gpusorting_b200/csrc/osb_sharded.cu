@@ -14,18 +14,11 @@
 //                keys cross HBM once (read) + NVLink once (write);
 //        staged: DigitBinningPass into a local send buffer, then ncclSend/ncclRecv per peer (baseline).
 //   5. local OneSweep (osb200_sort_keys_u32) on the received keys.
-#include <atomic>
-#include <chrono>
-#include <cstdio>
-#include <cstdlib>
 #include <cstring>
 #include <new>
 #include <vector>
 
-#include <fcntl.h>
 #include <nccl.h>
-#include <sys/mman.h>
-#include <unistd.h>
 
 #include "../../include/onesweep_b200.h"
 #include "osb_internal.h"
@@ -41,23 +34,6 @@ inline int cuda_status(cudaError_t e) { return e == cudaSuccess ? OSB200_OK : OS
         cudaError_t e__ = (expr);                        \
         if (e__ != cudaSuccess) return cuda_status(e__); \
     } while (0)
-// EXPERIMENT, off unless OSB_SHARDED_RENDEZVOUS is set: a host rendezvous of the ranks (POSIX shared memory, busy-polled) at
-// the entry of every sharded sort.  Written while chasing a skew between the ranks at the three collectives of a step at
-// N = 4 / 8 (every kernel at its expected duration, NCCL's tiny collectives fast in isolation).  Starting the steps together
-// with this rendezvous made it worse, so the skew did not come from the hosts entering the call at different times; it
-// came from the benchmark pinning every rank's main thread to core 0 (OMP_PROC_BIND, see bench.py).
-inline void host_rendezvous(std::atomic<unsigned long long>* arrivals, int world)
-{
-    if (!arrivals || world < 2) return;
-    const unsigned long long ticket = arrivals->fetch_add(1, std::memory_order_acq_rel);
-    const unsigned long long target = (ticket / static_cast<unsigned long long>(world) + 1) * static_cast<unsigned long long>(world);
-    const auto t0 = std::chrono::steady_clock::now();
-    unsigned spins = 0;
-    while (arrivals->load(std::memory_order_acquire) < target) {
-        for (int i = 0; i < 32; ++i) __builtin_ia32_pause();
-        if ((++spins & 0xfffu) == 0 && std::chrono::steady_clock::now() - t0 > std::chrono::seconds(1)) return;
-    }
-}
 
 // busy poll (see osb200_sharded_sort_keys_u32): returns as soon as the event has completed
 inline cudaError_t spin_until(cudaEvent_t e)
@@ -75,27 +51,6 @@ inline cudaError_t spin_until(cudaEvent_t e)
 
 }  // namespace
 
-
-// ---- EXPERIMENT (OSB_SHARDED_MAPPED=1, never measured): no copy-engine operations inside a step ---------------------------
-// The all-gathered histograms reach the host, and the plan reaches the device, through MAPPED pinned memory written / read by
-// tiny kernels on the same stream; the host polls a flag word in that memory.  Written while chasing the N = 4 / 8 skew
-// described at host_rendezvous under the hypothesis that a copy ordered behind a long-waiting compute kernel starts late;
-// the skew turned out to come from the benchmark (see bench.py).  Kept as an experiment; it has not been measured.
-__global__ void __launch_bounds__(256)
-publish_to_host_kernel(const unsigned long long* __restrict__ src, volatile unsigned long long* dst_mapped, int count,
-                       volatile unsigned long long* flag_mapped, unsigned long long step)
-{
-    for (int i = threadIdx.x; i < count; i += blockDim.x) dst_mapped[i] = src[i];
-    __threadfence_system();
-    __syncthreads();
-    if (threadIdx.x == 0) { *flag_mapped = step; __threadfence_system(); }
-}
-__global__ void __launch_bounds__(256)
-stage_from_host_kernel(const volatile unsigned long long* src_mapped, unsigned long long* __restrict__ dst, int count)
-{
-    for (int i = threadIdx.x; i < count; i += blockDim.x) dst[i] = src_mapped[i];
-}
-
 struct osb200_sharded_sorter {
     int rank = 0, world = 1;
     ncclComm_t comm = nullptr;
@@ -110,26 +65,13 @@ struct osb200_sharded_sorter {
     unsigned long long* h_hist_all = nullptr;  // pinned
     unsigned long long* h_out_base = nullptr;  // pinned
     unsigned long long* h_coarse_hist = nullptr;  // pinned
-    // device aliases of the three mapped pinned buffers above and of the flag word the host polls
-    unsigned long long* dm_hist_all = nullptr;
-    unsigned long long* dm_out_base = nullptr;
-    unsigned long long* dm_coarse_hist = nullptr;
-    unsigned long long* h_flag = nullptr;
-    unsigned long long* dm_flag = nullptr;
-    unsigned long long step = 0;
-    bool copy_engine = true;   // cudaMemcpyAsync for the 8 KB readback and the 4 KB plan; OSB_SHARDED_MAPPED=1: the kernels below
     uint32_t* d_flag = nullptr;                // 1-element all-reduce used as a stream-ordered cross-GPU barrier
     void* peer_recv[kMaxWorld] = {};           // IPC-mapped receive buffers of all ranks (own = recv_buf)
     bool fused = true;
     bool force_fine = false;  // always use the 256-bucket plan (tests)
     int last_bins = 0;
     cudaEvent_t ev[4] = {};
-    cudaEvent_t tev[3] = {};  // (OSB_SHARDED_TRACE) after the MSD histogram kernel, before / after the exchange kernel
-    bool tev_valid = false;
     cudaEvent_t sync_ev = nullptr;  // host wait for the all-gathered histograms (busy-polled)
-    // host rendezvous of the ranks (all on one node) in POSIX shared memory: keeps the ranks' steps in phase, see host_rendezvous
-    std::atomic<unsigned long long>* shm_arrivals = nullptr;
-    char shm_name[48] = {};
     float last_ms[4] = {0, 0, 0, 0};
 };
 
@@ -209,12 +151,8 @@ int osb200_sharded_destroy(osb200_sharded_handle h)
     cudaFreeHost(h->h_hist_all);
     cudaFreeHost(h->h_out_base);
     cudaFreeHost(h->h_coarse_hist);
-    cudaFreeHost(h->h_flag);
     for (cudaEvent_t e : h->ev) if (e) cudaEventDestroy(e);
-    for (cudaEvent_t e : h->tev) if (e) cudaEventDestroy(e);
     if (h->sync_ev) cudaEventDestroy(h->sync_ev);
-    if (h->shm_arrivals) munmap(static_cast<void*>(h->shm_arrivals), 4096);
-    if (h->shm_name[0] && h->rank == 0) shm_unlink(h->shm_name);
     if (h->comm) ncclCommDestroy(h->comm);
     delete h;
     return OSB200_OK;
@@ -239,21 +177,6 @@ int osb200_sharded_create(osb200_sharded_handle* out, const void* unique_id_128_
     std::memcpy(&id, unique_id_128_bytes, sizeof(id));
     if (ncclCommInitRank(&s->comm, world, id, rank) != ncclSuccess) { osb200_sharded_destroy(s); return OSB200_ERR_NCCL; }
 
-    if (world > 1 && std::getenv("OSB_SHARDED_RENDEZVOUS")) {  // opt-in experiment (measured: it did not help, see host_rendezvous)
-        unsigned long long tag = 0;
-        std::memcpy(&tag, unique_id_128_bytes, sizeof(tag));
-        unsigned long long tag2 = 0;
-        std::memcpy(&tag2, static_cast<const char*>(unique_id_128_bytes) + 8, sizeof(tag2));
-        std::snprintf(s->shm_name, sizeof(s->shm_name), "/osb200_%016llx%016llx", tag, tag2);
-        const int fd = shm_open(s->shm_name, O_CREAT | O_RDWR, 0600);
-        if (fd >= 0) {
-            if (ftruncate(fd, 4096) == 0) {
-                void* p = mmap(nullptr, 4096, PROT_READ | PROT_WRITE, MAP_SHARED, fd, 0);
-                if (p != MAP_FAILED) s->shm_arrivals = static_cast<std::atomic<unsigned long long>*>(p);  // zero-filled on creation
-            }
-            close(fd);
-        }
-    }
     int st = osb200_create(&s->exch, max_n_local, 4, 0);
     if (st == OSB200_OK) st = osb200_create(&s->local, s->capacity, 4, 0);
     if (st != OSB200_OK) { osb200_sharded_destroy(s); return st; }
@@ -262,21 +185,9 @@ int osb200_sharded_create(osb200_sharded_handle* out, const void* unique_id_128_
     ok = ok && cudaMalloc(&s->d_hist_all, static_cast<size_t>(world) * kRadix * sizeof(unsigned long long)) == cudaSuccess;
     ok = ok && cudaMalloc(&s->d_out_base, kRadix * sizeof(unsigned long long)) == cudaSuccess;
     ok = ok && cudaMalloc(&s->d_flag, 64) == cudaSuccess;
-    auto mapped = [&](unsigned long long** host, unsigned long long** dev, size_t count) {
-        void* hp = nullptr;
-        void* dp = nullptr;
-        if (cudaHostAlloc(&hp, count * sizeof(unsigned long long), cudaHostAllocMapped) != cudaSuccess) return false;
-        std::memset(hp, 0, count * sizeof(unsigned long long));
-        *host = static_cast<unsigned long long*>(hp);
-        if (cudaHostGetDevicePointer(&dp, hp, 0) != cudaSuccess) return false;
-        *dev = static_cast<unsigned long long*>(dp);
-        return true;
-    };
-    ok = ok && mapped(&s->h_hist_all, &s->dm_hist_all, static_cast<size_t>(world) * kRadix);
-    ok = ok && mapped(&s->h_out_base, &s->dm_out_base, kRadix);
-    ok = ok && mapped(&s->h_coarse_hist, &s->dm_coarse_hist, kRadix);
-    ok = ok && mapped(&s->h_flag, &s->dm_flag, 8);
-    s->copy_engine = std::getenv("OSB_SHARDED_MAPPED") == nullptr;  // default: cudaMemcpyAsync (the measured path)
+    ok = ok && cudaMallocHost(&s->h_hist_all, static_cast<size_t>(world) * kRadix * sizeof(unsigned long long)) == cudaSuccess;
+    ok = ok && cudaMallocHost(&s->h_out_base, kRadix * sizeof(unsigned long long)) == cudaSuccess;
+    ok = ok && cudaMallocHost(&s->h_coarse_hist, kRadix * sizeof(unsigned long long)) == cudaSuccess;
     for (auto& e : s->ev) ok = ok && cudaEventCreate(&e) == cudaSuccess;
     ok = ok && cudaEventCreateWithFlags(&s->sync_ev, cudaEventDisableTiming) == cudaSuccess;
     if (!ok) { cudaGetLastError(); osb200_sharded_destroy(s); return OSB200_ERR_ALLOC; }
@@ -367,62 +278,16 @@ int osb200_sharded_sort_keys_u32(osb200_sharded_handle h, const uint32_t* d_keys
     cudaStream_t q = static_cast<cudaStream_t>(stream);
     const int R = h->world;
 
-    // OSB_SHARDED_TRACE=1: host-side wall clock of this call's segments on stderr (diagnosis of straggling ranks)
-    static const bool trace = std::getenv("OSB_SHARDED_TRACE") != nullptr;
-    using clk = std::chrono::steady_clock;
-    if (h->shm_arrivals) host_rendezvous(h->shm_arrivals, R);
-    const clk::time_point t0 = clk::now();
-    if (trace) {
-        for (auto& e : h->tev) if (!e) OSB_TRY(cudaEventCreate(&e));
-        if (h->tev_valid) {  // kernel-only durations of the PREVIOUS call (its events have long completed)
-            float a = 0, b = 0, c = 0, d = 0;
-            cudaEventSynchronize(h->ev[3]);
-            cudaEventElapsedTime(&a, h->ev[0], h->tev[0]);
-            cudaEventElapsedTime(&b, h->tev[0], h->ev[1]);
-            cudaEventElapsedTime(&c, h->ev[1], h->tev[1]);
-            cudaEventElapsedTime(&d, h->tev[1], h->tev[2]);
-            float e2 = 0;
-            cudaEventElapsedTime(&e2, h->tev[2], h->ev[2]);
-            std::fprintf(stderr, "[osb sharded rank %d] prev call: MSD hist kernel %.3f ms, allgather+D2H+sync+plan %.3f ms, barrier1+H2D %.3f ms, exchange kernel %.3f ms, barrier2 %.3f ms\n",
-                         h->rank, a, b, c, d, e2);
-        }
-    }
     OSB_TRY(cudaEventRecord(h->ev[0], q));
     // 1-2. most-significant-digit histogram, all-gather
     int st = osb_internal_digit_histogram(h->exch, d_keys_local, n_local, 24, h->d_hist, q);
     if (st != OSB200_OK) return st;
-    if (trace) OSB_TRY(cudaEventRecord(h->tev[0], q));
     OSB_NCCL(ncclAllGather(h->d_hist, h->d_hist_all, kRadix, ncclUint64, h->comm, q));
-    const unsigned long long step = ++h->step;
-    if (h->copy_engine)
-        OSB_TRY(cudaMemcpyAsync(h->h_hist_all, h->d_hist_all, static_cast<size_t>(R) * kRadix * sizeof(unsigned long long),
-                                cudaMemcpyDeviceToHost, q));
-    else
-    {
-        publish_to_host_kernel<<<1, 256, 0, q>>>(h->d_hist_all, h->dm_hist_all, R * kRadix, h->dm_flag, step);
-        OSB_TRY(cudaGetLastError());
-    }
-    const clk::time_point t1 = clk::now();
-    // The plan (and the receive size) is needed on the host: the one host wait of a step.  It polls the flag word the
-    // publishing kernel writes into mapped pinned memory (see publish_to_host_kernel for why no copy engine is involved).
+    OSB_TRY(cudaMemcpyAsync(h->h_hist_all, h->d_hist_all, static_cast<size_t>(R) * kRadix * sizeof(unsigned long long),
+                            cudaMemcpyDeviceToHost, q));
+    // The plan (and the receive size) is needed on the host: the one host wait of a step, busy-polled.
     OSB_TRY(cudaEventRecord(h->sync_ev, q));
-    if (h->copy_engine) {
-        OSB_TRY(spin_until(h->sync_ev));
-    } else {
-        // the flag is written by the kernel after a system-scope fence; the event (recorded behind the kernel) is the safety net
-        const volatile unsigned long long* flag = h->h_flag;
-        unsigned polls = 0;
-        while (*flag != step) {
-            for (int i = 0; i < 16; ++i) __builtin_ia32_pause();
-            if ((++polls & 0x3ffu) == 0) {
-                const cudaError_t r = cudaEventQuery(h->sync_ev);
-                if (r == cudaSuccess) break;  // the kernel has completed: its writes are visible
-                if (r != cudaErrorNotReady) return cuda_status(r);
-            }
-        }
-        std::atomic_thread_fence(std::memory_order_acquire);
-    }
-    const clk::time_point t2 = clk::now();
+    OSB_TRY(spin_until(h->sync_ev));
 
     // 3. plan.  Preferred: R = 2^k ranks and the equal-width split of the key space fits the receive buffers ->
     //    exchange on the top k bits only (R bins instead of 256): runs of ~n/(tiles*R) keys (8 KB at R = 8) keep the
@@ -459,13 +324,7 @@ int osb200_sharded_sort_keys_u32(osb200_sharded_handle h, const uint32_t* d_keys
         for (int d = 0; d < kRadix; ++d) h->h_out_base[d / per] += my_hist[d];
         // (staged through its own pinned buffer: no host sync needed before h_out_base is filled again below)
         std::memcpy(h->h_coarse_hist, h->h_out_base, kRadix * sizeof(unsigned long long));
-        if (h->copy_engine)
-            OSB_TRY(cudaMemcpyAsync(h->d_hist, h->h_coarse_hist, kRadix * sizeof(unsigned long long), cudaMemcpyHostToDevice, q));
-        else
-        {
-            stage_from_host_kernel<<<1, 256, 0, q>>>(h->dm_coarse_hist, h->d_hist, kRadix);
-            OSB_TRY(cudaGetLastError());
-        }
+        OSB_TRY(cudaMemcpyAsync(h->d_hist, h->h_coarse_hist, kRadix * sizeof(unsigned long long), cudaMemcpyHostToDevice, q));
     } else {
         st = osb200_sharded_plan(reinterpret_cast<const uint64_t*>(h->h_hist_all), R, h->rank, dest, recv_count, recv_off);
         if (st != OSB200_OK) return st;
@@ -489,17 +348,9 @@ int osb200_sharded_sort_keys_u32(osb200_sharded_handle h, const uint32_t* d_keys
             const unsigned long long peer = reinterpret_cast<unsigned long long>(h->peer_recv[dest[d]]);
             h->h_out_base[d] = peer / sizeof(uint32_t) + recv_off[d];  // virtual element index relative to address 0
         }
-        if (h->copy_engine)
-            OSB_TRY(cudaMemcpyAsync(h->d_out_base, h->h_out_base, kRadix * sizeof(unsigned long long), cudaMemcpyHostToDevice, q));
-        else
-        {
-            stage_from_host_kernel<<<1, 256, 0, q>>>(h->dm_out_base, h->d_out_base, kRadix);
-            OSB_TRY(cudaGetLastError());
-        }
-        if (trace) OSB_TRY(cudaEventRecord(h->tev[1], q));
+        OSB_TRY(cudaMemcpyAsync(h->d_out_base, h->h_out_base, kRadix * sizeof(unsigned long long), cudaMemcpyHostToDevice, q));
         st = osb_internal_binning_pass(h->exch, d_keys_local, nullptr, n_local, xshift, h->d_hist, h->d_out_base, q);
         if (st != OSB200_OK) return st;
-        if (trace) { OSB_TRY(cudaEventRecord(h->tev[2], q)); h->tev_valid = true; }
         // every rank's scatter kernel has completed (and its NVLink stores are performed) before any local sort starts
         OSB_NCCL(ncclAllReduce(h->d_flag, h->d_flag, 1, ncclUint32, ncclSum, h->comm, q));
     } else {
@@ -532,12 +383,6 @@ int osb200_sharded_sort_keys_u32(osb200_sharded_handle h, const uint32_t* d_keys
     st = osb200_sort_keys_u32(h->local, h->recv_buf, mine, q);
     if (st != OSB200_OK) return st;
     OSB_TRY(cudaEventRecord(h->ev[3], q));
-    if (trace) {
-        const clk::time_point t3 = clk::now();
-        auto us = [](clk::time_point a, clk::time_point b) { return static_cast<long>(std::chrono::duration_cast<std::chrono::microseconds>(b - a).count()); };
-        std::fprintf(stderr, "[osb sharded rank %d] enqueue hist+allgather %ld us, wait %ld us, plan+enqueue exchange+local sort %ld us\n",
-                     h->rank, us(t0, t1), us(t1, t2), us(t2, t3));
-    }
     *d_out = h->recv_buf;
     *n_out = mine;
     return OSB200_OK;

@@ -1,5 +1,6 @@
-"""Sharded sort on >= 2 GPUs (NCCL, one process per GPU): fused NVLink scatter and staged NCCL exchange both
-produce the globally sorted, complete result.  Skipped on a single-GPU box.  -m gpu"""
+"""Sharded sort (NCCL, one process per GPU): fused NVLink scatter and staged NCCL exchange both produce the globally
+sorted, complete result.  The exchange tests need >= 2 GPUs and skip on a single-GPU box; the single-rank test runs the
+host side of the sharded sort on one GPU.  -m gpu"""
 import os
 
 import numpy as np
@@ -72,6 +73,21 @@ def test_sharded_sort_matches_global_sort(fused, fine):
         assert p.exitcode == 0
     res = sorted(q.get(timeout=5) for _ in range(world))
     assert all(ok for _, ok in res)
+
+
+def test_sharded_single_rank():
+    """World size 1: create and destroy, the MSD histogram and its all-gather, the copy to the host and the busy-polled
+    wait for it, the plan and the local sort, with every result compared element by element to np.sort."""
+    import torch.multiprocessing as mp
+
+    ctx = mp.get_context("spawn")
+    q = ctx.Queue()
+    port = 29800 + (os.getpid() % 1000)
+    p = ctx.Process(target=_worker, args=(0, 1, port, (1 << 20) + 12345, True, False, q))
+    p.start()
+    p.join(300)
+    assert p.exitcode == 0
+    assert q.get(timeout=5) == (0, True)
 
 
 def _overflow_worker(rank, world, port, n, q):

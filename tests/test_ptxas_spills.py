@@ -17,8 +17,8 @@ SOURCES = [os.path.join(CSRC, f) for f in ("osb_kernels.cu", "osb_common.cuh", "
     os.path.join(ROOT, "include", "onesweep_b200.h")]
 
 PROPS = re.compile(r"Function properties for (\S+)\s*\n\s*(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads")
-# digit_binning_wide_kernel<KeyT, PAIRS, K, WARPS, RANK_MODE, LOOK, STEP, MINB, HOT>
-WIDE = re.compile(r"_ZN3osb25digit_binning_wide_kernelI([jm])Lb([01])ELi(\d+)ELi(\d+)ELi(\d+)ELi(\d+)ELi(\d+)ELi(\d+)ELb([01])E")
+# digit_binning_wide_kernel<KeyT, PAIRS, K, WARPS, RANK_MODE, LOOK, MINB, HOT>
+WIDE = re.compile(r"_ZN3osb25digit_binning_wide_kernelI([jm])Lb([01])ELi(\d+)ELi(\d+)ELi(\d+)ELi(\d+)ELi(\d+)ELb([01])E")
 HIST = re.compile(r"_ZN3osb23global_histogram_kernelI([jm])Lb([01])E")
 RANK_ATOMIC = 0
 
@@ -46,13 +46,13 @@ def test_parse_report_reads_ptxas_format():
     assert parse_report(text) == [("_ZN3osb1kEv", 88, 92)]
 
 
-def test_hot_path_kernels_do_not_spill():
+def test_hot_path_instantiations_do_not_spill():
     report = _report()
     guarded, seen = [], set()
     for name, st, ld in report:
         w = WIDE.match(name)
         if w and int(w.group(5)) == RANK_ATOMIC:
-            key = ("u64" if w.group(1) == "m" else "u32") + ("/pairs" if w.group(2) == "1" else "/keys") + ("/hot" if w.group(9) == "1" else "")
+            key = ("u64" if w.group(1) == "m" else "u32") + ("/pairs" if w.group(2) == "1" else "/keys") + ("/hot" if w.group(8) == "1" else "")
             seen.add(key)
             guarded.append((f"digit_binning_wide_kernel {key}", st, ld))
         elif HIST.match(name):

@@ -1,4 +1,5 @@
-"""Development probe: per-phase wall clocks of the wide DigitBinningPass (library built with OSB_EXP bit 5 = 32)."""
+"""Development probe: per-phase wall clocks of the wide DigitBinningPass (library built with -DOSB_PHASE_PROBE=1, e.g.
+EXTRA_DEFS=-DOSB_PHASE_PROBE=1 tools/sweep.sh; OSB200_LIB names the library)."""
 import ctypes
 import os
 import sys
@@ -16,7 +17,7 @@ work = src.clone()
 s = g.OneSweepSorter(n, 4, 0)
 s.sort_keys(work)
 torch.cuda.synchronize()
-out = (ctypes.c_ulonglong * 16)()
+out = (ctypes.c_ulonglong * 11)()
 lib.osb200_debug_phases(out, 1)
 work.copy_(src)
 s.sort_keys(work)

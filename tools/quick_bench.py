@@ -11,9 +11,6 @@ from tests import oraclelib  # noqa: E402
 
 PEAK = 3350.0  # GB/s, H100 SXM data sheet (not a measured figure)
 REPS = int(os.environ.get("OSB_REPS", "5"))
-# OSB_PASS_ONLY=1 times single passes only, for the OSB_ABL builds: their passes write wrong keys, so in a whole sort the next
-# pass would get keys whose digit counts no longer match the global histogram its bases come from, and scatter outside its output
-PASS_ONLY = os.environ.get("OSB_PASS_ONLY", "0") not in ("", "0")
 
 
 def time_ms(fn, reps=REPS, prep=None):
@@ -48,7 +45,7 @@ def main():
         dst = torch.empty_like(src)
         for variant in VARIANTS:
             s.set_option("variant", variant)
-            for mode in [] if PASS_ONLY else MODES:
+            for mode in MODES:
                 s.set_option("rank_mode", mode)
                 med, best = time_ms(lambda: s.sort_keys(work), prep=lambda: work.copy_(src))
                 print(f"n=2^{e} keys u32 variant={variant} rank_mode={mode}: median {med:.3f} ms best {best:.3f} ms -> {n/med/1e6:.1f} Gkeys/s, "
@@ -58,9 +55,6 @@ def main():
                 pass_ms, _ = time_ms(lambda: s.digit_binning_pass(src, dst, shift))
                 print(f"   variant={variant} shift={shift}: hist+scan+one pass {pass_ms:.3f} ms => pass ~{pass_ms-hist_ms:.3f} ms "
                       f"({8*n/(pass_ms-hist_ms)/1e6:.0f} GB/s r+w)", flush=True)
-        if PASS_ONLY:
-            s.close()
-            continue
         assert s.validate(work) == 0
         s.close()
         del dst

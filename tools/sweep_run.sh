@@ -1,12 +1,8 @@
 #!/bin/bash
 # run sweep_check (bit-exactness) and quick_bench (keys u32, default variant) with every sweep library;
-# OSB_SKIP_PAIRS=0 times the pairs and u64 sorts as well.  Ablation builds (OSB_ABL != 0) write wrong keys: they are timed
-# one pass at a time from a correct input (OSB_PASS_ONLY), never as whole sorts.
+# OSB_SKIP_PAIRS=0 times the pairs and u64 sorts as well.
 for lib in tools/sweep/*.so; do
   echo "== $lib"
-  case "$lib" in
-    *_A0_*) pass_only=0; OSB200_LIB=$PWD/$lib timeout 120 python tools/sweep_check.py 2>&1 | tail -1;;
-    *) pass_only=1;;
-  esac
-  OSB200_LIB=$PWD/$lib OSB_PASS_ONLY=$pass_only OSB_SKIP_PAIRS=${OSB_SKIP_PAIRS-1} OSB_VARIANTS=2 timeout 180 python tools/quick_bench.py ${1:-30} 2>&1 | grep -E "variant=2|pairs|u64|Error|error|assert" | grep -v REFERENCE
+  OSB200_LIB=$PWD/$lib timeout 120 python tools/sweep_check.py 2>&1 | tail -1
+  OSB200_LIB=$PWD/$lib OSB_SKIP_PAIRS=${OSB_SKIP_PAIRS-1} OSB_VARIANTS=2 timeout 180 python tools/quick_bench.py ${1:-30} 2>&1 | grep -E "variant=2|pairs|u64|Error|error|assert" | grep -v REFERENCE
 done
