@@ -14,6 +14,7 @@ from .onesweep import (  # noqa: F401
     OneSweepDispatcher,
     OneSweepSorter,
     Sort,
+    argsort,
     init_random,
 )
 

@@ -24,7 +24,7 @@
 
 namespace {
 
-constexpr int kVersion = 1002;  // round 2: device plan, bit ranges, forward-progress fallback, hot passes, segmented sort
+constexpr int kVersion = 1003;  // 1002: device plan, bit ranges, forward-progress fallback, hot passes, segmented sort; 1003: argsort
 constexpr int kMaxPlaces = 8;
 
 inline int cuda_status(cudaError_t e) { return e == cudaSuccess ? OSB200_OK : OSB200_ERR_CUDA - static_cast<int>(e); }
@@ -141,8 +141,11 @@ int check_handle(const osb200_sorter* s) { return s ? OSB200_OK : OSB200_ERR_INV
 // The launch plan (reference: OneSweepDispatcher.cuh:311-363): GlobalHistogram, Scan, one DigitBinningPass per digit
 // place of [begin_bit, end_bit), then the (normally empty) copy-back.  Everything is enqueued on `stream`; which passes
 // actually move data is decided on the device (osb::SortPlan): the host never waits for the histogram.
+// keys_in != null is an argsort (osb200_argsort): d_keys / d_vals are its outputs, the keys and indices, and are not read.
+// The histogram reads keys_in, the first executed pass reads keys_in and makes the indices, and the copy-back also covers
+// a sort in which no pass executes.
 int sort_impl(osb200_sorter* s, void* d_keys, uint32_t* d_vals, uint64_t n, cudaStream_t stream,
-              const osb::KeyCodec* codec = nullptr, int begin_bit = 0, int end_bit = -1)
+              const osb::KeyCodec* codec = nullptr, int begin_bit = 0, int end_bit = -1, const void* keys_in = nullptr)
 {
     const int key_bits = s->key_bytes * 8;
     if (end_bit < 0) end_bit = key_bits;
@@ -167,7 +170,7 @@ int sort_impl(osb200_sorter* s, void* d_keys, uint32_t* d_vals, uint64_t n, cuda
         s->ev_count = 0;
         OSB_TRY(osb::launch_segment_sort(d_keys, d_vals, s->key_bytes, nullptr, 1, n, static_cast<uint32_t>(n),
                                          static_cast<uint32_t>(begin_bit), static_cast<uint32_t>(places), last_bits,
-                                         codec ? &c : nullptr, s->cfg.rank_mode, s->sm_count, stream));
+                                         codec ? &c : nullptr, s->cfg.rank_mode, s->sm_count, stream, keys_in));
         return OSB200_OK;
     }
 
@@ -193,7 +196,8 @@ int sort_impl(osb200_sorter* s, void* d_keys, uint32_t* d_vals, uint64_t n, cuda
     osb::KeyCodec enc;  // typed keys: the histogram and the first executed pass see encoded keys, the last one stores them decoded
     if (codec) { enc = *codec; enc.flags = osb::kCodecEncodeOnLoad; }
     if (whole_key)
-        OSB_TRY(osb::launch_global_histogram(d_keys, n, s->key_bytes, s->ghist(), s->sm_count, stream, codec ? &enc : nullptr));
+        OSB_TRY(osb::launch_global_histogram(keys_in ? keys_in : d_keys, n, s->key_bytes, s->ghist(), s->sm_count, stream,
+                                             codec ? &enc : nullptr));
     else
         OSB_TRY(osb::launch_global_histogram_bits(d_keys, n, s->key_bytes, s->ghist(), s->sm_count, stream, codec ? &enc : nullptr,
                                                   static_cast<uint32_t>(begin_bit), places, last_bits));
@@ -216,6 +220,7 @@ int sort_impl(osb200_sorter* s, void* d_keys, uint32_t* d_vals, uint64_t n, cuda
         cfg.place = static_cast<uint32_t>(p);
         if (use_plan) cfg.plan = s->plan();
         cfg.hot_passes = hot_passes;
+        cfg.argsort_in = keys_in;
         if (codec) {
             cfg.codec = *codec;
             cfg.codec.flags = use_plan ? osb::kCodecFromPlan
@@ -232,9 +237,13 @@ int sort_impl(osb200_sorter* s, void* d_keys, uint32_t* d_vals, uint64_t n, cuda
     }
     // an odd number of EXECUTED passes leaves the result in the alt buffers.  Without skipping the count is known here
     // (even for whole keys: no launch); with skipping only the device knows, and the kernel exits at once if it is even.
-    if (use_plan && (s->short_circuit || (places & 1)))
-        OSB_TRY(osb::launch_copy_back(s->plan(), s->alt_keys, d_keys, d_vals ? s->alt_vals : nullptr, d_vals, n, s->key_bytes,
-                                      s->sm_count, stream));
+    if (use_plan && (s->short_circuit || (places & 1))) {
+        if (keys_in)
+            OSB_TRY(osb::launch_argsort_copy_back(s->plan(), keys_in, s->alt_keys, d_keys, s->alt_vals, d_vals, n, s->sm_count, stream));
+        else
+            OSB_TRY(osb::launch_copy_back(s->plan(), s->alt_keys, d_keys, d_vals ? s->alt_vals : nullptr, d_vals, n, s->key_bytes,
+                                          s->sm_count, stream));
+    }
     if (capturing) OSB_TRY(cudaMemsetAsync(s->desc, 0, desc_bytes, stream));
     s->ev_count = ne;
     return OSB200_OK;
@@ -481,6 +490,33 @@ int osb200_sort_pairs_typed(osb200_handle h, void* d_keys, uint32_t* d_values, u
     if (h->cfg.variant != osb::kVariantWide) return OSB200_ERR_UNSUPPORTED;
     const bool plain = c.a == 0 && c.b == 0 && c.d == 0;
     return sort_impl(h, d_keys, d_values, n, static_cast<cudaStream_t>(stream), plain ? nullptr : &c);
+}
+
+int osb200_argsort(osb200_handle h, const void* d_keys_in, void* d_keys_out, uint32_t* d_indices, uint64_t n, int key_type,
+                   int descending, void* stream)
+{
+    if (check_handle(h) != OSB200_OK || h->key_bytes != 4 || h->value_bytes != 4) return OSB200_ERR_INVALID_ARG;
+    osb::KeyCodec c;
+    int st = make_codec(h, key_type, descending, &c);  // 64-bit key types: INVALID_ARG on this 4-byte handle
+    if (st != OSB200_OK) return st;
+    if (h->cfg.variant != osb::kVariantWide) return OSB200_ERR_UNSUPPORTED;  // the indices mode lives in the device plan
+    if (n == 0) return OSB200_OK;
+    const uintptr_t in = reinterpret_cast<uintptr_t>(d_keys_in), out = reinterpret_cast<uintptr_t>(d_keys_out),
+                    idx = reinterpret_cast<uintptr_t>(d_indices);
+    if (!in || !out || !idx || ((in | out | idx) & 15u)) return OSB200_ERR_INVALID_ARG;
+    if (n > h->max_n || n > (1ull << 32)) return OSB200_ERR_SIZE;  // the indices are 32-bit
+    // the input is read until the last pass; outputs that overlap it (or each other) would overwrite keys still to be read
+    const uint64_t bytes = n * sizeof(uint32_t);
+    auto overlap = [bytes](uintptr_t a, uintptr_t b) { return a < b + bytes && b < a + bytes; };
+    if (overlap(in, out) || overlap(in, idx) || overlap(out, idx)) return OSB200_ERR_INVALID_ARG;
+    cudaStream_t q = static_cast<cudaStream_t>(stream);
+    if (n == 1) {  // already sorted, but the outputs still have to be written
+        OSB_TRY(cudaMemcpyAsync(d_keys_out, d_keys_in, sizeof(uint32_t), cudaMemcpyDeviceToDevice, q));
+        OSB_TRY(cudaMemsetAsync(d_indices, 0, sizeof(uint32_t), q));
+        return OSB200_OK;
+    }
+    const bool plain = c.a == 0 && c.b == 0 && c.d == 0;
+    return sort_impl(h, d_keys_out, d_indices, n, q, plain ? nullptr : &c, 0, -1, d_keys_in);
 }
 
 int osb200_sort_host_keys_u32(osb200_handle h, uint32_t* h_keys, uint64_t n)

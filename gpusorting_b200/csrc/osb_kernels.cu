@@ -346,6 +346,39 @@ cudaError_t launch_copy_back(const SortPlan* plan, const void* alt_keys, void* k
     return cudaGetLastError();
 }
 
+// argsort: keys and indices in one launch.  Odd executed passes: both from the alt buffers.  No executed pass (all keys
+// equal): the input is its own stable sort -- keys from the untouched input, indices 0..n-1.  (All pointers 16-byte aligned.)
+__global__ void __launch_bounds__(512)
+argsort_copy_back_kernel(const SortPlan* __restrict__ plan, const uint32_t* __restrict__ keys_in, const uint32_t* __restrict__ alt_keys,
+                         uint32_t* __restrict__ keys, const uint32_t* __restrict__ alt_idx, uint32_t* __restrict__ idx, uint64_t n)
+{
+    const uint32_t ex = plan->executed;
+    if (ex != 0 && !(ex & 1u)) return;
+    const uint32_t* src = ex ? alt_keys : keys_in;
+    const uint64_t vecs = n / 4, stride = static_cast<uint64_t>(gridDim.x) * blockDim.x;
+    for (uint64_t i = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < vecs; i += stride) {
+        __stcs(reinterpret_cast<uint4*>(keys) + i, __ldcs(reinterpret_cast<const uint4*>(src) + i));
+        const uint32_t b = static_cast<uint32_t>(i * 4);
+        __stcs(reinterpret_cast<uint4*>(idx) + i, ex ? __ldcs(reinterpret_cast<const uint4*>(alt_idx) + i) : make_uint4(b, b + 1, b + 2, b + 3));
+    }
+    if (blockIdx.x == 0 && threadIdx.x < (n & 3u)) {
+        const uint64_t j = vecs * 4 + threadIdx.x;
+        keys[j] = src[j];
+        idx[j] = ex ? alt_idx[j] : static_cast<uint32_t>(j);
+    }
+}
+
+cudaError_t launch_argsort_copy_back(const SortPlan* plan, const void* keys_in, const void* alt_keys, void* keys,
+                                     const uint32_t* alt_idx, uint32_t* idx, uint64_t n, int sm_count, cudaStream_t stream)
+{
+    uint64_t want = (n / 4 + 511) / 512;
+    if (want < 1) want = 1;
+    const unsigned grid = static_cast<unsigned>(want < static_cast<uint64_t>(sm_count) * 4 ? want : sm_count * 4);
+    argsort_copy_back_kernel<<<grid, 512, 0, stream>>>(plan, static_cast<const uint32_t*>(keys_in), static_cast<const uint32_t*>(alt_keys),
+                                                       static_cast<uint32_t*>(keys), alt_idx, idx, n);
+    return cudaGetLastError();
+}
+
 // =====================================================================================================
 // Shared pieces of the digit-binning kernels
 // =====================================================================================================
@@ -801,7 +834,12 @@ struct PassParams {
     uint32_t spin_cap;     // lookback polls before the fallback re-reduction
     uint32_t stall_every;  // test hook (0 = off): tiles with tile % N == N-1 never publish their reduction
     const SortPlan* plan;  // device plan or null
+    const void* keys_in = nullptr;  // argsort (INDICES): the caller's untouched keys, read by the first executed pass
 };
+
+// plan_bits of an argsort pass (INDICES): this is the first executed pass -- its keys come from PassParams::keys_in and its
+// payloads are the keys' own input positions
+constexpr uint32_t kPlanBitsFirstIndices = 8u;
 
 // Reads a copy of a value the caller also holds in a register, kept in shared memory for this purpose: the compiler cannot
 // prove the two equal, so whatever is computed from the copy is computed again rather than taken from earlier expressions
@@ -824,16 +862,21 @@ struct WideSmem {
     uint32_t wtot[kRadix / 32];
     uint32_t wmax[kRadix / 32];                      // (HOT) per digit warp: max of (tile count << 8 | digit)
     uint32_t next_tile;                              // the tile this CTA works on after the current one (drawn ticket)
-    uint32_t plan_bits;                              // bit 0: source is the alt buffer; bits 1-2: codec flags of this pass
+    uint32_t plan_bits;                              // bit 0: source is the alt buffer; bits 1-2: codec flags of this pass;
+                                                     // bit 3: first pass of an argsort (kPlanBitsFirstIndices)
     uint32_t digit_shift, digit_mask;                // copies of the pass's digit, re-read by the rank phase (opaque_copy)
 };
 
-template <typename KeyT, bool PAIRS, int K, int WARPS, int RANK_MODE, int LOOK, int MINB, bool HOT = false>
+// INDICES (argsort, pairs only): buf0/val0 are the caller's output keys and indices, buf1/val1 the alt buffers.  The first
+// executed pass, which by the plan's parity would read the caller's side, reads its keys from pp.keys_in instead and makes
+// every payload from the key's position in the input; every other pass is the pairs pass as it is.
+template <typename KeyT, bool PAIRS, int K, int WARPS, int RANK_MODE, int LOOK, int MINB, bool HOT = false, bool INDICES = false>
 __global__ void __launch_bounds__(WARPS * 32, HOT ? OSB_HOT_MINB : MINB)
 digit_binning_wide_kernel(KeyT* buf0, KeyT* buf1, uint32_t* val0, uint32_t* val1, uint64_t n,
                           const unsigned long long* __restrict__ gbase, uint16_t* agg16, uint64_t* incl64,
                           uint32_t* ticket, PassParams pp, KeyCodec codec)
 {
+    static_assert(!INDICES || (PAIRS && sizeof(KeyT) == 4), "the indices are the 32-bit payloads of a pairs pass");
     using S = WideSmem<KeyT, PAIRS, K, WARPS>;
     constexpr int THREADS = S::THREADS;
     constexpr int T = S::T;
@@ -868,6 +911,7 @@ digit_binning_wide_kernel(KeyT* buf0, KeyT* buf1, uint32_t* val0, uint32_t* val1
         my_bits = plan_src_is_alt(pl, pp.place) ? 1u : 0u;
         if (codec.flags & kCodecFromPlan)
             my_bits |= (pp.place == pl.first_exec ? kCodecEncodeOnLoad << 1 : 0u) | (pp.place == pl.last_exec ? kCodecDecodeOnStore << 1 : 0u);
+        if constexpr (INDICES) my_bits |= pp.place == pl.first_exec ? kPlanBitsFirstIndices : 0u;
     }
     if (my_skip) return;  // all keys share this digit: nothing to move (the plan accounts for the parity)
     if (HOT != my_hot) return;  // a pass is executed by exactly one of the two instantiations the host enqueues
@@ -880,15 +924,23 @@ digit_binning_wide_kernel(KeyT* buf0, KeyT* buf1, uint32_t* val0, uint32_t* val1
     const uint32_t warp_off = warp * (32 * K) + lane;
     auto load_tile = [&](uint32_t t) {
         const bool swap = my_bits & 1u;
-        const KeyT* __restrict__ in = swap ? buf1 : buf0;
+        const bool iota = INDICES && (my_bits & kPlanBitsFirstIndices);  // argsort, first pass: payload = input position
+        const KeyT* __restrict__ in = iota ? static_cast<const KeyT*>(pp.keys_in) : swap ? buf1 : buf0;
         const uint32_t* __restrict__ in_val = swap ? val1 : val0;
         const uint64_t base = static_cast<uint64_t>(t) * T;
+        // (an argsort has n <= 2^32: every input position fits the 32-bit payload)
+        const uint32_t pos0 = static_cast<uint32_t>(base) + warp_off;
         if (base + T <= n) {
 #pragma unroll
             for (int i = 0; i < K; ++i) key[i] = ld_stream(in + base + warp_off + i * 32);
             if constexpr (PAIRS) {
+                if (iota) {
 #pragma unroll
-                for (int i = 0; i < K; ++i) val[i] = ld_stream(in_val + base + warp_off + i * 32);
+                    for (int i = 0; i < K; ++i) val[i] = pos0 + i * 32;
+                } else {
+#pragma unroll
+                    for (int i = 0; i < K; ++i) val[i] = ld_stream(in_val + base + warp_off + i * 32);
+                }
             }
         } else {
             const uint32_t live = base < n ? static_cast<uint32_t>(n - base) : 0u;
@@ -896,7 +948,7 @@ digit_binning_wide_kernel(KeyT* buf0, KeyT* buf1, uint32_t* val0, uint32_t* val1
             for (int i = 0; i < K; ++i) {
                 const uint32_t idx = warp_off + i * 32;
                 key[i] = idx < live ? in[base + idx] : static_cast<KeyT>(~static_cast<KeyT>(0));  // pad: ranks last
-                if constexpr (PAIRS) val[i] = idx < live ? in_val[base + idx] : 0u;
+                if constexpr (PAIRS) val[i] = iota ? pos0 + i * 32 : idx < live ? in_val[base + idx] : 0u;
             }
         }
     };
@@ -983,7 +1035,10 @@ digit_binning_wide_kernel(KeyT* buf0, KeyT* buf1, uint32_t* val0, uint32_t* val1
     auto chained_scan = [&]() {
         if (tid < kRadix) {
             TileRereduce<KeyT> rr;
-            rr.in = (sm.plan_bits & 1u) ? buf1 : buf0; rr.tile_keys = T; rr.shift = shift; rr.mask = dmask;
+            // (an argsort's first pass re-reduces the tile it would have loaded: the caller's input)
+            rr.in = (INDICES && (sm.plan_bits & kPlanBitsFirstIndices)) ? static_cast<const KeyT*>(pp.keys_in)
+                    : (sm.plan_bits & 1u) ? buf1 : buf0;
+            rr.tile_keys = T; rr.shift = shift; rr.mask = dmask;
             rr.encode = (sm.plan_bits >> 1) & kCodecEncodeOnLoad;
             rr.ca = static_cast<KeyT>(codec.a); rr.cb = static_cast<KeyT>(codec.b); rr.cd = static_cast<KeyT>(codec.d);
             const unsigned long long prior = lookback_wide<LOOK / 8, KeyT>(agg16, incl64, tile, tid, epoch, pp.spin_cap, rr);
@@ -1569,7 +1624,7 @@ template <> struct WideGeom<uint32_t, false> { static constexpr int K = OSB_WIDE
 template <> struct WideGeom<uint32_t, true>  { static constexpr int K = OSB_PAIRS_WIDE_K, WARPS = OSB_PAIRS_WIDE_WARPS, MINB = OSB_PAIRS_WIDE_MINB, LOOK = OSB_PAIRS_LOOK; };
 template <> struct WideGeom<uint64_t, false> { static constexpr int K = OSB_U64_K, WARPS = OSB_U64_WARPS, MINB = OSB_U64_MINB, LOOK = OSB_U64_LOOK; };
 
-template <typename KeyT, bool PAIRS, int RANK_MODE>
+template <typename KeyT, bool PAIRS, int RANK_MODE, bool INDICES = false>
 static cudaError_t launch_wide_variant(const void* in, void* out, const uint32_t* in_val, uint32_t* out_val, uint64_t n,
                                        uint32_t shift, const unsigned long long* gbase, uint16_t* agg16, uint64_t* incl64,
                                        uint32_t* ticket, uint32_t epoch, const BinningConfig& cfg, cudaStream_t stream)
@@ -1585,6 +1640,7 @@ static cudaError_t launch_wide_variant(const void* in, void* out, const uint32_t
     pp.spin_cap = cfg.spin_cap;
     pp.stall_every = cfg.debug_stall_every;
     pp.plan = cfg.plan;
+    pp.keys_in = cfg.argsort_in;
     // Persistent instantiations (all but the plain u64 keys and pairs passes, which run one CTA per tile): as many CTAs as can be resident
     // at once (capped by debug_max_ctas), at most one per tile; the tiles after the first of each CTA are handed out by
     // `ticket`, which the host zeroes before the pass.
@@ -1599,7 +1655,7 @@ static cudaError_t launch_wide_variant(const void* in, void* out, const uint32_t
         if (cfg.debug_max_ctas && cfg.debug_max_ctas < cap) cap = cfg.debug_max_ctas;
         return static_cast<unsigned>(tiles < cap ? tiles : cap);
     };
-    auto kern = digit_binning_wide_kernel<KeyT, PAIRS, G::K, G::WARPS, RANK_MODE, G::LOOK, G::MINB>;
+    auto kern = digit_binning_wide_kernel<KeyT, PAIRS, G::K, G::WARPS, RANK_MODE, G::LOOK, G::MINB, false, INDICES>;
     static int plain_per_sm = 0;  // (one value per instantiation of this function template)
     // with a device plan `in`/`out` are the caller's and the alt buffers (the kernel picks the direction); both are written
     kern<<<grid_for(kern, plain_per_sm, sizeof(KeyT) == 4 && !PAIRS), S::THREADS, sizeof(S), stream>>>(
@@ -1609,7 +1665,7 @@ static cudaError_t launch_wide_variant(const void* in, void* out, const uint32_t
         // the HOT instantiation of the same pass; returns at once unless the plan calls the pass hot, before drawing a ticket
         // (same geometry, one resident CTA per SM with up to 128 registers: no spills.  Two CTAs per SM at 64 registers
         // spill; 1,024 threads x 16 keys at 64 registers is slower than this)
-        auto hot = digit_binning_wide_kernel<KeyT, PAIRS, G::K, G::WARPS, RANK_MODE, G::LOOK, G::MINB, true>;
+        auto hot = digit_binning_wide_kernel<KeyT, PAIRS, G::K, G::WARPS, RANK_MODE, G::LOOK, G::MINB, true, INDICES>;
         static int hot_per_sm = 0;
         hot<<<grid_for(hot, hot_per_sm, true), S::THREADS, sizeof(S), stream>>>(
             static_cast<KeyT*>(const_cast<void*>(in)), static_cast<KeyT*>(out), const_cast<uint32_t*>(in_val), out_val, n, gbase,
@@ -1650,15 +1706,15 @@ static cudaError_t set_pairs_attr()
                                 cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(sizeof(S)));
 }
 
-template <typename KeyT, bool PAIRS, int RANK_MODE>
+template <typename KeyT, bool PAIRS, int RANK_MODE, bool INDICES = false>
 static cudaError_t set_wide_attr()
 {
     using G = WideGeom<KeyT, PAIRS>;
     using S = WideSmem<KeyT, PAIRS, G::K, G::WARPS>;
-    cudaError_t e = cudaFuncSetAttribute(digit_binning_wide_kernel<KeyT, PAIRS, G::K, G::WARPS, RANK_MODE, G::LOOK, G::MINB>,
+    cudaError_t e = cudaFuncSetAttribute(digit_binning_wide_kernel<KeyT, PAIRS, G::K, G::WARPS, RANK_MODE, G::LOOK, G::MINB, false, INDICES>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(sizeof(S)));
     if (e == cudaSuccess)
-        e = cudaFuncSetAttribute(digit_binning_wide_kernel<KeyT, PAIRS, G::K, G::WARPS, RANK_MODE, G::LOOK, G::MINB, true>,
+        e = cudaFuncSetAttribute(digit_binning_wide_kernel<KeyT, PAIRS, G::K, G::WARPS, RANK_MODE, G::LOOK, G::MINB, true, INDICES>,
                                  cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(sizeof(S)));
     return e;
 }
@@ -1748,6 +1804,8 @@ cudaError_t configure_kernels()
     if ((e = set_wide_attr<uint32_t, true, kRankBallot>()) != cudaSuccess) return e;
     if ((e = set_wide_attr<uint64_t, false, kRankAtomic>()) != cudaSuccess) return e;
     if ((e = set_wide_attr<uint64_t, false, kRankBallot>()) != cudaSuccess) return e;
+    if ((e = set_wide_attr<uint32_t, true, kRankAtomic, true>()) != cudaSuccess) return e;  // argsort
+    if ((e = set_wide_attr<uint32_t, true, kRankBallot, true>()) != cudaSuccess) return e;
     if ((e = set_pairs_attr<kRankAtomic>()) != cudaSuccess) return e;
     if ((e = set_pairs_attr<kRankBallot>()) != cudaSuccess) return e;
     return configure_segment_kernels();
@@ -1760,7 +1818,8 @@ cudaError_t launch_digit_binning(const void* in, void* out, const uint32_t* in_v
 {
     const bool pairs = in_val != nullptr;
     const bool ballot = cfg.rank_mode == kRankBallot;
-    if (cfg.variant != kVariantWide && (cfg.codec.flags || cfg.plan != nullptr || cfg.debug_stall_every)) return cudaErrorNotSupported;
+    if (cfg.variant != kVariantWide && (cfg.codec.flags || cfg.plan != nullptr || cfg.debug_stall_every || cfg.argsort_in))
+        return cudaErrorNotSupported;
     if (cfg.digit_bits < 1 || cfg.digit_bits > 8) return cudaErrorInvalidValue;
     // variants 0 and 1 always take 8-bit digits: a narrower digit is only correct for them when the bits above it do not exist
     if (cfg.variant != kVariantWide && cfg.digit_bits != 8 && shift + cfg.digit_bits != static_cast<uint32_t>(key_bytes) * 8u)
@@ -1771,6 +1830,13 @@ cudaError_t launch_digit_binning(const void* in, void* out, const uint32_t* in_v
                                                            ticket, epoch, cfg, stream)                                 \
             : launch_wide_variant<KEYT, PAIRS, kRankAtomic>(in, out, in_val, out_val, n, shift, gbase_place, agg16, desc, \
                                                            ticket, epoch, cfg, stream))
+        if (cfg.argsort_in != nullptr) {  // argsort: the first executed pass reads argsort_in and makes the indices
+            if (key_bytes != 4 || !pairs || cfg.plan == nullptr) return cudaErrorInvalidValue;
+            return ballot ? launch_wide_variant<uint32_t, true, kRankBallot, true>(in, out, in_val, out_val, n, shift, gbase_place, agg16,
+                                                                                  desc, ticket, epoch, cfg, stream)
+                          : launch_wide_variant<uint32_t, true, kRankAtomic, true>(in, out, in_val, out_val, n, shift, gbase_place, agg16,
+                                                                                  desc, ticket, epoch, cfg, stream);
+        }
         if (key_bytes == 4 && pairs && OSB_PAIRS16K)
             return ballot ? launch_pairs_variant<kRankBallot>(in, out, in_val, out_val, n, shift, gbase_place, agg16, desc, ticket, epoch, cfg, stream)
                           : launch_pairs_variant<kRankAtomic>(in, out, in_val, out_val, n, shift, gbase_place, agg16, desc, ticket, epoch, cfg, stream);
@@ -1820,11 +1886,14 @@ struct SegSmem {
     uint32_t wtot[kRadix / 32];
 };
 
-template <typename KeyT, bool PAIRS, int K, int WARPS, int RANK_MODE>
+// INDICES (argsort of the single segment): the keys come from keys_in, every payload is the key's position in the segment.
+template <typename KeyT, bool PAIRS, int K, int WARPS, int RANK_MODE, bool INDICES = false>
 __global__ void __launch_bounds__(WARPS * 32)
 segment_sort_kernel(KeyT* keys, uint32_t* vals, const unsigned long long* __restrict__ seg_off, uint64_t num_segments,
-                    uint64_t single_n, uint32_t begin_bit, uint32_t places, uint32_t last_bits, KeyCodec codec)
+                    uint64_t single_n, uint32_t begin_bit, uint32_t places, uint32_t last_bits, KeyCodec codec,
+                    const KeyT* __restrict__ keys_in)
 {
+    static_assert(!INDICES || PAIRS, "the indices are the payloads");
     using S = SegSmem<KeyT, PAIRS, K, WARPS>;
     constexpr int THREADS = S::THREADS;
     constexpr int T = S::T;
@@ -1849,10 +1918,10 @@ segment_sort_kernel(KeyT* keys, uint32_t* vals, const unsigned long long* __rest
 #pragma unroll
         for (int i = 0; i < K; ++i) {
             const uint32_t idx = warp_off + i * 32;
-            KeyT k = idx < len ? keys[lo + idx] : static_cast<KeyT>(0);
+            KeyT k = idx < len ? (INDICES ? keys_in : keys)[lo + idx] : static_cast<KeyT>(0);
             if (enc) k = codec_encode<KeyT>(k, ca, cb, cd);
             key[i] = idx < len ? k : static_cast<KeyT>(~static_cast<KeyT>(0));  // padding ranks last in every pass
-            if constexpr (PAIRS) val[i] = idx < len ? vals[lo + idx] : 0u;
+            if constexpr (PAIRS) val[i] = INDICES ? idx : idx < len ? vals[lo + idx] : 0u;
         }
 
         for (uint32_t p = 0; p < places; ++p) {
@@ -1921,11 +1990,11 @@ uint32_t segment_sort_capacity(int key_bytes, bool small)
     return small ? seg_cap<uint32_t, 1>() : seg_cap<uint32_t, 2>();
 }
 
-template <typename KeyT, bool PAIRS, int SIZE, int RANK_MODE>
+template <typename KeyT, bool PAIRS, int SIZE, int RANK_MODE, bool INDICES = false>
 static cudaError_t seg_attr()
 {
     using G = SegGeomN<KeyT, SIZE>;
-    return cudaFuncSetAttribute(segment_sort_kernel<KeyT, PAIRS, G::K, G::WARPS, RANK_MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    return cudaFuncSetAttribute(segment_sort_kernel<KeyT, PAIRS, G::K, G::WARPS, RANK_MODE, INDICES>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                 static_cast<int>(sizeof(SegSmem<KeyT, PAIRS, G::K, G::WARPS>)));
 }
 static cudaError_t configure_segment_kernels()
@@ -1942,33 +2011,42 @@ static cudaError_t configure_segment_kernels()
     OSB_SEG_ATTR(uint32_t, true)
     OSB_SEG_ATTR(uint64_t, false)
 #undef OSB_SEG_ATTR
+    // argsort: the single segment of a sort of at most one tile
+    if ((e = seg_attr<uint32_t, true, 2, kRankAtomic, true>()) != cudaSuccess) return e;
+    if ((e = seg_attr<uint32_t, true, 2, kRankBallot, true>()) != cudaSuccess) return e;
     return cudaSuccess;
 }
 
-template <typename KeyT, bool PAIRS, int SIZE>
+template <typename KeyT, bool PAIRS, int SIZE, bool INDICES = false>
 static cudaError_t launch_seg(void* keys, uint32_t* vals, const unsigned long long* seg_off, uint64_t num_segments, uint64_t single_n,
                               uint32_t begin_bit, uint32_t places, uint32_t last_bits, const KeyCodec& codec, int rank_mode, int sm_count,
-                              cudaStream_t stream)
+                              cudaStream_t stream, const void* keys_in = nullptr)
 {
     using G = SegGeomN<KeyT, SIZE>;
     using S = SegSmem<KeyT, PAIRS, G::K, G::WARPS>;
     const uint64_t cap = static_cast<uint64_t>(sm_count) * (SIZE == 2 ? 2 : 8);
     const unsigned grid = static_cast<unsigned>(num_segments < cap ? num_segments : cap);
+    const KeyT* in = static_cast<const KeyT*>(keys_in);
     if (rank_mode == kRankBallot)
-        segment_sort_kernel<KeyT, PAIRS, G::K, G::WARPS, kRankBallot><<<grid, S::THREADS, sizeof(S), stream>>>(
-            static_cast<KeyT*>(keys), vals, seg_off, num_segments, single_n, begin_bit, places, last_bits, codec);
+        segment_sort_kernel<KeyT, PAIRS, G::K, G::WARPS, kRankBallot, INDICES><<<grid, S::THREADS, sizeof(S), stream>>>(
+            static_cast<KeyT*>(keys), vals, seg_off, num_segments, single_n, begin_bit, places, last_bits, codec, in);
     else
-        segment_sort_kernel<KeyT, PAIRS, G::K, G::WARPS, kRankAtomic><<<grid, S::THREADS, sizeof(S), stream>>>(
-            static_cast<KeyT*>(keys), vals, seg_off, num_segments, single_n, begin_bit, places, last_bits, codec);
+        segment_sort_kernel<KeyT, PAIRS, G::K, G::WARPS, kRankAtomic, INDICES><<<grid, S::THREADS, sizeof(S), stream>>>(
+            static_cast<KeyT*>(keys), vals, seg_off, num_segments, single_n, begin_bit, places, last_bits, codec, in);
     return cudaGetLastError();
 }
 
 cudaError_t launch_segment_sort(void* keys, uint32_t* vals, int key_bytes, const unsigned long long* seg_off, uint64_t num_segments,
                                 uint64_t single_n, uint32_t max_len, uint32_t begin_bit, uint32_t places, uint32_t last_bits,
-                                const KeyCodec* codec_in, int rank_mode, int sm_count, cudaStream_t stream)
+                                const KeyCodec* codec_in, int rank_mode, int sm_count, cudaStream_t stream, const void* keys_in)
 {
     if (num_segments == 0) return cudaSuccess;
     const KeyCodec codec = codec_in ? *codec_in : KeyCodec();
+    if (keys_in != nullptr) {  // argsort: one segment of up to a tile, in the largest geometry (the only one instantiated for it)
+        if (key_bytes != 4 || !vals || seg_off || num_segments != 1 || max_len > seg_cap<uint32_t, 2>()) return cudaErrorInvalidValue;
+        return launch_seg<uint32_t, true, 2, true>(keys, vals, nullptr, 1, single_n, begin_bit, places, last_bits, codec, rank_mode,
+                                                   sm_count, stream, keys_in);
+    }
     const int size = max_len <= (key_bytes == 8 ? seg_cap<uint64_t, 0>() : seg_cap<uint32_t, 0>()) ? 0
                      : max_len <= segment_sort_capacity(key_bytes, true) ? 1 : 2;
     if (max_len > segment_sort_capacity(key_bytes, false)) return cudaErrorInvalidValue;

@@ -138,6 +138,24 @@ class OneSweepSorter:
                                               1 if descending else 0, _stream_ptr(stream)), "osb200_sort_pairs_typed")
         return keys, values
 
+    def argsort(self, keys: torch.Tensor, key_type: str, descending: bool = False, n: Optional[int] = None, stream=None):
+        """Stable sort of keys[:n] that leaves `keys` untouched (osb200_argsort; the shape of torch.sort(stable=True)).
+
+        Returns (sorted_keys, indices): new tensors of n elements on the keys' device, allocated with torch.empty (so the call
+        can be captured in a CUDA graph).  sorted_keys has the dtype of `keys`; indices[i] is the input position of
+        sorted_keys[i], stored as torch.int32, the container of the library's 32-bit payloads.  Positions >= 2^31 (n > 2^31)
+        read as negative in it: ``indices.long() & 0xFFFFFFFF`` recovers them.  key_type is "u32", "i32" or "f32"; equal keys
+        keep their input order in both directions.  Needs a (4, 4) sorter."""
+        n = keys.numel() if n is None else int(n)
+        _check_dev_tensor(keys, _TYPED_DTYPES_4, "keys", n, self.device)
+        with torch.cuda.stream(stream):  # (None: the current stream) the outputs belong to the stream that writes them
+            out = torch.empty(n, dtype=keys.dtype, device=keys.device)
+            idx = torch.empty(n, dtype=torch.int32, device=keys.device)
+        with torch.cuda.device(self.device):
+            check(lib.osb200_argsort(self._h, keys.data_ptr(), out.data_ptr(), idx.data_ptr(), n, KEY_TYPES[key_type],
+                                     1 if descending else 0, _stream_ptr(stream)), "osb200_argsort")
+        return out, idx
+
     def sort_bits(self, keys: torch.Tensor, begin_bit: int, end_bit: int, values: Optional[torch.Tensor] = None,
                   n: Optional[int] = None, stream=None):
         """Stable sort on the key bits [begin_bit, end_bit) only (osb200_sort_bits)."""
@@ -289,6 +307,18 @@ def Sort(keys: torch.Tensor, values: Optional[torch.Tensor] = None, n: Optional[
     if values is None:
         return s.sort_keys(keys, n, stream)
     return s.sort_pairs(keys, values, n, stream)
+
+
+def argsort(keys: torch.Tensor, key_type: str, descending: bool = False, n: Optional[int] = None, stream=None):
+    """Stable (sorted_keys, indices) of 32-bit keys, input untouched: OneSweepSorter.argsort on the cached (4, 4) sorter of
+    the stream (one handle per stream, as for Sort)."""
+    n = keys.numel() if n is None else int(n)
+    if not (isinstance(keys, torch.Tensor) and keys.is_cuda):
+        raise TypeError("keys must be a CUDA tensor")
+    with torch.cuda.device(keys.device.index):
+        sp = _stream_ptr(stream)
+    s = _cached_sorter(keys.device.index, 4, 4, n, sp)
+    return s.argsort(keys, key_type, descending, n, stream)
 
 
 class OneSweepDispatcher:

@@ -43,6 +43,13 @@ class OneSweepSorterB200 {
     {
         check(osb200_sort_keys_typed(h_, d_keys, n, key_type, descending ? 1 : 0, stream), "osb200_sort_keys_typed");
     }
+    // stable sort of d_keys_in (left untouched) into d_keys_out, with d_indices[i] = input position of d_keys_out[i]; 32-bit
+    // key types only, on a (4, 4) sorter; n <= 2^32
+    void ArgSort(const void* d_keys_in, void* d_keys_out, uint32_t* d_indices, uint64_t n, int key_type, bool descending,
+                 void* stream = nullptr)
+    {
+        check(osb200_argsort(h_, d_keys_in, d_keys_out, d_indices, n, key_type, descending ? 1 : 0, stream), "osb200_argsort");
+    }
     // every segment [offsets[i], offsets[i+1]) sorted ascending and stable in place, one thread block per segment
     // (reference: SplitSort, SegSort/SplitSort/SplitSort.cuh:702-938); d_values may be null; max_segment_len <= 16,384
     void SegmentedSort(uint32_t* d_keys, uint32_t* d_values, const uint64_t* d_segment_offsets, uint64_t num_segments,

@@ -102,6 +102,23 @@ OSB200_API int osb200_sort_keys_typed(osb200_handle h, void* d_keys, uint64_t n,
 OSB200_API int osb200_sort_pairs_typed(osb200_handle h, void* d_keys, uint32_t* d_values, uint64_t n, int key_type,
                                        int descending, void* stream);
 
+/* Argsort: the stable sort of d_keys_in[0..n) and its permutation, leaving the input as it is (the shape of torch.sort).
+ * d_keys_in is read and never written; d_keys_out receives the keys sorted, and d_indices[i] the input position of
+ * d_keys_out[i].  Equal keys keep their input order in both directions (the stable descending order of
+ * osb200_sort_pairs_typed).  key_type is OSB200_KEY_U32, _I32 or _F32, ordered as in osb200_sort_keys_typed.
+ * The handle must have key_bytes == 4 and value_bytes == 4: its alternate buffers are the ping-pong partners of d_keys_out
+ * and d_indices, so no other workspace is used.  The indices are made on the device rather than loaded: the histogram and
+ * the first executed digit pass read the keys from d_keys_in, and that pass writes each key's own position as its payload
+ * (every later pass is the pairs pass; a sort of at most 16,384 keys is one launch of the single-block sort).  Against
+ * copying the keys, writing 0..n-1 and calling osb200_sort_pairs_typed this saves the copy, the iota and a payload read.
+ * All three pointers must be 16-byte aligned, and none of the three arrays may overlap another.
+ * Returns OSB200_ERR_INVALID_ARG for a null, misaligned or overlapping pointer, a handle of another shape or a 64-bit
+ * key_type; OSB200_ERR_UNSUPPORTED unless option "variant" is 2 (the default); OSB200_ERR_SIZE when n > max_n or n > 2^32
+ * (the indices are uint32).  n == 0 is a no-op; n == 1 writes d_keys_out[0] = d_keys_in[0] and d_indices[0] = 0.
+ * Asynchronous and graph-capturable like the other single-GPU calls. */
+OSB200_API int osb200_argsort(osb200_handle h, const void* d_keys_in, void* d_keys_out, uint32_t* d_indices, uint64_t n,
+                              int key_type, int descending, void* stream);
+
 /* Sort on a bit range [begin_bit, end_bit) of the (unsigned) key only, CUB-style: keys that agree on those bits keep their
  * input order (stable).  ceil((end_bit-begin_bit)/8) digit passes instead of key_bytes; the last digit may be narrower
  * than 8 bits; an odd pass count is handled inside (the result is always returned in the caller's buffers).  d_values may
