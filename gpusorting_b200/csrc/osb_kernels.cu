@@ -1147,12 +1147,12 @@ digit_binning_wide_kernel(KeyT* buf0, KeyT* buf1, uint32_t* val0, uint32_t* val1
                         KeyT k = static_cast<KeyT>(e.x);
                         if (dec) k = codec_decode<KeyT>(k, ca, cb, cd);
                         KeyT* dst = reinterpret_cast<KeyT*>(kp) + x;
-                        st_stream(dst, k);
-                        st_stream(reinterpret_cast<uint32_t*>(reinterpret_cast<char*>(dst) + val_delta), e.y);
+                        st_scatter(dst, k);
+                        st_scatter(reinterpret_cast<uint32_t*>(reinterpret_cast<char*>(dst) + val_delta), e.y);
                     } else {
                         KeyT k = sm.sorted[x];
                         if (dec) k = codec_decode<KeyT>(k, ca, cb, cd);
-                        st_stream(reinterpret_cast<KeyT*>(kp) + x, k);
+                        st_scatter(reinterpret_cast<KeyT*>(kp) + x, k);
                     }
                 }
             }
@@ -1164,12 +1164,12 @@ digit_binning_wide_kernel(KeyT* buf0, KeyT* buf1, uint32_t* val0, uint32_t* val1
             if constexpr (PAIRS) {
                 const uint2 e = kv[idx];
                 KeyT* dst = reinterpret_cast<KeyT*>(sm.keyptr[digit_of(static_cast<KeyT>(e.x), shift, dmask)]) + idx;
-                st_stream(dst, static_cast<KeyT>(e.x));
-                st_stream(reinterpret_cast<uint32_t*>(reinterpret_cast<char*>(dst) + val_delta), e.y);
+                st_scatter(dst, static_cast<KeyT>(e.x));
+                st_scatter(reinterpret_cast<uint32_t*>(reinterpret_cast<char*>(dst) + val_delta), e.y);
             } else {
                 const KeyT k = sm.sorted[idx];
                 const uint32_t d = digit_of(k, shift, dmask);
-                st_stream(reinterpret_cast<KeyT*>(sm.keyptr[d]) + idx, k);
+                st_scatter(reinterpret_cast<KeyT*>(sm.keyptr[d]) + idx, k);
             }
         }
     } else {  // ragged last tile, or the last pass of a typed sort (keys leave decoded)
@@ -1181,12 +1181,12 @@ digit_binning_wide_kernel(KeyT* buf0, KeyT* buf1, uint32_t* val0, uint32_t* val1
                     const uint2 e = kv[idx];
                     const KeyT k = static_cast<KeyT>(e.x);
                     KeyT* dst = reinterpret_cast<KeyT*>(sm.keyptr[digit_of(k, shift, dmask)]) + idx;
-                    st_stream(dst, dec ? codec_decode<KeyT>(k, ca, cb, cd) : k);
-                    st_stream(reinterpret_cast<uint32_t*>(reinterpret_cast<char*>(dst) + val_delta), e.y);
+                    st_scatter(dst, dec ? codec_decode<KeyT>(k, ca, cb, cd) : k);
+                    st_scatter(reinterpret_cast<uint32_t*>(reinterpret_cast<char*>(dst) + val_delta), e.y);
                 } else {
                     const KeyT k = sm.sorted[idx];
                     const uint32_t d = digit_of(k, shift, dmask);
-                    st_stream(reinterpret_cast<KeyT*>(sm.keyptr[d]) + idx, dec ? codec_decode<KeyT>(k, ca, cb, cd) : k);
+                    st_scatter(reinterpret_cast<KeyT*>(sm.keyptr[d]) + idx, dec ? codec_decode<KeyT>(k, ca, cb, cd) : k);
                 }
             }
         }
