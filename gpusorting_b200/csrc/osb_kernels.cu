@@ -319,27 +319,37 @@ cudaError_t launch_global_histogram_bits(const void* keys, uint64_t n, int key_b
 // =====================================================================================================
 // copy_back: an odd number of executed passes leaves the result in the alt buffers
 // =====================================================================================================
+// W is the word each thread moves: uint4 when both buffers are 16-byte aligned, else uint32_t.  The caller's keys are
+// always 16-byte aligned (sort_impl checks them), but values need only their natural 4-byte alignment, and a 16-byte
+// access to a value buffer that starts at another offset is a misaligned-address fault.
+template <typename W>
 __global__ void __launch_bounds__(512)
-copy_back_kernel(const SortPlan* __restrict__ plan, const uint4* __restrict__ src, uint4* __restrict__ dst, uint64_t vecs,
+copy_back_kernel(const SortPlan* __restrict__ plan, const W* __restrict__ src, W* __restrict__ dst, uint64_t words,
                  const unsigned char* __restrict__ src_tail, unsigned char* __restrict__ dst_tail, uint32_t tail_bytes)
 {
     if (!(plan->executed & 1u)) return;
     const uint64_t stride = static_cast<uint64_t>(gridDim.x) * blockDim.x;
-    for (uint64_t i = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < vecs; i += stride) __stcs(dst + i, __ldcs(src + i));
+    for (uint64_t i = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < words; i += stride) __stcs(dst + i, __ldcs(src + i));
     if (blockIdx.x == 0 && threadIdx.x < tail_bytes) dst_tail[threadIdx.x] = src_tail[threadIdx.x];
 }
 
 cudaError_t launch_copy_back(const SortPlan* plan, const void* alt_keys, void* keys, const uint32_t* alt_vals, uint32_t* vals,
                              uint64_t n, int key_bytes, int sm_count, cudaStream_t stream)
 {
-    auto one = [&](const void* s, void* d, uint64_t bytes) {
-        const uint64_t vecs = bytes / 16;
-        uint64_t want = (vecs + 511) / 512;
+    auto launch = [&](auto word, const void* s, void* d, uint64_t bytes) {
+        using W = decltype(word);
+        const uint64_t words = bytes / sizeof(W);
+        uint64_t want = (words + 511) / 512;
         if (want < 1) want = 1;
         const unsigned grid = static_cast<unsigned>(want < static_cast<uint64_t>(sm_count) * 4 ? want : sm_count * 4);
-        copy_back_kernel<<<grid, 512, 0, stream>>>(plan, static_cast<const uint4*>(s), static_cast<uint4*>(d), vecs,
-                                                   static_cast<const unsigned char*>(s) + vecs * 16,
-                                                   static_cast<unsigned char*>(d) + vecs * 16, static_cast<uint32_t>(bytes - vecs * 16));
+        copy_back_kernel<W><<<grid, 512, 0, stream>>>(plan, static_cast<const W*>(s), static_cast<W*>(d), words,
+                                                      static_cast<const unsigned char*>(s) + words * sizeof(W),
+                                                      static_cast<unsigned char*>(d) + words * sizeof(W),
+                                                      static_cast<uint32_t>(bytes - words * sizeof(W)));
+    };
+    auto one = [&](const void* s, void* d, uint64_t bytes) {
+        if (((reinterpret_cast<uintptr_t>(s) | reinterpret_cast<uintptr_t>(d)) & 15u) == 0) launch(uint4{}, s, d, bytes);
+        else launch(uint32_t{}, s, d, bytes);
     };
     one(alt_keys, keys, n * key_bytes);
     if (vals) one(alt_vals, vals, n * sizeof(uint32_t));

@@ -130,6 +130,8 @@ class OneSweepSorter:
 
     def sort_pairs_typed(self, keys: torch.Tensor, values: torch.Tensor, key_type: str, descending: bool = False,
                          n: Optional[int] = None, stream=None):
+        """sort_keys_typed with 32-bit payloads that move with their keys (stable).  Keys must start on a 16-byte boundary
+        (OneSweepError status -1 otherwise); values need only their natural 4-byte alignment, so any contiguous view will do."""
         n = keys.numel() if n is None else int(n)
         _check_dev_tensor(keys, _TYPED_DTYPES_4, "keys", n, self.device)
         _check_dev_tensor(values, _TYPED_DTYPES_4, "values", n, self.device)
@@ -158,7 +160,8 @@ class OneSweepSorter:
 
     def sort_bits(self, keys: torch.Tensor, begin_bit: int, end_bit: int, values: Optional[torch.Tensor] = None,
                   n: Optional[int] = None, stream=None):
-        """Stable sort on the key bits [begin_bit, end_bit) only (osb200_sort_bits)."""
+        """Stable sort on the key bits [begin_bit, end_bit) only (osb200_sort_bits).  Keys must start on a 16-byte boundary
+        (OneSweepError status -1 otherwise); values need only their natural 4-byte alignment, so any contiguous view will do."""
         n = keys.numel() if n is None else int(n)
         _check_dev_tensor(keys, self._raw(), "keys", n, self.device)
         if values is not None:
@@ -191,6 +194,8 @@ class OneSweepSorter:
         return keys if values is None else (keys, values)
 
     def sort_pairs(self, keys: torch.Tensor, values: torch.Tensor, n: Optional[int] = None, stream=None):
+        """Stable sort of keys[:n] with 32-bit payloads values[:n], in place.  Keys must start on a 16-byte boundary
+        (OneSweepError status -1 otherwise); values need only their natural 4-byte alignment, so any contiguous view will do."""
         n = keys.numel() if n is None else int(n)
         _check_dev_tensor(keys, _KEY_DTYPES_4, "keys", n, self.device)
         _check_dev_tensor(values, _TYPED_DTYPES_4, "values", n, self.device)  # payloads are opaque 32-bit words
