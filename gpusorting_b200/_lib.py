@@ -50,6 +50,11 @@ SIGNATURES = {
     "osb200_sharded_plan": (c_int, [c_vp, c_int, c_int, c_vp, c_vp, c_vp]),
     "osb200_sharded_set_fused": (c_int, [c_vp, c_int]),
     "osb200_sharded_force_fine": (c_int, [c_vp, c_int]),
+    "osb200_sharded_capacity": (c_u64, [c_u64, c_int]),
+    "osb200_sharded_exchange_layout": (c_int, [c_vp, c_int, c_int, c_u64, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
+                                               c_vp, c_vp, c_vp]),
+    "osb200_debug_digit_histogram": (c_int, [c_vp, c_vp, c_u64, c_u32, c_vp, c_vp]),
+    "osb200_debug_exchange_pass": (c_int, [c_vp, c_vp, c_vp, c_u64, c_u32, c_vp, c_vp, c_vp]),
     "osb200_sharded_local_handle": (c_int, [c_vp, ctypes.POINTER(c_vp), ctypes.POINTER(c_vp)]),
     "osb200_sharded_last_timing": (c_int, [c_vp, ctypes.POINTER(ctypes.c_float)]),
 }

@@ -587,6 +587,33 @@ int osb200_digit_binning_pass(osb200_handle h, const void* d_in, void* d_out, co
     return OSB200_OK;
 }
 
+// Testing hooks: the two kernels of the sharded sort's exchange, on an ordinary handle (the sharded sort calls the internal
+// functions directly; nothing here is on a sort path).
+int osb200_debug_digit_histogram(osb200_handle h, const uint32_t* d_in, uint64_t n, uint32_t shift, uint64_t* d_hist256,
+                                 void* stream)
+{
+    if (check_handle(h) != OSB200_OK || h->key_bytes != 4 || !d_hist256 || shift >= 32) return OSB200_ERR_INVALID_ARG;
+    if (n && (!d_in || (reinterpret_cast<uintptr_t>(d_in) & 15u))) return OSB200_ERR_INVALID_ARG;
+    if (n > h->max_n) return OSB200_ERR_SIZE;
+    return osb_internal_digit_histogram(h, d_in, n, shift, reinterpret_cast<unsigned long long*>(d_hist256),
+                                        static_cast<cudaStream_t>(stream));
+}
+
+int osb200_debug_exchange_pass(osb200_handle h, const uint32_t* d_in, uint32_t* d_out, uint64_t n, uint32_t shift,
+                               const uint64_t* d_hist256, const uint64_t* d_out_base, void* stream)
+{
+    if (check_handle(h) != OSB200_OK || h->key_bytes != 4 || shift >= 32) return OSB200_ERR_INVALID_ARG;
+    // fused: the bases are absolute (virtual element indices), so there is no output pointer
+    if (d_out_base && d_out) return OSB200_ERR_INVALID_ARG;
+    if (n == 0) return OSB200_OK;
+    if (!d_in || (reinterpret_cast<uintptr_t>(d_in) & 15u) || d_in == d_out) return OSB200_ERR_INVALID_ARG;
+    // staged: an output and the histogram the pass scans
+    if (!d_out_base && (!d_out || !d_hist256 || (reinterpret_cast<uintptr_t>(d_out) & 3u))) return OSB200_ERR_INVALID_ARG;
+    if (n > h->max_n) return OSB200_ERR_SIZE;
+    return osb_internal_binning_pass(h, d_in, d_out, n, shift, reinterpret_cast<const unsigned long long*>(d_hist256),
+                                     reinterpret_cast<const unsigned long long*>(d_out_base), static_cast<cudaStream_t>(stream));
+}
+
 int osb200_validate(osb200_handle h, const void* d_keys, uint64_t n, uint64_t* h_err_count, void* stream)
 {
     if (check_handle(h) != OSB200_OK || !h_err_count) return OSB200_ERR_INVALID_ARG;

@@ -6,7 +6,8 @@
 //
 //   1. 256-bin histogram of the most significant digit of the local keys            (digit_histogram_kernel)
 //   2. all-gather of the R histograms                                                (ncclAllGather, 2 KB per rank)
-//   3. plan: contiguous bucket ranges -> ranks, balanced on the global counts        (osb200_sharded_plan, host)
+//   3. layout: top log2(R) bits split evenly, or contiguous ranges of 256 buckets      (osb200_sharded_exchange_layout,
+//      balanced on the global counts; bases and offsets of both exchange modes          host)
 //   4. exchange pass, two implementations:
 //        fused  (default): the ordinary DigitBinningPass kernel scatters straight into the peers' receive buffers
 //                through CUDA-IPC-mapped NVLink addresses -- its per-digit output bases are "virtual element indices"
@@ -64,12 +65,11 @@ struct osb200_sharded_sorter {
     unsigned long long* d_out_base = nullptr;  // [256] virtual element indices (fused mode)
     unsigned long long* h_hist_all = nullptr;  // pinned
     unsigned long long* h_out_base = nullptr;  // pinned
-    unsigned long long* h_coarse_hist = nullptr;  // pinned
+    unsigned long long* h_pass_hist = nullptr;  // pinned: the coarse histogram the exchange pass scans
     uint32_t* d_flag = nullptr;                // 1-element all-reduce used as a stream-ordered cross-GPU barrier
     void* peer_recv[kMaxWorld] = {};           // IPC-mapped receive buffers of all ranks (own = recv_buf)
     bool fused = true;
     bool force_fine = false;  // always use the 256-bucket plan (tests)
-    int last_bins = 0;
     cudaEvent_t ev[4] = {};
     cudaEvent_t sync_ev = nullptr;  // host wait for the all-gathered histograms (busy-polled)
     float last_ms[4] = {0, 0, 0, 0};
@@ -125,6 +125,77 @@ OSB200_API int osb200_sharded_plan(const uint64_t* hist_all, int world, int rank
     return OSB200_OK;
 }
 
+OSB200_API uint64_t osb200_sharded_capacity(uint64_t max_n_local, int slack_percent)
+{
+    if (slack_percent < 0 || slack_percent > 400) return 0;
+    return max_n_local + max_n_local / 100 * static_cast<uint64_t>(slack_percent) + 4096;
+}
+
+// The whole host-side layout of one exchange (see the header), as osb200_sharded_sort_keys_u32 uses it.
+//   Preferred: R = 2^k ranks and the equal-width split of the key space fits the receive buffers -> exchange on the top k
+//   bits only (R bins instead of 256): runs of ~n/(tiles*R) keys (8 KB at R = 8) keep the NVLink stores full-sector (short
+//   misaligned runs reach a fraction of the 128-B-aligned peer store rate, tools/microbench/p2p_store_ub.cu) and the ranking
+//   atomics nearly conflict-free.  Otherwise: 256 buckets, greedy (osb200_sharded_plan).
+OSB200_API int osb200_sharded_exchange_layout(const uint64_t* hist_all, int world, int rank, uint64_t capacity, int force_fine,
+                                              const uint64_t* recv_addrs, uint32_t* xshift, int32_t* bins, int32_t* dest,
+                                              uint64_t* recv_count, uint64_t* recv_off, uint64_t* pass_hist,
+                                              uint64_t* out_base, uint64_t* send_off, uint64_t* recv_from_off)
+{
+    if (!hist_all || !xshift || !bins || !dest || !recv_count || !recv_off || !pass_hist || !send_off || !recv_from_off ||
+        world < 1 || world > kMaxWorld || rank < 0 || rank >= world || (recv_addrs == nullptr) != (out_base == nullptr))
+        return OSB200_ERR_INVALID_ARG;
+    if (recv_addrs)
+        for (int q = 0; q < world; ++q)
+            if (recv_addrs[q] % sizeof(uint32_t)) return OSB200_ERR_INVALID_ARG;
+    const int R = world;
+    const uint64_t* mine = hist_all + static_cast<size_t>(rank) * kRadix;
+    int k = 0;
+    while ((1 << k) < R) ++k;
+    const int per = kRadix >> k;  // fine buckets per coarse bin
+    bool coarse = R > 1 && (1 << k) == R && !force_fine;
+    if (coarse) {
+        for (int q = 0; q < R; ++q) recv_count[q] = 0;
+        for (int src = 0; src < R; ++src)
+            for (int d = 0; d < kRadix; ++d) recv_count[d / per] += hist_all[static_cast<size_t>(src) * kRadix + d];
+        for (int q = 0; q < R; ++q) coarse = coarse && recv_count[q] <= capacity;
+    }
+    if (coarse) {
+        *xshift = 32 - k;
+        *bins = R;
+        for (int b = 0; b < kRadix; ++b) { dest[b] = b < R ? b : R - 1; recv_off[b] = 0; pass_hist[b] = 0; }
+        // bucket-major, source-minor: this rank's keys of bin b follow those of every lower source rank
+        for (int src = 0; src < rank; ++src)
+            for (int d = 0; d < kRadix; ++d) recv_off[d / per] += hist_all[static_cast<size_t>(src) * kRadix + d];
+        // the coarse histogram of THIS rank's keys, in the layout the pass expects (bins beyond R are empty)
+        for (int d = 0; d < kRadix; ++d) pass_hist[d / per] += mine[d];
+    } else {
+        *xshift = 24;
+        *bins = kRadix;
+        const int st = osb200_sharded_plan(hist_all, R, rank, dest, recv_count, recv_off);
+        if (st != OSB200_OK) return st;
+        for (int d = 0; d < kRadix; ++d) pass_hist[d] = mine[d];
+    }
+    // Bucket imbalance beyond the capacity.  Every rank computes the whole recv_count[] from the same histograms, so with the
+    // same capacity every rank takes this exit together.
+    for (int q = 0; q < R; ++q)
+        if (recv_count[q] > capacity) return OSB200_ERR_SIZE;
+    if (recv_addrs)
+        for (int d = 0; d < kRadix; ++d) out_base[d] = recv_addrs[dest[d]] / sizeof(uint32_t) + recv_off[d];
+    // staged: the pass output is bin-major and dest[] is non-decreasing, so the bins of one destination are contiguous in
+    // it; a destination receives source-major
+    for (int p = 0; p <= R; ++p) send_off[p] = 0;
+    for (int b = 0; b < kRadix; ++b) send_off[dest[b] + 1] += pass_hist[b];
+    for (int p = 0; p < R; ++p) send_off[p + 1] += send_off[p];
+    recv_from_off[0] = 0;
+    for (int src = 0; src < R; ++src) {
+        uint64_t c = 0;
+        for (int d = 0; d < kRadix; ++d)
+            if (dest[coarse ? d / per : d] == rank) c += hist_all[static_cast<size_t>(src) * kRadix + d];
+        recv_from_off[src + 1] = recv_from_off[src] + c;
+    }
+    return OSB200_OK;
+}
+
 int osb200_sharded_unique_id(void* out_128_bytes)
 {
     if (!out_128_bytes) return OSB200_ERR_INVALID_ARG;
@@ -150,7 +221,7 @@ int osb200_sharded_destroy(osb200_sharded_handle h)
     cudaFree(h->d_flag);
     cudaFreeHost(h->h_hist_all);
     cudaFreeHost(h->h_out_base);
-    cudaFreeHost(h->h_coarse_hist);
+    cudaFreeHost(h->h_pass_hist);
     for (cudaEvent_t e : h->ev) if (e) cudaEventDestroy(e);
     if (h->sync_ev) cudaEventDestroy(h->sync_ev);
     if (h->comm) ncclCommDestroy(h->comm);
@@ -171,7 +242,7 @@ int osb200_sharded_create(osb200_sharded_handle* out, const void* unique_id_128_
     s->rank = rank;
     s->world = world;
     s->max_n_local = max_n_local;
-    s->capacity = max_n_local + max_n_local / 100 * slack_percent + 4096;
+    s->capacity = osb200_sharded_capacity(max_n_local, slack_percent);
 
     ncclUniqueId id;
     std::memcpy(&id, unique_id_128_bytes, sizeof(id));
@@ -187,7 +258,7 @@ int osb200_sharded_create(osb200_sharded_handle* out, const void* unique_id_128_
     ok = ok && cudaMalloc(&s->d_flag, 64) == cudaSuccess;
     ok = ok && cudaMallocHost(&s->h_hist_all, static_cast<size_t>(world) * kRadix * sizeof(unsigned long long)) == cudaSuccess;
     ok = ok && cudaMallocHost(&s->h_out_base, kRadix * sizeof(unsigned long long)) == cudaSuccess;
-    ok = ok && cudaMallocHost(&s->h_coarse_hist, kRadix * sizeof(unsigned long long)) == cudaSuccess;
+    ok = ok && cudaMallocHost(&s->h_pass_hist, kRadix * sizeof(unsigned long long)) == cudaSuccess;
     for (auto& e : s->ev) ok = ok && cudaEventCreate(&e) == cudaSuccess;
     ok = ok && cudaEventCreateWithFlags(&s->sync_ev, cudaEventDisableTiming) == cudaSuccess;
     if (!ok) { cudaGetLastError(); osb200_sharded_destroy(s); return OSB200_ERR_ALLOC; }
@@ -289,65 +360,36 @@ int osb200_sharded_sort_keys_u32(osb200_sharded_handle h, const uint32_t* d_keys
     OSB_TRY(cudaEventRecord(h->sync_ev, q));
     OSB_TRY(spin_until(h->sync_ev));
 
-    // 3. plan.  Preferred: R = 2^k ranks and the equal-width split of the key space fits the receive buffers ->
-    //    exchange on the top k bits only (R bins instead of 256): runs of ~n/(tiles*R) keys (8 KB at R = 8) keep the
-    //    NVLink stores full-sector (short misaligned runs reach a fraction of the 128-B-aligned peer store rate,
-    //    tools/microbench/p2p_store_ub.cu) and the ranking atomics nearly conflict-free.  Otherwise: 256 buckets, greedy.
+    // 3. layout (osb200_sharded_exchange_layout): which bits the exchange pass bins on, where every bucket goes, the
+    //    histogram the pass scans, the fused pass's per-bucket bases and the staged send/receive offsets.  OSB200_ERR_SIZE
+    //    when the buckets do not fit the slack chosen at create: every rank holds the whole recv_count[] and the same
+    //    capacity (max_n_local and slack_percent must be identical on all ranks), so ALL ranks take this exit together,
+    //    before any collective or peer store of the exchange: nobody is left waiting in a barrier for a rank that bailed out.
     int32_t dest[kRadix];
-    uint64_t recv_count[kMaxWorld], recv_off[kRadix];
+    uint64_t recv_count[kMaxWorld], recv_off[kRadix], send_off[kMaxWorld + 1], roff[kMaxWorld + 1], recv_addrs[kMaxWorld];
     uint32_t xshift = 24;  // digit position of the exchange pass
-    int bins = kRadix;
-    int k = 0;
-    while ((1 << k) < R) ++k;
-    bool coarse = R > 1 && (1 << k) == R && !h->force_fine;
-    if (coarse) {
-        const int per = kRadix >> k;
-        for (int q2 = 0; q2 < R; ++q2) recv_count[q2] = 0;
-        for (int src = 0; src < R; ++src)
-            for (int d = 0; d < kRadix; ++d) recv_count[d / per] += h->h_hist_all[static_cast<size_t>(src) * kRadix + d];
-        for (int q2 = 0; q2 < R; ++q2) coarse = coarse && recv_count[q2] <= h->capacity;
-    }
-    if (coarse) {
-        const int per = kRadix >> k;
-        xshift = 32 - k;
-        bins = R;
-        for (int b = 0; b < kRadix; ++b) { dest[b] = b < R ? b : R - 1; recv_off[b] = 0; }
-        for (int b = 0; b < R; ++b) {
-            uint64_t off = 0;
-            for (int src = 0; src < h->rank; ++src)
-                for (int d = b * per; d < (b + 1) * per; ++d) off += h->h_hist_all[static_cast<size_t>(src) * kRadix + d];
-            recv_off[b] = off;
-        }
-        // the coarse histogram of THIS rank's keys, in the layout the pass expects (bins beyond R are empty)
-        for (int b = 0; b < kRadix; ++b) h->h_out_base[b] = 0;
-        const unsigned long long* my_hist = h->h_hist_all + static_cast<size_t>(h->rank) * kRadix;
-        for (int d = 0; d < kRadix; ++d) h->h_out_base[d / per] += my_hist[d];
-        // (staged through its own pinned buffer: no host sync needed before h_out_base is filled again below)
-        std::memcpy(h->h_coarse_hist, h->h_out_base, kRadix * sizeof(unsigned long long));
-        OSB_TRY(cudaMemcpyAsync(h->d_hist, h->h_coarse_hist, kRadix * sizeof(unsigned long long), cudaMemcpyHostToDevice, q));
-    } else {
-        st = osb200_sharded_plan(reinterpret_cast<const uint64_t*>(h->h_hist_all), R, h->rank, dest, recv_count, recv_off);
-        if (st != OSB200_OK) return st;
-    }
-    h->last_bins = bins;
+    int32_t bins = kRadix;
+    const bool fused = R > 1 && h->fused;
+    if (fused)
+        for (int r = 0; r < R; ++r) recv_addrs[r] = reinterpret_cast<uint64_t>(h->peer_recv[r]);
+    // (h_out_base and h_pass_hist are free: the wait above ordered the previous call's copies from them)
+    st = osb200_sharded_exchange_layout(reinterpret_cast<const uint64_t*>(h->h_hist_all), R, h->rank, h->capacity,
+                                        h->force_fine ? 1 : 0, fused ? recv_addrs : nullptr, &xshift, &bins, dest, recv_count,
+                                        recv_off, reinterpret_cast<uint64_t*>(h->h_pass_hist),
+                                        fused ? reinterpret_cast<uint64_t*>(h->h_out_base) : nullptr, send_off, roff);
+    if (st != OSB200_OK) return st;
     const uint64_t mine = recv_count[h->rank];
-    // Bucket imbalance beyond the slack chosen at create.  Every rank holds the whole recv_count[] and the same capacity
-    // (max_n_local and slack_percent must be identical on all ranks), so ALL ranks take this exit together, before any
-    // collective or peer store of the exchange: nobody is left waiting in a barrier for a rank that bailed out.
-    for (int r = 0; r < R; ++r)
-        if (recv_count[r] > h->capacity) return OSB200_ERR_SIZE;
+    // d_hist holds this rank's 256-bucket histogram already; a coarse pass scans the coarse one
+    if (bins != kRadix)
+        OSB_TRY(cudaMemcpyAsync(h->d_hist, h->h_pass_hist, kRadix * sizeof(unsigned long long), cudaMemcpyHostToDevice, q));
     OSB_TRY(cudaEventRecord(h->ev[1], q));
 
     // 4. exchange
     if (R == 1) {
         OSB_TRY(cudaMemcpyAsync(h->recv_buf, d_keys_local, n_local * sizeof(uint32_t), cudaMemcpyDeviceToDevice, q));
-    } else if (h->fused) {
+    } else if (fused) {
         // all ranks have finished reading their receive buffers from the previous call before anyone writes
         OSB_NCCL(ncclAllReduce(h->d_flag, h->d_flag, 1, ncclUint32, ncclSum, h->comm, q));
-        for (int d = 0; d < kRadix; ++d) {
-            const unsigned long long peer = reinterpret_cast<unsigned long long>(h->peer_recv[dest[d]]);
-            h->h_out_base[d] = peer / sizeof(uint32_t) + recv_off[d];  // virtual element index relative to address 0
-        }
         OSB_TRY(cudaMemcpyAsync(h->d_out_base, h->h_out_base, kRadix * sizeof(unsigned long long), cudaMemcpyHostToDevice, q));
         st = osb_internal_binning_pass(h->exch, d_keys_local, nullptr, n_local, xshift, h->d_hist, h->d_out_base, q);
         if (st != OSB200_OK) return st;
@@ -357,20 +399,10 @@ int osb200_sharded_sort_keys_u32(osb200_sharded_handle h, const uint32_t* d_keys
         st = osb_internal_binning_pass(h->exch, d_keys_local, h->send_buf, n_local, xshift, h->d_hist, nullptr, q);
         if (st != OSB200_OK) return st;
         // send_buf is bin-major; the bins of destination p are contiguous.  Receive source-major.
-        uint64_t send_off[kMaxWorld + 1] = {}, send_cnt[kMaxWorld] = {}, roff[kMaxWorld + 1] = {};
-        const int per = coarse ? (kRadix >> k) : 1;
-        const unsigned long long* my_hist = h->h_hist_all + static_cast<size_t>(h->rank) * kRadix;
-        for (int d = 0; d < kRadix; ++d) send_cnt[dest[coarse ? d / per : d]] += my_hist[d];
-        for (int p = 0; p < R; ++p) send_off[p + 1] = send_off[p] + send_cnt[p];
-        for (int src = 0; src < R; ++src) {
-            uint64_t c = 0;
-            for (int d = 0; d < kRadix; ++d)
-                if (dest[coarse ? d / per : d] == h->rank) c += h->h_hist_all[static_cast<size_t>(src) * kRadix + d];
-            roff[src + 1] = roff[src] + c;
-        }
         OSB_NCCL(ncclGroupStart());
         for (int p = 0; p < R; ++p) {
-            if (send_cnt[p]) OSB_NCCL(ncclSend(h->send_buf + send_off[p], send_cnt[p], ncclUint32, p, h->comm, q));
+            if (send_off[p + 1] - send_off[p])
+                OSB_NCCL(ncclSend(h->send_buf + send_off[p], send_off[p + 1] - send_off[p], ncclUint32, p, h->comm, q));
             if (roff[p + 1] - roff[p]) OSB_NCCL(ncclRecv(h->recv_buf + roff[p], roff[p + 1] - roff[p], ncclUint32, p, h->comm, q));
         }
         OSB_NCCL(ncclGroupEnd());

@@ -34,6 +34,38 @@ def plan(hist_all: np.ndarray, rank: int):
     return dest, recv_count, recv_off
 
 
+def capacity(max_n_local: int, slack_percent: int) -> int:
+    """Keys every rank's receive buffer holds (osb200_sharded_capacity)."""
+    c = int(lib.osb200_sharded_capacity(int(max_n_local), int(slack_percent)))
+    if c == 0:
+        raise ValueError(f"slack_percent={slack_percent} is outside 0..400")
+    return c
+
+
+def exchange_layout(hist_all: np.ndarray, rank: int, capacity: int, force_fine: bool = False, recv_addrs=None) -> dict:
+    """The sharded sort's host-side exchange layout (osb200_sharded_exchange_layout; pure function, usable without a GPU).
+
+    hist_all: [world, 256] uint64 top-byte counts of every rank; recv_addrs: the byte addresses of the world receive
+    buffers, or None.  Returns a dict with xshift, bins, dest, recv_count, recv_off, pass_hist, out_base (None without
+    recv_addrs), send_off and recv_from_off; raises OneSweepError with status -2 when neither split fits `capacity`."""
+    h = np.ascontiguousarray(hist_all, dtype=np.uint64)
+    world = h.shape[0]
+    xshift, bins = ctypes.c_uint32(0), ctypes.c_int32(0)
+    out = {"dest": np.empty(256, np.int32), "recv_count": np.empty(world, np.uint64), "recv_off": np.empty(256, np.uint64),
+           "pass_hist": np.empty(256, np.uint64), "send_off": np.empty(world + 1, np.uint64),
+           "recv_from_off": np.empty(world + 1, np.uint64)}
+    addrs = None if recv_addrs is None else np.ascontiguousarray(recv_addrs, dtype=np.uint64)
+    out["out_base"] = None if addrs is None else np.empty(256, np.uint64)
+    check(lib.osb200_sharded_exchange_layout(
+        h.ctypes.data, world, int(rank), int(capacity), 1 if force_fine else 0, None if addrs is None else addrs.ctypes.data,
+        ctypes.byref(xshift), ctypes.byref(bins), out["dest"].ctypes.data, out["recv_count"].ctypes.data,
+        out["recv_off"].ctypes.data, out["pass_hist"].ctypes.data,
+        None if addrs is None else out["out_base"].ctypes.data, out["send_off"].ctypes.data,
+        out["recv_from_off"].ctypes.data), "osb200_sharded_exchange_layout")
+    out["xshift"], out["bins"] = int(xshift.value), int(bins.value)
+    return out
+
+
 class _DevicePtr:
     """Zero-copy view of handle-owned device memory as a torch tensor (CUDA array interface)."""
 

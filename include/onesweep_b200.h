@@ -249,6 +249,32 @@ OSB200_API int osb200_sharded_sort_keys_u32(osb200_sharded_handle h, const uint3
  * source-rank-minor: the globally stable order of the MSD partition). */
 OSB200_API int osb200_sharded_plan(const uint64_t* hist_all /*[world][256]*/, int world, int rank, int32_t* dest,
                                    uint64_t* recv_count, uint64_t* recv_off);
+/* Keys every rank's receive buffer holds: max_n_local + max_n_local / 100 * slack_percent + 4096 (integer division), the
+ * capacity osb200_sharded_create allocates.  0 for a slack_percent outside 0..400. */
+OSB200_API uint64_t osb200_sharded_capacity(uint64_t max_n_local, int slack_percent);
+/* The whole host-side layout of one exchange, a pure function of the all-gathered histograms that
+ * osb200_sharded_sort_keys_u32 calls on every rank (exported so the layout and, with the two debug hooks below, the
+ * exchange pass itself can be tested without NCCL or a second GPU).  Inputs: hist_all[world][256] (the counts of every
+ * rank's top bytes), this `rank`, the receive `capacity` in keys, force_fine (see osb200_sharded_force_fine), and
+ * recv_addrs[world], the byte addresses of the receive buffers (4-byte aligned; NULL when no fused bases are wanted).
+ * Outputs:
+ *   *xshift, *bins   the exchange pass's digit: 32 - log2(world) and world bins when world is a power of two > 1, force_fine
+ *                    is 0 and every rank's share of the equal-width split fits `capacity` (coarse); else 24 and 256 (fine)
+ *   dest[256]        destination rank of every bin (coarse: bin b < world goes to rank b; fine: osb200_sharded_plan's)
+ *   recv_count[world] keys every rank receives
+ *   recv_off[256]    for this rank as a source, the element offset of its keys of bin b in dest[b]'s receive buffer:
+ *                    bucket-major, source-rank-minor, the stable order of the MSD partition
+ *   pass_hist[256]   the histogram the exchange pass scans: this rank's counts of its digit (coarse: bins 0..world-1)
+ *   out_base[256]    only if recv_addrs: the fused pass's base of every bin as a virtual element index,
+ *                    recv_addrs[dest[b]] / 4 + recv_off[b] (recv_addrs and out_base go together)
+ *   send_off[world+1]      staged: destination p's keys are [send_off[p], send_off[p+1]) of the pass's bin-major output
+ *   recv_from_off[world+1] staged: this rank receives source s's keys at [recv_from_off[s], recv_from_off[s+1])
+ * Returns OSB200_ERR_SIZE when neither split fits `capacity` -- the same on every rank, so all ranks stop together; then
+ * only xshift, bins, dest and recv_count are meaningful (the fine plan that does not fit). */
+OSB200_API int osb200_sharded_exchange_layout(const uint64_t* hist_all, int world, int rank, uint64_t capacity, int force_fine,
+                                              const uint64_t* recv_addrs, uint32_t* xshift, int32_t* bins, int32_t* dest,
+                                              uint64_t* recv_count, uint64_t* recv_off, uint64_t* pass_hist,
+                                              uint64_t* out_base, uint64_t* send_off, uint64_t* recv_from_off);
 /* 1 (default when CUDA IPC peer mapping works) = the exchange is the DigitBinningPass kernel scattering straight into
  * the peers' receive buffers over NVLink; 0 = staged: local pass + ncclSend/ncclRecv.  Same value on every rank. */
 OSB200_API int osb200_sharded_set_fused(osb200_sharded_handle h, int fused);
@@ -256,6 +282,20 @@ OSB200_API int osb200_sharded_set_fused(osb200_sharded_handle h, int fused);
  * receive buffers, the exchange bins on the top log2(world) bits only (long runs, full NVLink sectors); otherwise on
  * the top 8 bits with the greedy plan.  on=1 forces the 256-bucket plan (tests / skewed data).  Same on every rank. */
 OSB200_API int osb200_sharded_force_fine(osb200_sharded_handle h, int on);
+/* Testing hooks on an ordinary single-GPU handle (key_bytes 4), for running every rank's exchange pass in one process:
+ *   osb200_debug_digit_histogram  d_hist256[256] = counts of the digit (d_in[i] >> shift) & 0xFF over d_in[0..n), the
+ *                                 sharded sort's first step (shift 24)
+ *   osb200_debug_exchange_pass    the sharded sort's exchange pass over d_in[0..n), binning on the digit at `shift` (8 bits,
+ *                                 or 32 - shift bits above 24), stable.  With d_out_base (device [256]: the out_base of
+ *                                 osb200_sharded_exchange_layout) the keys of bin b go to the 4-byte words at virtual
+ *                                 element indices d_out_base[b], d_out_base[b] + 1, ... -- plain device addresses divided by
+ *                                 4 -- and d_out must be NULL (fused mode); without it the pass scans d_hist256, which must
+ *                                 hold the counts of that digit, into d_out (staged mode: the stable bin-major partition).
+ * d_in must be 16-byte aligned, n <= max_n, shift < 32.  Asynchronous on `stream`; not supported under graph capture. */
+OSB200_API int osb200_debug_digit_histogram(osb200_handle h, const uint32_t* d_in, uint64_t n, uint32_t shift,
+                                            uint64_t* d_hist256, void* stream);
+OSB200_API int osb200_debug_exchange_pass(osb200_handle h, const uint32_t* d_in, uint32_t* d_out, uint64_t n, uint32_t shift,
+                                          const uint64_t* d_hist256, const uint64_t* d_out_base, void* stream);
 /* The two single-GPU sorters inside a sharded sorter (exchange pass / local sort), e.g. to set options. */
 OSB200_API int osb200_sharded_local_handle(osb200_sharded_handle h, osb200_handle* exch, osb200_handle* local);
 /* Milliseconds of the phases of the last sharded sort on this rank: [0]=histogram+allgather,
