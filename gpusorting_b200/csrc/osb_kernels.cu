@@ -1897,10 +1897,11 @@ struct SegSmem {
 };
 
 // INDICES (argsort of the single segment): the keys come from keys_in, every payload is the key's position in the segment.
+// max_len: the caller's max_segment_len (<= T); longer segments are left as they are.
 template <typename KeyT, bool PAIRS, int K, int WARPS, int RANK_MODE, bool INDICES = false>
 __global__ void __launch_bounds__(WARPS * 32)
 segment_sort_kernel(KeyT* keys, uint32_t* vals, const unsigned long long* __restrict__ seg_off, uint64_t num_segments,
-                    uint64_t single_n, uint32_t begin_bit, uint32_t places, uint32_t last_bits, KeyCodec codec,
+                    uint64_t single_n, uint32_t max_len, uint32_t begin_bit, uint32_t places, uint32_t last_bits, KeyCodec codec,
                     const KeyT* __restrict__ keys_in)
 {
     static_assert(!INDICES || PAIRS, "the indices are the payloads");
@@ -1920,7 +1921,8 @@ segment_sort_kernel(KeyT* keys, uint32_t* vals, const unsigned long long* __rest
     for (uint64_t seg = blockIdx.x; seg < num_segments; seg += gridDim.x) {
         const uint64_t lo = seg_off ? seg_off[seg] : 0ull;
         const uint64_t hi = seg_off ? seg_off[seg + 1] : single_n;
-        if (hi <= lo + 1 || hi - lo > static_cast<uint64_t>(T)) continue;  // empty / one key / too long (caller's contract)
+        // empty / one key / longer than max_segment_len or the geometry (both the caller's contract: left untouched)
+        if (hi <= lo + 1 || hi - lo > static_cast<uint64_t>(max_len) || hi - lo > static_cast<uint64_t>(T)) continue;
         const uint32_t len = static_cast<uint32_t>(hi - lo);
 
         KeyT key[K];
@@ -2029,8 +2031,8 @@ static cudaError_t configure_segment_kernels()
 
 template <typename KeyT, bool PAIRS, int SIZE, bool INDICES = false>
 static cudaError_t launch_seg(void* keys, uint32_t* vals, const unsigned long long* seg_off, uint64_t num_segments, uint64_t single_n,
-                              uint32_t begin_bit, uint32_t places, uint32_t last_bits, const KeyCodec& codec, int rank_mode, int sm_count,
-                              cudaStream_t stream, const void* keys_in = nullptr)
+                              uint32_t max_len, uint32_t begin_bit, uint32_t places, uint32_t last_bits, const KeyCodec& codec,
+                              int rank_mode, int sm_count, cudaStream_t stream, const void* keys_in = nullptr)
 {
     using G = SegGeomN<KeyT, SIZE>;
     using S = SegSmem<KeyT, PAIRS, G::K, G::WARPS>;
@@ -2039,10 +2041,10 @@ static cudaError_t launch_seg(void* keys, uint32_t* vals, const unsigned long lo
     const KeyT* in = static_cast<const KeyT*>(keys_in);
     if (rank_mode == kRankBallot)
         segment_sort_kernel<KeyT, PAIRS, G::K, G::WARPS, kRankBallot, INDICES><<<grid, S::THREADS, sizeof(S), stream>>>(
-            static_cast<KeyT*>(keys), vals, seg_off, num_segments, single_n, begin_bit, places, last_bits, codec, in);
+            static_cast<KeyT*>(keys), vals, seg_off, num_segments, single_n, max_len, begin_bit, places, last_bits, codec, in);
     else
         segment_sort_kernel<KeyT, PAIRS, G::K, G::WARPS, kRankAtomic, INDICES><<<grid, S::THREADS, sizeof(S), stream>>>(
-            static_cast<KeyT*>(keys), vals, seg_off, num_segments, single_n, begin_bit, places, last_bits, codec, in);
+            static_cast<KeyT*>(keys), vals, seg_off, num_segments, single_n, max_len, begin_bit, places, last_bits, codec, in);
     return cudaGetLastError();
 }
 
@@ -2054,13 +2056,13 @@ cudaError_t launch_segment_sort(void* keys, uint32_t* vals, int key_bytes, const
     const KeyCodec codec = codec_in ? *codec_in : KeyCodec();
     if (keys_in != nullptr) {  // argsort: one segment of up to a tile, in the largest geometry (the only one instantiated for it)
         if (key_bytes != 4 || !vals || seg_off || num_segments != 1 || max_len > seg_cap<uint32_t, 2>()) return cudaErrorInvalidValue;
-        return launch_seg<uint32_t, true, 2, true>(keys, vals, nullptr, 1, single_n, begin_bit, places, last_bits, codec, rank_mode,
-                                                   sm_count, stream, keys_in);
+        return launch_seg<uint32_t, true, 2, true>(keys, vals, nullptr, 1, single_n, max_len, begin_bit, places, last_bits, codec,
+                                                   rank_mode, sm_count, stream, keys_in);
     }
     const int size = max_len <= (key_bytes == 8 ? seg_cap<uint64_t, 0>() : seg_cap<uint32_t, 0>()) ? 0
                      : max_len <= segment_sort_capacity(key_bytes, true) ? 1 : 2;
     if (max_len > segment_sort_capacity(key_bytes, false)) return cudaErrorInvalidValue;
-#define OSB_SEG_ARGS keys, vals, seg_off, num_segments, single_n, begin_bit, places, last_bits, codec, rank_mode, sm_count, stream
+#define OSB_SEG_ARGS keys, vals, seg_off, num_segments, single_n, max_len, begin_bit, places, last_bits, codec, rank_mode, sm_count, stream
 #define OSB_SEG(KEYT, PAIRS) \
     (size == 0 ? launch_seg<KEYT, PAIRS, 0>(OSB_SEG_ARGS) : size == 1 ? launch_seg<KEYT, PAIRS, 1>(OSB_SEG_ARGS) : launch_seg<KEYT, PAIRS, 2>(OSB_SEG_ARGS))
     if (key_bytes == 4) return vals ? OSB_SEG(uint32_t, true) : OSB_SEG(uint32_t, false);

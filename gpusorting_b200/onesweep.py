@@ -176,7 +176,7 @@ class OneSweepSorter:
         """Sort every segment [offsets[i], offsets[i+1]) of `keys` (and `values`) ascending and stable, in place, one thread
         block per segment (osb200_segmented_sort_u32; reference: SplitSort, SegSort/SplitSort/SplitSort.cuh:702-938).
         `segment_offsets`: int64 device tensor of num_segments + 1 offsets.  `max_segment_len` (default: computed here, which
-        costs a device->host read) must not exceed 16,384."""
+        costs a device->host read) must not exceed 16,384; segments longer than `max_segment_len` are left as they are."""
         _check_dev_tensor(keys, _KEY_DTYPES_4, "keys", keys.numel(), self.device)
         if values is not None:
             _check_dev_tensor(values, _TYPED_DTYPES_4, "values", keys.numel(), self.device)

@@ -117,6 +117,12 @@ def test_types_orders_and_sizes(g, key_type, descending):
                 kin = kin.view(torch.float32)
             out, idx = run(s, kin, key_type, descending)
             numpy_check(bits, key_type, descending, out, idx, f"n={n}")
+        for mode in rank_modes(s):  # the single-block path's instantiation of each rank mode
+            s.set_option("rank_mode", mode)
+            for n in [x for x in ns if x <= 16384]:
+                bits = typed_input(rng, n, key_type)
+                out, idx = run(s, dev(bits), key_type, descending)
+                numpy_check(bits, key_type, descending, out, idx, f"n={n} rank_mode={mode}")
         s.set_option("small_path", 0)  # the multi-kernel path at the single-block path's sizes
         for n in [x for x in ns if x <= 16384]:
             bits = typed_input(rng, n, key_type)

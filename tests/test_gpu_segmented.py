@@ -20,13 +20,15 @@ def seg_oracle(keys: np.ndarray, offs: np.ndarray):
     return out_k, out_v
 
 
-def run_segmented(g, lens, mask, pairs, seed, max_len=None):
+def run_segmented(g, lens, mask, pairs, seed, max_len=None, mode=None):
     rng = np.random.default_rng(seed)
     offs = np.concatenate([[0], np.cumsum(lens)]).astype(np.int64)
     n = int(offs[-1])
     keys = rng.integers(0, 1 << 32, n, dtype=np.uint64).astype(np.uint32) & np.uint32(mask)
     wk, wv = seg_oracle(keys, offs)
     with g.OneSweepSorter(max(n, 16), 4, 4 if pairs else 0) as s:
+        if mode is not None:
+            s.set_option("rank_mode", mode)
         tk = torch.from_numpy(keys.view(np.int32).copy()).cuda()
         tv = torch.arange(n, dtype=torch.int32, device="cuda") if pairs else None
         to = torch.from_numpy(offs).cuda()
@@ -36,21 +38,25 @@ def run_segmented(g, lens, mask, pairs, seed, max_len=None):
             assert np.array_equal(tv.cpu().numpy().view(np.uint32), wv)
 
 
+@pytest.mark.parametrize("mode", [0, 1])
 @pytest.mark.parametrize("pairs", [False, True])
-def test_segmented_random_lengths(pairs):
+def test_segmented_random_lengths(pairs, mode):
     import gpusorting_b200 as g
 
+    with g.OneSweepSorter(16, 4, 0) as s:
+        if mode not in ([0, 1] if s.info("atomic_order_ok") else [1]):
+            pytest.skip("the atomic rank mode does not keep lane order on this device")
     rng = np.random.default_rng(3)
     # short segments (the 2,048-key geometry), empty ones and single keys included
     lens = rng.integers(0, 2049, 700)
     lens[:6] = [0, 1, 2, 2048, 2047, 0]
-    run_segmented(g, lens, 0xFFFFFFFF, pairs, 11)
-    run_segmented(g, lens, 0xFF, pairs, 12)  # many ties: stability
+    run_segmented(g, lens, 0xFFFFFFFF, pairs, 11, mode=mode)
+    run_segmented(g, lens, 0xFF, pairs, 12, mode=mode)  # many ties: stability
     # up to a full tile (the 16,384-key geometry)
     lens = rng.integers(0, 16385, 60)
     lens[:5] = [16384, 16383, 2049, 0, 1]
-    run_segmented(g, lens, 0xFFFFFFFF, pairs, 13)
-    run_segmented(g, lens, 0xF0F, pairs, 14)
+    run_segmented(g, lens, 0xFFFFFFFF, pairs, 13, mode=mode)
+    run_segmented(g, lens, 0xF0F, pairs, 14, mode=mode)
 
 
 def test_segmented_many_tiny_segments_and_bounds():
@@ -109,7 +115,7 @@ def test_small_n_path_equals_the_ordinary_path(oracle, mode):
                 assert np.array_equal(t.cpu().numpy(), np.sort(f)[::-1]), (n, small)
             s.set_option("small_path", 1)
             if n <= 8192:
-                k8 = (k.astype(np.uint64) << np.uint64(32)) | np.uint64(n)
+                k8 = oracle.init_random_u64(n, 0, 900 + n)  # random in both words: every one of the 8 digit passes moves keys
                 for small in (1, 0):
                     s8.set_option("small_path", small)
                     t = torch.from_numpy(k8.view(np.int64).copy()).cuda()
