@@ -15,6 +15,7 @@ from .onesweep import (  # noqa: F401
     OneSweepSorter,
     Sort,
     argsort,
+    argsort16,
     init_random,
 )
 

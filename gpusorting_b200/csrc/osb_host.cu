@@ -24,7 +24,8 @@
 
 namespace {
 
-constexpr int kVersion = 1003;  // 1002: device plan, bit ranges, forward-progress fallback, hot passes, segmented sort; 1003: argsort
+constexpr int kVersion = 1004;  // 1002: device plan, bit ranges, forward-progress fallback, hot passes, segmented sort; 1003: argsort;
+                                // 1004: 16-bit keys (osb200_sort_keys16, osb200_sort_pairs16, osb200_argsort16)
 constexpr int kMaxPlaces = 8;
 
 inline int cuda_status(cudaError_t e) { return e == cudaSuccess ? OSB200_OK : OSB200_ERR_CUDA - static_cast<int>(e); }
@@ -144,10 +145,13 @@ int check_handle(const osb200_sorter* s) { return s ? OSB200_OK : OSB200_ERR_INV
 // keys_in != null is an argsort (osb200_argsort): d_keys / d_vals are its outputs, the keys and indices, and are not read.
 // The histogram reads keys_in, the first executed pass reads keys_in and makes the indices, and the copy-back also covers
 // a sort in which no pass executes.
-int sort_impl(osb200_sorter* s, void* d_keys, uint32_t* d_vals, uint64_t n, cudaStream_t stream,
+// key_bytes is the width of the keys being sorted: the handle's own, or 2 for the 16-bit calls (osb200_sort_keys16 & co.),
+// which run on a 4-byte handle -- its alternate buffers (4 B per key), descriptors (sized for its smallest tile, which the
+// 16-bit tiles are not below) and reductions (four digit places) cover a 16-bit sort of up to max_n keys.
+int sort_impl(osb200_sorter* s, int key_bytes, void* d_keys, uint32_t* d_vals, uint64_t n, cudaStream_t stream,
               const osb::KeyCodec* codec = nullptr, int begin_bit = 0, int end_bit = -1, const void* keys_in = nullptr)
 {
-    const int key_bits = s->key_bytes * 8;
+    const int key_bits = key_bytes * 8;
     if (end_bit < 0) end_bit = key_bits;
     if (begin_bit < 0 || end_bit > key_bits || begin_bit > end_bit) return OSB200_ERR_INVALID_ARG;
     if (n <= 1 || begin_bit == end_bit) return OSB200_OK;
@@ -164,11 +168,11 @@ int sort_impl(osb200_sorter* s, void* d_keys, uint32_t* d_vals, uint64_t n, cuda
     const bool use_plan = wide;
 
     // small-n path (SURVEY 8f rank 4): up to one tile of keys is sorted by ONE CTA in shared memory, one launch
-    if (wide && s->small_path && n <= osb::segment_sort_capacity(s->key_bytes, false)) {
+    if (wide && s->small_path && n <= osb::segment_sort_capacity(key_bytes, false)) {
         osb::KeyCodec c;
         if (codec) { c = *codec; c.flags = osb::kCodecEncodeOnLoad | osb::kCodecDecodeOnStore; }
         s->ev_count = 0;
-        OSB_TRY(osb::launch_segment_sort(d_keys, d_vals, s->key_bytes, nullptr, 1, n, static_cast<uint32_t>(n),
+        OSB_TRY(osb::launch_segment_sort(d_keys, d_vals, key_bytes, nullptr, 1, n, static_cast<uint32_t>(n),
                                          static_cast<uint32_t>(begin_bit), static_cast<uint32_t>(places), last_bits,
                                          codec ? &c : nullptr, s->cfg.rank_mode, s->sm_count, stream, keys_in));
         return OSB200_OK;
@@ -177,7 +181,7 @@ int sort_impl(osb200_sorter* s, void* d_keys, uint32_t* d_vals, uint64_t n, cuda
     bool capturing = false;
     int st = is_capturing(stream, &capturing);
     if (st != OSB200_OK) return st;
-    const uint32_t tile_keys = osb::binning_tile_keys(s->key_bytes, d_vals != nullptr, s->cfg);
+    const uint32_t tile_keys = osb::binning_tile_keys(key_bytes, d_vals != nullptr, s->cfg);
     const size_t desc_bytes = tiles_for(n, tile_keys) * osb::kRadix * sizeof(uint64_t);
     if (capturing) OSB_TRY(cudaMemsetAsync(s->desc, 0, desc_bytes, stream));
     OSB_TRY(cudaMemsetAsync(s->control, 0, ControlLayout::zeroed_bytes, stream));
@@ -196,10 +200,10 @@ int sort_impl(osb200_sorter* s, void* d_keys, uint32_t* d_vals, uint64_t n, cuda
     osb::KeyCodec enc;  // typed keys: the histogram and the first executed pass see encoded keys, the last one stores them decoded
     if (codec) { enc = *codec; enc.flags = osb::kCodecEncodeOnLoad; }
     if (whole_key)
-        OSB_TRY(osb::launch_global_histogram(keys_in ? keys_in : d_keys, n, s->key_bytes, s->ghist(), s->sm_count, stream,
+        OSB_TRY(osb::launch_global_histogram(keys_in ? keys_in : d_keys, n, key_bytes, s->ghist(), s->sm_count, stream,
                                              codec ? &enc : nullptr));
     else
-        OSB_TRY(osb::launch_global_histogram_bits(d_keys, n, s->key_bytes, s->ghist(), s->sm_count, stream, codec ? &enc : nullptr,
+        OSB_TRY(osb::launch_global_histogram_bits(d_keys, n, key_bytes, s->ghist(), s->sm_count, stream, codec ? &enc : nullptr,
                                                   static_cast<uint32_t>(begin_bit), places, last_bits));
     OSB_TRY(mark());
     // hot passes (low-entropy inputs): the default kernel has a second instantiation for them; both are enqueued per pass
@@ -228,7 +232,7 @@ int sort_impl(osb200_sorter* s, void* d_keys, uint32_t* d_vals, uint64_t n, cuda
         }
         // with a plan every launch gets (caller buffers, alt buffers) and picks its direction on the device
         OSB_TRY(osb::launch_digit_binning(use_plan ? d_keys : src, use_plan ? s->alt_keys : dst, use_plan ? d_vals : sv,
-                                          use_plan ? (d_vals ? s->alt_vals : nullptr) : dv, n, s->key_bytes,
+                                          use_plan ? (d_vals ? s->alt_vals : nullptr) : dv, n, key_bytes,
                                           static_cast<uint32_t>(begin_bit + 8 * p), s->gbase() + p * osb::kRadix, s->desc,
                                           s->agg16 + p * agg_stride, s->tickets() + p, epoch, cfg, stream));
         OSB_TRY(mark());
@@ -239,9 +243,10 @@ int sort_impl(osb200_sorter* s, void* d_keys, uint32_t* d_vals, uint64_t n, cuda
     // (even for whole keys: no launch); with skipping only the device knows, and the kernel exits at once if it is even.
     if (use_plan && (s->short_circuit || (places & 1))) {
         if (keys_in)
-            OSB_TRY(osb::launch_argsort_copy_back(s->plan(), keys_in, s->alt_keys, d_keys, s->alt_vals, d_vals, n, s->sm_count, stream));
+            OSB_TRY(osb::launch_argsort_copy_back(s->plan(), keys_in, s->alt_keys, d_keys, s->alt_vals, d_vals, n, key_bytes, s->sm_count,
+                                                      stream));
         else
-            OSB_TRY(osb::launch_copy_back(s->plan(), s->alt_keys, d_keys, d_vals ? s->alt_vals : nullptr, d_vals, n, s->key_bytes,
+            OSB_TRY(osb::launch_copy_back(s->plan(), s->alt_keys, d_keys, d_vals ? s->alt_vals : nullptr, d_vals, n, key_bytes,
                                           s->sm_count, stream));
     }
     if (capturing) OSB_TRY(cudaMemsetAsync(s->desc, 0, desc_bytes, stream));
@@ -271,7 +276,7 @@ int sort_host_impl(osb200_sorter* s, void* h_keys, uint32_t* h_vals, uint64_t n)
     cudaStream_t q = s->own_stream;
     OSB_TRY(cudaMemcpyAsync(s->stage_keys, h_keys, n * s->key_bytes, cudaMemcpyHostToDevice, q));
     if (h_vals) OSB_TRY(cudaMemcpyAsync(s->stage_vals, h_vals, n * sizeof(uint32_t), cudaMemcpyHostToDevice, q));
-    st = sort_impl(s, s->stage_keys, h_vals ? s->stage_vals : nullptr, n, q);
+    st = sort_impl(s, s->key_bytes, s->stage_keys, h_vals ? s->stage_vals : nullptr, n, q);
     if (st != OSB200_OK) return st;
     OSB_TRY(cudaMemcpyAsync(h_keys, s->stage_keys, n * s->key_bytes, cudaMemcpyDeviceToHost, q));
     if (h_vals) OSB_TRY(cudaMemcpyAsync(h_vals, s->stage_vals, n * sizeof(uint32_t), cudaMemcpyDeviceToHost, q));
@@ -412,20 +417,20 @@ int osb200_destroy(osb200_handle h)
 int osb200_sort_keys_u32(osb200_handle h, uint32_t* d_keys, uint64_t n, void* stream)
 {
     if (check_handle(h) != OSB200_OK || h->key_bytes != 4) return OSB200_ERR_INVALID_ARG;
-    return sort_impl(h, d_keys, nullptr, n, static_cast<cudaStream_t>(stream));  // a pairs-capable sorter may sort keys only
+    return sort_impl(h, h->key_bytes, d_keys, nullptr, n, static_cast<cudaStream_t>(stream));  // a pairs-capable sorter may sort keys only
 }
 
 int osb200_sort_pairs_u32(osb200_handle h, uint32_t* d_keys, uint32_t* d_values, uint64_t n, void* stream)
 {
     if (check_handle(h) != OSB200_OK || h->key_bytes != 4 || h->value_bytes != 4) return OSB200_ERR_INVALID_ARG;
     if (n > 1 && !d_values) return OSB200_ERR_INVALID_ARG;
-    return sort_impl(h, d_keys, d_values, n, static_cast<cudaStream_t>(stream));
+    return sort_impl(h, h->key_bytes, d_keys, d_values, n, static_cast<cudaStream_t>(stream));
 }
 
 int osb200_sort_keys_u64(osb200_handle h, uint64_t* d_keys, uint64_t n, void* stream)
 {
     if (check_handle(h) != OSB200_OK || h->key_bytes != 8) return OSB200_ERR_INVALID_ARG;
-    return sort_impl(h, d_keys, nullptr, n, static_cast<cudaStream_t>(stream));
+    return sort_impl(h, h->key_bytes, d_keys, nullptr, n, static_cast<cudaStream_t>(stream));
 }
 
 // Typed keys (SURVEY 8f rank 1).  key_type must match the handle's key width.
@@ -455,7 +460,7 @@ int osb200_sort_keys_typed(osb200_handle h, void* d_keys, uint64_t n, int key_ty
     if (st != OSB200_OK) return st;
     if (h->cfg.variant != osb::kVariantWide) return OSB200_ERR_UNSUPPORTED;
     const bool plain = c.a == 0 && c.b == 0 && c.d == 0;
-    return sort_impl(h, d_keys, nullptr, n, static_cast<cudaStream_t>(stream), plain ? nullptr : &c);
+    return sort_impl(h, h->key_bytes, d_keys, nullptr, n, static_cast<cudaStream_t>(stream), plain ? nullptr : &c);
 }
 
 int osb200_segmented_sort_u32(osb200_handle h, uint32_t* d_keys, uint32_t* d_values, const uint64_t* d_segment_offsets,
@@ -476,7 +481,7 @@ int osb200_sort_bits(osb200_handle h, void* d_keys, uint32_t* d_values, uint64_t
 {
     if (check_handle(h) != OSB200_OK) return OSB200_ERR_INVALID_ARG;
     if (d_values && (h->key_bytes != 4 || h->value_bytes != 4)) return OSB200_ERR_INVALID_ARG;
-    return sort_impl(h, d_keys, d_values, n, static_cast<cudaStream_t>(stream), nullptr, begin_bit, end_bit);
+    return sort_impl(h, h->key_bytes, d_keys, d_values, n, static_cast<cudaStream_t>(stream), nullptr, begin_bit, end_bit);
 }
 
 int osb200_sort_pairs_typed(osb200_handle h, void* d_keys, uint32_t* d_values, uint64_t n, int key_type, int descending,
@@ -489,7 +494,7 @@ int osb200_sort_pairs_typed(osb200_handle h, void* d_keys, uint32_t* d_values, u
     if (st != OSB200_OK) return st;
     if (h->cfg.variant != osb::kVariantWide) return OSB200_ERR_UNSUPPORTED;
     const bool plain = c.a == 0 && c.b == 0 && c.d == 0;
-    return sort_impl(h, d_keys, d_values, n, static_cast<cudaStream_t>(stream), plain ? nullptr : &c);
+    return sort_impl(h, h->key_bytes, d_keys, d_values, n, static_cast<cudaStream_t>(stream), plain ? nullptr : &c);
 }
 
 int osb200_argsort(osb200_handle h, const void* d_keys_in, void* d_keys_out, uint32_t* d_indices, uint64_t n, int key_type,
@@ -516,7 +521,76 @@ int osb200_argsort(osb200_handle h, const void* d_keys_in, void* d_keys_out, uin
         return OSB200_OK;
     }
     const bool plain = c.a == 0 && c.b == 0 && c.d == 0;
-    return sort_impl(h, d_keys_out, d_indices, n, q, plain ? nullptr : &c, 0, -1, d_keys_in);
+    return sort_impl(h, h->key_bytes, d_keys_out, d_indices, n, q, plain ? nullptr : &c, 0, -1, d_keys_in);
+}
+
+// 16-bit keys (osb200_key16_type) on a 4-byte handle: the same driver with a key width of 2 -- two digit passes.  F16 and
+// BF16 share the float codec (sign bit 15); they differ only in the dtype the caller keeps them in.
+static int make_codec16(int key_type, int descending, osb::KeyCodec* c)
+{
+    switch (key_type) {
+        case OSB200_KEY16_U16: c->a = 0; c->b = 0; break;
+        case OSB200_KEY16_I16: c->a = 0; c->b = 0x8000u; break;
+        case OSB200_KEY16_F16:
+        case OSB200_KEY16_BF16: c->a = 0xFFFFu; c->b = 0x8000u; break;
+        default: return OSB200_ERR_INVALID_ARG;
+    }
+    c->d = descending ? 0xFFFFu : 0;
+    c->flags = 0;
+    return OSB200_OK;
+}
+
+static int check_16(const osb200_sorter* h, bool pairs, int key_type, int descending, osb::KeyCodec* c)
+{
+    if (check_handle(h) != OSB200_OK || h->key_bytes != 4 || (pairs && h->value_bytes != 4)) return OSB200_ERR_INVALID_ARG;
+    const int st = make_codec16(key_type, descending, c);
+    if (st != OSB200_OK) return st;
+    if (h->cfg.variant != osb::kVariantWide) return OSB200_ERR_UNSUPPORTED;
+    return OSB200_OK;
+}
+
+int osb200_sort_keys16(osb200_handle h, void* d_keys, uint64_t n, int key_type, int descending, void* stream)
+{
+    osb::KeyCodec c;
+    const int st = check_16(h, false, key_type, descending, &c);
+    if (st != OSB200_OK) return st;
+    const bool plain = c.a == 0 && c.b == 0 && c.d == 0;
+    return sort_impl(h, 2, d_keys, nullptr, n, static_cast<cudaStream_t>(stream), plain ? nullptr : &c);
+}
+
+int osb200_sort_pairs16(osb200_handle h, void* d_keys, uint32_t* d_values, uint64_t n, int key_type, int descending, void* stream)
+{
+    osb::KeyCodec c;
+    const int st = check_16(h, true, key_type, descending, &c);
+    if (st != OSB200_OK) return st;
+    if (n > 1 && !d_values) return OSB200_ERR_INVALID_ARG;
+    const bool plain = c.a == 0 && c.b == 0 && c.d == 0;
+    return sort_impl(h, 2, d_keys, d_values, n, static_cast<cudaStream_t>(stream), plain ? nullptr : &c);
+}
+
+int osb200_argsort16(osb200_handle h, const void* d_keys_in, void* d_keys_out, uint32_t* d_indices, uint64_t n, int key_type,
+                     int descending, void* stream)
+{
+    osb::KeyCodec c;
+    const int st = check_16(h, true, key_type, descending, &c);
+    if (st != OSB200_OK) return st;
+    if (n == 0) return OSB200_OK;
+    const uintptr_t in = reinterpret_cast<uintptr_t>(d_keys_in), out = reinterpret_cast<uintptr_t>(d_keys_out),
+                    idx = reinterpret_cast<uintptr_t>(d_indices);
+    if (!in || !out || !idx || ((in | out | idx) & 15u)) return OSB200_ERR_INVALID_ARG;
+    if (n > h->max_n || n > (1ull << 32)) return OSB200_ERR_SIZE;  // the indices are 32-bit
+    // the key arrays are 2n bytes, the index array 4n
+    const uint64_t kb = n * sizeof(uint16_t), ib = n * sizeof(uint32_t);
+    auto overlap = [](uintptr_t a, uint64_t alen, uintptr_t b, uint64_t blen) { return a < b + blen && b < a + alen; };
+    if (overlap(in, kb, out, kb) || overlap(in, kb, idx, ib) || overlap(out, kb, idx, ib)) return OSB200_ERR_INVALID_ARG;
+    cudaStream_t q = static_cast<cudaStream_t>(stream);
+    if (n == 1) {  // already sorted, but the outputs still have to be written
+        OSB_TRY(cudaMemcpyAsync(d_keys_out, d_keys_in, sizeof(uint16_t), cudaMemcpyDeviceToDevice, q));
+        OSB_TRY(cudaMemsetAsync(d_indices, 0, sizeof(uint32_t), q));
+        return OSB200_OK;
+    }
+    const bool plain = c.a == 0 && c.b == 0 && c.d == 0;
+    return sort_impl(h, 2, d_keys_out, d_indices, n, q, plain ? nullptr : &c, 0, -1, d_keys_in);
 }
 
 int osb200_sort_host_keys_u32(osb200_handle h, uint32_t* h_keys, uint64_t n)

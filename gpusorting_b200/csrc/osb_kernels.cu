@@ -31,6 +31,7 @@ constexpr int kHistThreads = 1024;
 template <typename KeyT> struct HistGeom;
 template <> struct HistGeom<uint32_t> { static constexpr int COLS = 32; };
 template <> struct HistGeom<uint64_t> { static constexpr int COLS = 16; };
+template <> struct HistGeom<uint16_t> { static constexpr int COLS = 32; };  // 2 places x 256 digits x 32 columns: 64 KB
 
 // MASKED: a sort on the key bits [0, end_bit) -- only the first `places` byte places count and the last of them keeps
 // `last_mask` (the sharded path's local sort after an exchange on the top log2(R) bits: bits [0, 32 - log2 R))
@@ -60,6 +61,13 @@ __device__ __forceinline__ uint4 hist_encode_vec(uint4 v, const KeyCodec& c)
         const uint32_t a = static_cast<uint32_t>(c.a), b = static_cast<uint32_t>(c.b), d = static_cast<uint32_t>(c.d);
         v.x = codec_encode<uint32_t>(v.x, a, b, d); v.y = codec_encode<uint32_t>(v.y, a, b, d);
         v.z = codec_encode<uint32_t>(v.z, a, b, d); v.w = codec_encode<uint32_t>(v.w, a, b, d);
+    } else if constexpr (sizeof(KeyT) == 2) {
+        const uint16_t a = static_cast<uint16_t>(c.a), b = static_cast<uint16_t>(c.b), d = static_cast<uint16_t>(c.d);
+        auto enc2 = [&](uint32_t w) {  // the two keys of a 32-bit word
+            return static_cast<uint32_t>(codec_encode<uint16_t>(static_cast<uint16_t>(w), a, b, d)) |
+                   (static_cast<uint32_t>(codec_encode<uint16_t>(static_cast<uint16_t>(w >> 16), a, b, d)) << 16);
+        };
+        v.x = enc2(v.x); v.y = enc2(v.y); v.z = enc2(v.z); v.w = enc2(v.w);
     } else {
         unsigned long long k0 = (static_cast<unsigned long long>(v.y) << 32) | v.x, k1 = (static_cast<unsigned long long>(v.w) << 32) | v.z;
         k0 = codec_encode<unsigned long long>(k0, c.a, c.b, c.d); k1 = codec_encode<unsigned long long>(k1, c.a, c.b, c.d);
@@ -149,9 +157,14 @@ cudaError_t launch_global_histogram(const void* keys, uint64_t n, int key_bytes,
     if (key_bytes == 4)
         global_histogram_kernel<uint32_t><<<grid, kHistThreads, hist_smem_bytes<uint32_t>(), stream>>>(
             static_cast<const uint32_t*>(keys), n, ghist, codec);
-    else
+    else if (key_bytes == 8)
         global_histogram_kernel<uint64_t><<<grid, kHistThreads, hist_smem_bytes<uint64_t>(), stream>>>(
             static_cast<const uint64_t*>(keys), n, ghist, codec);
+    else if (key_bytes == 2)
+        global_histogram_kernel<uint16_t><<<grid, kHistThreads, hist_smem_bytes<uint16_t>(), stream>>>(
+            static_cast<const uint16_t*>(keys), n, ghist, codec);
+    else
+        return cudaErrorInvalidValue;
     return cudaGetLastError();
 }
 
@@ -358,16 +371,20 @@ cudaError_t launch_copy_back(const SortPlan* plan, const void* alt_keys, void* k
 
 // argsort: keys and indices in one launch.  Odd executed passes: both from the alt buffers.  No executed pass (all keys
 // equal): the input is its own stable sort -- keys from the untouched input, indices 0..n-1.  (All pointers 16-byte aligned.)
+// Four keys per step: one uint4 of 32-bit keys, one uint2 of 16-bit keys.
+template <typename KeyT>
 __global__ void __launch_bounds__(512)
-argsort_copy_back_kernel(const SortPlan* __restrict__ plan, const uint32_t* __restrict__ keys_in, const uint32_t* __restrict__ alt_keys,
-                         uint32_t* __restrict__ keys, const uint32_t* __restrict__ alt_idx, uint32_t* __restrict__ idx, uint64_t n)
+argsort_copy_back_kernel(const SortPlan* __restrict__ plan, const KeyT* __restrict__ keys_in, const KeyT* __restrict__ alt_keys,
+                         KeyT* __restrict__ keys, const uint32_t* __restrict__ alt_idx, uint32_t* __restrict__ idx, uint64_t n)
 {
+    using KV = typename std::conditional<sizeof(KeyT) == 4, uint4, uint2>::type;
+    static_assert(sizeof(KV) == 4 * sizeof(KeyT), "four keys per vector");
     const uint32_t ex = plan->executed;
     if (ex != 0 && !(ex & 1u)) return;
-    const uint32_t* src = ex ? alt_keys : keys_in;
+    const KeyT* src = ex ? alt_keys : keys_in;
     const uint64_t vecs = n / 4, stride = static_cast<uint64_t>(gridDim.x) * blockDim.x;
     for (uint64_t i = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < vecs; i += stride) {
-        __stcs(reinterpret_cast<uint4*>(keys) + i, __ldcs(reinterpret_cast<const uint4*>(src) + i));
+        __stcs(reinterpret_cast<KV*>(keys) + i, __ldcs(reinterpret_cast<const KV*>(src) + i));
         const uint32_t b = static_cast<uint32_t>(i * 4);
         __stcs(reinterpret_cast<uint4*>(idx) + i, ex ? __ldcs(reinterpret_cast<const uint4*>(alt_idx) + i) : make_uint4(b, b + 1, b + 2, b + 3));
     }
@@ -379,13 +396,22 @@ argsort_copy_back_kernel(const SortPlan* __restrict__ plan, const uint32_t* __re
 }
 
 cudaError_t launch_argsort_copy_back(const SortPlan* plan, const void* keys_in, const void* alt_keys, void* keys,
-                                     const uint32_t* alt_idx, uint32_t* idx, uint64_t n, int sm_count, cudaStream_t stream)
+                                     const uint32_t* alt_idx, uint32_t* idx, uint64_t n, int key_bytes, int sm_count,
+                                     cudaStream_t stream)
 {
     uint64_t want = (n / 4 + 511) / 512;
     if (want < 1) want = 1;
     const unsigned grid = static_cast<unsigned>(want < static_cast<uint64_t>(sm_count) * 4 ? want : sm_count * 4);
-    argsort_copy_back_kernel<<<grid, 512, 0, stream>>>(plan, static_cast<const uint32_t*>(keys_in), static_cast<const uint32_t*>(alt_keys),
-                                                       static_cast<uint32_t*>(keys), alt_idx, idx, n);
+    if (key_bytes == 4)
+        argsort_copy_back_kernel<uint32_t><<<grid, 512, 0, stream>>>(plan, static_cast<const uint32_t*>(keys_in),
+                                                                     static_cast<const uint32_t*>(alt_keys),
+                                                                     static_cast<uint32_t*>(keys), alt_idx, idx, n);
+    else if (key_bytes == 2)
+        argsort_copy_back_kernel<uint16_t><<<grid, 512, 0, stream>>>(plan, static_cast<const uint16_t*>(keys_in),
+                                                                     static_cast<const uint16_t*>(alt_keys),
+                                                                     static_cast<uint16_t*>(keys), alt_idx, idx, n);
+    else
+        return cudaErrorInvalidValue;
     return cudaGetLastError();
 }
 
@@ -863,8 +889,10 @@ template <typename KeyT, bool PAIRS, int K, int WARPS>
 struct WideSmem {
     static constexpr int THREADS = WARPS * 32;
     static constexpr int T = THREADS * K;
-    alignas(16) KeyT sorted[T];                      // digit-sorted tile
-    alignas(16) uint32_t sorted_val[PAIRS ? T : 4];  // payloads in the same order
+    // 16-bit pairs: `sorted` itself holds the tile's T {key, payload} uint2 words (8 B per slot; see the kernel)
+    static constexpr bool KV_IN_SORTED = PAIRS && sizeof(KeyT) == 2;
+    alignas(16) KeyT sorted[KV_IN_SORTED ? T * 8 / sizeof(KeyT) : T];  // digit-sorted tile
+    alignas(16) uint32_t sorted_val[PAIRS && !KV_IN_SORTED ? T : 4];   // payloads in the same order
     alignas(16) uint32_t hist[WARPS * kRadix];       // warp-private digit counters (counts, then running slots)
     unsigned long long keyptr[kRadix];               // per digit: byte address of out[first key of the digit - tile slot]
     unsigned long long valptr[PAIRS ? kRadix : 1];
@@ -886,7 +914,7 @@ digit_binning_wide_kernel(KeyT* buf0, KeyT* buf1, uint32_t* val0, uint32_t* val1
                           const unsigned long long* __restrict__ gbase, uint16_t* agg16, uint64_t* incl64,
                           uint32_t* ticket, PassParams pp, KeyCodec codec)
 {
-    static_assert(!INDICES || (PAIRS && sizeof(KeyT) == 4), "the indices are the 32-bit payloads of a pairs pass");
+    static_assert(!INDICES || (PAIRS && sizeof(KeyT) <= 4), "the indices are the 32-bit payloads of a pairs pass");
     using S = WideSmem<KeyT, PAIRS, K, WARPS>;
     constexpr int THREADS = S::THREADS;
     constexpr int T = S::T;
@@ -896,7 +924,9 @@ digit_binning_wide_kernel(KeyT* buf0, KeyT* buf1, uint32_t* val0, uint32_t* val1
     // pairs: key and payload of a tile slot are ONE 64-bit word of shared memory ({key, payload}; `sorted` and `sorted_val`
     // are adjacent and together hold T such words) -- one transposing STS.64 and one LDS.64 per pair instead of two of each,
     // and the payload's destination is the key's plus a constant (reference: OneSweep.cu:522-599 moves them separately)
-    static_assert(!PAIRS || (sizeof(KeyT) == 4 && offsetof(S, sorted_val) == offsetof(S, sorted) + sizeof(KeyT) * T), "kv layout");
+    // (16-bit keys: the word is {key zero-extended, payload}, and `sorted` is sized for T of them)
+    static_assert(!PAIRS || (sizeof(KeyT) == 4 && offsetof(S, sorted_val) == offsetof(S, sorted) + sizeof(KeyT) * T) ||
+                  (S::KV_IN_SORTED && sizeof(S::sorted) == sizeof(uint2) * T), "kv layout");
     uint2* const kv = reinterpret_cast<uint2*>(sm.sorted);
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -929,7 +959,10 @@ digit_binning_wide_kernel(KeyT* buf0, KeyT* buf1, uint32_t* val0, uint32_t* val1
 
     // ---- tile loads (warp-striped: every warp instruction reads one contiguous 128 B / 256 B row) ----------------
     // The ragged last tile is padded with all-ones keys (they rank last); a tile at or past num_tiles loads nothing.
-    KeyT key[K];
+    // (16-bit keys-only passes hold their keys zero-extended in 32-bit registers: as 16-bit values they spill in atomic mode;
+    // the pairs pass spills the other way round.)
+    using KeyReg = typename std::conditional<sizeof(KeyT) == 2 && !PAIRS, uint32_t, KeyT>::type;
+    KeyReg key[K];
     uint32_t val[PAIRS ? K : 1];
     const uint32_t warp_off = warp * (32 * K) + lane;
     auto load_tile = [&](uint32_t t) {
@@ -984,7 +1017,8 @@ digit_binning_wide_kernel(KeyT* buf0, KeyT* buf1, uint32_t* val0, uint32_t* val1
     // u64: with its window of 32 tiles the lookback holds four 16-byte blocks per round trip, and 16 prefetched keys held
     // across it spill (180 B per thread); issued after the lookback instead they made the pass 4 % slower on the H100.
     // Pairs: persistent, the pass was up to 0.9 % slower on the H100 (26.01 -> 25.79 Gpairs/s at 400 W).
-    constexpr bool kPersistent = (sizeof(KeyT) == 4 && !PAIRS) || HOT;
+    // 16-bit keys follow the u32 choices (same registers per key: a 16-bit key occupies a 32-bit register).
+    constexpr bool kPersistent = (sizeof(KeyT) <= 4 && !PAIRS) || HOT;
     while (true) {
     const uint64_t tile_base = static_cast<uint64_t>(tile) * T;
     const bool full = tile_base + T <= n;
@@ -998,7 +1032,7 @@ digit_binning_wide_kernel(KeyT* buf0, KeyT* buf1, uint32_t* val0, uint32_t* val1
         const KeyT ca = static_cast<KeyT>(codec.a), cb = static_cast<KeyT>(codec.b), cd = static_cast<KeyT>(codec.d);
 #pragma unroll
         for (int i = 0; i < K; ++i) {
-            key[i] = codec_encode<KeyT>(key[i], ca, cb, cd);
+            key[i] = codec_encode<KeyT>(static_cast<KeyT>(key[i]), ca, cb, cd);
             if (!full && warp_off + i * 32 >= valid) key[i] = static_cast<KeyT>(~static_cast<KeyT>(0));
         }
     }
@@ -1131,12 +1165,18 @@ digit_binning_wide_kernel(KeyT* buf0, KeyT* buf1, uint32_t* val0, uint32_t* val1
     // (partial-sector peer stores run well below it; tools/microbench/p2p_store_ub.cu measures both).
     const bool dec = (sm.plan_bits >> 1) & kCodecDecodeOnStore;
     const KeyT ca = static_cast<KeyT>(codec.a), cb = static_cast<KeyT>(codec.b), cd = static_cast<KeyT>(codec.d);
-    // pairs: a payload goes where its key goes, in the other output array (same element size: a constant byte distance)
+    // pairs: a payload goes where its key goes, in the other output array (same element size: a constant byte distance;
+    // 16-bit keys: the payload's own digit pointer)
     long long val_delta = 0;
-    if constexpr (PAIRS) {
+    if constexpr (PAIRS && sizeof(KeyT) == 4) {
         const bool swap = sm.plan_bits & 1u;
         val_delta = reinterpret_cast<const char*>(swap ? val0 : val1) - reinterpret_cast<const char*>(swap ? buf0 : buf1);
     }
+    auto val_dst = [&](KeyT* dst, uint32_t d, uint32_t x) -> uint32_t* {
+        if constexpr (sizeof(KeyT) == 4) return reinterpret_cast<uint32_t*>(reinterpret_cast<char*>(dst) + val_delta);
+        else return reinterpret_cast<uint32_t*>(sm.valptr[d]) + x;
+    };
+    (void)val_dst;
     auto slot_key = [&](uint32_t x) -> KeyT { if constexpr (PAIRS) return static_cast<KeyT>(kv[x].x); else return sm.sorted[x]; };
     (void)slot_key;
     if (pp.dbits <= 5) {
@@ -1158,7 +1198,7 @@ digit_binning_wide_kernel(KeyT* buf0, KeyT* buf1, uint32_t* val0, uint32_t* val1
                         if (dec) k = codec_decode<KeyT>(k, ca, cb, cd);
                         KeyT* dst = reinterpret_cast<KeyT*>(kp) + x;
                         st_scatter(dst, k);
-                        st_scatter(reinterpret_cast<uint32_t*>(reinterpret_cast<char*>(dst) + val_delta), e.y);
+                        st_scatter(val_dst(dst, b, x), e.y);
                     } else {
                         KeyT k = sm.sorted[x];
                         if (dec) k = codec_decode<KeyT>(k, ca, cb, cd);
@@ -1173,9 +1213,10 @@ digit_binning_wide_kernel(KeyT* buf0, KeyT* buf1, uint32_t* val0, uint32_t* val1
             const uint32_t idx = j * THREADS + tid;
             if constexpr (PAIRS) {
                 const uint2 e = kv[idx];
-                KeyT* dst = reinterpret_cast<KeyT*>(sm.keyptr[digit_of(static_cast<KeyT>(e.x), shift, dmask)]) + idx;
+                const uint32_t d = digit_of(static_cast<KeyT>(e.x), shift, dmask);
+                KeyT* dst = reinterpret_cast<KeyT*>(sm.keyptr[d]) + idx;
                 st_scatter(dst, static_cast<KeyT>(e.x));
-                st_scatter(reinterpret_cast<uint32_t*>(reinterpret_cast<char*>(dst) + val_delta), e.y);
+                st_scatter(val_dst(dst, d, idx), e.y);
             } else {
                 const KeyT k = sm.sorted[idx];
                 const uint32_t d = digit_of(k, shift, dmask);
@@ -1190,9 +1231,10 @@ digit_binning_wide_kernel(KeyT* buf0, KeyT* buf1, uint32_t* val0, uint32_t* val1
                 if constexpr (PAIRS) {
                     const uint2 e = kv[idx];
                     const KeyT k = static_cast<KeyT>(e.x);
-                    KeyT* dst = reinterpret_cast<KeyT*>(sm.keyptr[digit_of(k, shift, dmask)]) + idx;
+                    const uint32_t d = digit_of(k, shift, dmask);
+                    KeyT* dst = reinterpret_cast<KeyT*>(sm.keyptr[d]) + idx;
                     st_scatter(dst, dec ? codec_decode<KeyT>(k, ca, cb, cd) : k);
-                    st_scatter(reinterpret_cast<uint32_t*>(reinterpret_cast<char*>(dst) + val_delta), e.y);
+                    st_scatter(val_dst(dst, d, idx), e.y);
                 } else {
                     const KeyT k = sm.sorted[idx];
                     const uint32_t d = digit_of(k, shift, dmask);
@@ -1633,6 +1675,22 @@ template <typename KeyT, bool PAIRS> struct WideGeom;
 template <> struct WideGeom<uint32_t, false> { static constexpr int K = OSB_WIDE_K, WARPS = OSB_WIDE_WARPS, MINB = OSB_WIDE_MINB, LOOK = OSB_LOOK; };
 template <> struct WideGeom<uint32_t, true>  { static constexpr int K = OSB_PAIRS_WIDE_K, WARPS = OSB_PAIRS_WIDE_WARPS, MINB = OSB_PAIRS_WIDE_MINB, LOOK = OSB_PAIRS_LOOK; };
 template <> struct WideGeom<uint64_t, false> { static constexpr int K = OSB_U64_K, WARPS = OSB_U64_WARPS, MINB = OSB_U64_MINB, LOOK = OSB_U64_LOOK; };
+// 16-bit keys (osb200_sort_keys16 & co., run on a 4-byte handle).  A 16-bit key takes a 32-bit register like a u32 key;
+// each tile load is one warp-striped 16-bit load per key (64 B per warp instruction, tile order = input order, so the
+// stability argument of the u32 pass is unchanged).  Keys: 24 keys per thread (12,288-key tiles) -- with the u32 kernel's 32
+// the atomic-mode pass spills on sm_90a (12 B; 28 and 30 keys spill too, 24 does not).  Pairs: the u32 pairs geometry.
+// DESIGN §4.4.
+#ifndef OSB_K16_K  // geometry of the 16-bit keys-only kernel, overridable for sweeps
+#define OSB_K16_K 24
+#define OSB_K16_WARPS 16
+#endif
+#ifndef OSB_P16_K  // geometry of the 16-bit pairs / argsort kernel
+#define OSB_P16_K 16
+#define OSB_P16_WARPS 16
+#endif
+template <> struct WideGeom<uint16_t, false> { static constexpr int K = OSB_K16_K, WARPS = OSB_K16_WARPS, MINB = 2, LOOK = OSB_LOOK; };
+template <> struct WideGeom<uint16_t, true>  { static constexpr int K = OSB_P16_K, WARPS = OSB_P16_WARPS, MINB = 2, LOOK = OSB_PAIRS_LOOK; };
+template <typename KeyT, bool PAIRS> constexpr uint32_t wide_tile() { return WideGeom<KeyT, PAIRS>::K * WideGeom<KeyT, PAIRS>::WARPS * 32; }
 
 template <typename KeyT, bool PAIRS, int RANK_MODE, bool INDICES = false>
 static cudaError_t launch_wide_variant(const void* in, void* out, const uint32_t* in_val, uint32_t* out_val, uint64_t n,
@@ -1668,7 +1726,7 @@ static cudaError_t launch_wide_variant(const void* in, void* out, const uint32_t
     auto kern = digit_binning_wide_kernel<KeyT, PAIRS, G::K, G::WARPS, RANK_MODE, G::LOOK, G::MINB, false, INDICES>;
     static int plain_per_sm = 0;  // (one value per instantiation of this function template)
     // with a device plan `in`/`out` are the caller's and the alt buffers (the kernel picks the direction); both are written
-    kern<<<grid_for(kern, plain_per_sm, sizeof(KeyT) == 4 && !PAIRS), S::THREADS, sizeof(S), stream>>>(
+    kern<<<grid_for(kern, plain_per_sm, sizeof(KeyT) <= 4 && !PAIRS), S::THREADS, sizeof(S), stream>>>(
         static_cast<KeyT*>(const_cast<void*>(in)), static_cast<KeyT*>(out), const_cast<uint32_t*>(in_val), out_val, n, gbase,
         agg16, incl64, ticket, pp, cfg.codec);
     if (cfg.plan != nullptr && cfg.hot_passes) {
@@ -1758,8 +1816,21 @@ static cudaError_t launch_tile_variant(const void* in, void* out, const uint32_t
     return cudaGetLastError();
 }
 
+// 16-bit keys run on a 4-byte handle, whose descriptors and reductions are sized for its smallest tile (smallest_tile in
+// osb_host.cu: the minimum over the variants of the 4-byte tiles): their tiles must not be smaller.
+constexpr uint32_t cmin(uint32_t a, uint32_t b) { return a < b ? a : b; }
+constexpr uint32_t kSmallestTileU32Keys = cmin(cmin(TileGeom<uint32_t, false>::WARPS * 32 * TileGeom<uint32_t, false>::K,
+                                                    RingGeom<uint32_t>::K * RingGeom<uint32_t>::WARPS * 32), wide_tile<uint32_t, false>());
+constexpr uint32_t kSmallestTileU32Pairs = cmin(TileGeom<uint32_t, true>::WARPS * 32 * TileGeom<uint32_t, true>::K, wide_tile<uint32_t, true>());
+static_assert(wide_tile<uint16_t, false>() >= kSmallestTileU32Keys && wide_tile<uint16_t, false>() >= kSmallestTileU32Pairs,
+              "16-bit keys (either 4-byte handle): a smaller tile would need more descriptors than the handle has");
+static_assert(wide_tile<uint16_t, true>() >= kSmallestTileU32Pairs,
+              "16-bit pairs (a (4, 4) handle): a smaller tile would need more descriptors than the handle has");
+static_assert(wide_tile<uint16_t, false>() < 32768 && wide_tile<uint16_t, true>() < 32768, "agg16 holds 15-bit counts");
+
 uint32_t binning_tile_keys(int key_bytes, bool pairs, const BinningConfig& cfg)
 {
+    if (key_bytes == 2) return pairs ? wide_tile<uint16_t, true>() : wide_tile<uint16_t, false>();  // (the wide kernel only)
     if (cfg.variant == kVariantPersistent && !pairs)
         return key_bytes == 8 ? RingGeom<uint64_t>::K * RingGeom<uint64_t>::WARPS * 32 : RingGeom<uint32_t>::K * RingGeom<uint32_t>::WARPS * 32;
     if (cfg.variant == kVariantWide) {
@@ -1816,6 +1887,15 @@ cudaError_t configure_kernels()
     if ((e = set_wide_attr<uint64_t, false, kRankBallot>()) != cudaSuccess) return e;
     if ((e = set_wide_attr<uint32_t, true, kRankAtomic, true>()) != cudaSuccess) return e;  // argsort
     if ((e = set_wide_attr<uint32_t, true, kRankBallot, true>()) != cudaSuccess) return e;
+    // 16-bit keys: histogram, keys, pairs, argsort
+    if ((e = cudaFuncSetAttribute(global_histogram_kernel<uint16_t>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  static_cast<int>(hist_smem_bytes<uint16_t>()))) != cudaSuccess) return e;
+    if ((e = set_wide_attr<uint16_t, false, kRankAtomic>()) != cudaSuccess) return e;
+    if ((e = set_wide_attr<uint16_t, false, kRankBallot>()) != cudaSuccess) return e;
+    if ((e = set_wide_attr<uint16_t, true, kRankAtomic>()) != cudaSuccess) return e;
+    if ((e = set_wide_attr<uint16_t, true, kRankBallot>()) != cudaSuccess) return e;
+    if ((e = set_wide_attr<uint16_t, true, kRankAtomic, true>()) != cudaSuccess) return e;
+    if ((e = set_wide_attr<uint16_t, true, kRankBallot, true>()) != cudaSuccess) return e;
     if ((e = set_pairs_attr<kRankAtomic>()) != cudaSuccess) return e;
     if ((e = set_pairs_attr<kRankBallot>()) != cudaSuccess) return e;
     return configure_segment_kernels();
@@ -1841,12 +1921,18 @@ cudaError_t launch_digit_binning(const void* in, void* out, const uint32_t* in_v
             : launch_wide_variant<KEYT, PAIRS, kRankAtomic>(in, out, in_val, out_val, n, shift, gbase_place, agg16, desc, \
                                                            ticket, epoch, cfg, stream))
         if (cfg.argsort_in != nullptr) {  // argsort: the first executed pass reads argsort_in and makes the indices
-            if (key_bytes != 4 || !pairs || cfg.plan == nullptr) return cudaErrorInvalidValue;
+            if ((key_bytes != 4 && key_bytes != 2) || !pairs || cfg.plan == nullptr) return cudaErrorInvalidValue;
+            if (key_bytes == 2)
+                return ballot ? launch_wide_variant<uint16_t, true, kRankBallot, true>(in, out, in_val, out_val, n, shift, gbase_place,
+                                                                                      agg16, desc, ticket, epoch, cfg, stream)
+                              : launch_wide_variant<uint16_t, true, kRankAtomic, true>(in, out, in_val, out_val, n, shift, gbase_place,
+                                                                                      agg16, desc, ticket, epoch, cfg, stream);
             return ballot ? launch_wide_variant<uint32_t, true, kRankBallot, true>(in, out, in_val, out_val, n, shift, gbase_place, agg16,
                                                                                   desc, ticket, epoch, cfg, stream)
                           : launch_wide_variant<uint32_t, true, kRankAtomic, true>(in, out, in_val, out_val, n, shift, gbase_place, agg16,
                                                                                   desc, ticket, epoch, cfg, stream);
         }
+        if (key_bytes == 2) return pairs ? OSB_WIDE(uint16_t, true) : OSB_WIDE(uint16_t, false);
         if (key_bytes == 4 && pairs && OSB_PAIRS16K)
             return ballot ? launch_pairs_variant<kRankBallot>(in, out, in_val, out_val, n, shift, gbase_place, agg16, desc, ticket, epoch, cfg, stream)
                           : launch_pairs_variant<kRankAtomic>(in, out, in_val, out_val, n, shift, gbase_place, agg16, desc, ticket, epoch, cfg, stream);
@@ -1994,10 +2080,13 @@ template <> struct SegGeomN<uint32_t, 2> { static constexpr int K = 32, WARPS = 
 template <> struct SegGeomN<uint64_t, 0> { static constexpr int K = 1,  WARPS = 8; };   //    256 keys
 template <> struct SegGeomN<uint64_t, 1> { static constexpr int K = 8,  WARPS = 8; };   //  2,048 keys
 template <> struct SegGeomN<uint64_t, 2> { static constexpr int K = 16, WARPS = 16; };  //  8,192 keys
+// 16-bit keys: only the small-n path of their sorts (one segment of up to 16,384 keys; no segmented sort of 16-bit keys)
+template <> struct SegGeomN<uint16_t, 2> { static constexpr int K = 32, WARPS = 16; };  // 16,384 keys, 512 threads
 template <typename KeyT, int SIZE> constexpr uint32_t seg_cap() { return SegGeomN<KeyT, SIZE>::K * SegGeomN<KeyT, SIZE>::WARPS * 32; }
 
 uint32_t segment_sort_capacity(int key_bytes, bool small)
 {
+    if (key_bytes == 2) return seg_cap<uint16_t, 2>();
     if (key_bytes == 8) return small ? seg_cap<uint64_t, 1>() : seg_cap<uint64_t, 2>();
     return small ? seg_cap<uint32_t, 1>() : seg_cap<uint32_t, 2>();
 }
@@ -2026,6 +2115,13 @@ static cudaError_t configure_segment_kernels()
     // argsort: the single segment of a sort of at most one tile
     if ((e = seg_attr<uint32_t, true, 2, kRankAtomic, true>()) != cudaSuccess) return e;
     if ((e = seg_attr<uint32_t, true, 2, kRankBallot, true>()) != cudaSuccess) return e;
+    // 16-bit keys: the single segment of a sort of at most one tile -- keys, pairs, argsort
+    if ((e = seg_attr<uint16_t, false, 2, kRankAtomic>()) != cudaSuccess) return e;
+    if ((e = seg_attr<uint16_t, false, 2, kRankBallot>()) != cudaSuccess) return e;
+    if ((e = seg_attr<uint16_t, true, 2, kRankAtomic>()) != cudaSuccess) return e;
+    if ((e = seg_attr<uint16_t, true, 2, kRankBallot>()) != cudaSuccess) return e;
+    if ((e = seg_attr<uint16_t, true, 2, kRankAtomic, true>()) != cudaSuccess) return e;
+    if ((e = seg_attr<uint16_t, true, 2, kRankBallot, true>()) != cudaSuccess) return e;
     return cudaSuccess;
 }
 
@@ -2055,9 +2151,20 @@ cudaError_t launch_segment_sort(void* keys, uint32_t* vals, int key_bytes, const
     if (num_segments == 0) return cudaSuccess;
     const KeyCodec codec = codec_in ? *codec_in : KeyCodec();
     if (keys_in != nullptr) {  // argsort: one segment of up to a tile, in the largest geometry (the only one instantiated for it)
-        if (key_bytes != 4 || !vals || seg_off || num_segments != 1 || max_len > seg_cap<uint32_t, 2>()) return cudaErrorInvalidValue;
+        if ((key_bytes != 4 && key_bytes != 2) || !vals || seg_off || num_segments != 1 || max_len > segment_sort_capacity(key_bytes, false))
+            return cudaErrorInvalidValue;
+        if (key_bytes == 2)
+            return launch_seg<uint16_t, true, 2, true>(keys, vals, nullptr, 1, single_n, max_len, begin_bit, places, last_bits, codec,
+                                                       rank_mode, sm_count, stream, keys_in);
         return launch_seg<uint32_t, true, 2, true>(keys, vals, nullptr, 1, single_n, max_len, begin_bit, places, last_bits, codec,
                                                    rank_mode, sm_count, stream, keys_in);
+    }
+    if (key_bytes == 2) {  // 16-bit keys: the single segment of a small sort, in the 16,384-key geometry
+        if (seg_off || num_segments != 1 || max_len > seg_cap<uint16_t, 2>()) return cudaErrorInvalidValue;
+        return vals ? launch_seg<uint16_t, true, 2>(keys, vals, nullptr, 1, single_n, max_len, begin_bit, places, last_bits, codec,
+                                                    rank_mode, sm_count, stream)
+                    : launch_seg<uint16_t, false, 2>(keys, vals, nullptr, 1, single_n, max_len, begin_bit, places, last_bits, codec,
+                                                     rank_mode, sm_count, stream);
     }
     const int size = max_len <= (key_bytes == 8 ? seg_cap<uint64_t, 0>() : seg_cap<uint32_t, 0>()) ? 0
                      : max_len <= segment_sort_capacity(key_bytes, true) ? 1 : 2;

@@ -30,6 +30,9 @@ _KEY_DTYPES_8 = (torch.int64, torch.uint64)
 _TYPED_DTYPES_4 = (torch.int32, torch.uint32, torch.float32)
 _TYPED_DTYPES_8 = (torch.int64, torch.uint64, torch.float64)
 KEY_TYPES = {"u32": 0, "i32": 1, "f32": 2, "u64": 3, "i64": 4, "f64": 5}
+# 16-bit keys (sort_keys16 / sort_pairs16 / argsort16, on a 4-byte sorter): key_type states the order, the dtype the width
+_TYPED_DTYPES_2 = (torch.int16, torch.uint16, torch.float16, torch.bfloat16)
+KEY16_TYPES = {"u16": 0, "i16": 1, "f16": 2, "bf16": 3}
 
 
 def _stream_ptr(stream: Optional[torch.cuda.Stream]) -> int:
@@ -156,6 +159,45 @@ class OneSweepSorter:
         with torch.cuda.device(self.device):
             check(lib.osb200_argsort(self._h, keys.data_ptr(), out.data_ptr(), idx.data_ptr(), n, KEY_TYPES[key_type],
                                      1 if descending else 0, _stream_ptr(stream)), "osb200_argsort")
+        return out, idx
+
+    # -- 16-bit keys: two digit passes over 2-byte keys, on this (4-byte) sorter's workspace --------------------------
+    def sort_keys16(self, keys: torch.Tensor, key_type: str, descending: bool = False, n: Optional[int] = None,
+                    stream=None) -> torch.Tensor:
+        """Stable in-place sort of int16 / uint16 / float16 / bfloat16 keys (osb200_sort_keys16).  key_type in KEY16_TYPES
+        ("u16", "i16", "f16", "bf16") states how the bits are ordered; floats follow the total order of their bit patterns.
+        Keys must start on a 16-byte boundary (OneSweepError status -1 otherwise).  Needs a sorter with key_bytes == 4."""
+        n = keys.numel() if n is None else int(n)
+        _check_dev_tensor(keys, _TYPED_DTYPES_2, "keys", n, self.device)
+        with torch.cuda.device(self.device):
+            check(lib.osb200_sort_keys16(self._h, keys.data_ptr(), n, KEY16_TYPES[key_type], 1 if descending else 0,
+                                         _stream_ptr(stream)), "osb200_sort_keys16")
+        return keys
+
+    def sort_pairs16(self, keys: torch.Tensor, values: torch.Tensor, key_type: str, descending: bool = False,
+                     n: Optional[int] = None, stream=None):
+        """sort_keys16 with 32-bit payloads that move with their keys (osb200_sort_pairs16).  Values need only their natural
+        4-byte alignment.  Needs a (4, 4) sorter."""
+        n = keys.numel() if n is None else int(n)
+        _check_dev_tensor(keys, _TYPED_DTYPES_2, "keys", n, self.device)
+        _check_dev_tensor(values, _TYPED_DTYPES_4, "values", n, self.device)
+        with torch.cuda.device(self.device):
+            check(lib.osb200_sort_pairs16(self._h, keys.data_ptr(), values.data_ptr(), n, KEY16_TYPES[key_type],
+                                          1 if descending else 0, _stream_ptr(stream)), "osb200_sort_pairs16")
+        return keys, values
+
+    def argsort16(self, keys: torch.Tensor, key_type: str, descending: bool = False, n: Optional[int] = None, stream=None):
+        """argsort of 16-bit keys (osb200_argsort16): returns (sorted_keys, indices), new tensors of n elements, sorted_keys in
+        the dtype of `keys` and indices as torch.int32 (positions >= 2^31 read as negative: ``indices.long() & 0xFFFFFFFF``).
+        `keys` is left untouched.  Needs a (4, 4) sorter."""
+        n = keys.numel() if n is None else int(n)
+        _check_dev_tensor(keys, _TYPED_DTYPES_2, "keys", n, self.device)
+        with torch.cuda.stream(stream):  # (None: the current stream) the outputs belong to the stream that writes them
+            out = torch.empty(n, dtype=keys.dtype, device=keys.device)
+            idx = torch.empty(n, dtype=torch.int32, device=keys.device)
+        with torch.cuda.device(self.device):
+            check(lib.osb200_argsort16(self._h, keys.data_ptr(), out.data_ptr(), idx.data_ptr(), n, KEY16_TYPES[key_type],
+                                       1 if descending else 0, _stream_ptr(stream)), "osb200_argsort16")
         return out, idx
 
     def sort_bits(self, keys: torch.Tensor, begin_bit: int, end_bit: int, values: Optional[torch.Tensor] = None,
@@ -324,6 +366,18 @@ def argsort(keys: torch.Tensor, key_type: str, descending: bool = False, n: Opti
         sp = _stream_ptr(stream)
     s = _cached_sorter(keys.device.index, 4, 4, n, sp)
     return s.argsort(keys, key_type, descending, n, stream)
+
+
+def argsort16(keys: torch.Tensor, key_type: str, descending: bool = False, n: Optional[int] = None, stream=None):
+    """Stable (sorted_keys, indices) of 16-bit keys (int16, uint16, float16, bfloat16; key_type "u16", "i16", "f16" or
+    "bf16"), input untouched: OneSweepSorter.argsort16 on the stream's cached (4, 4) sorter, the one argsort uses."""
+    n = keys.numel() if n is None else int(n)
+    if not (isinstance(keys, torch.Tensor) and keys.is_cuda):
+        raise TypeError("keys must be a CUDA tensor")
+    with torch.cuda.device(keys.device.index):
+        sp = _stream_ptr(stream)
+    s = _cached_sorter(keys.device.index, 4, 4, n, sp)
+    return s.argsort16(keys, key_type, descending, n, stream)
 
 
 class OneSweepDispatcher:

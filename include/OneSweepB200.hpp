@@ -50,6 +50,21 @@ class OneSweepSorterB200 {
     {
         check(osb200_argsort(h_, d_keys_in, d_keys_out, d_indices, n, key_type, descending ? 1 : 0, stream), "osb200_argsort");
     }
+    // 16-bit keys (osb200_key16_type: uint16, int16, float16, bfloat16) in two digit passes, on a 4-byte sorter; pairs and
+    // argsort need a (4, 4) sorter
+    void SortKeys16(void* d_keys, uint64_t n, int key_type, bool descending, void* stream = nullptr)
+    {
+        check(osb200_sort_keys16(h_, d_keys, n, key_type, descending ? 1 : 0, stream), "osb200_sort_keys16");
+    }
+    void SortPairs16(void* d_keys, uint32_t* d_values, uint64_t n, int key_type, bool descending, void* stream = nullptr)
+    {
+        check(osb200_sort_pairs16(h_, d_keys, d_values, n, key_type, descending ? 1 : 0, stream), "osb200_sort_pairs16");
+    }
+    void ArgSort16(const void* d_keys_in, void* d_keys_out, uint32_t* d_indices, uint64_t n, int key_type, bool descending,
+                   void* stream = nullptr)
+    {
+        check(osb200_argsort16(h_, d_keys_in, d_keys_out, d_indices, n, key_type, descending ? 1 : 0, stream), "osb200_argsort16");
+    }
     // every segment [offsets[i], offsets[i+1]) sorted ascending and stable in place, one thread block per segment
     // (reference: SplitSort, SegSort/SplitSort/SplitSort.cuh:702-938); d_values may be null; max_segment_len <= 16,384
     void SegmentedSort(uint32_t* d_keys, uint32_t* d_values, const uint64_t* d_segment_offsets, uint64_t num_segments,

@@ -122,6 +122,31 @@ OSB200_API int osb200_sort_pairs_typed(osb200_handle h, void* d_keys, uint32_t* 
 OSB200_API int osb200_argsort(osb200_handle h, const void* d_keys_in, void* d_keys_out, uint32_t* d_indices, uint64_t n,
                               int key_type, int descending, void* stream);
 
+/* 16-bit keys: uint16, int16, IEEE half (float16) and bfloat16, sorted in TWO digit passes over 2-byte keys (instead of
+ * converting them to float32 and running four passes over 4-byte keys).  They run on a handle with key_bytes == 4, which
+ * owns all the workspace they need; a caller sorting both float32 and bfloat16 keys uses one handle.
+ *   osb200_sort_keys16   as osb200_sort_keys_typed: d_keys sorted in place; any 4-byte handle
+ *   osb200_sort_pairs16  as osb200_sort_pairs_typed: uint32 payloads move with their keys; needs value_bytes == 4
+ *   osb200_argsort16     as osb200_argsort: d_keys_in untouched, d_keys_out sorted, d_indices[i] = input position of
+ *                        d_keys_out[i] (uint32, so n <= 2^32); needs value_bytes == 4
+ * Stable in both directions (descending is the complement of the transformed key).  F16 and BF16 are ordered by the total
+ * order of their bit patterns (-NaN < -inf < ... < -0.0 < +0.0 < ... < +inf < +NaN) and share one transform.
+ * Keys must be 16-byte aligned (argsort16: all three pointers); values need 4-byte alignment; the argsort16 arrays (keys 2n
+ * bytes, indices 4n bytes) must not overlap.  Returns OSB200_ERR_INVALID_ARG for a handle with key_bytes != 4 (or without
+ * payloads, for pairs16 / argsort16), a key_type outside osb200_key16_type, a null, misaligned or overlapping pointer;
+ * OSB200_ERR_SIZE for n > max_n (argsort16 also for n > 2^32); OSB200_ERR_UNSUPPORTED unless option "variant" is 2.  n <= 1
+ * is a no-op, except that argsort16 with n == 1 writes both outputs.  Options and info keys apply as to the 32-bit sorts
+ * (profile intervals: [hist, scan, pass0, pass1]); a sort of at most 16,384 keys is one launch of the single-block sort.
+ * Asynchronous, no host synchronisation, graph-capturable. */
+typedef enum osb200_key16_type {
+    OSB200_KEY16_U16 = 0, OSB200_KEY16_I16 = 1, OSB200_KEY16_F16 = 2, OSB200_KEY16_BF16 = 3
+} osb200_key16_type;
+OSB200_API int osb200_sort_keys16(osb200_handle h, void* d_keys, uint64_t n, int key_type, int descending, void* stream);
+OSB200_API int osb200_sort_pairs16(osb200_handle h, void* d_keys, uint32_t* d_values, uint64_t n, int key_type,
+                                   int descending, void* stream);
+OSB200_API int osb200_argsort16(osb200_handle h, const void* d_keys_in, void* d_keys_out, uint32_t* d_indices, uint64_t n,
+                                int key_type, int descending, void* stream);
+
 /* Sort on a bit range [begin_bit, end_bit) of the (unsigned) key only, CUB-style: keys that agree on those bits keep their
  * input order (stable).  ceil((end_bit-begin_bit)/8) digit passes instead of key_bytes; the last digit may be narrower
  * than 8 bits; an odd pass count is handled inside (the result is always returned in the caller's buffers).  d_values may
