@@ -17,6 +17,7 @@ from .onesweep import (  # noqa: F401
     argsort,
     argsort16,
     init_random,
+    sort_rows,
 )
 
 __version__ = "0.1.0"

@@ -24,8 +24,9 @@
 
 namespace {
 
-constexpr int kVersion = 1004;  // 1002: device plan, bit ranges, forward-progress fallback, hot passes, segmented sort; 1003: argsort;
-                                // 1004: 16-bit keys (osb200_sort_keys16, osb200_sort_pairs16, osb200_argsort16)
+constexpr int kVersion = 1005;  // 1002: device plan, bit ranges, forward-progress fallback, hot passes, segmented sort; 1003: argsort;
+                                // 1004: 16-bit keys (osb200_sort_keys16, osb200_sort_pairs16, osb200_argsort16);
+                                // 1005: row sort (osb200_sort_rows)
 constexpr int kMaxPlaces = 8;
 
 inline int cuda_status(cudaError_t e) { return e == cudaSuccess ? OSB200_OK : OSB200_ERR_CUDA - static_cast<int>(e); }
@@ -60,6 +61,7 @@ struct osb200_sorter {
     bool short_circuit = true;   // skip passes whose digit is the same for all keys (decided on the device, no host sync)
     bool small_path = true;      // n <= one tile: the single-CTA shared-memory sort (one launch)
     bool hot_passes = true;      // low-entropy digit places run in the HOT instantiation of the pass (decided on the device)
+    bool debug_rows_block = false;  // test hook: osb200_sort_rows sorts rows of <= 256 keys on the block path, not the warp path
 
     void* alt_keys = nullptr;
     uint32_t* alt_vals = nullptr;
@@ -433,10 +435,10 @@ int osb200_sort_keys_u64(osb200_handle h, uint64_t* d_keys, uint64_t n, void* st
     return sort_impl(h, h->key_bytes, d_keys, nullptr, n, static_cast<cudaStream_t>(stream));
 }
 
-// Typed keys (SURVEY 8f rank 1).  key_type must match the handle's key width.
-static int make_codec(const osb200_sorter* h, int key_type, int descending, osb::KeyCodec* c)
+// Typed keys (SURVEY 8f rank 1).  key_type must match the key width (the handle's, or the row sort's key_bytes).
+static int make_codec(int key_bytes, int key_type, int descending, osb::KeyCodec* c)
 {
-    const bool wide64 = h->key_bytes == 8;
+    const bool wide64 = key_bytes == 8;
     const unsigned long long all = wide64 ? ~0ull : 0xffffffffull, sign = wide64 ? (1ull << 63) : (1ull << 31);
     switch (key_type) {
         case OSB200_KEY_U32: if (wide64) return OSB200_ERR_INVALID_ARG; c->a = 0; c->b = 0; break;
@@ -456,7 +458,7 @@ int osb200_sort_keys_typed(osb200_handle h, void* d_keys, uint64_t n, int key_ty
 {
     if (check_handle(h) != OSB200_OK) return OSB200_ERR_INVALID_ARG;
     osb::KeyCodec c;
-    int st = make_codec(h, key_type, descending, &c);
+    int st = make_codec(h->key_bytes, key_type, descending, &c);
     if (st != OSB200_OK) return st;
     if (h->cfg.variant != osb::kVariantWide) return OSB200_ERR_UNSUPPORTED;
     const bool plain = c.a == 0 && c.b == 0 && c.d == 0;
@@ -490,7 +492,7 @@ int osb200_sort_pairs_typed(osb200_handle h, void* d_keys, uint32_t* d_values, u
     if (check_handle(h) != OSB200_OK || h->key_bytes != 4 || h->value_bytes != 4) return OSB200_ERR_INVALID_ARG;
     if (n > 1 && !d_values) return OSB200_ERR_INVALID_ARG;
     osb::KeyCodec c;
-    int st = make_codec(h, key_type, descending, &c);
+    int st = make_codec(h->key_bytes, key_type, descending, &c);
     if (st != OSB200_OK) return st;
     if (h->cfg.variant != osb::kVariantWide) return OSB200_ERR_UNSUPPORTED;
     const bool plain = c.a == 0 && c.b == 0 && c.d == 0;
@@ -502,7 +504,7 @@ int osb200_argsort(osb200_handle h, const void* d_keys_in, void* d_keys_out, uin
 {
     if (check_handle(h) != OSB200_OK || h->key_bytes != 4 || h->value_bytes != 4) return OSB200_ERR_INVALID_ARG;
     osb::KeyCodec c;
-    int st = make_codec(h, key_type, descending, &c);  // 64-bit key types: INVALID_ARG on this 4-byte handle
+    int st = make_codec(h->key_bytes, key_type, descending, &c);  // 64-bit key types: INVALID_ARG on this 4-byte handle
     if (st != OSB200_OK) return st;
     if (h->cfg.variant != osb::kVariantWide) return OSB200_ERR_UNSUPPORTED;  // the indices mode lives in the device plan
     if (n == 0) return OSB200_OK;
@@ -591,6 +593,45 @@ int osb200_argsort16(osb200_handle h, const void* d_keys_in, void* d_keys_out, u
     }
     const bool plain = c.a == 0 && c.b == 0 && c.d == 0;
     return sort_impl(h, 2, d_keys_out, d_indices, n, q, plain ? nullptr : &c, 0, -1, d_keys_in);
+}
+
+// Row sort: one launch, no workspace -- only the handle's device, rank mode and SM count are used, so any handle will do.
+int osb200_sort_rows(osb200_handle h, const void* d_keys_in, void* d_keys_out, uint32_t* d_indices, uint64_t num_rows,
+                     uint32_t row_len, int key_bytes, int key_type, int descending, void* stream)
+{
+    if (check_handle(h) != OSB200_OK) return OSB200_ERR_INVALID_ARG;
+    osb::KeyCodec c;
+    int st = key_bytes == 2 ? make_codec16(key_type, descending, &c)
+             : key_bytes == 4 || key_bytes == 8 ? make_codec(key_bytes, key_type, descending, &c)
+                                                : OSB200_ERR_INVALID_ARG;
+    if (st != OSB200_OK) return st;
+    if (num_rows == 0 || row_len == 0) return OSB200_OK;
+    const uintptr_t in = reinterpret_cast<uintptr_t>(d_keys_in), out = reinterpret_cast<uintptr_t>(d_keys_out),
+                    idx = reinterpret_cast<uintptr_t>(d_indices);
+    if (!in || !out) return OSB200_ERR_INVALID_ARG;
+    // the kernels load and store element by element: natural alignment is enough
+    if (((in | out) & static_cast<uintptr_t>(key_bytes - 1)) || (idx & 3u)) return OSB200_ERR_INVALID_ARG;
+    // the array sizes in bytes must fit in 64 bits
+    if (num_rows > UINT64_MAX / row_len) return OSB200_ERR_INVALID_ARG;
+    const uint64_t n = num_rows * row_len;
+    if (n > UINT64_MAX / 8) return OSB200_ERR_INVALID_ARG;
+    const uint64_t kb = n * static_cast<uint64_t>(key_bytes), ib = n * sizeof(uint32_t);
+    auto overlap = [](uintptr_t a, uint64_t alen, uintptr_t b, uint64_t blen) { return a < b + blen && b < a + alen; };
+    // in place (out == in) is fine: a row is read whole before it is written; any other overlap is not
+    if ((in != out && overlap(in, kb, out, kb)) || (idx && (overlap(in, kb, idx, ib) || overlap(out, kb, idx, ib))))
+        return OSB200_ERR_INVALID_ARG;
+    if (row_len > osb::row_sort_capacity(key_bytes)) return OSB200_ERR_SIZE;
+    cudaStream_t q = static_cast<cudaStream_t>(stream);
+    if (row_len == 1) {  // every row is sorted already
+        if (in != out) OSB_TRY(cudaMemcpyAsync(d_keys_out, d_keys_in, kb, cudaMemcpyDeviceToDevice, q));
+        if (idx) OSB_TRY(cudaMemsetAsync(d_indices, 0, ib, q));
+        return OSB200_OK;
+    }
+    const bool plain = c.a == 0 && c.b == 0 && c.d == 0;
+    c.flags = osb::kCodecEncodeOnLoad | osb::kCodecDecodeOnStore;
+    OSB_TRY(osb::launch_row_sort(d_keys_in, d_keys_out, d_indices, num_rows, row_len, key_bytes, plain ? nullptr : &c,
+                                 h->cfg.rank_mode, h->debug_rows_block, h->sm_count, q));
+    return OSB200_OK;
 }
 
 int osb200_sort_host_keys_u32(osb200_handle h, uint32_t* h_keys, uint64_t n)
@@ -742,6 +783,7 @@ int osb200_set_option(osb200_handle h, const char* key, int64_t value)
         h->cfg.debug_max_ctas = static_cast<uint32_t>(value);
         return OSB200_OK;
     }
+    if (!std::strcmp(key, "debug_rows_block")) { h->debug_rows_block = value != 0; return OSB200_OK; }
     if (!std::strcmp(key, "debug_epoch")) {  // test hook: the epoch counter, to reach the wrap-around or reuse epochs
         if (value < 0 || value > osb::kEpochMax) return OSB200_ERR_INVALID_ARG;
         h->epoch = static_cast<uint32_t>(value);

@@ -1982,10 +1982,14 @@ struct SegSmem {
     uint32_t wtot[kRadix / 32];
 };
 
-// INDICES (argsort of the single segment): the keys come from keys_in, every payload is the key's position in the segment.
+// INDICES (argsort): the keys come from keys_in, every payload is the key's position in its segment.
+// ROWS (row sort, osb200_sort_rows): segment s is row s, [s * single_n, (s + 1) * single_n) (seg_off is not read), and the
+// keys are always read from keys_in (== keys in place).  A compile-time flag rather than a runtime one, so that the
+// segmented sort's and small path's instantiations compile as before (a runtime select cost the 8,192-key u64 kernel spills).
 // max_len: the caller's max_segment_len (<= T); longer segments are left as they are.
-template <typename KeyT, bool PAIRS, int K, int WARPS, int RANK_MODE, bool INDICES = false>
-__global__ void __launch_bounds__(WARPS * 32)
+// (ROWS: one resident CTA per SM is stated, or ptxas caps some 512-thread instantiations at 64 registers and spills.)
+template <typename KeyT, bool PAIRS, int K, int WARPS, int RANK_MODE, bool INDICES = false, bool ROWS = false>
+__global__ void __launch_bounds__(WARPS * 32, ROWS ? 1 : 0)
 segment_sort_kernel(KeyT* keys, uint32_t* vals, const unsigned long long* __restrict__ seg_off, uint64_t num_segments,
                     uint64_t single_n, uint32_t max_len, uint32_t begin_bit, uint32_t places, uint32_t last_bits, KeyCodec codec,
                     const KeyT* __restrict__ keys_in)
@@ -2005,8 +2009,8 @@ segment_sort_kernel(KeyT* keys, uint32_t* vals, const unsigned long long* __rest
     const bool enc = codec.flags & kCodecEncodeOnLoad, dec = codec.flags & kCodecDecodeOnStore;
 
     for (uint64_t seg = blockIdx.x; seg < num_segments; seg += gridDim.x) {
-        const uint64_t lo = seg_off ? seg_off[seg] : 0ull;
-        const uint64_t hi = seg_off ? seg_off[seg + 1] : single_n;
+        const uint64_t lo = ROWS ? seg * single_n : seg_off ? seg_off[seg] : 0ull;
+        const uint64_t hi = ROWS ? lo + single_n : seg_off ? seg_off[seg + 1] : single_n;
         // empty / one key / longer than max_segment_len or the geometry (both the caller's contract: left untouched)
         if (hi <= lo + 1 || hi - lo > static_cast<uint64_t>(max_len) || hi - lo > static_cast<uint64_t>(T)) continue;
         const uint32_t len = static_cast<uint32_t>(hi - lo);
@@ -2016,12 +2020,20 @@ segment_sort_kernel(KeyT* keys, uint32_t* vals, const unsigned long long* __rest
 #pragma unroll
         for (int i = 0; i < K; ++i) {
             const uint32_t idx = warp_off + i * 32;
-            KeyT k = idx < len ? (INDICES ? keys_in : keys)[lo + idx] : static_cast<KeyT>(0);
+            KeyT k = idx < len ? (INDICES || ROWS ? keys_in : keys)[lo + idx] : static_cast<KeyT>(0);
             if (enc) k = codec_encode<KeyT>(k, ca, cb, cd);
             key[i] = idx < len ? k : static_cast<KeyT>(~static_cast<KeyT>(0));  // padding ranks last in every pass
             if constexpr (PAIRS) val[i] = INDICES ? idx : idx < len ? vals[lo + idx] : 0u;
         }
 
+        // ROWS: a warp's 32 keys of step i that all lie behind the row are padding, and every padding key has digit 255 in
+        // every pass: ranking them costs one serialised same-address atomic per key.  Such chunks are neither counted nor
+        // ranked (what they read back from slots nobody wrote is never used).  The padding of the one chunk that straddles
+        // `len` is ranked; it follows every real key in tile order, so it takes the slots from `len` on, which are its own
+        // positions.  (The condition is warp-uniform, so the ballot ranking sees full warps.)
+        const uint32_t warp_lo = warp * (32 * K);  // this warp's chunks: [warp_lo + 32 i, warp_lo + 32 i + 32)
+        const uint32_t live_chunks = ROWS ? (len > warp_lo ? (len - warp_lo + 31) / 32 : 0u) : static_cast<uint32_t>(K);
+        auto live = [&](int i) { return !ROWS || static_cast<uint32_t>(i) < live_chunks; };
         for (uint32_t p = 0; p < places; ++p) {
             const uint32_t shift = begin_bit + 8u * p;
             const uint32_t dmask = p == places - 1 ? (1u << last_bits) - 1u : 255u;
@@ -2032,7 +2044,8 @@ segment_sort_kernel(KeyT* keys, uint32_t* vals, const unsigned long long* __rest
             }
             __syncthreads();
 #pragma unroll
-            for (int i = 0; i < K; ++i) atomicAdd(&wh[digit_of(key[i], shift, dmask)], 1u);
+            for (int i = 0; i < K; ++i)
+                if (live(i)) atomicAdd(&wh[digit_of(key[i], shift, dmask)], 1u);
             __syncthreads();
             uint32_t tile_count = 0;
             if (tid < kRadix) {
@@ -2048,6 +2061,7 @@ segment_sort_kernel(KeyT* keys, uint32_t* vals, const unsigned long long* __rest
             __syncthreads();
 #pragma unroll
             for (int i = 0; i < K; ++i) {
+                if (!live(i)) continue;
                 const uint32_t slot = warp_rank_and_count<RANK_MODE>(wh, digit_of(key[i], shift, dmask), lt);
                 sm.sorted[slot] = key[i];
                 if constexpr (PAIRS) sm.sorted_val[slot] = val[i];
@@ -2080,7 +2094,8 @@ template <> struct SegGeomN<uint32_t, 2> { static constexpr int K = 32, WARPS = 
 template <> struct SegGeomN<uint64_t, 0> { static constexpr int K = 1,  WARPS = 8; };   //    256 keys
 template <> struct SegGeomN<uint64_t, 1> { static constexpr int K = 8,  WARPS = 8; };   //  2,048 keys
 template <> struct SegGeomN<uint64_t, 2> { static constexpr int K = 16, WARPS = 16; };  //  8,192 keys
-// 16-bit keys: only the small-n path of their sorts (one segment of up to 16,384 keys; no segmented sort of 16-bit keys)
+// 16-bit keys: the small-n path of their sorts (one segment of up to 16,384 keys) and the row sort; no segmented sort
+template <> struct SegGeomN<uint16_t, 1> { static constexpr int K = 8,  WARPS = 8; };   //  2,048 keys (row sort only)
 template <> struct SegGeomN<uint16_t, 2> { static constexpr int K = 32, WARPS = 16; };  // 16,384 keys, 512 threads
 template <typename KeyT, int SIZE> constexpr uint32_t seg_cap() { return SegGeomN<KeyT, SIZE>::K * SegGeomN<KeyT, SIZE>::WARPS * 32; }
 
@@ -2091,11 +2106,12 @@ uint32_t segment_sort_capacity(int key_bytes, bool small)
     return small ? seg_cap<uint32_t, 1>() : seg_cap<uint32_t, 2>();
 }
 
-template <typename KeyT, bool PAIRS, int SIZE, int RANK_MODE, bool INDICES = false>
+template <typename KeyT, bool PAIRS, int SIZE, int RANK_MODE, bool INDICES = false, bool ROWS = false>
 static cudaError_t seg_attr()
 {
     using G = SegGeomN<KeyT, SIZE>;
-    return cudaFuncSetAttribute(segment_sort_kernel<KeyT, PAIRS, G::K, G::WARPS, RANK_MODE, INDICES>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    return cudaFuncSetAttribute(segment_sort_kernel<KeyT, PAIRS, G::K, G::WARPS, RANK_MODE, INDICES, ROWS>,
+                                cudaFuncAttributeMaxDynamicSharedMemorySize,
                                 static_cast<int>(sizeof(SegSmem<KeyT, PAIRS, G::K, G::WARPS>)));
 }
 static cudaError_t configure_segment_kernels()
@@ -2122,10 +2138,22 @@ static cudaError_t configure_segment_kernels()
     if ((e = seg_attr<uint16_t, true, 2, kRankBallot>()) != cudaSuccess) return e;
     if ((e = seg_attr<uint16_t, true, 2, kRankAtomic, true>()) != cudaSuccess) return e;
     if ((e = seg_attr<uint16_t, true, 2, kRankBallot, true>()) != cudaSuccess) return e;
+    // row sort (launch_row_sort): geometries 1 and 2 of every key width, keys only and with indices
+#define OSB_ROW_ATTR_SIZE(KEYT, SIZE)                                                                      \
+    if ((e = seg_attr<KEYT, false, SIZE, kRankAtomic, false, true>()) != cudaSuccess) return e;            \
+    if ((e = seg_attr<KEYT, false, SIZE, kRankBallot, false, true>()) != cudaSuccess) return e;            \
+    if ((e = seg_attr<KEYT, true, SIZE, kRankAtomic, true, true>()) != cudaSuccess) return e;              \
+    if ((e = seg_attr<KEYT, true, SIZE, kRankBallot, true, true>()) != cudaSuccess) return e;
+#define OSB_ROW_ATTR(KEYT) OSB_ROW_ATTR_SIZE(KEYT, 1) OSB_ROW_ATTR_SIZE(KEYT, 2)
+    OSB_ROW_ATTR(uint16_t)
+    OSB_ROW_ATTR(uint32_t)
+    OSB_ROW_ATTR(uint64_t)
+#undef OSB_ROW_ATTR
+#undef OSB_ROW_ATTR_SIZE
     return cudaSuccess;
 }
 
-template <typename KeyT, bool PAIRS, int SIZE, bool INDICES = false>
+template <typename KeyT, bool PAIRS, int SIZE, bool INDICES = false, bool ROWS = false>
 static cudaError_t launch_seg(void* keys, uint32_t* vals, const unsigned long long* seg_off, uint64_t num_segments, uint64_t single_n,
                               uint32_t max_len, uint32_t begin_bit, uint32_t places, uint32_t last_bits, const KeyCodec& codec,
                               int rank_mode, int sm_count, cudaStream_t stream, const void* keys_in = nullptr)
@@ -2136,10 +2164,10 @@ static cudaError_t launch_seg(void* keys, uint32_t* vals, const unsigned long lo
     const unsigned grid = static_cast<unsigned>(num_segments < cap ? num_segments : cap);
     const KeyT* in = static_cast<const KeyT*>(keys_in);
     if (rank_mode == kRankBallot)
-        segment_sort_kernel<KeyT, PAIRS, G::K, G::WARPS, kRankBallot, INDICES><<<grid, S::THREADS, sizeof(S), stream>>>(
+        segment_sort_kernel<KeyT, PAIRS, G::K, G::WARPS, kRankBallot, INDICES, ROWS><<<grid, S::THREADS, sizeof(S), stream>>>(
             static_cast<KeyT*>(keys), vals, seg_off, num_segments, single_n, max_len, begin_bit, places, last_bits, codec, in);
     else
-        segment_sort_kernel<KeyT, PAIRS, G::K, G::WARPS, kRankAtomic, INDICES><<<grid, S::THREADS, sizeof(S), stream>>>(
+        segment_sort_kernel<KeyT, PAIRS, G::K, G::WARPS, kRankAtomic, INDICES, ROWS><<<grid, S::THREADS, sizeof(S), stream>>>(
             static_cast<KeyT*>(keys), vals, seg_off, num_segments, single_n, max_len, begin_bit, places, last_bits, codec, in);
     return cudaGetLastError();
 }
@@ -2177,6 +2205,177 @@ cudaError_t launch_segment_sort(void* keys, uint32_t* vals, int key_bytes, const
 #undef OSB_SEG_ARGS
 #undef OSB_SEG
     return cudaErrorInvalidValue;
+}
+
+// =====================================================================================================
+// Row sort, warp path: rows of at most 256 keys, ONE WARP sorts one row at a time (grid-stride over the rows).  The block
+// path would pad such a row to a block's tile and pay six block barriers and an 8 x 256-bin histogram clear and scan per
+// pass; a warp needs no block barrier at all.  Reference: SplitSort packs short segments at warp level
+// (SegSort/SplitSort/SplitSort.cuh:31-130); the ranking here is the DigitBinningPass's (warp_rank_and_count), so the order is
+// stable by the same lane-order property (or the ballot mode).
+//
+// Per pass: count the row's digits in the warp's own 256 bins (real keys only), one lane scans 8 bins and the warp scans
+// the lane totals with shuffles, every key is ranked in tile order (key i*32 + lane) and stored at its slot in the warp's
+// staging area, and read back in tile order.  The padding keys (all ones) rank after every real key, at slots >= row_len.
+// A pass in which one bin holds the whole row would leave the order as it is, so the warp skips it: 64-bit rows of small
+// values execute only the passes of their low digits.
+// =====================================================================================================
+constexpr int kRowWarps = 8;  // warps per CTA (independent: no block barrier)
+
+template <typename KeyT, int K, bool INDICES>
+struct RowWarpSmem {  // one per warp: 1 KB of bins + the staging area (at most 4 KB: 64-bit keys with indices, K = 8)
+    alignas(16) uint32_t hist[kRadix];
+    alignas(16) KeyT keys[32 * K];
+    uint32_t idx[INDICES ? 32 * K : 1];
+};
+
+template <typename KeyT, int K, int RANK_MODE, bool INDICES>
+__global__ void __launch_bounds__(kRowWarps * 32)
+row_sort_warp_kernel(const KeyT* in, KeyT* out, uint32_t* __restrict__ idx_out, uint64_t num_rows, uint32_t row_len,
+                     KeyCodec codec)
+{
+    using W = RowWarpSmem<KeyT, K, INDICES>;
+    extern __shared__ __align__(16) unsigned char s_raw[];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    W& sm = reinterpret_cast<W*>(s_raw)[warp];
+    uint4* h4 = reinterpret_cast<uint4*>(sm.hist);  // lane l owns bins 8l .. 8l+7 (h4[2l], h4[2l+1])
+    const uint32_t lt = lanemask_lt();
+    const KeyT ca = static_cast<KeyT>(codec.a), cb = static_cast<KeyT>(codec.b), cd = static_cast<KeyT>(codec.d);
+    const bool enc = codec.flags & kCodecEncodeOnLoad, dec = codec.flags & kCodecDecodeOnStore;
+
+    for (uint64_t row = static_cast<uint64_t>(blockIdx.x) * kRowWarps + warp; row < num_rows;
+         row += static_cast<uint64_t>(gridDim.x) * kRowWarps) {
+        const uint64_t base = row * row_len;
+        KeyT key[K];
+        uint32_t val[INDICES ? K : 1];
+#pragma unroll
+        for (int i = 0; i < K; ++i) {
+            const uint32_t idx = i * 32 + lane;
+            KeyT k = idx < row_len ? in[base + idx] : static_cast<KeyT>(0);
+            if (enc) k = codec_encode<KeyT>(k, ca, cb, cd);
+            key[i] = idx < row_len ? k : static_cast<KeyT>(~static_cast<KeyT>(0));
+            if constexpr (INDICES) val[i] = idx;
+        }
+#pragma unroll 1
+        for (uint32_t shift = 0; shift < sizeof(KeyT) * 8; shift += 8) {
+            h4[2 * lane] = make_uint4(0, 0, 0, 0);
+            h4[2 * lane + 1] = make_uint4(0, 0, 0, 0);
+            __syncwarp();
+#pragma unroll
+            for (int i = 0; i < K; ++i)
+                if (i * 32 + lane < row_len) atomicAdd(&sm.hist[digit_of(key[i], shift)], 1u);
+            __syncwarp();
+            const uint4 lo4 = h4[2 * lane], hi4 = h4[2 * lane + 1];
+            const uint32_t c[8] = {lo4.x, lo4.y, lo4.z, lo4.w, hi4.x, hi4.y, hi4.z, hi4.w};
+            uint32_t sum = 0;
+            bool whole = false;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) { sum += c[j]; whole |= c[j] == row_len; }
+            if (__any_sync(0xffffffffu, whole)) continue;  // one digit for the whole row: this pass keeps the order
+            uint32_t incl = sum;
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+                const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o);
+                if (lane >= o) incl += t;
+            }
+            uint32_t run = incl - sum, e[8];
+#pragma unroll
+            for (int j = 0; j < 8; ++j) { e[j] = run; run += c[j]; }
+            h4[2 * lane] = make_uint4(e[0], e[1], e[2], e[3]);
+            h4[2 * lane + 1] = make_uint4(e[4], e[5], e[6], e[7]);
+            __syncwarp();
+#pragma unroll
+            for (int i = 0; i < K; ++i) {
+                const uint32_t slot = warp_rank_and_count<RANK_MODE>(sm.hist, digit_of(key[i], shift), lt);
+                sm.keys[slot] = key[i];
+                if constexpr (INDICES) sm.idx[slot] = val[i];
+            }
+            __syncwarp();
+#pragma unroll
+            for (int i = 0; i < K; ++i) {
+                key[i] = sm.keys[i * 32 + lane];
+                if constexpr (INDICES) val[i] = sm.idx[i * 32 + lane];
+            }
+            __syncwarp();
+        }
+#pragma unroll
+        for (int i = 0; i < K; ++i) {
+            const uint32_t idx = i * 32 + lane;
+            if (idx < row_len) {
+                KeyT k = key[i];
+                if (dec) k = codec_decode<KeyT>(k, ca, cb, cd);
+                out[base + idx] = k;
+                if constexpr (INDICES) idx_out[base + idx] = val[i];
+            }
+        }
+    }
+}
+
+// CTAs of one kernel that are resident on one SM (the warp path's grid: a grid-stride loop over the rows wants every CTA
+// resident from the start)
+template <typename KeyT, int K, int RANK_MODE, bool INDICES>
+static cudaError_t launch_row_warp(const void* in, void* out, uint32_t* idx, uint64_t num_rows, uint32_t row_len,
+                                   const KeyCodec& codec, int sm_count, cudaStream_t stream)
+{
+    auto kern = row_sort_warp_kernel<KeyT, K, RANK_MODE, INDICES>;
+    constexpr size_t smem = kRowWarps * sizeof(RowWarpSmem<KeyT, K, INDICES>);
+    static const int per_sm = [&] {
+        int b = 0;
+        return cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, kern, kRowWarps * 32, smem) == cudaSuccess ? b : 0;
+    }();
+    if (per_sm <= 0) return cudaErrorLaunchOutOfResources;
+    const uint64_t need = (num_rows + kRowWarps - 1) / kRowWarps, cap = static_cast<uint64_t>(sm_count) * per_sm;
+    kern<<<static_cast<unsigned>(need < cap ? need : cap), kRowWarps * 32, smem, stream>>>(
+        static_cast<const KeyT*>(in), static_cast<KeyT*>(out), idx, num_rows, row_len, codec);
+    return cudaGetLastError();
+}
+
+template <typename KeyT, int RANK_MODE, bool INDICES>
+static cudaError_t launch_row_warp_k(const void* in, void* out, uint32_t* idx, uint64_t num_rows, uint32_t row_len,
+                                     const KeyCodec& codec, int sm_count, cudaStream_t stream)
+{
+    if (row_len <= 32) return launch_row_warp<KeyT, 1, RANK_MODE, INDICES>(in, out, idx, num_rows, row_len, codec, sm_count, stream);
+    if (row_len <= 64) return launch_row_warp<KeyT, 2, RANK_MODE, INDICES>(in, out, idx, num_rows, row_len, codec, sm_count, stream);
+    if (row_len <= 128) return launch_row_warp<KeyT, 4, RANK_MODE, INDICES>(in, out, idx, num_rows, row_len, codec, sm_count, stream);
+    return launch_row_warp<KeyT, 8, RANK_MODE, INDICES>(in, out, idx, num_rows, row_len, codec, sm_count, stream);
+}
+
+template <typename KeyT>
+static cudaError_t launch_rows(const void* keys_in, void* keys_out, uint32_t* indices, uint64_t num_rows, uint32_t row_len,
+                               const KeyCodec& codec, int rank_mode, bool block_only, int sm_count, cudaStream_t stream)
+{
+    if (row_len <= kRowWarpMaxLen && !block_only) {
+        if (rank_mode == kRankBallot)
+            return indices ? launch_row_warp_k<KeyT, kRankBallot, true>(keys_in, keys_out, indices, num_rows, row_len, codec, sm_count, stream)
+                           : launch_row_warp_k<KeyT, kRankBallot, false>(keys_in, keys_out, indices, num_rows, row_len, codec, sm_count, stream);
+        return indices ? launch_row_warp_k<KeyT, kRankAtomic, true>(keys_in, keys_out, indices, num_rows, row_len, codec, sm_count, stream)
+                       : launch_row_warp_k<KeyT, kRankAtomic, false>(keys_in, keys_out, indices, num_rows, row_len, codec, sm_count, stream);
+    }
+    // block path: segment s of segment_sort_kernel is row s
+    const bool small = row_len <= seg_cap<KeyT, 1>();
+#define OSB_ROW_ARGS keys_out, indices, nullptr, num_rows, row_len, row_len, 0u, static_cast<uint32_t>(sizeof(KeyT)), 8u, codec, \
+                     rank_mode, sm_count, stream, keys_in
+    if (indices)
+        return small ? launch_seg<KeyT, true, 1, true, true>(OSB_ROW_ARGS) : launch_seg<KeyT, true, 2, true, true>(OSB_ROW_ARGS);
+    return small ? launch_seg<KeyT, false, 1, false, true>(OSB_ROW_ARGS) : launch_seg<KeyT, false, 2, false, true>(OSB_ROW_ARGS);
+#undef OSB_ROW_ARGS
+}
+
+uint32_t row_sort_capacity(int key_bytes) { return key_bytes == 8 ? seg_cap<uint64_t, 2>() : seg_cap<uint32_t, 2>(); }
+
+cudaError_t launch_row_sort(const void* keys_in, void* keys_out, uint32_t* indices, uint64_t num_rows, uint32_t row_len,
+                            int key_bytes, const KeyCodec* codec_in, int rank_mode, bool block_only, int sm_count,
+                            cudaStream_t stream)
+{
+    if (num_rows == 0 || row_len == 0) return cudaSuccess;
+    if (row_len > row_sort_capacity(key_bytes)) return cudaErrorInvalidValue;
+    const KeyCodec codec = codec_in ? *codec_in : KeyCodec();
+    switch (key_bytes) {
+        case 2: return launch_rows<uint16_t>(keys_in, keys_out, indices, num_rows, row_len, codec, rank_mode, block_only, sm_count, stream);
+        case 4: return launch_rows<uint32_t>(keys_in, keys_out, indices, num_rows, row_len, codec, rank_mode, block_only, sm_count, stream);
+        case 8: return launch_rows<uint64_t>(keys_in, keys_out, indices, num_rows, row_len, codec, rank_mode, block_only, sm_count, stream);
+        default: return cudaErrorInvalidValue;
+    }
 }
 
 // =====================================================================================================

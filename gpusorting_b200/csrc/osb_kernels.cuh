@@ -94,6 +94,18 @@ cudaError_t launch_segment_sort(void* keys, uint32_t* vals, int key_bytes, const
                                 const KeyCodec* codec, int rank_mode, int sm_count, cudaStream_t stream,
                                 const void* keys_in = nullptr);
 
+// Row sort: row r = elements [r * row_len, (r + 1) * row_len) of keys_in, sorted stable into the same row of keys_out
+// (keys_out == keys_in: in place); indices (may be null) receives every output key's position within its row.  Rows of at
+// most kRowWarpMaxLen keys are sorted one per warp (row_sort_warp_kernel) unless block_only; longer rows, up to
+// row_sort_capacity(key_bytes), one per CTA by segment_sort_kernel (2,048- or 16,384-key geometry).  key_bytes 2, 4 or 8; the
+// codec (both flags set, or null for plain unsigned ascending keys) is applied on load and undone on store.  The caller
+// handles row_len == 1, which the block path leaves untouched.
+constexpr uint32_t kRowWarpMaxLen = 256;
+uint32_t row_sort_capacity(int key_bytes);
+cudaError_t launch_row_sort(const void* keys_in, void* keys_out, uint32_t* indices, uint64_t num_rows, uint32_t row_len,
+                            int key_bytes, const KeyCodec* codec, int rank_mode, bool block_only, int sm_count,
+                            cudaStream_t stream);
+
 // Validate (reference: Validate, UtilityKernels.cuh:403-429): err_count += #(keys[i] > keys[i+1]).
 cudaError_t launch_validate(const void* keys, uint64_t n, int key_bytes, unsigned long long* err_count, int sm_count,
                             cudaStream_t stream);

@@ -33,6 +33,10 @@ KEY_TYPES = {"u32": 0, "i32": 1, "f32": 2, "u64": 3, "i64": 4, "f64": 5}
 # 16-bit keys (sort_keys16 / sort_pairs16 / argsort16, on a 4-byte sorter): key_type states the order, the dtype the width
 _TYPED_DTYPES_2 = (torch.int16, torch.uint16, torch.float16, torch.bfloat16)
 KEY16_TYPES = {"u16": 0, "i16": 1, "f16": 2, "bf16": 3}
+# row sort (sort_rows): the key type of every dtype it takes
+_ROW_KEY_TYPES = {torch.int16: "i16", torch.uint16: "u16", torch.float16: "f16", torch.bfloat16: "bf16",
+                  torch.int32: "i32", torch.uint32: "u32", torch.float32: "f32",
+                  torch.int64: "i64", torch.uint64: "u64", torch.float64: "f64"}
 
 
 def _stream_ptr(stream: Optional[torch.cuda.Stream]) -> int:
@@ -199,6 +203,34 @@ class OneSweepSorter:
             check(lib.osb200_argsort16(self._h, keys.data_ptr(), out.data_ptr(), idx.data_ptr(), n, KEY16_TYPES[key_type],
                                        1 if descending else 0, _stream_ptr(stream)), "osb200_argsort16")
         return out, idx
+
+    # -- row sort: every row of a batch along its last dimension, no workspace (any sorter will do) -------------------
+    def sort_rows(self, x: torch.Tensor, key_type: str, descending: bool = False, return_indices: bool = True,
+                  inplace: bool = False, stream=None):
+        """Stable sort of every row of `x` along its last dimension (osb200_sort_rows), the shape of
+        ``torch.sort(x, dim=-1, stable=True)``.  `x` is a contiguous CUDA tensor of rank >= 1 of any of the ten key dtypes;
+        key_type states how its bits are ordered: one of KEY16_TYPES for 2-byte dtypes, of KEY_TYPES of the dtype's width
+        otherwise.  Floats follow the total order of their bit patterns; equal keys keep their order in both directions.
+
+        Returns (values, indices) shaped like `x`, indices as torch.int32 positions within the row, or `values` alone with
+        return_indices=False.  The outputs are new tensors allocated with torch.empty on the stream; inplace=True sorts `x`
+        itself and returns it as `values`.  The last dimension may hold at most 16,384 keys (8,192 for 8-byte dtypes)."""
+        if not (isinstance(x, torch.Tensor) and x.is_cuda and x.is_contiguous() and x.dim() >= 1 and x.dtype in _ROW_KEY_TYPES):
+            raise TypeError(f"x must be a contiguous CUDA tensor of rank >= 1 with dtype in {tuple(_ROW_KEY_TYPES)}")
+        if x.device.index != self.device:
+            raise ValueError(f"x lives on cuda:{x.device.index}, the sorter on cuda:{self.device}")
+        kb = x.element_size()
+        kt = (KEY16_TYPES if kb == 2 else KEY_TYPES)[key_type]
+        row_len = x.shape[-1]
+        num_rows = x.numel() // row_len if row_len else 0
+        with torch.cuda.stream(stream):  # (None: the current stream) the outputs belong to the stream that writes them
+            out = x if inplace else torch.empty_like(x)
+            idx = torch.empty(x.shape, dtype=torch.int32, device=x.device) if return_indices else None
+        with torch.cuda.device(self.device):
+            check(lib.osb200_sort_rows(self._h, x.data_ptr(), out.data_ptr(), idx.data_ptr() if idx is not None else None,
+                                       num_rows, row_len, kb, kt, 1 if descending else 0, _stream_ptr(stream)),
+                  "osb200_sort_rows")
+        return (out, idx) if return_indices else out
 
     def sort_bits(self, keys: torch.Tensor, begin_bit: int, end_bit: int, values: Optional[torch.Tensor] = None,
                   n: Optional[int] = None, stream=None):
@@ -378,6 +410,20 @@ def argsort16(keys: torch.Tensor, key_type: str, descending: bool = False, n: Op
         sp = _stream_ptr(stream)
     s = _cached_sorter(keys.device.index, 4, 4, n, sp)
     return s.argsort16(keys, key_type, descending, n, stream)
+
+
+def sort_rows(x: torch.Tensor, descending: bool = False, return_indices: bool = True, stream=None):
+    """``torch.sort(x, dim=-1, stable=True)`` for a contiguous CUDA tensor of int16, uint16, float16, bfloat16, int32, uint32,
+    float32, int64, uint64 or float64: (values, int32 indices), or values alone.  The key type follows the dtype.
+    OneSweepSorter.sort_rows on the stream's cached (4, 4) sorter, the one argsort uses (the row sort needs no workspace)."""
+    if not (isinstance(x, torch.Tensor) and x.is_cuda):
+        raise TypeError("x must be a CUDA tensor")
+    if x.dtype not in _ROW_KEY_TYPES:
+        raise TypeError(f"x.dtype must be one of {tuple(_ROW_KEY_TYPES)}")
+    with torch.cuda.device(x.device.index):
+        sp = _stream_ptr(stream)
+    s = _cached_sorter(x.device.index, 4, 4, 1, sp)
+    return s.sort_rows(x, _ROW_KEY_TYPES[x.dtype], descending, return_indices, False, stream)
 
 
 class OneSweepDispatcher:

@@ -65,6 +65,16 @@ class OneSweepSorterB200 {
     {
         check(osb200_argsort16(h_, d_keys_in, d_keys_out, d_indices, n, key_type, descending ? 1 : 0, stream), "osb200_argsort16");
     }
+    // every row [r*row_len, (r+1)*row_len) of d_keys_in sorted stable into d_keys_out (== d_keys_in: in place), with
+    // d_indices (may be null) = positions within the row; key_bytes 2 (osb200_key16_type) or 4 / 8 (osb200_key_type);
+    // row_len <= 16,384 (8,192 for 8-byte keys); any sorter
+    void SortRows(const void* d_keys_in, void* d_keys_out, uint32_t* d_indices, uint64_t num_rows, uint32_t row_len,
+                  int key_bytes, int key_type, bool descending, void* stream = nullptr)
+    {
+        check(osb200_sort_rows(h_, d_keys_in, d_keys_out, d_indices, num_rows, row_len, key_bytes, key_type, descending ? 1 : 0,
+                               stream),
+              "osb200_sort_rows");
+    }
     // every segment [offsets[i], offsets[i+1]) sorted ascending and stable in place, one thread block per segment
     // (reference: SplitSort, SegSort/SplitSort/SplitSort.cuh:702-938); d_values may be null; max_segment_len <= 16,384
     void SegmentedSort(uint32_t* d_keys, uint32_t* d_values, const uint64_t* d_segment_offsets, uint64_t num_segments,

@@ -147,6 +147,25 @@ OSB200_API int osb200_sort_pairs16(osb200_handle h, void* d_keys, uint32_t* d_va
 OSB200_API int osb200_argsort16(osb200_handle h, const void* d_keys_in, void* d_keys_out, uint32_t* d_indices, uint64_t n,
                                 int key_type, int descending, void* stream);
 
+/* Row sort: every row of a batch sorted along its last dimension, the shape of torch.sort(x, dim=-1, stable=True).
+ * Row r of d_keys_in is elements [r*row_len, (r+1)*row_len); it is sorted stable into the same row of d_keys_out, ascending
+ * or descending (the complement of the encoded key, as in osb200_sort_keys_typed: equal keys keep their input order in both
+ * directions).  d_indices may be NULL (keys only); otherwise d_indices[r*row_len + j] is the position within row r of
+ * output key j (uint32).
+ *   key_bytes 2: key_type is an osb200_key16_type;  4 or 8: an osb200_key_type of that width.  Floats follow the total order
+ *                of their bit patterns, as everywhere else in this library.
+ * Any handle will do, whatever its key or value width: the call uses only the handle's device, rank mode and SM count, and
+ * allocates nothing.  d_keys_out == d_keys_in sorts in place; any other overlap among the three arrays is
+ * OSB200_ERR_INVALID_ARG.  Only natural alignment is required (the kernels load element by element).
+ * Returns OSB200_ERR_INVALID_ARG for a null handle or key pointer, a misaligned pointer, a key_bytes / key_type that do not
+ * match, or array sizes that overflow 64 bits; OSB200_ERR_SIZE for row_len above 16,384 (2- and 4-byte keys) or 8,192 (8-byte
+ * keys).  num_rows == 0 or row_len == 0 is a no-op; row_len == 1 copies the keys and writes zero indices.
+ * Rows of at most 256 keys are sorted one per warp, longer rows one per thread block in shared memory (option
+ * "debug_rows_block" = 1 sends the short rows to the block path too; a test hook).  One launch: asynchronous, no host
+ * synchronisation, graph-capturable (there is nothing to clear under capture). */
+OSB200_API int osb200_sort_rows(osb200_handle h, const void* d_keys_in, void* d_keys_out, uint32_t* d_indices, uint64_t num_rows,
+                                uint32_t row_len, int key_bytes, int key_type, int descending, void* stream);
+
 /* Sort on a bit range [begin_bit, end_bit) of the (unsigned) key only, CUB-style: keys that agree on those bits keep their
  * input order (stable).  ceil((end_bit-begin_bit)/8) digit passes instead of key_bytes; the last digit may be narrower
  * than 8 bits; an odd pass count is handled inside (the result is always returned in the caller's buffers).  d_values may
@@ -221,6 +240,8 @@ OSB200_API int osb200_init_random_u32(uint32_t* d_keys, uint32_t* d_payload, uin
  *   "debug_stall_every"  test hook for that fallback: N > 0 makes every N-th tile withhold its reduction
  *   "debug_max_ctas" test hook of the persistent DigitBinningPass (uint32 keys, HOT passes): N > 0 runs it on at most N CTAs (the tiles after
  *                    each CTA's first are handed out by an atomic ticket); 0 (default) = as many as can be resident
+ *   "debug_rows_block"  test hook of osb200_sort_rows: 1 = rows of at most 256 keys go through the block path (2,048-key
+ *                    geometry) instead of one warp per row, to compare the two paths; 0 (default) = the warp path
  *   "debug_epoch"    test hook of the descriptor epochs: sets the handle's epoch counter (0 .. 2^24 - 1; info "epoch"), so
  *                    that the next passes cross the wrap-around (which clears every descriptor) or reuse the epochs of a
  *                    captured sort
