@@ -23,6 +23,7 @@ SIGNATURES = {
     "osb200_version": (c_int, []),
     "osb200_status_string": (ctypes.c_char_p, [c_int]),
     "osb200_create": (c_int, [ctypes.POINTER(c_vp), c_u64, c_int, c_int]),
+    "osb200_create_pairs64": (c_int, [ctypes.POINTER(c_vp), c_u64]),
     "osb200_destroy": (c_int, [c_vp]),
     "osb200_workspace_bytes": (c_u64, [c_u64, c_int, c_int]),
     "osb200_sort_keys_u32": (c_int, [c_vp, c_vp, c_u64, c_vp]),

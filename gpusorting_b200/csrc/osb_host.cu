@@ -24,9 +24,10 @@
 
 namespace {
 
-constexpr int kVersion = 1005;  // 1002: device plan, bit ranges, forward-progress fallback, hot passes, segmented sort; 1003: argsort;
+constexpr int kVersion = 1006;  // 1002: device plan, bit ranges, forward-progress fallback, hot passes, segmented sort; 1003: argsort;
                                 // 1004: 16-bit keys (osb200_sort_keys16, osb200_sort_pairs16, osb200_argsort16);
-                                // 1005: row sort (osb200_sort_rows)
+                                // 1005: row sort (osb200_sort_rows);
+                                // 1006: 64-bit keys with uint32 payloads and their argsort (osb200_create_pairs64)
 constexpr int kMaxPlaces = 8;
 
 inline int cuda_status(cudaError_t e) { return e == cudaSuccess ? OSB200_OK : OSB200_ERR_CUDA - static_cast<int>(e); }
@@ -352,12 +353,14 @@ uint64_t osb200_workspace_bytes(uint64_t max_n, int key_bytes, int value_bytes)
            (tiles + 8) * osb::kRadix * sizeof(uint16_t) * key_bytes + ControlLayout::total;
 }
 
-int osb200_create(osb200_handle* out, uint64_t max_n, int key_bytes, int value_bytes)
+}  // extern "C"
+
+namespace {
+
+// What osb200_create and osb200_create_pairs64 share once the shape is accepted: the size check, the device check, the
+// workspace, and the rank-mode self-test.
+int create_impl(osb200_handle* out, uint64_t max_n, int key_bytes, int value_bytes)
 {
-    if (!out) return OSB200_ERR_INVALID_ARG;
-    *out = nullptr;
-    if ((key_bytes != 4 && key_bytes != 8) || (value_bytes != 0 && value_bytes != 4)) return OSB200_ERR_INVALID_ARG;
-    if (key_bytes == 8 && value_bytes != 0) return OSB200_ERR_UNSUPPORTED;
     if (max_n == 0 || max_n > (1ull << 34)) return OSB200_ERR_INVALID_ARG;
 
     int dev = 0;
@@ -398,6 +401,26 @@ int osb200_create(osb200_handle* out, uint64_t max_n, int key_bytes, int value_b
     s->cfg.rank_mode = s->atomic_order_ok ? osb::kRankAtomic : osb::kRankBallot;
     *out = s;
     return OSB200_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int osb200_create(osb200_handle* out, uint64_t max_n, int key_bytes, int value_bytes)
+{
+    if (!out) return OSB200_ERR_INVALID_ARG;
+    *out = nullptr;
+    if ((key_bytes != 4 && key_bytes != 8) || (value_bytes != 0 && value_bytes != 4)) return OSB200_ERR_INVALID_ARG;
+    if (key_bytes == 8 && value_bytes != 0) return OSB200_ERR_UNSUPPORTED;  // osb200_create_pairs64 makes that shape
+    return create_impl(out, max_n, key_bytes, value_bytes);
+}
+
+int osb200_create_pairs64(osb200_handle* out, uint64_t max_n)
+{
+    if (!out) return OSB200_ERR_INVALID_ARG;
+    *out = nullptr;
+    return create_impl(out, max_n, 8, 4);
 }
 
 int osb200_destroy(osb200_handle h)
@@ -486,10 +509,11 @@ int osb200_sort_bits(osb200_handle h, void* d_keys, uint32_t* d_values, uint64_t
     return sort_impl(h, h->key_bytes, d_keys, d_values, n, static_cast<cudaStream_t>(stream), nullptr, begin_bit, end_bit);
 }
 
+// Pairs and argsort take a (4, 4) handle with 32-bit key types or a (8, 4) handle (osb200_create_pairs64) with 64-bit ones.
 int osb200_sort_pairs_typed(osb200_handle h, void* d_keys, uint32_t* d_values, uint64_t n, int key_type, int descending,
                             void* stream)
 {
-    if (check_handle(h) != OSB200_OK || h->key_bytes != 4 || h->value_bytes != 4) return OSB200_ERR_INVALID_ARG;
+    if (check_handle(h) != OSB200_OK || h->value_bytes != 4) return OSB200_ERR_INVALID_ARG;
     if (n > 1 && !d_values) return OSB200_ERR_INVALID_ARG;
     osb::KeyCodec c;
     int st = make_codec(h->key_bytes, key_type, descending, &c);
@@ -502,9 +526,9 @@ int osb200_sort_pairs_typed(osb200_handle h, void* d_keys, uint32_t* d_values, u
 int osb200_argsort(osb200_handle h, const void* d_keys_in, void* d_keys_out, uint32_t* d_indices, uint64_t n, int key_type,
                    int descending, void* stream)
 {
-    if (check_handle(h) != OSB200_OK || h->key_bytes != 4 || h->value_bytes != 4) return OSB200_ERR_INVALID_ARG;
+    if (check_handle(h) != OSB200_OK || h->value_bytes != 4) return OSB200_ERR_INVALID_ARG;
     osb::KeyCodec c;
-    int st = make_codec(h->key_bytes, key_type, descending, &c);  // 64-bit key types: INVALID_ARG on this 4-byte handle
+    int st = make_codec(h->key_bytes, key_type, descending, &c);  // a key type of the other width: INVALID_ARG
     if (st != OSB200_OK) return st;
     if (h->cfg.variant != osb::kVariantWide) return OSB200_ERR_UNSUPPORTED;  // the indices mode lives in the device plan
     if (n == 0) return OSB200_OK;
@@ -513,12 +537,13 @@ int osb200_argsort(osb200_handle h, const void* d_keys_in, void* d_keys_out, uin
     if (!in || !out || !idx || ((in | out | idx) & 15u)) return OSB200_ERR_INVALID_ARG;
     if (n > h->max_n || n > (1ull << 32)) return OSB200_ERR_SIZE;  // the indices are 32-bit
     // the input is read until the last pass; outputs that overlap it (or each other) would overwrite keys still to be read
-    const uint64_t bytes = n * sizeof(uint32_t);
-    auto overlap = [bytes](uintptr_t a, uintptr_t b) { return a < b + bytes && b < a + bytes; };
-    if (overlap(in, out) || overlap(in, idx) || overlap(out, idx)) return OSB200_ERR_INVALID_ARG;
+    // (the key arrays are key_bytes * n bytes, the index array 4n)
+    const uint64_t kb = n * static_cast<uint64_t>(h->key_bytes), ib = n * sizeof(uint32_t);
+    auto overlap = [](uintptr_t a, uint64_t alen, uintptr_t b, uint64_t blen) { return a < b + blen && b < a + alen; };
+    if (overlap(in, kb, out, kb) || overlap(in, kb, idx, ib) || overlap(out, kb, idx, ib)) return OSB200_ERR_INVALID_ARG;
     cudaStream_t q = static_cast<cudaStream_t>(stream);
     if (n == 1) {  // already sorted, but the outputs still have to be written
-        OSB_TRY(cudaMemcpyAsync(d_keys_out, d_keys_in, sizeof(uint32_t), cudaMemcpyDeviceToDevice, q));
+        OSB_TRY(cudaMemcpyAsync(d_keys_out, d_keys_in, h->key_bytes, cudaMemcpyDeviceToDevice, q));
         OSB_TRY(cudaMemsetAsync(d_indices, 0, sizeof(uint32_t), q));
         return OSB200_OK;
     }

@@ -371,20 +371,23 @@ cudaError_t launch_copy_back(const SortPlan* plan, const void* alt_keys, void* k
 
 // argsort: keys and indices in one launch.  Odd executed passes: both from the alt buffers.  No executed pass (all keys
 // equal): the input is its own stable sort -- keys from the untouched input, indices 0..n-1.  (All pointers 16-byte aligned.)
-// Four keys per step: one uint4 of 32-bit keys, one uint2 of 16-bit keys.
+// Four keys per step: one uint4 of 32-bit keys, one uint2 of 16-bit keys, two uint4 of 64-bit keys.
 template <typename KeyT>
 __global__ void __launch_bounds__(512)
 argsort_copy_back_kernel(const SortPlan* __restrict__ plan, const KeyT* __restrict__ keys_in, const KeyT* __restrict__ alt_keys,
                          KeyT* __restrict__ keys, const uint32_t* __restrict__ alt_idx, uint32_t* __restrict__ idx, uint64_t n)
 {
-    using KV = typename std::conditional<sizeof(KeyT) == 4, uint4, uint2>::type;
-    static_assert(sizeof(KV) == 4 * sizeof(KeyT), "four keys per vector");
+    using KV = typename std::conditional<sizeof(KeyT) == 2, uint2, uint4>::type;
+    constexpr int KV_PER_STEP = 4 * sizeof(KeyT) / sizeof(KV);
+    static_assert(KV_PER_STEP * sizeof(KV) == 4 * sizeof(KeyT), "four keys per step");
     const uint32_t ex = plan->executed;
     if (ex != 0 && !(ex & 1u)) return;
     const KeyT* src = ex ? alt_keys : keys_in;
     const uint64_t vecs = n / 4, stride = static_cast<uint64_t>(gridDim.x) * blockDim.x;
     for (uint64_t i = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < vecs; i += stride) {
-        __stcs(reinterpret_cast<KV*>(keys) + i, __ldcs(reinterpret_cast<const KV*>(src) + i));
+#pragma unroll
+        for (int v = 0; v < KV_PER_STEP; ++v)
+            __stcs(reinterpret_cast<KV*>(keys) + i * KV_PER_STEP + v, __ldcs(reinterpret_cast<const KV*>(src) + i * KV_PER_STEP + v));
         const uint32_t b = static_cast<uint32_t>(i * 4);
         __stcs(reinterpret_cast<uint4*>(idx) + i, ex ? __ldcs(reinterpret_cast<const uint4*>(alt_idx) + i) : make_uint4(b, b + 1, b + 2, b + 3));
     }
@@ -410,6 +413,10 @@ cudaError_t launch_argsort_copy_back(const SortPlan* plan, const void* keys_in, 
         argsort_copy_back_kernel<uint16_t><<<grid, 512, 0, stream>>>(plan, static_cast<const uint16_t*>(keys_in),
                                                                      static_cast<const uint16_t*>(alt_keys),
                                                                      static_cast<uint16_t*>(keys), alt_idx, idx, n);
+    else if (key_bytes == 8)
+        argsort_copy_back_kernel<uint64_t><<<grid, 512, 0, stream>>>(plan, static_cast<const uint64_t*>(keys_in),
+                                                                     static_cast<const uint64_t*>(alt_keys),
+                                                                     static_cast<uint64_t*>(keys), alt_idx, idx, n);
     else
         return cudaErrorInvalidValue;
     return cudaGetLastError();
@@ -890,6 +897,7 @@ struct WideSmem {
     static constexpr int THREADS = WARPS * 32;
     static constexpr int T = THREADS * K;
     // 16-bit pairs: `sorted` itself holds the tile's T {key, payload} uint2 words (8 B per slot; see the kernel)
+    // (64-bit pairs: the keys in `sorted`, the payloads in `sorted_val` -- no {key, payload} word)
     static constexpr bool KV_IN_SORTED = PAIRS && sizeof(KeyT) == 2;
     alignas(16) KeyT sorted[KV_IN_SORTED ? T * 8 / sizeof(KeyT) : T];  // digit-sorted tile
     alignas(16) uint32_t sorted_val[PAIRS && !KV_IN_SORTED ? T : 4];   // payloads in the same order
@@ -914,7 +922,7 @@ digit_binning_wide_kernel(KeyT* buf0, KeyT* buf1, uint32_t* val0, uint32_t* val1
                           const unsigned long long* __restrict__ gbase, uint16_t* agg16, uint64_t* incl64,
                           uint32_t* ticket, PassParams pp, KeyCodec codec)
 {
-    static_assert(!INDICES || (PAIRS && sizeof(KeyT) <= 4), "the indices are the 32-bit payloads of a pairs pass");
+    static_assert(!INDICES || PAIRS, "the indices are the 32-bit payloads of a pairs pass");
     using S = WideSmem<KeyT, PAIRS, K, WARPS>;
     constexpr int THREADS = S::THREADS;
     constexpr int T = S::T;
@@ -925,9 +933,23 @@ digit_binning_wide_kernel(KeyT* buf0, KeyT* buf1, uint32_t* val0, uint32_t* val1
     // are adjacent and together hold T such words) -- one transposing STS.64 and one LDS.64 per pair instead of two of each,
     // and the payload's destination is the key's plus a constant (reference: OneSweep.cu:522-599 moves them separately)
     // (16-bit keys: the word is {key zero-extended, payload}, and `sorted` is sized for T of them)
+    // (64-bit keys: a 12-byte slot has no such word; keys and payloads are staged in their own arrays, and every payload is
+    // stored through its digit's own pointer, as for 16-bit keys)
+    constexpr bool KV_WORD = PAIRS && sizeof(KeyT) <= 4;
     static_assert(!PAIRS || (sizeof(KeyT) == 4 && offsetof(S, sorted_val) == offsetof(S, sorted) + sizeof(KeyT) * T) ||
-                  (S::KV_IN_SORTED && sizeof(S::sorted) == sizeof(uint2) * T), "kv layout");
+                  (S::KV_IN_SORTED && sizeof(S::sorted) == sizeof(uint2) * T) ||
+                  (sizeof(KeyT) == 8 && sizeof(S::sorted) == sizeof(KeyT) * T && sizeof(S::sorted_val) == sizeof(uint32_t) * T),
+                  "kv layout");
     uint2* const kv = reinterpret_cast<uint2*>(sm.sorted);
+    // a tile slot's key and payload: stored by the rank phase, read by the scatter
+    auto put_slot = [&](uint32_t slot, KeyT k, uint32_t v) {
+        if constexpr (KV_WORD) kv[slot] = make_uint2(static_cast<uint32_t>(k), v);
+        else { sm.sorted[slot] = k; sm.sorted_val[slot] = v; }
+    };
+    auto get_slot = [&](uint32_t x, KeyT& k, uint32_t& v) {
+        if constexpr (KV_WORD) { const uint2 e = kv[x]; k = static_cast<KeyT>(e.x); v = e.y; }
+        else { k = sm.sorted[x]; v = sm.sorted_val[x]; }
+    };
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const uint32_t lt = lanemask_lt();
@@ -1126,14 +1148,14 @@ digit_binning_wide_kernel(KeyT* buf0, KeyT* buf1, uint32_t* val0, uint32_t* val1
             uint32_t slot = hot_run + __popc(b & lt);
             if (!is_hot) slot = warp_rank_and_count<RANK_MODE>(wh, d, lt);
             hot_run += __popc(b);
-            if constexpr (PAIRS) kv[slot] = make_uint2(static_cast<uint32_t>(key[i]), val[i]);
+            if constexpr (PAIRS) put_slot(slot, key[i], val[i]);
             else sm.sorted[slot] = key[i];
         }
     } else {
 #pragma unroll
         for (int i = 0; i < K; ++i) {
             const uint32_t slot = warp_rank_and_count<RANK_MODE>(wh, digit_of(key[i], rshift, rmask), lt);
-            if constexpr (PAIRS) kv[slot] = make_uint2(static_cast<uint32_t>(key[i]), val[i]);
+            if constexpr (PAIRS) put_slot(slot, key[i], val[i]);
             else sm.sorted[slot] = key[i];
         }
     }
@@ -1166,7 +1188,7 @@ digit_binning_wide_kernel(KeyT* buf0, KeyT* buf1, uint32_t* val0, uint32_t* val1
     const bool dec = (sm.plan_bits >> 1) & kCodecDecodeOnStore;
     const KeyT ca = static_cast<KeyT>(codec.a), cb = static_cast<KeyT>(codec.b), cd = static_cast<KeyT>(codec.d);
     // pairs: a payload goes where its key goes, in the other output array (same element size: a constant byte distance;
-    // 16-bit keys: the payload's own digit pointer)
+    // 16- and 64-bit keys: the payload's own digit pointer)
     long long val_delta = 0;
     if constexpr (PAIRS && sizeof(KeyT) == 4) {
         const bool swap = sm.plan_bits & 1u;
@@ -1177,7 +1199,7 @@ digit_binning_wide_kernel(KeyT* buf0, KeyT* buf1, uint32_t* val0, uint32_t* val1
         else return reinterpret_cast<uint32_t*>(sm.valptr[d]) + x;
     };
     (void)val_dst;
-    auto slot_key = [&](uint32_t x) -> KeyT { if constexpr (PAIRS) return static_cast<KeyT>(kv[x].x); else return sm.sorted[x]; };
+    auto slot_key = [&](uint32_t x) -> KeyT { if constexpr (KV_WORD) return static_cast<KeyT>(kv[x].x); else return sm.sorted[x]; };
     (void)slot_key;
     if (pp.dbits <= 5) {
         const uint32_t nbins = 1u << pp.dbits;
@@ -1193,12 +1215,13 @@ digit_binning_wide_kernel(KeyT* buf0, KeyT* buf1, uint32_t* val0, uint32_t* val1
                 if (p >= ga) {
                     const uint32_t x = lo + p - ga;
                     if constexpr (PAIRS) {
-                        const uint2 e = kv[x];
-                        KeyT k = static_cast<KeyT>(e.x);
+                        KeyT k;
+                        uint32_t v;
+                        get_slot(x, k, v);
                         if (dec) k = codec_decode<KeyT>(k, ca, cb, cd);
                         KeyT* dst = reinterpret_cast<KeyT*>(kp) + x;
                         st_scatter(dst, k);
-                        st_scatter(val_dst(dst, b, x), e.y);
+                        st_scatter(val_dst(dst, b, x), v);
                     } else {
                         KeyT k = sm.sorted[x];
                         if (dec) k = codec_decode<KeyT>(k, ca, cb, cd);
@@ -1212,11 +1235,13 @@ digit_binning_wide_kernel(KeyT* buf0, KeyT* buf1, uint32_t* val0, uint32_t* val1
         for (int j = 0; j < K; ++j) {
             const uint32_t idx = j * THREADS + tid;
             if constexpr (PAIRS) {
-                const uint2 e = kv[idx];
-                const uint32_t d = digit_of(static_cast<KeyT>(e.x), shift, dmask);
+                KeyT k;
+                uint32_t v;
+                get_slot(idx, k, v);
+                const uint32_t d = digit_of(k, shift, dmask);
                 KeyT* dst = reinterpret_cast<KeyT*>(sm.keyptr[d]) + idx;
-                st_scatter(dst, static_cast<KeyT>(e.x));
-                st_scatter(val_dst(dst, d, idx), e.y);
+                st_scatter(dst, k);
+                st_scatter(val_dst(dst, d, idx), v);
             } else {
                 const KeyT k = sm.sorted[idx];
                 const uint32_t d = digit_of(k, shift, dmask);
@@ -1229,12 +1254,13 @@ digit_binning_wide_kernel(KeyT* buf0, KeyT* buf1, uint32_t* val0, uint32_t* val1
             const uint32_t idx = j * THREADS + tid;
             if (idx < valid) {
                 if constexpr (PAIRS) {
-                    const uint2 e = kv[idx];
-                    const KeyT k = static_cast<KeyT>(e.x);
+                    KeyT k;
+                    uint32_t v;
+                    get_slot(idx, k, v);
                     const uint32_t d = digit_of(k, shift, dmask);
                     KeyT* dst = reinterpret_cast<KeyT*>(sm.keyptr[d]) + idx;
                     st_scatter(dst, dec ? codec_decode<KeyT>(k, ca, cb, cd) : k);
-                    st_scatter(val_dst(dst, d, idx), e.y);
+                    st_scatter(val_dst(dst, d, idx), v);
                 } else {
                     const KeyT k = sm.sorted[idx];
                     const uint32_t d = digit_of(k, shift, dmask);
@@ -1690,6 +1716,19 @@ template <> struct WideGeom<uint64_t, false> { static constexpr int K = OSB_U64_
 #endif
 template <> struct WideGeom<uint16_t, false> { static constexpr int K = OSB_K16_K, WARPS = OSB_K16_WARPS, MINB = 2, LOOK = OSB_LOOK; };
 template <> struct WideGeom<uint16_t, true>  { static constexpr int K = OSB_P16_K, WARPS = OSB_P16_WARPS, MINB = 2, LOOK = OSB_PAIRS_LOOK; };
+// 64-bit keys with 32-bit payloads (osb200_create_pairs64: osb200_sort_pairs_typed, osb200_argsort).  A pair takes three
+// registers, so the u32 pairs shape (16 pairs per thread at 64 registers) does not fit.  16 pairs per thread with ONE CTA
+// per SM (8,192-pair tiles, 116 KiB of shared memory, up to 128 registers: no spills) beat 8 and 12 pairs per thread at two
+// CTAs per SM by 23 % and 15 % on the H100 (2^30 keys, argsort: 91 against 118 and 107 ms).  DESIGN §4.11.
+#ifndef OSB_P64_K  // geometry of the 64-bit pairs / argsort kernel, overridable for sweeps
+#define OSB_P64_K 16
+#define OSB_P64_WARPS 16
+#define OSB_P64_MINB 1
+#endif
+#ifndef OSB_P64_LOOK
+#define OSB_P64_LOOK 32
+#endif
+template <> struct WideGeom<uint64_t, true>  { static constexpr int K = OSB_P64_K, WARPS = OSB_P64_WARPS, MINB = OSB_P64_MINB, LOOK = OSB_P64_LOOK; };
 template <typename KeyT, bool PAIRS> constexpr uint32_t wide_tile() { return WideGeom<KeyT, PAIRS>::K * WideGeom<KeyT, PAIRS>::WARPS * 32; }
 
 template <typename KeyT, bool PAIRS, int RANK_MODE, bool INDICES = false>
@@ -1827,6 +1866,11 @@ static_assert(wide_tile<uint16_t, false>() >= kSmallestTileU32Keys && wide_tile<
 static_assert(wide_tile<uint16_t, true>() >= kSmallestTileU32Pairs,
               "16-bit pairs (a (4, 4) handle): a smaller tile would need more descriptors than the handle has");
 static_assert(wide_tile<uint16_t, false>() < 32768 && wide_tile<uint16_t, true>() < 32768, "agg16 holds 15-bit counts");
+// A (8, 4) handle sizes its descriptors and reductions for smallest_tile(8, true): the variant-0 u64 tile (osb200_workspace_bytes
+// relies on it as well).
+static_assert(wide_tile<uint64_t, true>() >= TileGeom<uint64_t, false>::WARPS * 32 * TileGeom<uint64_t, false>::K,
+              "64-bit pairs: a smaller tile would need more descriptors than the handle has");
+static_assert(wide_tile<uint64_t, true>() < 32768, "agg16 holds 15-bit counts");
 
 uint32_t binning_tile_keys(int key_bytes, bool pairs, const BinningConfig& cfg)
 {
@@ -1834,7 +1878,7 @@ uint32_t binning_tile_keys(int key_bytes, bool pairs, const BinningConfig& cfg)
     if (cfg.variant == kVariantPersistent && !pairs)
         return key_bytes == 8 ? RingGeom<uint64_t>::K * RingGeom<uint64_t>::WARPS * 32 : RingGeom<uint32_t>::K * RingGeom<uint32_t>::WARPS * 32;
     if (cfg.variant == kVariantWide) {
-        if (key_bytes == 8) return WideGeom<uint64_t, false>::K * WideGeom<uint64_t, false>::WARPS * 32;
+        if (key_bytes == 8) return pairs ? wide_tile<uint64_t, true>() : wide_tile<uint64_t, false>();
         return pairs ? (OSB_PAIRS16K ? kPairsK * kPairsWarps * 32 : WideGeom<uint32_t, true>::K * WideGeom<uint32_t, true>::WARPS * 32)
                      : WideGeom<uint32_t, false>::K * WideGeom<uint32_t, false>::WARPS * 32;
     }
@@ -1896,6 +1940,11 @@ cudaError_t configure_kernels()
     if ((e = set_wide_attr<uint16_t, true, kRankBallot>()) != cudaSuccess) return e;
     if ((e = set_wide_attr<uint16_t, true, kRankAtomic, true>()) != cudaSuccess) return e;
     if ((e = set_wide_attr<uint16_t, true, kRankBallot, true>()) != cudaSuccess) return e;
+    // 64-bit keys with payloads: pairs, argsort
+    if ((e = set_wide_attr<uint64_t, true, kRankAtomic>()) != cudaSuccess) return e;
+    if ((e = set_wide_attr<uint64_t, true, kRankBallot>()) != cudaSuccess) return e;
+    if ((e = set_wide_attr<uint64_t, true, kRankAtomic, true>()) != cudaSuccess) return e;
+    if ((e = set_wide_attr<uint64_t, true, kRankBallot, true>()) != cudaSuccess) return e;
     if ((e = set_pairs_attr<kRankAtomic>()) != cudaSuccess) return e;
     if ((e = set_pairs_attr<kRankBallot>()) != cudaSuccess) return e;
     return configure_segment_kernels();
@@ -1921,12 +1970,18 @@ cudaError_t launch_digit_binning(const void* in, void* out, const uint32_t* in_v
             : launch_wide_variant<KEYT, PAIRS, kRankAtomic>(in, out, in_val, out_val, n, shift, gbase_place, agg16, desc, \
                                                            ticket, epoch, cfg, stream))
         if (cfg.argsort_in != nullptr) {  // argsort: the first executed pass reads argsort_in and makes the indices
-            if ((key_bytes != 4 && key_bytes != 2) || !pairs || cfg.plan == nullptr) return cudaErrorInvalidValue;
+            if (!pairs || cfg.plan == nullptr) return cudaErrorInvalidValue;
             if (key_bytes == 2)
                 return ballot ? launch_wide_variant<uint16_t, true, kRankBallot, true>(in, out, in_val, out_val, n, shift, gbase_place,
                                                                                       agg16, desc, ticket, epoch, cfg, stream)
                               : launch_wide_variant<uint16_t, true, kRankAtomic, true>(in, out, in_val, out_val, n, shift, gbase_place,
                                                                                       agg16, desc, ticket, epoch, cfg, stream);
+            if (key_bytes == 8)
+                return ballot ? launch_wide_variant<uint64_t, true, kRankBallot, true>(in, out, in_val, out_val, n, shift, gbase_place,
+                                                                                      agg16, desc, ticket, epoch, cfg, stream)
+                              : launch_wide_variant<uint64_t, true, kRankAtomic, true>(in, out, in_val, out_val, n, shift, gbase_place,
+                                                                                      agg16, desc, ticket, epoch, cfg, stream);
+            if (key_bytes != 4) return cudaErrorInvalidValue;
             return ballot ? launch_wide_variant<uint32_t, true, kRankBallot, true>(in, out, in_val, out_val, n, shift, gbase_place, agg16,
                                                                                   desc, ticket, epoch, cfg, stream)
                           : launch_wide_variant<uint32_t, true, kRankAtomic, true>(in, out, in_val, out_val, n, shift, gbase_place, agg16,
@@ -1937,7 +1992,7 @@ cudaError_t launch_digit_binning(const void* in, void* out, const uint32_t* in_v
             return ballot ? launch_pairs_variant<kRankBallot>(in, out, in_val, out_val, n, shift, gbase_place, agg16, desc, ticket, epoch, cfg, stream)
                           : launch_pairs_variant<kRankAtomic>(in, out, in_val, out_val, n, shift, gbase_place, agg16, desc, ticket, epoch, cfg, stream);
         if (key_bytes == 4) return pairs ? OSB_WIDE(uint32_t, true) : OSB_WIDE(uint32_t, false);
-        if (key_bytes == 8 && !pairs) return OSB_WIDE(uint64_t, false);
+        if (key_bytes == 8) return pairs ? OSB_WIDE(uint64_t, true) : OSB_WIDE(uint64_t, false);
 #undef OSB_WIDE
         return cudaErrorInvalidValue;
     }
@@ -2138,6 +2193,11 @@ static cudaError_t configure_segment_kernels()
     if ((e = seg_attr<uint16_t, true, 2, kRankBallot>()) != cudaSuccess) return e;
     if ((e = seg_attr<uint16_t, true, 2, kRankAtomic, true>()) != cudaSuccess) return e;
     if ((e = seg_attr<uint16_t, true, 2, kRankBallot, true>()) != cudaSuccess) return e;
+    // 64-bit keys with payloads: the single segment of a sort of at most one tile -- pairs, argsort
+    if ((e = seg_attr<uint64_t, true, 2, kRankAtomic>()) != cudaSuccess) return e;
+    if ((e = seg_attr<uint64_t, true, 2, kRankBallot>()) != cudaSuccess) return e;
+    if ((e = seg_attr<uint64_t, true, 2, kRankAtomic, true>()) != cudaSuccess) return e;
+    if ((e = seg_attr<uint64_t, true, 2, kRankBallot, true>()) != cudaSuccess) return e;
     // row sort (launch_row_sort): geometries 1 and 2 of every key width, keys only and with indices
 #define OSB_ROW_ATTR_SIZE(KEYT, SIZE)                                                                      \
     if ((e = seg_attr<KEYT, false, SIZE, kRankAtomic, false, true>()) != cudaSuccess) return e;            \
@@ -2179,11 +2239,15 @@ cudaError_t launch_segment_sort(void* keys, uint32_t* vals, int key_bytes, const
     if (num_segments == 0) return cudaSuccess;
     const KeyCodec codec = codec_in ? *codec_in : KeyCodec();
     if (keys_in != nullptr) {  // argsort: one segment of up to a tile, in the largest geometry (the only one instantiated for it)
-        if ((key_bytes != 4 && key_bytes != 2) || !vals || seg_off || num_segments != 1 || max_len > segment_sort_capacity(key_bytes, false))
+        if (!vals || seg_off || num_segments != 1 || max_len > segment_sort_capacity(key_bytes, false))
             return cudaErrorInvalidValue;
         if (key_bytes == 2)
             return launch_seg<uint16_t, true, 2, true>(keys, vals, nullptr, 1, single_n, max_len, begin_bit, places, last_bits, codec,
                                                        rank_mode, sm_count, stream, keys_in);
+        if (key_bytes == 8)
+            return launch_seg<uint64_t, true, 2, true>(keys, vals, nullptr, 1, single_n, max_len, begin_bit, places, last_bits, codec,
+                                                       rank_mode, sm_count, stream, keys_in);
+        if (key_bytes != 4) return cudaErrorInvalidValue;
         return launch_seg<uint32_t, true, 2, true>(keys, vals, nullptr, 1, single_n, max_len, begin_bit, places, last_bits, codec,
                                                    rank_mode, sm_count, stream, keys_in);
     }
@@ -2193,6 +2257,11 @@ cudaError_t launch_segment_sort(void* keys, uint32_t* vals, int key_bytes, const
                                                     rank_mode, sm_count, stream)
                     : launch_seg<uint16_t, false, 2>(keys, vals, nullptr, 1, single_n, max_len, begin_bit, places, last_bits, codec,
                                                      rank_mode, sm_count, stream);
+    }
+    if (key_bytes == 8 && vals) {  // 64-bit pairs: the single segment of a small sort, in the 8,192-key geometry
+        if (seg_off || num_segments != 1 || max_len > seg_cap<uint64_t, 2>()) return cudaErrorInvalidValue;
+        return launch_seg<uint64_t, true, 2>(keys, vals, nullptr, 1, single_n, max_len, begin_bit, places, last_bits, codec,
+                                             rank_mode, sm_count, stream);
     }
     const int size = max_len <= (key_bytes == 8 ? seg_cap<uint64_t, 0>() : seg_cap<uint32_t, 0>()) ? 0
                      : max_len <= segment_sort_capacity(key_bytes, true) ? 1 : 2;

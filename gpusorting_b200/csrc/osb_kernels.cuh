@@ -32,7 +32,7 @@ struct BinningConfig {
     uint32_t debug_stall_every = 0;   // test hook: tiles with tile % N == N-1 never publish their reduction (0 = off)
     uint32_t debug_max_ctas = 0;      // test hook: at most this many persistent CTAs per pass (0 = as many as can be resident)
     bool hot_passes = false;          // also enqueue the HOT instantiation (the plan decides which of the two runs the pass)
-    const void* argsort_in = nullptr; // argsort (u32/u16 pairs, needs the plan): the first executed pass reads its keys from here
+    const void* argsort_in = nullptr; // argsort (u32/u16/u64 pairs, needs the plan): the first executed pass reads its keys from here
                                       // and makes every payload from the key's input position (in/in_val: output keys/indices)
 };
 
@@ -66,7 +66,7 @@ cudaError_t launch_global_histogram_bits(const void* keys, uint64_t n, int key_b
 // If the plan says an odd number of passes ran, the sorted data sits in the alt buffers: move it to the caller's.
 cudaError_t launch_copy_back(const SortPlan* plan, const void* alt_keys, void* keys, const uint32_t* alt_vals, uint32_t* vals,
                              uint64_t n, int key_bytes, int sm_count, cudaStream_t stream);
-// The same for an argsort (32- or 16-bit keys, u32 indices): an odd number of executed passes -> move keys and indices from
+// The same for an argsort (16-, 32- or 64-bit keys, u32 indices): an odd number of executed passes -> move keys and indices from
 // the alt buffers; none (every digit place constant) -> the keys are copied from the untouched input and the indices are 0..n-1.
 cudaError_t launch_argsort_copy_back(const SortPlan* plan, const void* keys_in, const void* alt_keys, void* keys,
                                      const uint32_t* alt_idx, uint32_t* idx, uint64_t n, int key_bytes, int sm_count,
@@ -85,9 +85,10 @@ cudaError_t launch_digit_binning(const void* in, void* out, const uint32_t* in_v
 // Segment sort / small-n path: one CTA sorts one segment (<= segment_sort_capacity keys) in shared memory, all digit passes
 // in one launch.  seg_off == nullptr: the single segment [0, single_n).  max_len (an upper bound of the segment lengths)
 // picks the geometry; segments longer than the capacity are skipped by the kernel (the caller must not pass them).
-// keys_in != null (argsort of the single segment; u32 or u16 keys, vals = indices): the keys are read from keys_in, the payloads
-// are the keys' input positions, and the sorted keys and indices are stored to keys / vals.
-// key_bytes 2 (16-bit keys): only the single segment of a sort (seg_off null), up to 16,384 keys.
+// keys_in != null (argsort of the single segment; u16, u32 or u64 keys, vals = indices): the keys are read from keys_in, the
+// payloads are the keys' input positions, and the sorted keys and indices are stored to keys / vals.
+// key_bytes 2 (16-bit keys), and key_bytes 8 with vals: only the single segment of a sort (seg_off null), up to 16,384 keys
+// (8,192 for 64-bit keys).
 uint32_t segment_sort_capacity(int key_bytes, bool small);
 cudaError_t launch_segment_sort(void* keys, uint32_t* vals, int key_bytes, const unsigned long long* seg_off, uint64_t num_segments,
                                 uint64_t single_n, uint32_t max_len, uint32_t begin_bit, uint32_t places, uint32_t last_bits,

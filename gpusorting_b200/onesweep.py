@@ -58,6 +58,7 @@ class OneSweepSorter:
 
     Keys are ordered by their UNSIGNED bit pattern, as in the reference CUDA path (uint32 keys,
     OneSweep.cuh:24-52); int32/int64 tensors are accepted as raw 32/64-bit containers.
+    (8, 4) -- 64-bit keys with 32-bit payloads -- is created by osb200_create_pairs64.
     """
 
     def __init__(self, max_n: int, key_bytes: int = 4, value_bytes: int = 0, device: Optional[int] = None):
@@ -67,7 +68,10 @@ class OneSweepSorter:
         self.max_n, self.key_bytes, self.value_bytes = int(max_n), int(key_bytes), int(value_bytes)
         h = ctypes.c_void_p()
         with torch.cuda.device(self.device):
-            check(lib.osb200_create(ctypes.byref(h), self.max_n, self.key_bytes, self.value_bytes), "osb200_create")
+            if (self.key_bytes, self.value_bytes) == (8, 4):
+                check(lib.osb200_create_pairs64(ctypes.byref(h), self.max_n), "osb200_create_pairs64")
+            else:
+                check(lib.osb200_create(ctypes.byref(h), self.max_n, self.key_bytes, self.value_bytes), "osb200_create")
         self._h = h
 
     # -- lifetime ---------------------------------------------------------------------------------
@@ -138,9 +142,10 @@ class OneSweepSorter:
     def sort_pairs_typed(self, keys: torch.Tensor, values: torch.Tensor, key_type: str, descending: bool = False,
                          n: Optional[int] = None, stream=None):
         """sort_keys_typed with 32-bit payloads that move with their keys (stable).  Keys must start on a 16-byte boundary
-        (OneSweepError status -1 otherwise); values need only their natural 4-byte alignment, so any contiguous view will do."""
+        (OneSweepError status -1 otherwise); values need only their natural 4-byte alignment, so any contiguous view will do.
+        Keys are 32-bit on a (4, 4) sorter and int64 / uint64 / float64 on a (8, 4) sorter."""
         n = keys.numel() if n is None else int(n)
-        _check_dev_tensor(keys, _TYPED_DTYPES_4, "keys", n, self.device)
+        _check_dev_tensor(keys, self._typed(), "keys", n, self.device)
         _check_dev_tensor(values, _TYPED_DTYPES_4, "values", n, self.device)
         with torch.cuda.device(self.device):
             check(lib.osb200_sort_pairs_typed(self._h, keys.data_ptr(), values.data_ptr(), n, KEY_TYPES[key_type],
@@ -153,10 +158,11 @@ class OneSweepSorter:
         Returns (sorted_keys, indices): new tensors of n elements on the keys' device, allocated with torch.empty (so the call
         can be captured in a CUDA graph).  sorted_keys has the dtype of `keys`; indices[i] is the input position of
         sorted_keys[i], stored as torch.int32, the container of the library's 32-bit payloads.  Positions >= 2^31 (n > 2^31)
-        read as negative in it: ``indices.long() & 0xFFFFFFFF`` recovers them.  key_type is "u32", "i32" or "f32"; equal keys
-        keep their input order in both directions.  Needs a (4, 4) sorter."""
+        read as negative in it: ``indices.long() & 0xFFFFFFFF`` recovers them.  key_type is "u32", "i32" or "f32" on a (4, 4)
+        sorter, "u64", "i64" or "f64" (int64 / uint64 / float64 keys) on a (8, 4) sorter; equal keys keep their input order in
+        both directions."""
         n = keys.numel() if n is None else int(n)
-        _check_dev_tensor(keys, _TYPED_DTYPES_4, "keys", n, self.device)
+        _check_dev_tensor(keys, self._typed(), "keys", n, self.device)
         with torch.cuda.stream(stream):  # (None: the current stream) the outputs belong to the stream that writes them
             out = torch.empty(n, dtype=keys.dtype, device=keys.device)
             idx = torch.empty(n, dtype=torch.int32, device=keys.device)
@@ -269,10 +275,13 @@ class OneSweepSorter:
 
     def sort_pairs(self, keys: torch.Tensor, values: torch.Tensor, n: Optional[int] = None, stream=None):
         """Stable sort of keys[:n] with 32-bit payloads values[:n], in place.  Keys must start on a 16-byte boundary
-        (OneSweepError status -1 otherwise); values need only their natural 4-byte alignment, so any contiguous view will do."""
+        (OneSweepError status -1 otherwise); values need only their natural 4-byte alignment, so any contiguous view will do.
+        On a (8, 4) sorter the keys are int64 / uint64 containers ordered by their unsigned bits (key type "u64")."""
         n = keys.numel() if n is None else int(n)
-        _check_dev_tensor(keys, _KEY_DTYPES_4, "keys", n, self.device)
+        _check_dev_tensor(keys, self._raw(), "keys", n, self.device)
         _check_dev_tensor(values, _TYPED_DTYPES_4, "values", n, self.device)  # payloads are opaque 32-bit words
+        if self.key_bytes == 8:
+            return self.sort_pairs_typed(keys, values, "u64", False, n, stream)
         with torch.cuda.device(self.device):
             check(lib.osb200_sort_pairs_u32(self._h, keys.data_ptr(), values.data_ptr(), n, _stream_ptr(stream)),
                   "osb200_sort_pairs_u32")
@@ -389,14 +398,14 @@ def Sort(keys: torch.Tensor, values: Optional[torch.Tensor] = None, n: Optional[
 
 
 def argsort(keys: torch.Tensor, key_type: str, descending: bool = False, n: Optional[int] = None, stream=None):
-    """Stable (sorted_keys, indices) of 32-bit keys, input untouched: OneSweepSorter.argsort on the cached (4, 4) sorter of
-    the stream (one handle per stream, as for Sort)."""
+    """Stable (sorted_keys, indices) of 32- or 64-bit keys, input untouched: OneSweepSorter.argsort on the stream's cached
+    (4, 4) sorter, or its (8, 4) sorter for int64 / uint64 / float64 keys (one handle per stream, as for Sort)."""
     n = keys.numel() if n is None else int(n)
     if not (isinstance(keys, torch.Tensor) and keys.is_cuda):
         raise TypeError("keys must be a CUDA tensor")
     with torch.cuda.device(keys.device.index):
         sp = _stream_ptr(stream)
-    s = _cached_sorter(keys.device.index, 4, 4, n, sp)
+    s = _cached_sorter(keys.device.index, 8 if keys.element_size() == 8 else 4, 4, n, sp)
     return s.argsort(keys, key_type, descending, n, stream)
 
 

@@ -19,9 +19,11 @@
 
 class OneSweepSorterB200 {
   public:
+    // (8, 4) -- 64-bit keys with uint32 payloads -- is made by osb200_create_pairs64
     OneSweepSorterB200(uint64_t max_n, int key_bytes, int value_bytes) : max_n_(max_n)
     {
-        check(osb200_create(&h_, max_n, key_bytes, value_bytes), "osb200_create");
+        if (key_bytes == 8 && value_bytes == 4) check(osb200_create_pairs64(&h_, max_n), "osb200_create_pairs64");
+        else check(osb200_create(&h_, max_n, key_bytes, value_bytes), "osb200_create");
     }
     ~OneSweepSorterB200() { if (h_) osb200_destroy(h_); }
     OneSweepSorterB200(const OneSweepSorterB200&) = delete;
@@ -32,6 +34,11 @@ class OneSweepSorterB200 {
     void SortPairs(uint32_t* d_keys, uint32_t* d_values, uint64_t n, void* stream = nullptr)
     {
         check(osb200_sort_pairs_u32(h_, d_keys, d_values, n, stream), "osb200_sort_pairs_u32");
+    }
+    // uint64 keys with uint32 payloads, on a (8, 4) sorter
+    void SortPairs(uint64_t* d_keys, uint32_t* d_values, uint64_t n, void* stream = nullptr)
+    {
+        check(osb200_sort_pairs_typed(h_, d_keys, d_values, n, OSB200_KEY_U64, 0, stream), "osb200_sort_pairs_typed");
     }
     // stable sort on the key bits [begin_bit, end_bit) only; d_values may be null
     void SortBits(void* d_keys, uint32_t* d_values, uint64_t n, int begin_bit, int end_bit, void* stream = nullptr)
@@ -44,7 +51,7 @@ class OneSweepSorterB200 {
         check(osb200_sort_keys_typed(h_, d_keys, n, key_type, descending ? 1 : 0, stream), "osb200_sort_keys_typed");
     }
     // stable sort of d_keys_in (left untouched) into d_keys_out, with d_indices[i] = input position of d_keys_out[i]; 32-bit
-    // key types only, on a (4, 4) sorter; n <= 2^32
+    // key types on a (4, 4) sorter, 64-bit key types on a (8, 4) sorter; n <= 2^32
     void ArgSort(const void* d_keys_in, void* d_keys_out, uint32_t* d_indices, uint64_t n, int key_type, bool descending,
                  void* stream = nullptr)
     {
@@ -123,5 +130,9 @@ inline void Sort(uint64_t* d_keys, uint64_t n, void* stream = nullptr) { detail:
 inline void Sort(uint32_t* d_keys, uint32_t* d_values, uint64_t n, void* stream = nullptr)
 {
     detail::sorter(4, 4, n).SortPairs(d_keys, d_values, n, stream);
+}
+inline void Sort(uint64_t* d_keys, uint32_t* d_values, uint64_t n, void* stream = nullptr)
+{
+    detail::sorter(8, 4, n).SortPairs(d_keys, d_values, n, stream);
 }
 }  // namespace OneSweep

@@ -72,8 +72,17 @@ OSB200_API const char* osb200_status_string(int status);
  *   value_bytes 0 (keys only == keysOnly=true) or 4 (uint32 payload == keysOnly=false)
  *   max_n       largest n a sort call may pass (reference: maxSize), up to 2^34
  * The device is the calling thread's current CUDA device.
+ * key_bytes 8 with value_bytes 4 returns OSB200_ERR_UNSUPPORTED here: that shape comes from osb200_create_pairs64.
  * ---------------------------------------------------------------------------------------------- */
 OSB200_API int osb200_create(osb200_handle* out, uint64_t max_n, int key_bytes, int value_bytes);
+/* A handle for 64-bit keys with uint32 payloads (key_bytes 8, value_bytes 4): osb200_sort_pairs_typed and osb200_argsort with
+ * OSB200_KEY_U64, _I64 or _F64 keys.  Its workspace is alternate keys (8 * max_n bytes) and payloads (4 * max_n), the tile
+ * descriptors and reductions, and the control block; osb200_workspace_bytes(max_n, 8, 4) is what it allocates.  The keys-only
+ * calls (osb200_sort_keys_u64, osb200_sort_keys_typed, osb200_sort_host_keys_u64) work on it as on a (8, 0) handle.
+ * osb200_sort_pairs_u32, the host-buffer pairs call, the segmented sort and osb200_sort_bits with values do not take 64-bit
+ * keys: they return OSB200_ERR_INVALID_ARG on it, as on any 8-byte handle.  Argument errors and OSB200_ERR_NO_DEVICE as for
+ * osb200_create (a null `out`, max_n == 0 or max_n > 2^34: OSB200_ERR_INVALID_ARG). */
+OSB200_API int osb200_create_pairs64(osb200_handle* out, uint64_t max_n);
 OSB200_API int osb200_destroy(osb200_handle h);
 /* Device bytes a handle with these parameters allocates (alt buffers + control state). */
 OSB200_API uint64_t osb200_workspace_bytes(uint64_t max_n, int key_bytes, int value_bytes);
@@ -97,7 +106,9 @@ OSB200_API int osb200_sort_keys_u64(osb200_handle h, uint64_t* d_keys, uint64_t 
  * into the first pass (and the histogram) and undone in the last pass's stores: no extra traffic.  Floats follow the
  * IEEE total order of their bit patterns (-0.0 < +0.0, NaNs at the ends), as the reference's transform does.
  * Descending is the complement of the transformed key, so equal keys KEEP their input order (stable) -- unlike the
- * reference's index reversal, which reverses ties.  key_type must match the handle's key width. */
+ * reference's index reversal, which reverses ties.  key_type must match the handle's key width.
+ * osb200_sort_pairs_typed needs value_bytes == 4: a (4, 4) handle with 32-bit key types, or a (8, 4) handle
+ * (osb200_create_pairs64) with 64-bit ones.  Keys must be 16-byte aligned, values 4-byte aligned. */
 typedef enum osb200_key_type {
     OSB200_KEY_U32 = 0, OSB200_KEY_I32 = 1, OSB200_KEY_F32 = 2, OSB200_KEY_U64 = 3, OSB200_KEY_I64 = 4, OSB200_KEY_F64 = 5
 } osb200_key_type;
@@ -108,16 +119,18 @@ OSB200_API int osb200_sort_pairs_typed(osb200_handle h, void* d_keys, uint32_t* 
 /* Argsort: the stable sort of d_keys_in[0..n) and its permutation, leaving the input as it is (the shape of torch.sort).
  * d_keys_in is read and never written; d_keys_out receives the keys sorted, and d_indices[i] the input position of
  * d_keys_out[i].  Equal keys keep their input order in both directions (the stable descending order of
- * osb200_sort_pairs_typed).  key_type is OSB200_KEY_U32, _I32 or _F32, ordered as in osb200_sort_keys_typed.
- * The handle must have key_bytes == 4 and value_bytes == 4: its alternate buffers are the ping-pong partners of d_keys_out
- * and d_indices, so no other workspace is used.  The indices are made on the device rather than loaded: the histogram and
- * the first executed digit pass read the keys from d_keys_in, and that pass writes each key's own position as its payload
- * (every later pass is the pairs pass; a sort of at most 16,384 keys is one launch of the single-block sort).  Against
- * copying the keys, writing 0..n-1 and calling osb200_sort_pairs_typed this saves the copy, the iota and a payload read.
- * All three pointers must be 16-byte aligned, and none of the three arrays may overlap another.
- * Returns OSB200_ERR_INVALID_ARG for a null, misaligned or overlapping pointer, a handle of another shape or a 64-bit
- * key_type; OSB200_ERR_UNSUPPORTED unless option "variant" is 2 (the default); OSB200_ERR_SIZE when n > max_n or n > 2^32
- * (the indices are uint32).  n == 0 is a no-op; n == 1 writes d_keys_out[0] = d_keys_in[0] and d_indices[0] = 0.
+ * osb200_sort_pairs_typed).  key_type is ordered as in osb200_sort_keys_typed: OSB200_KEY_U32, _I32 or _F32 on a handle
+ * with key_bytes == 4 and value_bytes == 4, OSB200_KEY_U64, _I64 or _F64 on a (8, 4) handle (osb200_create_pairs64).  The
+ * handle's alternate buffers are the ping-pong partners of d_keys_out and d_indices, so no other workspace is used.  The
+ * indices are made on the device rather than loaded: the histogram and the first executed digit pass read the keys from
+ * d_keys_in, and that pass writes each key's own position as its payload (every later pass is the pairs pass; a sort of at
+ * most 16,384 keys, 8,192 64-bit keys, is one launch of the single-block sort).  Against copying the keys, writing 0..n-1
+ * and calling osb200_sort_pairs_typed this saves the copy, the iota and a payload read.
+ * All three pointers must be 16-byte aligned, and none of the three arrays (keys key_bytes * n bytes, indices 4n) may
+ * overlap another.
+ * Returns OSB200_ERR_INVALID_ARG for a null, misaligned or overlapping pointer, a handle without payloads or a key_type of
+ * the other width; OSB200_ERR_UNSUPPORTED unless option "variant" is 2 (the default); OSB200_ERR_SIZE when n > max_n or
+ * n > 2^32 (the indices are uint32).  n == 0 is a no-op; n == 1 writes d_keys_out[0] = d_keys_in[0] and d_indices[0] = 0.
  * Asynchronous and graph-capturable like the other single-GPU calls. */
 OSB200_API int osb200_argsort(osb200_handle h, const void* d_keys_in, void* d_keys_out, uint32_t* d_indices, uint64_t n,
                               int key_type, int descending, void* stream);
