@@ -142,6 +142,8 @@ int is_capturing(cudaStream_t stream, bool* out)
 
 int check_handle(const osb200_sorter* s) { return s ? OSB200_OK : OSB200_ERR_INVALID_ARG; }
 
+bool overlaps(uintptr_t a, uint64_t alen, uintptr_t b, uint64_t blen) { return a < b + blen && b < a + alen; }
+
 // The launch plan (reference: OneSweepDispatcher.cuh:311-363): GlobalHistogram, Scan, one DigitBinningPass per digit
 // place of [begin_bit, end_bit), then the (normally empty) copy-back.  Everything is enqueued on `stream`; which passes
 // actually move data is decided on the device (osb::SortPlan): the host never waits for the histogram.
@@ -171,7 +173,7 @@ int sort_impl(osb200_sorter* s, int key_bytes, void* d_keys, uint32_t* d_vals, u
     const bool use_plan = wide;
 
     // small-n path (SURVEY 8f rank 4): up to one tile of keys is sorted by ONE CTA in shared memory, one launch
-    if (wide && s->small_path && n <= osb::segment_sort_capacity(key_bytes, false)) {
+    if (wide && s->small_path && n <= osb::segment_sort_capacity(key_bytes)) {
         osb::KeyCodec c;
         if (codec) { c = *codec; c.flags = osb::kCodecEncodeOnLoad | osb::kCodecDecodeOnStore; }
         s->ev_count = 0;
@@ -210,7 +212,7 @@ int sort_impl(osb200_sorter* s, int key_bytes, void* d_keys, uint32_t* d_vals, u
                                                   static_cast<uint32_t>(begin_bit), places, last_bits));
     OSB_TRY(mark());
     // hot passes (low-entropy inputs): the default kernel has a second instantiation for them; both are enqueued per pass
-    const bool hot_passes = use_plan && s->hot_passes && !(d_vals && osb::binning_tile_keys(4, true, s->cfg) == 16384);
+    const bool hot_passes = use_plan && s->hot_passes && osb::binning_has_hot_twin(key_bytes, d_vals != nullptr, keys_in != nullptr, s->cfg);
     OSB_TRY(osb::launch_scan(s->ghist(), s->gbase(), places, stream, use_plan ? s->plan() : nullptr, n, s->short_circuit, hot_passes));
     OSB_TRY(mark());
 
@@ -458,8 +460,9 @@ int osb200_sort_keys_u64(osb200_handle h, uint64_t* d_keys, uint64_t n, void* st
     return sort_impl(h, h->key_bytes, d_keys, nullptr, n, static_cast<cudaStream_t>(stream));
 }
 
-// Typed keys (SURVEY 8f rank 1).  key_type must match the key width (the handle's, or the row sort's key_bytes).
-static int make_codec(int key_bytes, int key_type, int descending, osb::KeyCodec* c)
+// Typed keys (SURVEY 8f rank 1).  key_type must match the key width (the handle's, or the row sort's key_bytes).  *codec is
+// c, or null for plain unsigned ascending keys, which the kernels sort as they are.
+static int make_codec(int key_bytes, int key_type, int descending, osb::KeyCodec* c, const osb::KeyCodec** codec)
 {
     const bool wide64 = key_bytes == 8;
     const unsigned long long all = wide64 ? ~0ull : 0xffffffffull, sign = wide64 ? (1ull << 63) : (1ull << 31);
@@ -474,18 +477,78 @@ static int make_codec(int key_bytes, int key_type, int descending, osb::KeyCodec
     }
     c->d = descending ? all : 0;
     c->flags = 0;
+    *codec = c->a == 0 && c->b == 0 && c->d == 0 ? nullptr : c;
     return OSB200_OK;
+}
+
+// 16-bit keys (osb200_key16_type) on a 4-byte handle: the same driver with a key width of 2 -- two digit passes.  F16 and
+// BF16 share the float codec (sign bit 15); they differ only in the dtype the caller keeps them in.
+static int make_codec16(int key_type, int descending, osb::KeyCodec* c, const osb::KeyCodec** codec)
+{
+    switch (key_type) {
+        case OSB200_KEY16_U16: c->a = 0; c->b = 0; break;
+        case OSB200_KEY16_I16: c->a = 0; c->b = 0x8000u; break;
+        case OSB200_KEY16_F16:
+        case OSB200_KEY16_BF16: c->a = 0xFFFFu; c->b = 0x8000u; break;
+        default: return OSB200_ERR_INVALID_ARG;
+    }
+    c->d = descending ? 0xFFFFu : 0;
+    c->flags = 0;
+    *codec = c->a == 0 && c->b == 0 && c->d == 0 ? nullptr : c;
+    return OSB200_OK;
+}
+
+// What every typed sort and argsort checks once the handle's shape is accepted: the key type (a type of another width:
+// INVALID_ARG), then the variant (typed keys and the indices mode live in the default pass's device plan).
+static int typed_codec(const osb200_sorter* h, int key_bytes, int key_type, int descending, osb::KeyCodec* c, const osb::KeyCodec** codec)
+{
+    const int st = key_bytes == 2 ? make_codec16(key_type, descending, c, codec) : make_codec(key_bytes, key_type, descending, c, codec);
+    if (st != OSB200_OK) return st;
+    return h->cfg.variant == osb::kVariantWide ? OSB200_OK : OSB200_ERR_UNSUPPORTED;
+}
+
+// The typed keys and pairs sorts once the handle's shape is accepted; pairs: d_vals may be null only when n <= 1.
+static int typed_sort(osb200_sorter* h, int key_bytes, void* d_keys, uint32_t* d_vals, bool pairs, uint64_t n, int key_type,
+                      int descending, void* stream)
+{
+    osb::KeyCodec c;
+    const osb::KeyCodec* codec = nullptr;
+    const int st = typed_codec(h, key_bytes, key_type, descending, &c, &codec);
+    if (st != OSB200_OK) return st;
+    if (pairs && n > 1 && !d_vals) return OSB200_ERR_INVALID_ARG;
+    return sort_impl(h, key_bytes, d_keys, d_vals, n, static_cast<cudaStream_t>(stream), codec);
+}
+
+// The argsorts once the handle's shape is accepted: keys of key_bytes (the handle's, or 2), 32-bit indices.
+static int argsort_impl(osb200_sorter* h, int key_bytes, const void* d_keys_in, void* d_keys_out, uint32_t* d_indices, uint64_t n,
+                        int key_type, int descending, void* stream)
+{
+    osb::KeyCodec c;
+    const osb::KeyCodec* codec = nullptr;
+    const int st = typed_codec(h, key_bytes, key_type, descending, &c, &codec);
+    if (st != OSB200_OK) return st;
+    if (n == 0) return OSB200_OK;
+    const uintptr_t in = reinterpret_cast<uintptr_t>(d_keys_in), out = reinterpret_cast<uintptr_t>(d_keys_out),
+                    idx = reinterpret_cast<uintptr_t>(d_indices);
+    if (!in || !out || !idx || ((in | out | idx) & 15u)) return OSB200_ERR_INVALID_ARG;
+    if (n > h->max_n || n > (1ull << 32)) return OSB200_ERR_SIZE;  // the indices are 32-bit
+    // the input is read until the last pass; outputs that overlap it (or each other) would overwrite keys still to be read
+    // (the key arrays are key_bytes * n bytes, the index array 4n)
+    const uint64_t kb = n * static_cast<uint64_t>(key_bytes), ib = n * sizeof(uint32_t);
+    if (overlaps(in, kb, out, kb) || overlaps(in, kb, idx, ib) || overlaps(out, kb, idx, ib)) return OSB200_ERR_INVALID_ARG;
+    cudaStream_t q = static_cast<cudaStream_t>(stream);
+    if (n == 1) {  // already sorted, but the outputs still have to be written
+        OSB_TRY(cudaMemcpyAsync(d_keys_out, d_keys_in, key_bytes, cudaMemcpyDeviceToDevice, q));
+        OSB_TRY(cudaMemsetAsync(d_indices, 0, sizeof(uint32_t), q));
+        return OSB200_OK;
+    }
+    return sort_impl(h, key_bytes, d_keys_out, d_indices, n, q, codec, 0, -1, d_keys_in);
 }
 
 int osb200_sort_keys_typed(osb200_handle h, void* d_keys, uint64_t n, int key_type, int descending, void* stream)
 {
     if (check_handle(h) != OSB200_OK) return OSB200_ERR_INVALID_ARG;
-    osb::KeyCodec c;
-    int st = make_codec(h->key_bytes, key_type, descending, &c);
-    if (st != OSB200_OK) return st;
-    if (h->cfg.variant != osb::kVariantWide) return OSB200_ERR_UNSUPPORTED;
-    const bool plain = c.a == 0 && c.b == 0 && c.d == 0;
-    return sort_impl(h, h->key_bytes, d_keys, nullptr, n, static_cast<cudaStream_t>(stream), plain ? nullptr : &c);
+    return typed_sort(h, h->key_bytes, d_keys, nullptr, false, n, key_type, descending, stream);
 }
 
 int osb200_segmented_sort_u32(osb200_handle h, uint32_t* d_keys, uint32_t* d_values, const uint64_t* d_segment_offsets,
@@ -495,7 +558,7 @@ int osb200_segmented_sort_u32(osb200_handle h, uint32_t* d_keys, uint32_t* d_val
     if (h->key_bytes != 4 || (d_values && h->value_bytes != 4)) return OSB200_ERR_INVALID_ARG;
     if (num_segments == 0 || max_segment_len <= 1) return OSB200_OK;
     if (!d_keys || !d_segment_offsets) return OSB200_ERR_INVALID_ARG;
-    if (max_segment_len > osb::segment_sort_capacity(4, false)) return OSB200_ERR_SIZE;  // sort longer segments with osb200_sort_*
+    if (max_segment_len > osb::segment_sort_capacity(4)) return OSB200_ERR_SIZE;  // sort longer segments with osb200_sort_*
     OSB_TRY(osb::launch_segment_sort(d_keys, d_values, 4, reinterpret_cast<const unsigned long long*>(d_segment_offsets), num_segments,
                                      0, max_segment_len, 0, 4, 8, nullptr, h->cfg.rank_mode, h->sm_count,
                                      static_cast<cudaStream_t>(stream)));
@@ -514,110 +577,34 @@ int osb200_sort_pairs_typed(osb200_handle h, void* d_keys, uint32_t* d_values, u
                             void* stream)
 {
     if (check_handle(h) != OSB200_OK || h->value_bytes != 4) return OSB200_ERR_INVALID_ARG;
-    if (n > 1 && !d_values) return OSB200_ERR_INVALID_ARG;
-    osb::KeyCodec c;
-    int st = make_codec(h->key_bytes, key_type, descending, &c);
-    if (st != OSB200_OK) return st;
-    if (h->cfg.variant != osb::kVariantWide) return OSB200_ERR_UNSUPPORTED;
-    const bool plain = c.a == 0 && c.b == 0 && c.d == 0;
-    return sort_impl(h, h->key_bytes, d_keys, d_values, n, static_cast<cudaStream_t>(stream), plain ? nullptr : &c);
+    if (n > 1 && !d_values) return OSB200_ERR_INVALID_ARG;  // before the key type, unlike osb200_sort_pairs16
+    return typed_sort(h, h->key_bytes, d_keys, d_values, true, n, key_type, descending, stream);
 }
 
 int osb200_argsort(osb200_handle h, const void* d_keys_in, void* d_keys_out, uint32_t* d_indices, uint64_t n, int key_type,
                    int descending, void* stream)
 {
     if (check_handle(h) != OSB200_OK || h->value_bytes != 4) return OSB200_ERR_INVALID_ARG;
-    osb::KeyCodec c;
-    int st = make_codec(h->key_bytes, key_type, descending, &c);  // a key type of the other width: INVALID_ARG
-    if (st != OSB200_OK) return st;
-    if (h->cfg.variant != osb::kVariantWide) return OSB200_ERR_UNSUPPORTED;  // the indices mode lives in the device plan
-    if (n == 0) return OSB200_OK;
-    const uintptr_t in = reinterpret_cast<uintptr_t>(d_keys_in), out = reinterpret_cast<uintptr_t>(d_keys_out),
-                    idx = reinterpret_cast<uintptr_t>(d_indices);
-    if (!in || !out || !idx || ((in | out | idx) & 15u)) return OSB200_ERR_INVALID_ARG;
-    if (n > h->max_n || n > (1ull << 32)) return OSB200_ERR_SIZE;  // the indices are 32-bit
-    // the input is read until the last pass; outputs that overlap it (or each other) would overwrite keys still to be read
-    // (the key arrays are key_bytes * n bytes, the index array 4n)
-    const uint64_t kb = n * static_cast<uint64_t>(h->key_bytes), ib = n * sizeof(uint32_t);
-    auto overlap = [](uintptr_t a, uint64_t alen, uintptr_t b, uint64_t blen) { return a < b + blen && b < a + alen; };
-    if (overlap(in, kb, out, kb) || overlap(in, kb, idx, ib) || overlap(out, kb, idx, ib)) return OSB200_ERR_INVALID_ARG;
-    cudaStream_t q = static_cast<cudaStream_t>(stream);
-    if (n == 1) {  // already sorted, but the outputs still have to be written
-        OSB_TRY(cudaMemcpyAsync(d_keys_out, d_keys_in, h->key_bytes, cudaMemcpyDeviceToDevice, q));
-        OSB_TRY(cudaMemsetAsync(d_indices, 0, sizeof(uint32_t), q));
-        return OSB200_OK;
-    }
-    const bool plain = c.a == 0 && c.b == 0 && c.d == 0;
-    return sort_impl(h, h->key_bytes, d_keys_out, d_indices, n, q, plain ? nullptr : &c, 0, -1, d_keys_in);
-}
-
-// 16-bit keys (osb200_key16_type) on a 4-byte handle: the same driver with a key width of 2 -- two digit passes.  F16 and
-// BF16 share the float codec (sign bit 15); they differ only in the dtype the caller keeps them in.
-static int make_codec16(int key_type, int descending, osb::KeyCodec* c)
-{
-    switch (key_type) {
-        case OSB200_KEY16_U16: c->a = 0; c->b = 0; break;
-        case OSB200_KEY16_I16: c->a = 0; c->b = 0x8000u; break;
-        case OSB200_KEY16_F16:
-        case OSB200_KEY16_BF16: c->a = 0xFFFFu; c->b = 0x8000u; break;
-        default: return OSB200_ERR_INVALID_ARG;
-    }
-    c->d = descending ? 0xFFFFu : 0;
-    c->flags = 0;
-    return OSB200_OK;
-}
-
-static int check_16(const osb200_sorter* h, bool pairs, int key_type, int descending, osb::KeyCodec* c)
-{
-    if (check_handle(h) != OSB200_OK || h->key_bytes != 4 || (pairs && h->value_bytes != 4)) return OSB200_ERR_INVALID_ARG;
-    const int st = make_codec16(key_type, descending, c);
-    if (st != OSB200_OK) return st;
-    if (h->cfg.variant != osb::kVariantWide) return OSB200_ERR_UNSUPPORTED;
-    return OSB200_OK;
+    return argsort_impl(h, h->key_bytes, d_keys_in, d_keys_out, d_indices, n, key_type, descending, stream);
 }
 
 int osb200_sort_keys16(osb200_handle h, void* d_keys, uint64_t n, int key_type, int descending, void* stream)
 {
-    osb::KeyCodec c;
-    const int st = check_16(h, false, key_type, descending, &c);
-    if (st != OSB200_OK) return st;
-    const bool plain = c.a == 0 && c.b == 0 && c.d == 0;
-    return sort_impl(h, 2, d_keys, nullptr, n, static_cast<cudaStream_t>(stream), plain ? nullptr : &c);
+    if (check_handle(h) != OSB200_OK || h->key_bytes != 4) return OSB200_ERR_INVALID_ARG;
+    return typed_sort(h, 2, d_keys, nullptr, false, n, key_type, descending, stream);
 }
 
 int osb200_sort_pairs16(osb200_handle h, void* d_keys, uint32_t* d_values, uint64_t n, int key_type, int descending, void* stream)
 {
-    osb::KeyCodec c;
-    const int st = check_16(h, true, key_type, descending, &c);
-    if (st != OSB200_OK) return st;
-    if (n > 1 && !d_values) return OSB200_ERR_INVALID_ARG;
-    const bool plain = c.a == 0 && c.b == 0 && c.d == 0;
-    return sort_impl(h, 2, d_keys, d_values, n, static_cast<cudaStream_t>(stream), plain ? nullptr : &c);
+    if (check_handle(h) != OSB200_OK || h->key_bytes != 4 || h->value_bytes != 4) return OSB200_ERR_INVALID_ARG;
+    return typed_sort(h, 2, d_keys, d_values, true, n, key_type, descending, stream);
 }
 
 int osb200_argsort16(osb200_handle h, const void* d_keys_in, void* d_keys_out, uint32_t* d_indices, uint64_t n, int key_type,
                      int descending, void* stream)
 {
-    osb::KeyCodec c;
-    const int st = check_16(h, true, key_type, descending, &c);
-    if (st != OSB200_OK) return st;
-    if (n == 0) return OSB200_OK;
-    const uintptr_t in = reinterpret_cast<uintptr_t>(d_keys_in), out = reinterpret_cast<uintptr_t>(d_keys_out),
-                    idx = reinterpret_cast<uintptr_t>(d_indices);
-    if (!in || !out || !idx || ((in | out | idx) & 15u)) return OSB200_ERR_INVALID_ARG;
-    if (n > h->max_n || n > (1ull << 32)) return OSB200_ERR_SIZE;  // the indices are 32-bit
-    // the key arrays are 2n bytes, the index array 4n
-    const uint64_t kb = n * sizeof(uint16_t), ib = n * sizeof(uint32_t);
-    auto overlap = [](uintptr_t a, uint64_t alen, uintptr_t b, uint64_t blen) { return a < b + blen && b < a + alen; };
-    if (overlap(in, kb, out, kb) || overlap(in, kb, idx, ib) || overlap(out, kb, idx, ib)) return OSB200_ERR_INVALID_ARG;
-    cudaStream_t q = static_cast<cudaStream_t>(stream);
-    if (n == 1) {  // already sorted, but the outputs still have to be written
-        OSB_TRY(cudaMemcpyAsync(d_keys_out, d_keys_in, sizeof(uint16_t), cudaMemcpyDeviceToDevice, q));
-        OSB_TRY(cudaMemsetAsync(d_indices, 0, sizeof(uint32_t), q));
-        return OSB200_OK;
-    }
-    const bool plain = c.a == 0 && c.b == 0 && c.d == 0;
-    return sort_impl(h, 2, d_keys_out, d_indices, n, q, plain ? nullptr : &c, 0, -1, d_keys_in);
+    if (check_handle(h) != OSB200_OK || h->key_bytes != 4 || h->value_bytes != 4) return OSB200_ERR_INVALID_ARG;
+    return argsort_impl(h, 2, d_keys_in, d_keys_out, d_indices, n, key_type, descending, stream);
 }
 
 // Row sort: one launch, no workspace -- only the handle's device, rank mode and SM count are used, so any handle will do.
@@ -626,8 +613,9 @@ int osb200_sort_rows(osb200_handle h, const void* d_keys_in, void* d_keys_out, u
 {
     if (check_handle(h) != OSB200_OK) return OSB200_ERR_INVALID_ARG;
     osb::KeyCodec c;
-    int st = key_bytes == 2 ? make_codec16(key_type, descending, &c)
-             : key_bytes == 4 || key_bytes == 8 ? make_codec(key_bytes, key_type, descending, &c)
+    const osb::KeyCodec* codec = nullptr;
+    int st = key_bytes == 2 ? make_codec16(key_type, descending, &c, &codec)
+             : key_bytes == 4 || key_bytes == 8 ? make_codec(key_bytes, key_type, descending, &c, &codec)
                                                 : OSB200_ERR_INVALID_ARG;
     if (st != OSB200_OK) return st;
     if (num_rows == 0 || row_len == 0) return OSB200_OK;
@@ -641,9 +629,8 @@ int osb200_sort_rows(osb200_handle h, const void* d_keys_in, void* d_keys_out, u
     const uint64_t n = num_rows * row_len;
     if (n > UINT64_MAX / 8) return OSB200_ERR_INVALID_ARG;
     const uint64_t kb = n * static_cast<uint64_t>(key_bytes), ib = n * sizeof(uint32_t);
-    auto overlap = [](uintptr_t a, uint64_t alen, uintptr_t b, uint64_t blen) { return a < b + blen && b < a + alen; };
     // in place (out == in) is fine: a row is read whole before it is written; any other overlap is not
-    if ((in != out && overlap(in, kb, out, kb)) || (idx && (overlap(in, kb, idx, ib) || overlap(out, kb, idx, ib))))
+    if ((in != out && overlaps(in, kb, out, kb)) || (idx && (overlaps(in, kb, idx, ib) || overlaps(out, kb, idx, ib))))
         return OSB200_ERR_INVALID_ARG;
     if (row_len > osb::row_sort_capacity(key_bytes)) return OSB200_ERR_SIZE;
     cudaStream_t q = static_cast<cudaStream_t>(stream);
@@ -652,9 +639,8 @@ int osb200_sort_rows(osb200_handle h, const void* d_keys_in, void* d_keys_out, u
         if (idx) OSB_TRY(cudaMemsetAsync(d_indices, 0, ib, q));
         return OSB200_OK;
     }
-    const bool plain = c.a == 0 && c.b == 0 && c.d == 0;
     c.flags = osb::kCodecEncodeOnLoad | osb::kCodecDecodeOnStore;
-    OSB_TRY(osb::launch_row_sort(d_keys_in, d_keys_out, d_indices, num_rows, row_len, key_bytes, plain ? nullptr : &c,
+    OSB_TRY(osb::launch_row_sort(d_keys_in, d_keys_out, d_indices, num_rows, row_len, key_bytes, codec,
                                  h->cfg.rank_mode, h->debug_rows_block, h->sm_count, q));
     return OSB200_OK;
 }
@@ -850,7 +836,7 @@ int64_t osb200_get_info(osb200_handle h, const char* key)
         if (cudaMemcpy(&pl, h->plan(), sizeof(pl), cudaMemcpyDeviceToHost) != cudaSuccess) return -1;
         return static_cast<int>((pl.skip_mask >> osb::kPlanHotShift) & 0xffu);
     }
-    if (!std::strcmp(key, "small_path_max_n")) return osb::segment_sort_capacity(h->key_bytes, false);
+    if (!std::strcmp(key, "small_path_max_n")) return osb::segment_sort_capacity(h->key_bytes);
     if (!std::strcmp(key, "spin_cap")) return h->cfg.spin_cap;
     if (!std::strcmp(key, "last_skip_mask") || !std::strcmp(key, "last_executed_passes")) {
         // the plan of the last sort on this handle (synchronises the device: introspection / tests only)

@@ -12,10 +12,78 @@
 // its values to same-address lanes of a warp instruction in ascending lane order -- checked by a device self-test when a
 // sorter is created -- it is a single-instruction stable multisplit.  The ballot formulation is kept as
 // RankMode::kRankBallot and is used when the self-test fails.
+#include <type_traits>
+
 #include "osb_kernels.cuh"
 #include "osb_common.cuh"
 
 namespace osb {
+
+// =====================================================================================================
+// Host-side dispatch.  Each kernel family lists the instantiations it is compiled for once, as a TypeList of shapes;
+// configure_kernels() walks the lists and the launchers find the shape that matches their run-time arguments in the same
+// list, so every launched instantiation is a configured one.
+// =====================================================================================================
+template <typename... Ts> struct TypeList {};
+
+// f(T{}) for every type of the list, in order, until one returns an error
+template <typename... Ts, typename F>
+static cudaError_t for_each_type(TypeList<Ts...>, F&& f)
+{
+    cudaError_t e = cudaSuccess;
+    (void)(((e = f(Ts{})) == cudaSuccess) && ...);
+    return e;
+}
+
+// f(T{}) for the first type of the list that `match` accepts; cudaErrorInvalidValue if there is none
+template <typename... Ts, typename M, typename F>
+static cudaError_t find_type(TypeList<Ts...>, M&& match, F&& f)
+{
+    cudaError_t e = cudaErrorInvalidValue;
+    (void)((match(Ts{}) && ((e = f(Ts{})), true)) || ...);
+    return e;
+}
+
+// The key type of the list that is key_bytes wide: f(KeyT{}); cudaErrorInvalidValue if the launcher has none that wide.
+template <typename... Keys, typename F>
+static cudaError_t with_key_type(TypeList<Keys...> keys, int key_bytes, F&& f)
+{
+    return find_type(keys, [&](auto k) { return key_bytes == static_cast<int>(sizeof(k)); }, f);
+}
+
+// The rank mode as a compile-time constant: f(std::integral_constant<int, RANK_MODE>{}).
+template <typename F>
+static cudaError_t with_rank_mode(int rank_mode, F&& f)
+{
+    return rank_mode == kRankBallot ? f(std::integral_constant<int, kRankBallot>{}) : f(std::integral_constant<int, kRankAtomic>{});
+}
+
+// ceil(work / per_cta) CTAs, at least one and at most cap
+static unsigned capped_grid(uint64_t work, uint64_t per_cta, uint64_t cap)
+{
+    uint64_t want = (work + per_cta - 1) / per_cta;
+    if (want < 1) want = 1;
+    return static_cast<unsigned>(want < cap ? want : cap);
+}
+
+template <typename K>
+static cudaError_t set_smem(K* kernel, size_t bytes)
+{
+    return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bytes));
+}
+
+// Opts both rank modes of a shape's kernel (and of its HOT twin, if it has one) into the shape's dynamic shared memory.
+template <typename Shape>
+static cudaError_t configure_shape(Shape)
+{
+    cudaError_t e = set_smem(Shape::template kernel<kRankAtomic>(), Shape::smem);
+    if (e == cudaSuccess) e = set_smem(Shape::template kernel<kRankBallot>(), Shape::smem);
+    if constexpr (Shape::has_hot) {
+        if (e == cudaSuccess) e = set_smem(Shape::template kernel<kRankAtomic, true>(), Shape::smem);
+        if (e == cudaSuccess) e = set_smem(Shape::template kernel<kRankBallot, true>(), Shape::smem);
+    }
+    return e;
+}
 
 // =====================================================================================================
 // GlobalHistogram
@@ -146,26 +214,26 @@ global_histogram_kernel(const KeyT* __restrict__ keys, uint64_t n, unsigned long
 
 template <typename KeyT> constexpr size_t hist_smem_bytes() { return sizeof(KeyT) * kRadix * HistGeom<KeyT>::COLS * sizeof(uint32_t); }
 
+using HistKeys = TypeList<uint16_t, uint32_t, uint64_t>;  // global_histogram_kernel of whole keys
+using HistBitsKeys = TypeList<uint32_t, uint64_t>;        // its MASKED form and global_histogram_bits_kernel (bit-range sorts)
+
+template <typename KeyT, bool MASKED>
+static cudaError_t launch_histogram_vec(const void* keys, uint64_t n, unsigned long long* ghist, int sm_count, cudaStream_t stream,
+                                        const KeyCodec& codec, int places = 0, uint32_t last_mask = 255u)
+{
+    const unsigned grid = capped_grid(n / (16 / sizeof(KeyT)), kHistThreads, sm_count);
+    global_histogram_kernel<KeyT, MASKED><<<grid, kHistThreads, hist_smem_bytes<KeyT>(), stream>>>(
+        static_cast<const KeyT*>(keys), n, ghist, codec, places, last_mask);
+    return cudaGetLastError();
+}
+
 cudaError_t launch_global_histogram(const void* keys, uint64_t n, int key_bytes, unsigned long long* ghist,
                                     int sm_count, cudaStream_t stream, const KeyCodec* codec_in)
 {
     const KeyCodec codec = codec_in ? *codec_in : KeyCodec();
-    const uint64_t vecs = n / (16 / key_bytes);
-    uint64_t want = (vecs + kHistThreads - 1) / kHistThreads;
-    if (want < 1) want = 1;
-    const unsigned grid = static_cast<unsigned>(want < static_cast<uint64_t>(sm_count) ? want : sm_count);
-    if (key_bytes == 4)
-        global_histogram_kernel<uint32_t><<<grid, kHistThreads, hist_smem_bytes<uint32_t>(), stream>>>(
-            static_cast<const uint32_t*>(keys), n, ghist, codec);
-    else if (key_bytes == 8)
-        global_histogram_kernel<uint64_t><<<grid, kHistThreads, hist_smem_bytes<uint64_t>(), stream>>>(
-            static_cast<const uint64_t*>(keys), n, ghist, codec);
-    else if (key_bytes == 2)
-        global_histogram_kernel<uint16_t><<<grid, kHistThreads, hist_smem_bytes<uint16_t>(), stream>>>(
-            static_cast<const uint16_t*>(keys), n, ghist, codec);
-    else
-        return cudaErrorInvalidValue;
-    return cudaGetLastError();
+    return with_key_type(HistKeys{}, key_bytes, [&](auto k) {
+        return launch_histogram_vec<decltype(k), false>(keys, n, ghist, sm_count, stream, codec);
+    });
 }
 
 // Single digit place (the sharded path's most-significant-digit histogram): one atomic per key, same
@@ -201,14 +269,12 @@ digit_histogram_kernel(const KeyT* __restrict__ keys, uint64_t n, uint32_t shift
 cudaError_t launch_digit_histogram(const void* keys, uint64_t n, int key_bytes, uint32_t shift,
                                    unsigned long long* hist256, int sm_count, cudaStream_t stream)
 {
-    uint64_t want = (n + kHistThreads * 4 - 1) / (kHistThreads * 4);
-    if (want < 1) want = 1;
-    const unsigned grid = static_cast<unsigned>(want < static_cast<uint64_t>(sm_count) * 2 ? want : sm_count * 2);
-    if (key_bytes == 4)
-        digit_histogram_kernel<uint32_t><<<grid, kHistThreads, 0, stream>>>(static_cast<const uint32_t*>(keys), n, shift, hist256);
-    else
-        digit_histogram_kernel<uint64_t><<<grid, kHistThreads, 0, stream>>>(static_cast<const uint64_t*>(keys), n, shift, hist256);
-    return cudaGetLastError();
+    const unsigned grid = capped_grid(n, kHistThreads * 4, static_cast<uint64_t>(sm_count) * 2);
+    return with_key_type(TypeList<uint32_t, uint64_t>{}, key_bytes, [&](auto k) {
+        using KeyT = decltype(k);
+        digit_histogram_kernel<KeyT><<<grid, kHistThreads, 0, stream>>>(static_cast<const KeyT*>(keys), n, shift, hist256);
+        return cudaGetLastError();
+    });
 }
 
 // =====================================================================================================
@@ -304,29 +370,14 @@ cudaError_t launch_global_histogram_bits(const void* keys, uint64_t n, int key_b
 {
     const KeyCodec codec = codec_in ? *codec_in : KeyCodec();
     const uint32_t last_mask = (1u << last_bits) - 1u;
-    if (begin_bit == 0) {  // byte-aligned places: the fast kernel slices the loaded words, the last place keeps last_bits
-        const uint64_t vecs = n / (16 / key_bytes);
-        uint64_t w2 = (vecs + kHistThreads - 1) / kHistThreads;
-        if (w2 < 1) w2 = 1;
-        const unsigned g2 = static_cast<unsigned>(w2 < static_cast<uint64_t>(sm_count) ? w2 : sm_count);
-        if (key_bytes == 4)
-            global_histogram_kernel<uint32_t, true><<<g2, kHistThreads, hist_smem_bytes<uint32_t>(), stream>>>(
-                static_cast<const uint32_t*>(keys), n, ghist, codec, places, last_mask);
-        else
-            global_histogram_kernel<uint64_t, true><<<g2, kHistThreads, hist_smem_bytes<uint64_t>(), stream>>>(
-                static_cast<const uint64_t*>(keys), n, ghist, codec, places, last_mask);
+    return with_key_type(HistBitsKeys{}, key_bytes, [&](auto k) {
+        using KeyT = decltype(k);
+        // byte-aligned places: the fast kernel slices the loaded words, the last place keeps last_bits
+        if (begin_bit == 0) return launch_histogram_vec<KeyT, true>(keys, n, ghist, sm_count, stream, codec, places, last_mask);
+        global_histogram_bits_kernel<KeyT><<<capped_grid(n, kHistThreads * 4, sm_count), kHistThreads, hist_smem_bytes<KeyT>(), stream>>>(
+            static_cast<const KeyT*>(keys), n, ghist, codec, begin_bit, places, last_mask);
         return cudaGetLastError();
-    }
-    uint64_t want = (n + kHistThreads * 4 - 1) / (kHistThreads * 4);
-    if (want < 1) want = 1;
-    const unsigned grid = static_cast<unsigned>(want < static_cast<uint64_t>(sm_count) ? want : sm_count);
-    if (key_bytes == 4)
-        global_histogram_bits_kernel<uint32_t><<<grid, kHistThreads, hist_smem_bytes<uint32_t>(), stream>>>(
-            static_cast<const uint32_t*>(keys), n, ghist, codec, begin_bit, places, last_mask);
-    else
-        global_histogram_bits_kernel<uint64_t><<<grid, kHistThreads, hist_smem_bytes<uint64_t>(), stream>>>(
-            static_cast<const uint64_t*>(keys), n, ghist, codec, begin_bit, places, last_mask);
-    return cudaGetLastError();
+    });
 }
 
 // =====================================================================================================
@@ -352,10 +403,7 @@ cudaError_t launch_copy_back(const SortPlan* plan, const void* alt_keys, void* k
     auto launch = [&](auto word, const void* s, void* d, uint64_t bytes) {
         using W = decltype(word);
         const uint64_t words = bytes / sizeof(W);
-        uint64_t want = (words + 511) / 512;
-        if (want < 1) want = 1;
-        const unsigned grid = static_cast<unsigned>(want < static_cast<uint64_t>(sm_count) * 4 ? want : sm_count * 4);
-        copy_back_kernel<W><<<grid, 512, 0, stream>>>(plan, static_cast<const W*>(s), static_cast<W*>(d), words,
+        copy_back_kernel<W><<<capped_grid(words, 512, static_cast<uint64_t>(sm_count) * 4), 512, 0, stream>>>(plan, static_cast<const W*>(s), static_cast<W*>(d), words,
                                                       static_cast<const unsigned char*>(s) + words * sizeof(W),
                                                       static_cast<unsigned char*>(d) + words * sizeof(W),
                                                       static_cast<uint32_t>(bytes - words * sizeof(W)));
@@ -402,24 +450,13 @@ cudaError_t launch_argsort_copy_back(const SortPlan* plan, const void* keys_in, 
                                      const uint32_t* alt_idx, uint32_t* idx, uint64_t n, int key_bytes, int sm_count,
                                      cudaStream_t stream)
 {
-    uint64_t want = (n / 4 + 511) / 512;
-    if (want < 1) want = 1;
-    const unsigned grid = static_cast<unsigned>(want < static_cast<uint64_t>(sm_count) * 4 ? want : sm_count * 4);
-    if (key_bytes == 4)
-        argsort_copy_back_kernel<uint32_t><<<grid, 512, 0, stream>>>(plan, static_cast<const uint32_t*>(keys_in),
-                                                                     static_cast<const uint32_t*>(alt_keys),
-                                                                     static_cast<uint32_t*>(keys), alt_idx, idx, n);
-    else if (key_bytes == 2)
-        argsort_copy_back_kernel<uint16_t><<<grid, 512, 0, stream>>>(plan, static_cast<const uint16_t*>(keys_in),
-                                                                     static_cast<const uint16_t*>(alt_keys),
-                                                                     static_cast<uint16_t*>(keys), alt_idx, idx, n);
-    else if (key_bytes == 8)
-        argsort_copy_back_kernel<uint64_t><<<grid, 512, 0, stream>>>(plan, static_cast<const uint64_t*>(keys_in),
-                                                                     static_cast<const uint64_t*>(alt_keys),
-                                                                     static_cast<uint64_t*>(keys), alt_idx, idx, n);
-    else
-        return cudaErrorInvalidValue;
-    return cudaGetLastError();
+    const unsigned grid = capped_grid(n / 4, 512, static_cast<uint64_t>(sm_count) * 4);
+    return with_key_type(TypeList<uint16_t, uint32_t, uint64_t>{}, key_bytes, [&](auto k) {
+        using KeyT = decltype(k);
+        argsort_copy_back_kernel<KeyT><<<grid, 512, 0, stream>>>(plan, static_cast<const KeyT*>(keys_in), static_cast<const KeyT*>(alt_keys),
+                                                                 static_cast<KeyT*>(keys), alt_idx, idx, n);
+        return cudaGetLastError();
+    });
 }
 
 // =====================================================================================================
@@ -1651,30 +1688,58 @@ template <typename KeyT> struct RingGeom;
 template <> struct RingGeom<uint32_t> { static constexpr int K = OSB_RING_K, WARPS = 16, LOOK = OSB_LOOK; };
 template <> struct RingGeom<uint64_t> { static constexpr int K = 8,  WARPS = 16, LOOK = OSB_LOOK; };
 
-template <typename KeyT, int RANK_MODE>
-static cudaError_t launch_ring_variant(const void* in, void* out, uint64_t n, uint32_t shift, const unsigned long long* gbase,
-                                       uint16_t* agg16, uint64_t* incl64, uint32_t* ticket, uint32_t epoch, int sm_count,
-                                       cudaStream_t stream)
-{
-    using G = RingGeom<KeyT>;
-    using S = RingSmem<KeyT, G::K, G::WARPS>;
-    const uint64_t tiles = (n + S::T - 1) / S::T;
-    const uint64_t cap = static_cast<uint64_t>(sm_count) * (sizeof(KeyT) == 4 ? OSB_RING_MINB : 2);
-    const unsigned grid = static_cast<unsigned>(tiles < cap ? tiles : cap);
-    auto kern = digit_binning_ring_kernel<KeyT, G::K, G::WARPS, RANK_MODE, G::LOOK>;
-    kern<<<grid, S::THREADS, sizeof(S), stream>>>(static_cast<const KeyT*>(in), static_cast<KeyT*>(out), n, shift, gbase, agg16,
-                                                   incl64, ticket, epoch, static_cast<uint32_t>(tiles));
-    return cudaGetLastError();
-}
+// ---- what every DigitBinningPass shape has ------------------------------------------------------------
+// The arguments of one pass, whichever kernel runs it.
+struct PassArgs {
+    const void* in; void* out; const uint32_t* in_val; uint32_t* out_val; uint64_t n; uint32_t shift;
+    const unsigned long long* gbase; uint64_t* desc; uint16_t* agg16; uint32_t* ticket; uint32_t epoch;
+    const BinningConfig& cfg; cudaStream_t stream;
 
-template <typename KeyT, int RANK_MODE>
-static cudaError_t set_ring_attr()
-{
+    PassParams params() const
+    {
+        PassParams pp;
+        pp.shift = shift;
+        pp.dbits = cfg.digit_bits;
+        pp.epoch = epoch;
+        pp.place = cfg.place;
+        pp.spin_cap = cfg.spin_cap;
+        pp.stall_every = cfg.debug_stall_every;
+        pp.plan = cfg.plan;
+        pp.keys_in = cfg.argsort_in;
+        return pp;
+    }
+};
+
+// A pass shape: the keys, pairs and indices it sorts.  Each family adds its tile T, its dynamic shared memory `smem`,
+// kernel<RANK_MODE, HOT>() and launch<RANK_MODE>(const PassArgs&).
+template <typename KeyT, bool PAIRS, bool INDICES = false>
+struct PassShape {
+    using Key = KeyT;
+    static constexpr bool pairs = PAIRS, indices = INDICES;
+    static constexpr bool enabled = true;   // whether launch_digit_binning runs it (the shape is configured either way)
+    static constexpr bool has_hot = false;  // whether it has a HOT twin for low-entropy passes
+};
+
+template <typename KeyT>
+struct RingShape : PassShape<KeyT, false> {
     using G = RingGeom<KeyT>;
     using S = RingSmem<KeyT, G::K, G::WARPS>;
-    return cudaFuncSetAttribute(digit_binning_ring_kernel<KeyT, G::K, G::WARPS, RANK_MODE, G::LOOK>,
-                                cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(sizeof(S)));
-}
+    static constexpr uint32_t T = S::T;
+    static constexpr size_t smem = sizeof(S);
+    template <int RANK_MODE, bool HOT = false>
+    static auto kernel() { return digit_binning_ring_kernel<KeyT, G::K, G::WARPS, RANK_MODE, G::LOOK>; }
+    template <int RANK_MODE>
+    static cudaError_t launch(const PassArgs& a)
+    {
+        const uint64_t tiles = (a.n + T - 1) / T;
+        const uint64_t cap = static_cast<uint64_t>(a.cfg.sm_count) * (sizeof(KeyT) == 4 ? OSB_RING_MINB : 2);
+        const auto kern = kernel<RANK_MODE>();
+        kern<<<static_cast<unsigned>(tiles < cap ? tiles : cap), S::THREADS, smem, a.stream>>>(
+            static_cast<const KeyT*>(a.in), static_cast<KeyT*>(a.out), a.n, a.shift, a.gbase, a.agg16, a.desc, a.ticket, a.epoch,
+            static_cast<uint32_t>(tiles));
+        return cudaGetLastError();
+    }
+};
 
 // Geometry and lookback window: 16,384-key tiles on 2 x 512 threads per SM (~82 KB of shared memory per CTA, inside
 // H100's 227 KB per block and 228 KB per SM).  Re-swept on the H100 with tools/sweep.sh (DESIGN §4.2): 8,192-key tiles on
@@ -1729,102 +1794,74 @@ template <> struct WideGeom<uint16_t, true>  { static constexpr int K = OSB_P16_
 #define OSB_P64_LOOK 32
 #endif
 template <> struct WideGeom<uint64_t, true>  { static constexpr int K = OSB_P64_K, WARPS = OSB_P64_WARPS, MINB = OSB_P64_MINB, LOOK = OSB_P64_LOOK; };
-template <typename KeyT, bool PAIRS> constexpr uint32_t wide_tile() { return WideGeom<KeyT, PAIRS>::K * WideGeom<KeyT, PAIRS>::WARPS * 32; }
-
-template <typename KeyT, bool PAIRS, int RANK_MODE, bool INDICES = false>
-static cudaError_t launch_wide_variant(const void* in, void* out, const uint32_t* in_val, uint32_t* out_val, uint64_t n,
-                                       uint32_t shift, const unsigned long long* gbase, uint16_t* agg16, uint64_t* incl64,
-                                       uint32_t* ticket, uint32_t epoch, const BinningConfig& cfg, cudaStream_t stream)
-{
+template <typename KeyT, bool PAIRS, bool INDICES = false>
+struct WideShape : PassShape<KeyT, PAIRS, INDICES> {
     using G = WideGeom<KeyT, PAIRS>;
     using S = WideSmem<KeyT, PAIRS, G::K, G::WARPS>;
-    const uint64_t tiles = (n + S::T - 1) / S::T;
-    PassParams pp;
-    pp.shift = shift;
-    pp.dbits = cfg.digit_bits;
-    pp.epoch = epoch;
-    pp.place = cfg.place;
-    pp.spin_cap = cfg.spin_cap;
-    pp.stall_every = cfg.debug_stall_every;
-    pp.plan = cfg.plan;
-    pp.keys_in = cfg.argsort_in;
-    // Persistent instantiations (all but the plain u64 keys and pairs passes, which run one CTA per tile): as many CTAs as can be resident
-    // at once (capped by debug_max_ctas), at most one per tile; the tiles after the first of each CTA are handed out by
-    // `ticket`, which the host zeroes before the pass.
-    auto grid_for = [&](auto kernel, int& per_sm, bool persistent) -> unsigned {
-        if (!persistent) return static_cast<unsigned>(tiles);
-        if (per_sm == 0) {
-            int b = 0;
-            if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, kernel, S::THREADS, sizeof(S)) != cudaSuccess || b < 1) b = 1;
-            per_sm = b;
+    static constexpr uint32_t T = S::T;
+    static constexpr size_t smem = sizeof(S);
+    static constexpr bool has_hot = true;
+    template <int RANK_MODE, bool HOT = false>
+    static auto kernel() { return digit_binning_wide_kernel<KeyT, PAIRS, G::K, G::WARPS, RANK_MODE, G::LOOK, G::MINB, HOT, INDICES>; }
+    template <int RANK_MODE>
+    static cudaError_t launch(const PassArgs& a)
+    {
+        const uint64_t tiles = (a.n + T - 1) / T;
+        const PassParams pp = a.params();
+        // Persistent instantiations (all but the plain u64 keys and pairs passes, which run one CTA per tile): as many CTAs as can be resident
+        // at once (capped by debug_max_ctas), at most one per tile; the tiles after the first of each CTA are handed out by
+        // `ticket`, which the host zeroes before the pass.
+        auto grid_for = [&](auto kernel, int& per_sm, bool persistent) -> unsigned {
+            if (!persistent) return static_cast<unsigned>(tiles);
+            if (per_sm == 0) {
+                int b = 0;
+                if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, kernel, S::THREADS, smem) != cudaSuccess || b < 1) b = 1;
+                per_sm = b;
+            }
+            uint64_t cap = static_cast<uint64_t>(a.cfg.sm_count) * per_sm;
+            if (a.cfg.debug_max_ctas && a.cfg.debug_max_ctas < cap) cap = a.cfg.debug_max_ctas;
+            return static_cast<unsigned>(tiles < cap ? tiles : cap);
+        };
+        KeyT* buf0 = static_cast<KeyT*>(const_cast<void*>(a.in));
+        uint32_t* val0 = const_cast<uint32_t*>(a.in_val);
+        const auto kern = kernel<RANK_MODE>();
+        static int plain_per_sm = 0;  // (one value per instantiation)
+        // with a device plan `in`/`out` are the caller's and the alt buffers (the kernel picks the direction); both are written
+        kern<<<grid_for(kern, plain_per_sm, sizeof(KeyT) <= 4 && !PAIRS), S::THREADS, smem, a.stream>>>(
+            buf0, static_cast<KeyT*>(a.out), val0, a.out_val, a.n, a.gbase, a.agg16, a.desc, a.ticket, pp, a.cfg.codec);
+        if (a.cfg.plan != nullptr && a.cfg.hot_passes) {
+            // the HOT instantiation of the same pass; returns at once unless the plan calls the pass hot, before drawing a ticket
+            // (same geometry, one resident CTA per SM with up to 128 registers: no spills.  Two CTAs per SM at 64 registers
+            // spill; 1,024 threads x 16 keys at 64 registers is slower than this)
+            const auto hot = kernel<RANK_MODE, true>();
+            static int hot_per_sm = 0;
+            hot<<<grid_for(hot, hot_per_sm, true), S::THREADS, smem, a.stream>>>(
+                buf0, static_cast<KeyT*>(a.out), val0, a.out_val, a.n, a.gbase, a.agg16, a.desc, a.ticket, pp, a.cfg.codec);
         }
-        uint64_t cap = static_cast<uint64_t>(cfg.sm_count) * per_sm;
-        if (cfg.debug_max_ctas && cfg.debug_max_ctas < cap) cap = cfg.debug_max_ctas;
-        return static_cast<unsigned>(tiles < cap ? tiles : cap);
-    };
-    auto kern = digit_binning_wide_kernel<KeyT, PAIRS, G::K, G::WARPS, RANK_MODE, G::LOOK, G::MINB, false, INDICES>;
-    static int plain_per_sm = 0;  // (one value per instantiation of this function template)
-    // with a device plan `in`/`out` are the caller's and the alt buffers (the kernel picks the direction); both are written
-    kern<<<grid_for(kern, plain_per_sm, sizeof(KeyT) <= 4 && !PAIRS), S::THREADS, sizeof(S), stream>>>(
-        static_cast<KeyT*>(const_cast<void*>(in)), static_cast<KeyT*>(out), const_cast<uint32_t*>(in_val), out_val, n, gbase,
-        agg16, incl64, ticket, pp, cfg.codec);
-    if (cfg.plan != nullptr && cfg.hot_passes) {
-        // the HOT instantiation of the same pass; returns at once unless the plan calls the pass hot, before drawing a ticket
-        // (same geometry, one resident CTA per SM with up to 128 registers: no spills.  Two CTAs per SM at 64 registers
-        // spill; 1,024 threads x 16 keys at 64 registers is slower than this)
-        auto hot = digit_binning_wide_kernel<KeyT, PAIRS, G::K, G::WARPS, RANK_MODE, G::LOOK, G::MINB, true, INDICES>;
-        static int hot_per_sm = 0;
-        hot<<<grid_for(hot, hot_per_sm, true), S::THREADS, sizeof(S), stream>>>(
-            static_cast<KeyT*>(const_cast<void*>(in)), static_cast<KeyT*>(out), const_cast<uint32_t*>(in_val), out_val, n, gbase,
-            agg16, incl64, ticket, pp, cfg.codec);
+        return cudaGetLastError();
     }
-    return cudaGetLastError();
-}
+};
 
 constexpr int kPairsK = 32, kPairsWarps = 16;
 
-template <int RANK_MODE>
-static cudaError_t launch_pairs_variant(const void* in, void* out, const uint32_t* in_val, uint32_t* out_val, uint64_t n,
-                                        uint32_t shift, const unsigned long long* gbase, uint16_t* agg16, uint64_t* incl64,
-                                        uint32_t* ticket, uint32_t epoch, const BinningConfig& cfg, cudaStream_t stream)
-{
+// u32 pairs in 16,384-pair tiles: the default pass's shape only in a -DOSB_PAIRS16K=1 build
+struct Pairs16KShape : PassShape<uint32_t, true> {
+    static constexpr bool enabled = OSB_PAIRS16K != 0;
     using S = PairsSmem<kPairsWarps, kPairsK>;
-    const uint64_t tiles = (n + S::T - 1) / S::T;
-    PassParams pp;
-    pp.shift = shift;
-    pp.dbits = cfg.digit_bits;
-    pp.epoch = epoch;
-    pp.place = cfg.place;
-    pp.spin_cap = cfg.spin_cap;
-    pp.stall_every = cfg.debug_stall_every;
-    pp.plan = cfg.plan;
-    auto kern = digit_binning_pairs_kernel<kPairsK, kPairsWarps, RANK_MODE, OSB_PAIRS_LOOK>;
-    kern<<<static_cast<unsigned>(tiles), S::THREADS, sizeof(S), stream>>>(
-        static_cast<uint32_t*>(const_cast<void*>(in)), static_cast<uint32_t*>(out), const_cast<uint32_t*>(in_val), out_val, n,
-        gbase, agg16, incl64, ticket, pp, cfg.codec);
-    return cudaGetLastError();
-}
-
-template <int RANK_MODE>
-static cudaError_t set_pairs_attr()
-{
-    using S = PairsSmem<kPairsWarps, kPairsK>;
-    return cudaFuncSetAttribute(digit_binning_pairs_kernel<kPairsK, kPairsWarps, RANK_MODE, OSB_PAIRS_LOOK>,
-                                cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(sizeof(S)));
-}
-
-template <typename KeyT, bool PAIRS, int RANK_MODE, bool INDICES = false>
-static cudaError_t set_wide_attr()
-{
-    using G = WideGeom<KeyT, PAIRS>;
-    using S = WideSmem<KeyT, PAIRS, G::K, G::WARPS>;
-    cudaError_t e = cudaFuncSetAttribute(digit_binning_wide_kernel<KeyT, PAIRS, G::K, G::WARPS, RANK_MODE, G::LOOK, G::MINB, false, INDICES>,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(sizeof(S)));
-    if (e == cudaSuccess)
-        e = cudaFuncSetAttribute(digit_binning_wide_kernel<KeyT, PAIRS, G::K, G::WARPS, RANK_MODE, G::LOOK, G::MINB, true, INDICES>,
-                                 cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(sizeof(S)));
-    return e;
-}
+    static constexpr uint32_t T = S::T;
+    static constexpr size_t smem = sizeof(S);
+    template <int RANK_MODE, bool HOT = false>
+    static auto kernel() { return digit_binning_pairs_kernel<kPairsK, kPairsWarps, RANK_MODE, OSB_PAIRS_LOOK>; }
+    template <int RANK_MODE>
+    static cudaError_t launch(const PassArgs& a)
+    {
+        const auto kern = kernel<RANK_MODE>();
+        kern<<<static_cast<unsigned>((a.n + T - 1) / T), S::THREADS, smem, a.stream>>>(
+            static_cast<uint32_t*>(const_cast<void*>(a.in)), static_cast<uint32_t*>(a.out), const_cast<uint32_t*>(a.in_val), a.out_val,
+            a.n, a.gbase, a.agg16, a.desc, a.ticket, a.params(), a.cfg.codec);
+        return cudaGetLastError();
+    }
+};
 
 // ---- variant-0 geometry ------------------------------------------------------------------------------
 template <typename KeyT, bool PAIRS> struct TileGeom;
@@ -1833,121 +1870,77 @@ template <> struct TileGeom<uint32_t, true>  { static constexpr int K = 16, WARP
 template <> struct TileGeom<uint64_t, false> { static constexpr int K = 8,  WARPS = 16; };
 
 template <typename KeyT, bool PAIRS>
-constexpr size_t tile_smem_bytes()
-{
+struct TileShape : PassShape<KeyT, PAIRS> {
     using G = TileGeom<KeyT, PAIRS>;
-    const size_t hist = static_cast<size_t>(G::WARPS) * kRadix * 4;
-    const size_t keys = static_cast<size_t>(G::WARPS) * 32 * G::K * sizeof(KeyT);
-    return hist > keys ? hist : keys;
-}
+    static constexpr uint32_t T = G::WARPS * 32 * G::K;
+    static constexpr size_t hist_bytes = static_cast<size_t>(G::WARPS) * kRadix * 4, keys_bytes = T * sizeof(KeyT);
+    static constexpr size_t smem = hist_bytes > keys_bytes ? hist_bytes : keys_bytes;  // the histograms, then the sorted tile
+    template <int RANK_MODE, bool HOT = false>
+    static auto kernel() { return digit_binning_tile_kernel<KeyT, PAIRS, G::K, G::WARPS, RANK_MODE>; }
+    template <int RANK_MODE>
+    static cudaError_t launch(const PassArgs& a)
+    {
+        const auto kern = kernel<RANK_MODE>();
+        kern<<<static_cast<unsigned>((a.n + T - 1) / T), G::WARPS * 32, smem, a.stream>>>(
+            static_cast<const KeyT*>(a.in), static_cast<KeyT*>(a.out), a.in_val, a.out_val, a.n, a.shift, a.gbase, a.desc, a.ticket,
+            a.epoch);
+        return cudaGetLastError();
+    }
+};
 
-template <typename KeyT, bool PAIRS, int RANK_MODE>
-static cudaError_t launch_tile_variant(const void* in, void* out, const uint32_t* in_val, uint32_t* out_val, uint64_t n,
-                                       uint32_t shift, const unsigned long long* gbase, uint64_t* desc, uint32_t* ticket,
-                                       uint32_t epoch, cudaStream_t stream)
+// The instantiations of each variant.  Variant 2, the default pass: 16-, 32- and 64-bit keys, pairs and argsort, each with a
+// HOT twin (and the 16K-pair kernel, which takes the u32 pairs when enabled).
+using DefaultPassShapes = TypeList<Pairs16KShape,
+                                   WideShape<uint16_t, false>, WideShape<uint16_t, true>, WideShape<uint16_t, true, true>,
+                                   WideShape<uint32_t, false>, WideShape<uint32_t, true>, WideShape<uint32_t, true, true>,
+                                   WideShape<uint64_t, false>, WideShape<uint64_t, true>, WideShape<uint64_t, true, true>>;
+using RingShapes = TypeList<RingShape<uint32_t>, RingShape<uint64_t>>;  // variant 1: keys only
+using TileShapes = TypeList<TileShape<uint32_t, false>, TileShape<uint32_t, true>, TileShape<uint64_t, false>>;  // variant 0
+
+// f(Shape{}) for the pass launch_digit_binning runs on these keys in this variant: variant 1 has no pairs kernel, and
+// runs pairs in variant 0's.  cudaErrorInvalidValue if the variant has no such pass.
+template <typename F>
+static cudaError_t with_pass_shape(int key_bytes, bool pairs, bool indices, int variant, F&& f)
 {
-    using G = TileGeom<KeyT, PAIRS>;
-    constexpr int T = G::WARPS * 32 * G::K;
-    const uint64_t tiles = (n + T - 1) / T;
-    auto kern = digit_binning_tile_kernel<KeyT, PAIRS, G::K, G::WARPS, RANK_MODE>;
-    kern<<<static_cast<unsigned>(tiles), G::WARPS * 32, tile_smem_bytes<KeyT, PAIRS>(), stream>>>(
-        static_cast<const KeyT*>(in), static_cast<KeyT*>(out), in_val, out_val, n, shift, gbase, desc, ticket, epoch);
-    return cudaGetLastError();
+    auto match = [&](auto s) {
+        using S = decltype(s);
+        return S::enabled && key_bytes == static_cast<int>(sizeof(typename S::Key)) && S::pairs == pairs && S::indices == indices;
+    };
+    if (variant == kVariantWide) return find_type(DefaultPassShapes{}, match, f);
+    if (variant == kVariantPersistent && !pairs) return find_type(RingShapes{}, match, f);
+    return find_type(TileShapes{}, match, f);
 }
 
 // 16-bit keys run on a 4-byte handle, whose descriptors and reductions are sized for its smallest tile (smallest_tile in
 // osb_host.cu: the minimum over the variants of the 4-byte tiles): their tiles must not be smaller.
 constexpr uint32_t cmin(uint32_t a, uint32_t b) { return a < b ? a : b; }
-constexpr uint32_t kSmallestTileU32Keys = cmin(cmin(TileGeom<uint32_t, false>::WARPS * 32 * TileGeom<uint32_t, false>::K,
-                                                    RingGeom<uint32_t>::K * RingGeom<uint32_t>::WARPS * 32), wide_tile<uint32_t, false>());
-constexpr uint32_t kSmallestTileU32Pairs = cmin(TileGeom<uint32_t, true>::WARPS * 32 * TileGeom<uint32_t, true>::K, wide_tile<uint32_t, true>());
-static_assert(wide_tile<uint16_t, false>() >= kSmallestTileU32Keys && wide_tile<uint16_t, false>() >= kSmallestTileU32Pairs,
+constexpr uint32_t kSmallestTileU32Keys = cmin(cmin(TileShape<uint32_t, false>::T, RingShape<uint32_t>::T), WideShape<uint32_t, false>::T);
+constexpr uint32_t kSmallestTileU32Pairs = cmin(TileShape<uint32_t, true>::T, WideShape<uint32_t, true>::T);
+static_assert(WideShape<uint16_t, false>::T >= kSmallestTileU32Keys && WideShape<uint16_t, false>::T >= kSmallestTileU32Pairs,
               "16-bit keys (either 4-byte handle): a smaller tile would need more descriptors than the handle has");
-static_assert(wide_tile<uint16_t, true>() >= kSmallestTileU32Pairs,
+static_assert(WideShape<uint16_t, true>::T >= kSmallestTileU32Pairs,
               "16-bit pairs (a (4, 4) handle): a smaller tile would need more descriptors than the handle has");
-static_assert(wide_tile<uint16_t, false>() < 32768 && wide_tile<uint16_t, true>() < 32768, "agg16 holds 15-bit counts");
+static_assert(WideShape<uint16_t, false>::T < 32768 && WideShape<uint16_t, true>::T < 32768, "agg16 holds 15-bit counts");
 // A (8, 4) handle sizes its descriptors and reductions for smallest_tile(8, true): the variant-0 u64 tile (osb200_workspace_bytes
 // relies on it as well).
-static_assert(wide_tile<uint64_t, true>() >= TileGeom<uint64_t, false>::WARPS * 32 * TileGeom<uint64_t, false>::K,
+static_assert(WideShape<uint64_t, true>::T >= TileShape<uint64_t, false>::T,
               "64-bit pairs: a smaller tile would need more descriptors than the handle has");
-static_assert(wide_tile<uint64_t, true>() < 32768, "agg16 holds 15-bit counts");
+static_assert(WideShape<uint64_t, true>::T < 32768, "agg16 holds 15-bit counts");
 
 uint32_t binning_tile_keys(int key_bytes, bool pairs, const BinningConfig& cfg)
 {
-    if (key_bytes == 2) return pairs ? wide_tile<uint16_t, true>() : wide_tile<uint16_t, false>();  // (the wide kernel only)
-    if (cfg.variant == kVariantPersistent && !pairs)
-        return key_bytes == 8 ? RingGeom<uint64_t>::K * RingGeom<uint64_t>::WARPS * 32 : RingGeom<uint32_t>::K * RingGeom<uint32_t>::WARPS * 32;
-    if (cfg.variant == kVariantWide) {
-        if (key_bytes == 8) return pairs ? wide_tile<uint64_t, true>() : wide_tile<uint64_t, false>();
-        return pairs ? (OSB_PAIRS16K ? kPairsK * kPairsWarps * 32 : WideGeom<uint32_t, true>::K * WideGeom<uint32_t, true>::WARPS * 32)
-                     : WideGeom<uint32_t, false>::K * WideGeom<uint32_t, false>::WARPS * 32;
-    }
-    if (key_bytes == 8) return TileGeom<uint64_t, false>::WARPS * 32 * TileGeom<uint64_t, false>::K;
-    if (pairs) return TileGeom<uint32_t, true>::WARPS * 32 * TileGeom<uint32_t, true>::K;
-    return TileGeom<uint32_t, false>::WARPS * 32 * TileGeom<uint32_t, false>::K;
+    uint32_t t = 0;
+    auto tile = [&](auto s) { t = decltype(s)::T; return cudaSuccess; };
+    // pairs in a variant without a pairs pass for these keys (variant 0, 64-bit keys): the tile of its keys pass
+    if (with_pass_shape(key_bytes, pairs, false, cfg.variant, tile) != cudaSuccess) with_pass_shape(key_bytes, false, false, cfg.variant, tile);
+    return t;
 }
 
-template <typename KeyT, bool PAIRS, int RANK_MODE>
-static cudaError_t set_tile_attr()
+bool binning_has_hot_twin(int key_bytes, bool pairs, bool indices, const BinningConfig& cfg)
 {
-    using G = TileGeom<KeyT, PAIRS>;
-    return cudaFuncSetAttribute(digit_binning_tile_kernel<KeyT, PAIRS, G::K, G::WARPS, RANK_MODE>,
-                                cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                static_cast<int>(tile_smem_bytes<KeyT, PAIRS>()));
-}
-
-static cudaError_t configure_segment_kernels();
-
-cudaError_t configure_kernels()
-{
-    cudaError_t e;
-    if ((e = cudaFuncSetAttribute(global_histogram_kernel<uint32_t>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                  static_cast<int>(hist_smem_bytes<uint32_t>()))) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(global_histogram_kernel<uint64_t>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                  static_cast<int>(hist_smem_bytes<uint64_t>()))) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(global_histogram_kernel<uint32_t, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                  static_cast<int>(hist_smem_bytes<uint32_t>()))) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(global_histogram_kernel<uint64_t, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                  static_cast<int>(hist_smem_bytes<uint64_t>()))) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(global_histogram_bits_kernel<uint32_t>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                  static_cast<int>(hist_smem_bytes<uint32_t>()))) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(global_histogram_bits_kernel<uint64_t>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                  static_cast<int>(hist_smem_bytes<uint64_t>()))) != cudaSuccess) return e;
-    if ((e = set_tile_attr<uint32_t, false, kRankAtomic>()) != cudaSuccess) return e;
-    if ((e = set_tile_attr<uint32_t, false, kRankBallot>()) != cudaSuccess) return e;
-    if ((e = set_tile_attr<uint32_t, true, kRankAtomic>()) != cudaSuccess) return e;
-    if ((e = set_tile_attr<uint32_t, true, kRankBallot>()) != cudaSuccess) return e;
-    if ((e = set_tile_attr<uint64_t, false, kRankAtomic>()) != cudaSuccess) return e;
-    if ((e = set_tile_attr<uint64_t, false, kRankBallot>()) != cudaSuccess) return e;
-    if ((e = set_ring_attr<uint32_t, kRankAtomic>()) != cudaSuccess) return e;
-    if ((e = set_ring_attr<uint32_t, kRankBallot>()) != cudaSuccess) return e;
-    if ((e = set_ring_attr<uint64_t, kRankAtomic>()) != cudaSuccess) return e;
-    if ((e = set_ring_attr<uint64_t, kRankBallot>()) != cudaSuccess) return e;
-    if ((e = set_wide_attr<uint32_t, false, kRankAtomic>()) != cudaSuccess) return e;
-    if ((e = set_wide_attr<uint32_t, false, kRankBallot>()) != cudaSuccess) return e;
-    if ((e = set_wide_attr<uint32_t, true, kRankAtomic>()) != cudaSuccess) return e;
-    if ((e = set_wide_attr<uint32_t, true, kRankBallot>()) != cudaSuccess) return e;
-    if ((e = set_wide_attr<uint64_t, false, kRankAtomic>()) != cudaSuccess) return e;
-    if ((e = set_wide_attr<uint64_t, false, kRankBallot>()) != cudaSuccess) return e;
-    if ((e = set_wide_attr<uint32_t, true, kRankAtomic, true>()) != cudaSuccess) return e;  // argsort
-    if ((e = set_wide_attr<uint32_t, true, kRankBallot, true>()) != cudaSuccess) return e;
-    // 16-bit keys: histogram, keys, pairs, argsort
-    if ((e = cudaFuncSetAttribute(global_histogram_kernel<uint16_t>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                  static_cast<int>(hist_smem_bytes<uint16_t>()))) != cudaSuccess) return e;
-    if ((e = set_wide_attr<uint16_t, false, kRankAtomic>()) != cudaSuccess) return e;
-    if ((e = set_wide_attr<uint16_t, false, kRankBallot>()) != cudaSuccess) return e;
-    if ((e = set_wide_attr<uint16_t, true, kRankAtomic>()) != cudaSuccess) return e;
-    if ((e = set_wide_attr<uint16_t, true, kRankBallot>()) != cudaSuccess) return e;
-    if ((e = set_wide_attr<uint16_t, true, kRankAtomic, true>()) != cudaSuccess) return e;
-    if ((e = set_wide_attr<uint16_t, true, kRankBallot, true>()) != cudaSuccess) return e;
-    // 64-bit keys with payloads: pairs, argsort
-    if ((e = set_wide_attr<uint64_t, true, kRankAtomic>()) != cudaSuccess) return e;
-    if ((e = set_wide_attr<uint64_t, true, kRankBallot>()) != cudaSuccess) return e;
-    if ((e = set_wide_attr<uint64_t, true, kRankAtomic, true>()) != cudaSuccess) return e;
-    if ((e = set_wide_attr<uint64_t, true, kRankBallot, true>()) != cudaSuccess) return e;
-    if ((e = set_pairs_attr<kRankAtomic>()) != cudaSuccess) return e;
-    if ((e = set_pairs_attr<kRankBallot>()) != cudaSuccess) return e;
-    return configure_segment_kernels();
+    bool hot = false;
+    with_pass_shape(key_bytes, pairs, indices, cfg.variant, [&](auto s) { hot = decltype(s)::has_hot; return cudaSuccess; });
+    return hot;
 }
 
 cudaError_t launch_digit_binning(const void* in, void* out, const uint32_t* in_val, uint32_t* out_val, uint64_t n,
@@ -1956,63 +1949,20 @@ cudaError_t launch_digit_binning(const void* in, void* out, const uint32_t* in_v
                                  cudaStream_t stream)
 {
     const bool pairs = in_val != nullptr;
-    const bool ballot = cfg.rank_mode == kRankBallot;
     if (cfg.variant != kVariantWide && (cfg.codec.flags || cfg.plan != nullptr || cfg.debug_stall_every || cfg.argsort_in))
         return cudaErrorNotSupported;
     if (cfg.digit_bits < 1 || cfg.digit_bits > 8) return cudaErrorInvalidValue;
     // variants 0 and 1 always take 8-bit digits: a narrower digit is only correct for them when the bits above it do not exist
     if (cfg.variant != kVariantWide && cfg.digit_bits != 8 && shift + cfg.digit_bits != static_cast<uint32_t>(key_bytes) * 8u)
         return cudaErrorNotSupported;
-    if (cfg.variant == kVariantWide) {
-#define OSB_WIDE(KEYT, PAIRS)                                                                                          \
-    (ballot ? launch_wide_variant<KEYT, PAIRS, kRankBallot>(in, out, in_val, out_val, n, shift, gbase_place, agg16, desc, \
-                                                           ticket, epoch, cfg, stream)                                 \
-            : launch_wide_variant<KEYT, PAIRS, kRankAtomic>(in, out, in_val, out_val, n, shift, gbase_place, agg16, desc, \
-                                                           ticket, epoch, cfg, stream))
-        if (cfg.argsort_in != nullptr) {  // argsort: the first executed pass reads argsort_in and makes the indices
-            if (!pairs || cfg.plan == nullptr) return cudaErrorInvalidValue;
-            if (key_bytes == 2)
-                return ballot ? launch_wide_variant<uint16_t, true, kRankBallot, true>(in, out, in_val, out_val, n, shift, gbase_place,
-                                                                                      agg16, desc, ticket, epoch, cfg, stream)
-                              : launch_wide_variant<uint16_t, true, kRankAtomic, true>(in, out, in_val, out_val, n, shift, gbase_place,
-                                                                                      agg16, desc, ticket, epoch, cfg, stream);
-            if (key_bytes == 8)
-                return ballot ? launch_wide_variant<uint64_t, true, kRankBallot, true>(in, out, in_val, out_val, n, shift, gbase_place,
-                                                                                      agg16, desc, ticket, epoch, cfg, stream)
-                              : launch_wide_variant<uint64_t, true, kRankAtomic, true>(in, out, in_val, out_val, n, shift, gbase_place,
-                                                                                      agg16, desc, ticket, epoch, cfg, stream);
-            if (key_bytes != 4) return cudaErrorInvalidValue;
-            return ballot ? launch_wide_variant<uint32_t, true, kRankBallot, true>(in, out, in_val, out_val, n, shift, gbase_place, agg16,
-                                                                                  desc, ticket, epoch, cfg, stream)
-                          : launch_wide_variant<uint32_t, true, kRankAtomic, true>(in, out, in_val, out_val, n, shift, gbase_place, agg16,
-                                                                                  desc, ticket, epoch, cfg, stream);
-        }
-        if (key_bytes == 2) return pairs ? OSB_WIDE(uint16_t, true) : OSB_WIDE(uint16_t, false);
-        if (key_bytes == 4 && pairs && OSB_PAIRS16K)
-            return ballot ? launch_pairs_variant<kRankBallot>(in, out, in_val, out_val, n, shift, gbase_place, agg16, desc, ticket, epoch, cfg, stream)
-                          : launch_pairs_variant<kRankAtomic>(in, out, in_val, out_val, n, shift, gbase_place, agg16, desc, ticket, epoch, cfg, stream);
-        if (key_bytes == 4) return pairs ? OSB_WIDE(uint32_t, true) : OSB_WIDE(uint32_t, false);
-        if (key_bytes == 8) return pairs ? OSB_WIDE(uint64_t, true) : OSB_WIDE(uint64_t, false);
-#undef OSB_WIDE
-        return cudaErrorInvalidValue;
-    }
-    if (cfg.variant == kVariantPersistent && !pairs) {
-        if (key_bytes == 4)
-            return ballot ? launch_ring_variant<uint32_t, kRankBallot>(in, out, n, shift, gbase_place, agg16, desc, ticket, epoch, cfg.sm_count, stream)
-                          : launch_ring_variant<uint32_t, kRankAtomic>(in, out, n, shift, gbase_place, agg16, desc, ticket, epoch, cfg.sm_count, stream);
-        if (key_bytes == 8)
-            return ballot ? launch_ring_variant<uint64_t, kRankBallot>(in, out, n, shift, gbase_place, agg16, desc, ticket, epoch, cfg.sm_count, stream)
-                          : launch_ring_variant<uint64_t, kRankAtomic>(in, out, n, shift, gbase_place, agg16, desc, ticket, epoch, cfg.sm_count, stream);
-    }
-#define OSB_DISPATCH(KEYT, PAIRS)                                                                                   \
-    (ballot ? launch_tile_variant<KEYT, PAIRS, kRankBallot>(in, out, in_val, out_val, n, shift, gbase_place, desc,  \
-                                                           ticket, epoch, stream)                                   \
-            : launch_tile_variant<KEYT, PAIRS, kRankAtomic>(in, out, in_val, out_val, n, shift, gbase_place, desc,  \
-                                                           ticket, epoch, stream))
-    if (key_bytes == 4) return pairs ? OSB_DISPATCH(uint32_t, true) : OSB_DISPATCH(uint32_t, false);
-    if (key_bytes == 8 && !pairs) return OSB_DISPATCH(uint64_t, false);
-#undef OSB_DISPATCH
-    return cudaErrorInvalidValue;
+    // argsort: the first executed pass reads argsort_in and makes the indices
+    const bool indices = cfg.argsort_in != nullptr;
+    if (indices && (!pairs || cfg.plan == nullptr)) return cudaErrorInvalidValue;
+    const PassArgs a{in, out, in_val, out_val, n, shift, gbase_place, desc, agg16, ticket, epoch, cfg, stream};
+    return with_rank_mode(cfg.rank_mode, [&](auto r) {
+        return with_pass_shape(key_bytes, pairs, indices, cfg.variant,
+                               [&](auto s) { return decltype(s)::template launch<decltype(r)::value>(a); });
+    });
 }
 
 // =====================================================================================================
@@ -2152,84 +2102,63 @@ template <> struct SegGeomN<uint64_t, 2> { static constexpr int K = 16, WARPS = 
 // 16-bit keys: the small-n path of their sorts (one segment of up to 16,384 keys) and the row sort; no segmented sort
 template <> struct SegGeomN<uint16_t, 1> { static constexpr int K = 8,  WARPS = 8; };   //  2,048 keys (row sort only)
 template <> struct SegGeomN<uint16_t, 2> { static constexpr int K = 32, WARPS = 16; };  // 16,384 keys, 512 threads
-template <typename KeyT, int SIZE> constexpr uint32_t seg_cap() { return SegGeomN<KeyT, SIZE>::K * SegGeomN<KeyT, SIZE>::WARPS * 32; }
-
-uint32_t segment_sort_capacity(int key_bytes, bool small)
-{
-    if (key_bytes == 2) return seg_cap<uint16_t, 2>();
-    if (key_bytes == 8) return small ? seg_cap<uint64_t, 1>() : seg_cap<uint64_t, 2>();
-    return small ? seg_cap<uint32_t, 1>() : seg_cap<uint32_t, 2>();
-}
-
-template <typename KeyT, bool PAIRS, int SIZE, int RANK_MODE, bool INDICES = false, bool ROWS = false>
-static cudaError_t seg_attr()
-{
-    using G = SegGeomN<KeyT, SIZE>;
-    return cudaFuncSetAttribute(segment_sort_kernel<KeyT, PAIRS, G::K, G::WARPS, RANK_MODE, INDICES, ROWS>,
-                                cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                static_cast<int>(sizeof(SegSmem<KeyT, PAIRS, G::K, G::WARPS>)));
-}
-static cudaError_t configure_segment_kernels()
-{
-    cudaError_t e;
-#define OSB_SEG_ATTR(KEYT, PAIRS)                                                                          \
-    if ((e = seg_attr<KEYT, PAIRS, 0, kRankAtomic>()) != cudaSuccess) return e;                             \
-    if ((e = seg_attr<KEYT, PAIRS, 0, kRankBallot>()) != cudaSuccess) return e;                             \
-    if ((e = seg_attr<KEYT, PAIRS, 1, kRankAtomic>()) != cudaSuccess) return e;                             \
-    if ((e = seg_attr<KEYT, PAIRS, 1, kRankBallot>()) != cudaSuccess) return e;                             \
-    if ((e = seg_attr<KEYT, PAIRS, 2, kRankAtomic>()) != cudaSuccess) return e;                             \
-    if ((e = seg_attr<KEYT, PAIRS, 2, kRankBallot>()) != cudaSuccess) return e;
-    OSB_SEG_ATTR(uint32_t, false)
-    OSB_SEG_ATTR(uint32_t, true)
-    OSB_SEG_ATTR(uint64_t, false)
-#undef OSB_SEG_ATTR
-    // argsort: the single segment of a sort of at most one tile
-    if ((e = seg_attr<uint32_t, true, 2, kRankAtomic, true>()) != cudaSuccess) return e;
-    if ((e = seg_attr<uint32_t, true, 2, kRankBallot, true>()) != cudaSuccess) return e;
-    // 16-bit keys: the single segment of a sort of at most one tile -- keys, pairs, argsort
-    if ((e = seg_attr<uint16_t, false, 2, kRankAtomic>()) != cudaSuccess) return e;
-    if ((e = seg_attr<uint16_t, false, 2, kRankBallot>()) != cudaSuccess) return e;
-    if ((e = seg_attr<uint16_t, true, 2, kRankAtomic>()) != cudaSuccess) return e;
-    if ((e = seg_attr<uint16_t, true, 2, kRankBallot>()) != cudaSuccess) return e;
-    if ((e = seg_attr<uint16_t, true, 2, kRankAtomic, true>()) != cudaSuccess) return e;
-    if ((e = seg_attr<uint16_t, true, 2, kRankBallot, true>()) != cudaSuccess) return e;
-    // 64-bit keys with payloads: the single segment of a sort of at most one tile -- pairs, argsort
-    if ((e = seg_attr<uint64_t, true, 2, kRankAtomic>()) != cudaSuccess) return e;
-    if ((e = seg_attr<uint64_t, true, 2, kRankBallot>()) != cudaSuccess) return e;
-    if ((e = seg_attr<uint64_t, true, 2, kRankAtomic, true>()) != cudaSuccess) return e;
-    if ((e = seg_attr<uint64_t, true, 2, kRankBallot, true>()) != cudaSuccess) return e;
-    // row sort (launch_row_sort): geometries 1 and 2 of every key width, keys only and with indices
-#define OSB_ROW_ATTR_SIZE(KEYT, SIZE)                                                                      \
-    if ((e = seg_attr<KEYT, false, SIZE, kRankAtomic, false, true>()) != cudaSuccess) return e;            \
-    if ((e = seg_attr<KEYT, false, SIZE, kRankBallot, false, true>()) != cudaSuccess) return e;            \
-    if ((e = seg_attr<KEYT, true, SIZE, kRankAtomic, true, true>()) != cudaSuccess) return e;              \
-    if ((e = seg_attr<KEYT, true, SIZE, kRankBallot, true, true>()) != cudaSuccess) return e;
-#define OSB_ROW_ATTR(KEYT) OSB_ROW_ATTR_SIZE(KEYT, 1) OSB_ROW_ATTR_SIZE(KEYT, 2)
-    OSB_ROW_ATTR(uint16_t)
-    OSB_ROW_ATTR(uint32_t)
-    OSB_ROW_ATTR(uint64_t)
-#undef OSB_ROW_ATTR
-#undef OSB_ROW_ATTR_SIZE
-    return cudaSuccess;
-}
-
 template <typename KeyT, bool PAIRS, int SIZE, bool INDICES = false, bool ROWS = false>
-static cudaError_t launch_seg(void* keys, uint32_t* vals, const unsigned long long* seg_off, uint64_t num_segments, uint64_t single_n,
-                              uint32_t max_len, uint32_t begin_bit, uint32_t places, uint32_t last_bits, const KeyCodec& codec,
-                              int rank_mode, int sm_count, cudaStream_t stream, const void* keys_in = nullptr)
-{
+struct SegShape {
+    using Key = KeyT;
+    static constexpr bool pairs = PAIRS, indices = INDICES, rows = ROWS, has_hot = false;
     using G = SegGeomN<KeyT, SIZE>;
     using S = SegSmem<KeyT, PAIRS, G::K, G::WARPS>;
-    const uint64_t cap = static_cast<uint64_t>(sm_count) * (SIZE == 2 ? 2 : 8);
+    static constexpr uint32_t T = S::T;  // the longest segment it sorts
+    static constexpr size_t smem = sizeof(S);
+    static constexpr int ctas_per_sm = SIZE == 2 ? 2 : 8;
+    template <int RANK_MODE, bool HOT = false>
+    static auto kernel() { return segment_sort_kernel<KeyT, PAIRS, G::K, G::WARPS, RANK_MODE, INDICES, ROWS>; }
+};
+template <typename KeyT, int SIZE, bool INDICES> using RowShape = SegShape<KeyT, INDICES, SIZE, INDICES, true>;
+
+// Each kind of sort lists its geometries smallest first: the launchers take the first one that holds the longest segment.
+using SegShapes = TypeList<
+    // segmented sort and small path: 32-bit keys and pairs, 64-bit keys
+    SegShape<uint32_t, false, 0>, SegShape<uint32_t, false, 1>, SegShape<uint32_t, false, 2>,
+    SegShape<uint32_t, true, 0>, SegShape<uint32_t, true, 1>, SegShape<uint32_t, true, 2>,
+    SegShape<uint64_t, false, 0>, SegShape<uint64_t, false, 1>, SegShape<uint64_t, false, 2>,
+    // small path only (the single segment of a sort of at most one tile): 16-bit keys and pairs, 64-bit pairs, every argsort
+    SegShape<uint16_t, false, 2>, SegShape<uint16_t, true, 2>, SegShape<uint64_t, true, 2>,
+    SegShape<uint16_t, true, 2, true>, SegShape<uint32_t, true, 2, true>, SegShape<uint64_t, true, 2, true>,
+    // row sort, block path: keys only and with indices
+    RowShape<uint16_t, 1, false>, RowShape<uint16_t, 2, false>, RowShape<uint16_t, 1, true>, RowShape<uint16_t, 2, true>,
+    RowShape<uint32_t, 1, false>, RowShape<uint32_t, 2, false>, RowShape<uint32_t, 1, true>, RowShape<uint32_t, 2, true>,
+    RowShape<uint64_t, 1, false>, RowShape<uint64_t, 2, false>, RowShape<uint64_t, 1, true>, RowShape<uint64_t, 2, true>>;
+
+// the longest segment (ROWS: row) of key_bytes-wide keys that a shape of the list sorts; 0 if there is none
+template <bool ROWS>
+static uint32_t seg_capacity(int key_bytes)
+{
+    uint32_t cap = 0;
+    for_each_type(SegShapes{}, [&](auto s) {
+        using S = decltype(s);
+        if (S::rows == ROWS && key_bytes == static_cast<int>(sizeof(typename S::Key)) && S::T > cap) cap = S::T;
+        return cudaSuccess;
+    });
+    return cap;
+}
+
+uint32_t segment_sort_capacity(int key_bytes) { return seg_capacity<false>(key_bytes); }
+
+template <typename Shape>
+static cudaError_t launch_seg(Shape, void* keys, uint32_t* vals, const unsigned long long* seg_off, uint64_t num_segments,
+                              uint64_t single_n, uint32_t max_len, uint32_t begin_bit, uint32_t places, uint32_t last_bits,
+                              const KeyCodec& codec, int rank_mode, int sm_count, cudaStream_t stream, const void* keys_in)
+{
+    using KeyT = typename Shape::Key;
+    const uint64_t cap = static_cast<uint64_t>(sm_count) * Shape::ctas_per_sm;
     const unsigned grid = static_cast<unsigned>(num_segments < cap ? num_segments : cap);
-    const KeyT* in = static_cast<const KeyT*>(keys_in);
-    if (rank_mode == kRankBallot)
-        segment_sort_kernel<KeyT, PAIRS, G::K, G::WARPS, kRankBallot, INDICES, ROWS><<<grid, S::THREADS, sizeof(S), stream>>>(
-            static_cast<KeyT*>(keys), vals, seg_off, num_segments, single_n, max_len, begin_bit, places, last_bits, codec, in);
-    else
-        segment_sort_kernel<KeyT, PAIRS, G::K, G::WARPS, kRankAtomic, INDICES, ROWS><<<grid, S::THREADS, sizeof(S), stream>>>(
-            static_cast<KeyT*>(keys), vals, seg_off, num_segments, single_n, max_len, begin_bit, places, last_bits, codec, in);
-    return cudaGetLastError();
+    return with_rank_mode(rank_mode, [&](auto r) {
+        const auto kern = Shape::template kernel<decltype(r)::value>();
+        kern<<<grid, Shape::S::THREADS, Shape::smem, stream>>>(static_cast<KeyT*>(keys), vals, seg_off, num_segments, single_n, max_len,
+                                                              begin_bit, places, last_bits, codec, static_cast<const KeyT*>(keys_in));
+        return cudaGetLastError();
+    });
 }
 
 cudaError_t launch_segment_sort(void* keys, uint32_t* vals, int key_bytes, const unsigned long long* seg_off, uint64_t num_segments,
@@ -2237,43 +2166,21 @@ cudaError_t launch_segment_sort(void* keys, uint32_t* vals, int key_bytes, const
                                 const KeyCodec* codec_in, int rank_mode, int sm_count, cudaStream_t stream, const void* keys_in)
 {
     if (num_segments == 0) return cudaSuccess;
+    const bool pairs = vals != nullptr, indices = keys_in != nullptr;
+    // argsort, 16-bit keys and 64-bit pairs: only the single segment of a small sort
+    if ((indices || key_bytes == 2 || (key_bytes == 8 && pairs)) && (seg_off || num_segments != 1)) return cudaErrorInvalidValue;
     const KeyCodec codec = codec_in ? *codec_in : KeyCodec();
-    if (keys_in != nullptr) {  // argsort: one segment of up to a tile, in the largest geometry (the only one instantiated for it)
-        if (!vals || seg_off || num_segments != 1 || max_len > segment_sort_capacity(key_bytes, false))
-            return cudaErrorInvalidValue;
-        if (key_bytes == 2)
-            return launch_seg<uint16_t, true, 2, true>(keys, vals, nullptr, 1, single_n, max_len, begin_bit, places, last_bits, codec,
-                                                       rank_mode, sm_count, stream, keys_in);
-        if (key_bytes == 8)
-            return launch_seg<uint64_t, true, 2, true>(keys, vals, nullptr, 1, single_n, max_len, begin_bit, places, last_bits, codec,
-                                                       rank_mode, sm_count, stream, keys_in);
-        if (key_bytes != 4) return cudaErrorInvalidValue;
-        return launch_seg<uint32_t, true, 2, true>(keys, vals, nullptr, 1, single_n, max_len, begin_bit, places, last_bits, codec,
-                                                   rank_mode, sm_count, stream, keys_in);
-    }
-    if (key_bytes == 2) {  // 16-bit keys: the single segment of a small sort, in the 16,384-key geometry
-        if (seg_off || num_segments != 1 || max_len > seg_cap<uint16_t, 2>()) return cudaErrorInvalidValue;
-        return vals ? launch_seg<uint16_t, true, 2>(keys, vals, nullptr, 1, single_n, max_len, begin_bit, places, last_bits, codec,
-                                                    rank_mode, sm_count, stream)
-                    : launch_seg<uint16_t, false, 2>(keys, vals, nullptr, 1, single_n, max_len, begin_bit, places, last_bits, codec,
-                                                     rank_mode, sm_count, stream);
-    }
-    if (key_bytes == 8 && vals) {  // 64-bit pairs: the single segment of a small sort, in the 8,192-key geometry
-        if (seg_off || num_segments != 1 || max_len > seg_cap<uint64_t, 2>()) return cudaErrorInvalidValue;
-        return launch_seg<uint64_t, true, 2>(keys, vals, nullptr, 1, single_n, max_len, begin_bit, places, last_bits, codec,
-                                             rank_mode, sm_count, stream);
-    }
-    const int size = max_len <= (key_bytes == 8 ? seg_cap<uint64_t, 0>() : seg_cap<uint32_t, 0>()) ? 0
-                     : max_len <= segment_sort_capacity(key_bytes, true) ? 1 : 2;
-    if (max_len > segment_sort_capacity(key_bytes, false)) return cudaErrorInvalidValue;
-#define OSB_SEG_ARGS keys, vals, seg_off, num_segments, single_n, max_len, begin_bit, places, last_bits, codec, rank_mode, sm_count, stream
-#define OSB_SEG(KEYT, PAIRS) \
-    (size == 0 ? launch_seg<KEYT, PAIRS, 0>(OSB_SEG_ARGS) : size == 1 ? launch_seg<KEYT, PAIRS, 1>(OSB_SEG_ARGS) : launch_seg<KEYT, PAIRS, 2>(OSB_SEG_ARGS))
-    if (key_bytes == 4) return vals ? OSB_SEG(uint32_t, true) : OSB_SEG(uint32_t, false);
-    if (key_bytes == 8 && !vals) return OSB_SEG(uint64_t, false);
-#undef OSB_SEG_ARGS
-#undef OSB_SEG
-    return cudaErrorInvalidValue;
+    return find_type(
+        SegShapes{},
+        [&](auto s) {
+            using S = decltype(s);
+            return !S::rows && key_bytes == static_cast<int>(sizeof(typename S::Key)) && S::pairs == pairs && S::indices == indices &&
+                   max_len <= S::T;
+        },
+        [&](auto s) {
+            return launch_seg(s, keys, vals, seg_off, num_segments, single_n, max_len, begin_bit, places, last_bits, codec, rank_mode,
+                              sm_count, stream, keys_in);
+        });
 }
 
 // =====================================================================================================
@@ -2409,28 +2316,7 @@ static cudaError_t launch_row_warp_k(const void* in, void* out, uint32_t* idx, u
     return launch_row_warp<KeyT, 8, RANK_MODE, INDICES>(in, out, idx, num_rows, row_len, codec, sm_count, stream);
 }
 
-template <typename KeyT>
-static cudaError_t launch_rows(const void* keys_in, void* keys_out, uint32_t* indices, uint64_t num_rows, uint32_t row_len,
-                               const KeyCodec& codec, int rank_mode, bool block_only, int sm_count, cudaStream_t stream)
-{
-    if (row_len <= kRowWarpMaxLen && !block_only) {
-        if (rank_mode == kRankBallot)
-            return indices ? launch_row_warp_k<KeyT, kRankBallot, true>(keys_in, keys_out, indices, num_rows, row_len, codec, sm_count, stream)
-                           : launch_row_warp_k<KeyT, kRankBallot, false>(keys_in, keys_out, indices, num_rows, row_len, codec, sm_count, stream);
-        return indices ? launch_row_warp_k<KeyT, kRankAtomic, true>(keys_in, keys_out, indices, num_rows, row_len, codec, sm_count, stream)
-                       : launch_row_warp_k<KeyT, kRankAtomic, false>(keys_in, keys_out, indices, num_rows, row_len, codec, sm_count, stream);
-    }
-    // block path: segment s of segment_sort_kernel is row s
-    const bool small = row_len <= seg_cap<KeyT, 1>();
-#define OSB_ROW_ARGS keys_out, indices, nullptr, num_rows, row_len, row_len, 0u, static_cast<uint32_t>(sizeof(KeyT)), 8u, codec, \
-                     rank_mode, sm_count, stream, keys_in
-    if (indices)
-        return small ? launch_seg<KeyT, true, 1, true, true>(OSB_ROW_ARGS) : launch_seg<KeyT, true, 2, true, true>(OSB_ROW_ARGS);
-    return small ? launch_seg<KeyT, false, 1, false, true>(OSB_ROW_ARGS) : launch_seg<KeyT, false, 2, false, true>(OSB_ROW_ARGS);
-#undef OSB_ROW_ARGS
-}
-
-uint32_t row_sort_capacity(int key_bytes) { return key_bytes == 8 ? seg_cap<uint64_t, 2>() : seg_cap<uint32_t, 2>(); }
+uint32_t row_sort_capacity(int key_bytes) { return seg_capacity<true>(key_bytes); }
 
 cudaError_t launch_row_sort(const void* keys_in, void* keys_out, uint32_t* indices, uint64_t num_rows, uint32_t row_len,
                             int key_bytes, const KeyCodec* codec_in, int rank_mode, bool block_only, int sm_count,
@@ -2439,13 +2325,48 @@ cudaError_t launch_row_sort(const void* keys_in, void* keys_out, uint32_t* indic
     if (num_rows == 0 || row_len == 0) return cudaSuccess;
     if (row_len > row_sort_capacity(key_bytes)) return cudaErrorInvalidValue;
     const KeyCodec codec = codec_in ? *codec_in : KeyCodec();
-    switch (key_bytes) {
-        case 2: return launch_rows<uint16_t>(keys_in, keys_out, indices, num_rows, row_len, codec, rank_mode, block_only, sm_count, stream);
-        case 4: return launch_rows<uint32_t>(keys_in, keys_out, indices, num_rows, row_len, codec, rank_mode, block_only, sm_count, stream);
-        case 8: return launch_rows<uint64_t>(keys_in, keys_out, indices, num_rows, row_len, codec, rank_mode, block_only, sm_count, stream);
-        default: return cudaErrorInvalidValue;
+    if (row_len <= kRowWarpMaxLen && !block_only) {
+        return with_key_type(TypeList<uint16_t, uint32_t, uint64_t>{}, key_bytes, [&](auto k) {
+            return with_rank_mode(rank_mode, [&](auto r) {
+                using KeyT = decltype(k);
+                constexpr int R = decltype(r)::value;
+                return indices ? launch_row_warp_k<KeyT, R, true>(keys_in, keys_out, indices, num_rows, row_len, codec, sm_count, stream)
+                               : launch_row_warp_k<KeyT, R, false>(keys_in, keys_out, indices, num_rows, row_len, codec, sm_count, stream);
+            });
+        });
     }
+    // block path: segment s of segment_sort_kernel is row s
+    return find_type(
+        SegShapes{},
+        [&](auto s) {
+            using S = decltype(s);
+            return S::rows && key_bytes == static_cast<int>(sizeof(typename S::Key)) && S::indices == (indices != nullptr) && row_len <= S::T;
+        },
+        [&](auto s) {
+            return launch_seg(s, keys_out, indices, nullptr, num_rows, row_len, row_len, 0u, static_cast<uint32_t>(key_bytes), 8u, codec,
+                              rank_mode, sm_count, stream, keys_in);
+        });
 }
+
+cudaError_t configure_kernels()
+{
+    cudaError_t e = for_each_type(HistKeys{}, [](auto k) {
+        using KeyT = decltype(k);
+        return set_smem(global_histogram_kernel<KeyT>, hist_smem_bytes<KeyT>());
+    });
+    if (e == cudaSuccess) e = for_each_type(HistBitsKeys{}, [](auto k) {
+        using KeyT = decltype(k);
+        const cudaError_t m = set_smem(global_histogram_kernel<KeyT, true>, hist_smem_bytes<KeyT>());
+        return m != cudaSuccess ? m : set_smem(global_histogram_bits_kernel<KeyT>, hist_smem_bytes<KeyT>());
+    });
+    auto shape = [](auto s) { return configure_shape(s); };
+    if (e == cudaSuccess) e = for_each_type(DefaultPassShapes{}, shape);
+    if (e == cudaSuccess) e = for_each_type(RingShapes{}, shape);
+    if (e == cudaSuccess) e = for_each_type(TileShapes{}, shape);
+    if (e == cudaSuccess) e = for_each_type(SegShapes{}, shape);
+    return e;
+}
+
 
 // =====================================================================================================
 // Validate: adjacent-inversion count (reference: UtilityKernels.cuh:403-429)
@@ -2465,10 +2386,11 @@ validate_kernel(const KeyT* __restrict__ keys, uint64_t n, unsigned long long* e
 cudaError_t launch_validate(const void* keys, uint64_t n, int key_bytes, unsigned long long* err_count, int sm_count,
                             cudaStream_t stream)
 {
-    const unsigned grid = static_cast<unsigned>(sm_count) * 8;
-    if (key_bytes == 4) validate_kernel<uint32_t><<<grid, 256, 0, stream>>>(static_cast<const uint32_t*>(keys), n, err_count);
-    else validate_kernel<uint64_t><<<grid, 256, 0, stream>>>(static_cast<const uint64_t*>(keys), n, err_count);
-    return cudaGetLastError();
+    return with_key_type(TypeList<uint32_t, uint64_t>{}, key_bytes, [&](auto k) {
+        using KeyT = decltype(k);
+        validate_kernel<KeyT><<<static_cast<unsigned>(sm_count) * 8, 256, 0, stream>>>(static_cast<const KeyT*>(keys), n, err_count);
+        return cudaGetLastError();
+    });
 }
 
 // =====================================================================================================

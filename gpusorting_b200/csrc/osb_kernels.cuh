@@ -38,6 +38,8 @@ struct BinningConfig {
 
 // keys per partition tile for a key width / pairs flag / variant (host needs it to size descriptors)
 uint32_t binning_tile_keys(int key_bytes, bool pairs, const BinningConfig& cfg);
+// whether the pass that runs these keys in cfg.variant has a HOT instantiation (BinningConfig::hot_passes)
+bool binning_has_hot_twin(int key_bytes, bool pairs, bool indices, const BinningConfig& cfg);
 
 // One-time per-process kernel attribute setup (dynamic shared memory opt-in). Returns cudaError_t.
 cudaError_t configure_kernels();
@@ -89,7 +91,7 @@ cudaError_t launch_digit_binning(const void* in, void* out, const uint32_t* in_v
 // payloads are the keys' input positions, and the sorted keys and indices are stored to keys / vals.
 // key_bytes 2 (16-bit keys), and key_bytes 8 with vals: only the single segment of a sort (seg_off null), up to 16,384 keys
 // (8,192 for 64-bit keys).
-uint32_t segment_sort_capacity(int key_bytes, bool small);
+uint32_t segment_sort_capacity(int key_bytes);
 cudaError_t launch_segment_sort(void* keys, uint32_t* vals, int key_bytes, const unsigned long long* seg_off, uint64_t num_segments,
                                 uint64_t single_n, uint32_t max_len, uint32_t begin_bit, uint32_t places, uint32_t last_bits,
                                 const KeyCodec* codec, int rank_mode, int sm_count, cudaStream_t stream,
