@@ -122,4 +122,23 @@ __device__ __forceinline__ bool plan_src_is_alt(const SortPlan& pl, uint32_t pla
     return __popc(~pl.skip_mask & ((1u << place) - 1u)) & 1u;
 }
 
+// ---- fused first pass (whole-key u32 keys-only sorts, DESIGN §4.12) ----------------------------------------------------
+// The first digit pass counts the global histogram itself and scatters digit d into a region of fixed capacity c(n) at
+// d * c(n) of the alt buffer, so it needs no digit bases and no GlobalHistogram in front of it.  SortPlan::skip_mask bit
+// kPlanFusedKept says its result stands; otherwise the classic GlobalHistogram, Scan and first pass run after it.
+constexpr uint32_t kPlanFusedKept = 1u << 24;
+// Region capacity: n/256 plus 1/32 of it plus 1,024 keys, in whole 128-byte lines (uniform keys: ~64 standard deviations of
+// slack at n = 2^30, ~18 at 2^20).
+__host__ __device__ constexpr uint64_t fused_region_keys(uint64_t n)
+{
+    const uint64_t q = (n + 255) / 256;
+    return (q + q / 32 + 1024 + 31) / 32 * 32;
+}
+// the first executed pass after place 0 of a fused sort reads the gapped layout the fused pass left
+__device__ __forceinline__ bool plan_reads_gapped(const SortPlan& pl, uint32_t place)
+{
+    const uint32_t later = ~pl.skip_mask & 0xfeu;
+    return (pl.skip_mask & kPlanFusedKept) && later && place == static_cast<uint32_t>(__ffs(later) - 1);
+}
+
 }  // namespace osb

@@ -63,8 +63,10 @@ struct osb200_sorter {
     bool small_path = true;      // n <= one tile: the single-CTA shared-memory sort (one launch)
     bool hot_passes = true;      // low-entropy digit places run in the HOT instantiation of the pass (decided on the device)
     bool debug_rows_block = false;  // test hook: osb200_sort_rows sorts rows of <= 256 keys on the block path, not the warp path
+    bool fused_histogram = true;    // whole-key u32 keys-only sorts of >= kFusedMinTiles tiles: the fused first pass (§4.12)
 
     void* alt_keys = nullptr;
+    uint64_t alt_key_slots = 0;        // keys (of key_bytes) the alt key buffer holds: max_n, or the fused regions' 256 c(max_n)
     uint32_t* alt_vals = nullptr;
     unsigned char* control = nullptr;  // ControlLayout
     uint64_t* desc = nullptr;          // [tiles][256] 64-bit descriptors (epoch-stamped, cleared only by captured sorts)
@@ -72,10 +74,15 @@ struct osb200_sorter {
     uint64_t desc_tiles = 0;
     uint32_t epoch = 0;
 
-    // optional per-kernel timing of the last sort (osb200_set_option "profile"): events on the launching stream
+    // optional per-kernel timing of the last sort (osb200_set_option "profile"): events on the launching stream, and the
+    // spans between them that make up each reported entry ([histogram, scan, pass 0, pass 1, ...])
     bool profile = false;
-    cudaEvent_t ev[kMaxPlaces + 3] = {};
+    static constexpr int kMaxEvents = kMaxPlaces + 6;
+    cudaEvent_t ev[kMaxEvents] = {};
     int ev_count = 0;
+    struct Span { int entry, from, to; };
+    Span spans[kMaxEvents] = {};
+    int span_count = 0;
 
     // lazily created staging for the host-buffer entry points
     void* stage_keys = nullptr;
@@ -98,6 +105,26 @@ struct osb200_sorter {
 namespace {
 
 uint64_t tiles_for(uint64_t n, uint32_t tile_keys) { return (n + tile_keys - 1) / tile_keys; }
+
+// Fused sorts (DESIGN §4.12): whole-key u32 keys-only sorts on the default pass of at least this many tiles, and below 2^32
+// keys (the fused pass counts in 32-bit words).  Smaller sorts keep the classic launch plan: there the saved read is a few
+// microseconds, and a region's slack is a large share of its keys.
+constexpr uint64_t kFusedMinTiles = 64;
+constexpr int kFusedTicket = 4, kFusedAbort = 5;  // control-block slots of the fused pass (a u32 sort uses tickets 0-3)
+
+bool fused_size(uint64_t n)
+{
+    osb::BinningConfig wide;
+    wide.variant = osb::kVariantWide;
+    return n < (1ull << 32) && tiles_for(n, osb::binning_tile_keys(4, false, wide)) >= kFusedMinTiles;
+}
+
+// keys the alt key buffer of a handle holds: max_n, or the fused pass's 256 regions when a u32 sort of max_n keys is fused
+uint64_t alt_key_slots_for(uint64_t max_n, int key_bytes)
+{
+    const uint64_t regions = key_bytes == 4 && fused_size(max_n) ? osb::kRadix * osb::fused_region_keys(max_n) : 0;
+    return regions > max_n ? regions : max_n;
+}
 // the compact reductions are stored in blocks of 8 tiles ([tile/8][digit][tile%8], see osb_kernels.cu agg_index)
 uint64_t agg_tiles_for(uint64_t n, uint32_t tile_keys) { return (tiles_for(n, tile_keys) + 7) / 8 * 8; }
 
@@ -194,42 +221,84 @@ int sort_impl(osb200_sorter* s, int key_bytes, void* d_keys, uint32_t* d_vals, u
     const uint64_t agg_stride = agg_tiles_for(n, tile_keys) * osb::kRadix;
     // reductions carry no epoch (16-bit words): they are cleared per sort, 512 B per tile and place (128 MiB at n = 2^30)
     if (compact) OSB_TRY(cudaMemsetAsync(s->agg16, 0, agg_stride * places * sizeof(uint16_t), stream));
+    // profile: events in stream order, and the spans between them that make up each entry of osb200_get_profile
     int ne = 0;
+    s->span_count = 0;
     auto mark = [&]() -> cudaError_t {
         if (!s->profile) return cudaSuccess;
         if (!s->ev[ne]) { cudaError_t e = cudaEventCreate(&s->ev[ne]); if (e != cudaSuccess) return e; }
         return cudaEventRecord(s->ev[ne++], stream);
     };
+    auto span = [&](int entry) -> cudaError_t {  // entry: the launches since the previous mark
+        if (s->profile) s->spans[s->span_count++] = {entry, ne - 1, ne};
+        return mark();
+    };
     s->ev_count = 0;
     OSB_TRY(mark());
     osb::KeyCodec enc;  // typed keys: the histogram and the first executed pass see encoded keys, the last one stores them decoded
     if (codec) { enc = *codec; enc.flags = osb::kCodecEncodeOnLoad; }
-    if (whole_key)
-        OSB_TRY(osb::launch_global_histogram(keys_in ? keys_in : d_keys, n, key_bytes, s->ghist(), s->sm_count, stream,
-                                             codec ? &enc : nullptr));
-    else
-        OSB_TRY(osb::launch_global_histogram_bits(d_keys, n, key_bytes, s->ghist(), s->sm_count, stream, codec ? &enc : nullptr,
-                                                  static_cast<uint32_t>(begin_bit), places, last_bits));
-    OSB_TRY(mark());
     // hot passes (low-entropy inputs): the default kernel has a second instantiation for them; both are enqueued per pass
     const bool hot_passes = use_plan && s->hot_passes && osb::binning_has_hot_twin(key_bytes, d_vals != nullptr, keys_in != nullptr, s->cfg);
-    OSB_TRY(osb::launch_scan(s->ghist(), s->gbase(), places, stream, use_plan ? s->plan() : nullptr, n, s->short_circuit, hot_passes));
-    OSB_TRY(mark());
+    // Fused sort (DESIGN §4.12): the first pass counts the global histogram and scatters into fixed regions of the alt
+    // buffer; the scan after it keeps that result or calls the fallback -- the classic histogram, scan and first pass,
+    // enqueued always and returning at once when the fused pass stands.
+    const uint64_t region = osb::fused_region_keys(n);
+    const bool fused = s->fused_histogram && use_plan && whole_key && key_bytes == 4 && !d_vals && !keys_in && fused_size(n) &&
+                       osb::kRadix * region <= s->alt_key_slots;
+    // (the fused pass runs on place 0's epoch: one epoch per digit place, as in the classic plan)
+    uint32_t fused_epoch = 0;
+    if (fused) {
+        st = next_epoch(s, stream, &fused_epoch);
+        if (st != OSB200_OK) return st;
+        const uint32_t epoch = fused_epoch;
+        osb::BinningConfig cfg = s->cfg;
+        if (codec) cfg.codec = enc;
+        unsigned long long* fallback_hist = s->ghist() + 4 * osb::kRadix;  // a 4-place sort's unused places 4-7
+        uint32_t* abort_word = s->tickets() + kFusedAbort;
+        uint32_t ctas = 0;
+        OSB_TRY(osb::launch_fused_first_pass(static_cast<const uint32_t*>(d_keys), static_cast<uint32_t*>(s->alt_keys), n, region,
+                                             s->ghist(), abort_word, s->desc, s->agg16, s->tickets() + kFusedTicket, epoch, cfg, stream,
+                                             &ctas));
+        OSB_TRY(span(2));
+        OSB_TRY(osb::launch_scan_fused(s->ghist(), s->gbase(), places, stream, s->plan(), n, s->short_circuit, hot_passes, false,
+                                       abort_word, region));
+        OSB_TRY(span(1));
+        OSB_TRY(osb::launch_fused_fallback_zero(s->plan(), s->tickets() + kFusedTicket, ctas, tiles_for(n, tile_keys), s->agg16, s->desc,
+                                                s->sm_count, stream));
+        OSB_TRY(osb::launch_global_histogram(d_keys, n, key_bytes, fallback_hist, s->sm_count, stream, codec ? &enc : nullptr, s->plan()));
+        OSB_TRY(span(0));
+        OSB_TRY(osb::launch_scan_fused(fallback_hist, s->gbase(), places, stream, s->plan(), n, s->short_circuit, hot_passes, true,
+                                       nullptr, 0));
+        OSB_TRY(span(1));
+    } else {
+        if (whole_key)
+            OSB_TRY(osb::launch_global_histogram(keys_in ? keys_in : d_keys, n, key_bytes, s->ghist(), s->sm_count, stream,
+                                                 codec ? &enc : nullptr));
+        else
+            OSB_TRY(osb::launch_global_histogram_bits(d_keys, n, key_bytes, s->ghist(), s->sm_count, stream, codec ? &enc : nullptr,
+                                                      static_cast<uint32_t>(begin_bit), places, last_bits));
+        OSB_TRY(span(0));
+        OSB_TRY(osb::launch_scan(s->ghist(), s->gbase(), places, stream, use_plan ? s->plan() : nullptr, n, s->short_circuit, hot_passes));
+        OSB_TRY(span(1));
+    }
 
     void* src = d_keys;
     void* dst = s->alt_keys;
     uint32_t* sv = d_vals;
     uint32_t* dv = d_vals ? s->alt_vals : nullptr;
     for (int p = 0; p < places; ++p) {
-        uint32_t epoch = 0;
-        st = next_epoch(s, stream, &epoch);
-        if (st != OSB200_OK) return st;
+        uint32_t epoch = fused_epoch;
+        if (!fused || p > 0) {
+            st = next_epoch(s, stream, &epoch);
+            if (st != OSB200_OK) return st;
+        }
         osb::BinningConfig cfg = s->cfg;
         cfg.digit_bits = p == places - 1 ? last_bits : 8u;
         cfg.place = static_cast<uint32_t>(p);
         if (use_plan) cfg.plan = s->plan();
         cfg.hot_passes = hot_passes;
         cfg.argsort_in = keys_in;
+        if (fused) { cfg.fused_region = region; cfg.fused_dense_base0 = s->gbase(); }
         if (codec) {
             cfg.codec = *codec;
             cfg.codec.flags = use_plan ? osb::kCodecFromPlan
@@ -240,7 +309,7 @@ int sort_impl(osb200_sorter* s, int key_bytes, void* d_keys, uint32_t* d_vals, u
                                           use_plan ? (d_vals ? s->alt_vals : nullptr) : dv, n, key_bytes,
                                           static_cast<uint32_t>(begin_bit + 8 * p), s->gbase() + p * osb::kRadix, s->desc,
                                           s->agg16 + p * agg_stride, s->tickets() + p, epoch, cfg, stream));
-        OSB_TRY(mark());
+        OSB_TRY(span(2 + p));
         void* t = src; src = dst; dst = t;
         uint32_t* tv = sv; sv = dv; dv = tv;
     }
@@ -351,7 +420,7 @@ uint64_t osb200_workspace_bytes(uint64_t max_n, int key_bytes, int value_bytes)
 {
     if ((key_bytes != 4 && key_bytes != 8) || (value_bytes != 0 && value_bytes != 4)) return 0;
     const uint64_t tiles = tiles_for(max_n ? max_n : 1, smallest_tile(key_bytes, value_bytes != 0));
-    return max_n * key_bytes + max_n * value_bytes + tiles * osb::kRadix * sizeof(uint64_t) +
+    return alt_key_slots_for(max_n, key_bytes) * key_bytes + max_n * value_bytes + tiles * osb::kRadix * sizeof(uint64_t) +
            (tiles + 8) * osb::kRadix * sizeof(uint16_t) * key_bytes + ControlLayout::total;
 }
 
@@ -385,7 +454,8 @@ int create_impl(osb200_handle* out, uint64_t max_n, int key_bytes, int value_byt
     if (e != cudaSuccess) { delete s; return cuda_status(e); }
 
     s->desc_tiles = tiles_for(max_n, smallest_tile(key_bytes, value_bytes != 0));
-    bool ok = cudaMalloc(&s->alt_keys, max_n * key_bytes) == cudaSuccess;
+    s->alt_key_slots = alt_key_slots_for(max_n, key_bytes);
+    bool ok = cudaMalloc(&s->alt_keys, s->alt_key_slots * key_bytes) == cudaSuccess;
     if (ok && value_bytes) ok = cudaMalloc(&s->alt_vals, max_n * sizeof(uint32_t)) == cudaSuccess;
     ok = ok && cudaMalloc(&s->control, ControlLayout::total) == cudaSuccess;
     ok = ok && cudaMalloc(&s->desc, s->desc_tiles * osb::kRadix * sizeof(uint64_t)) == cudaSuccess;
@@ -779,6 +849,7 @@ int osb200_set_option(osb200_handle h, const char* key, int64_t value)
     if (!std::strcmp(key, "short_circuit")) { h->short_circuit = value != 0; return OSB200_OK; }
     if (!std::strcmp(key, "small_path")) { h->small_path = value != 0; return OSB200_OK; }
     if (!std::strcmp(key, "hot_passes")) { h->hot_passes = value != 0; return OSB200_OK; }
+    if (!std::strcmp(key, "fused_histogram")) { h->fused_histogram = value != 0; return OSB200_OK; }
     if (!std::strcmp(key, "spin_cap")) {
         if (value < 1 || value > (1ll << 30)) return OSB200_ERR_INVALID_ARG;
         h->cfg.spin_cap = static_cast<uint32_t>(value);
@@ -814,7 +885,14 @@ int osb200_get_profile(osb200_handle h, float* out_ms, int capacity)
     if (h->ev_count < 2) return 0;
     OSB_TRY(cudaEventSynchronize(h->ev[h->ev_count - 1]));
     int k = 0;
-    for (int i = 0; i + 1 < h->ev_count && k < capacity; ++i, ++k) OSB_TRY(cudaEventElapsedTime(&out_ms[k], h->ev[i], h->ev[i + 1]));
+    for (int i = 0; i < h->span_count; ++i) {
+        const osb200_sorter::Span& sp = h->spans[i];
+        if (sp.entry >= capacity) continue;
+        for (; k <= sp.entry; ++k) out_ms[k] = 0.0f;
+        float ms = 0.0f;
+        OSB_TRY(cudaEventElapsedTime(&ms, h->ev[sp.from], h->ev[sp.to]));
+        out_ms[sp.entry] += ms;
+    }
     return k;
 }
 
@@ -831,6 +909,12 @@ int64_t osb200_get_info(osb200_handle h, const char* key)
     if (!std::strcmp(key, "short_circuit")) return h->short_circuit ? 1 : 0;
     if (!std::strcmp(key, "small_path")) return h->small_path ? 1 : 0;
     if (!std::strcmp(key, "hot_passes")) return h->hot_passes ? 1 : 0;
+    if (!std::strcmp(key, "fused_histogram")) return h->fused_histogram ? 1 : 0;
+    if (!std::strcmp(key, "last_fused_kept")) {  // 1: the last sort's fused first pass stood (0 also for a sort that was not fused)
+        osb::SortPlan pl;
+        if (cudaMemcpy(&pl, h->plan(), sizeof(pl), cudaMemcpyDeviceToHost) != cudaSuccess) return OSB200_ERR_CUDA;
+        return (pl.skip_mask & osb::kPlanFusedKept) ? 1 : 0;
+    }
     if (!std::strcmp(key, "last_hot_mask")) {
         osb::SortPlan pl;
         if (cudaMemcpy(&pl, h->plan(), sizeof(pl), cudaMemcpyDeviceToHost) != cudaSuccess) return -1;

@@ -156,8 +156,9 @@ __device__ __forceinline__ void hist_count_vec(uint32_t* s_col, const uint4& v, 
 template <typename KeyT, bool MASKED = false>
 __global__ void __launch_bounds__(kHistThreads, 1)
 global_histogram_kernel(const KeyT* __restrict__ keys, uint64_t n, unsigned long long* __restrict__ ghist, KeyCodec codec,
-                        int places = 0, uint32_t last_mask = 255u)
+                        int places = 0, uint32_t last_mask = 255u, const SortPlan* gate = nullptr)
 {
+    if (gate != nullptr && (gate->skip_mask & kPlanFusedKept)) return;  // fallback of a fused sort whose first pass stood
     constexpr int PLACES = sizeof(KeyT);
     constexpr int VEC = 16 / sizeof(KeyT);
     constexpr int COLS = HistGeom<KeyT>::COLS;
@@ -219,21 +220,48 @@ using HistBitsKeys = TypeList<uint32_t, uint64_t>;        // its MASKED form and
 
 template <typename KeyT, bool MASKED>
 static cudaError_t launch_histogram_vec(const void* keys, uint64_t n, unsigned long long* ghist, int sm_count, cudaStream_t stream,
-                                        const KeyCodec& codec, int places = 0, uint32_t last_mask = 255u)
+                                        const KeyCodec& codec, int places = 0, uint32_t last_mask = 255u,
+                                        const SortPlan* gate = nullptr)
 {
     const unsigned grid = capped_grid(n / (16 / sizeof(KeyT)), kHistThreads, sm_count);
     global_histogram_kernel<KeyT, MASKED><<<grid, kHistThreads, hist_smem_bytes<KeyT>(), stream>>>(
-        static_cast<const KeyT*>(keys), n, ghist, codec, places, last_mask);
+        static_cast<const KeyT*>(keys), n, ghist, codec, places, last_mask, gate);
     return cudaGetLastError();
 }
 
 cudaError_t launch_global_histogram(const void* keys, uint64_t n, int key_bytes, unsigned long long* ghist,
-                                    int sm_count, cudaStream_t stream, const KeyCodec* codec_in)
+                                    int sm_count, cudaStream_t stream, const KeyCodec* codec_in, const SortPlan* gate)
 {
     const KeyCodec codec = codec_in ? *codec_in : KeyCodec();
     return with_key_type(HistKeys{}, key_bytes, [&](auto k) {
-        return launch_histogram_vec<decltype(k), false>(keys, n, ghist, sm_count, stream, codec);
+        return launch_histogram_vec<decltype(k), false>(keys, n, ghist, sm_count, stream, codec, 0, 255u, gate);
     });
+}
+
+// The fallback of a fused sort clears what the fused pass left for place 0's classic pass, which runs on the same
+// reductions and the same epoch: place 0's reductions and the descriptors of the tiles it reached -- at most its first
+// CTAs' tiles and those drawn from its ticket (few when it stopped early).  Returns at once when the fused pass stood.
+__global__ void __launch_bounds__(512)
+fused_fallback_zero_kernel(const SortPlan* __restrict__ plan, const uint32_t* __restrict__ ticket, uint32_t ctas, uint64_t tiles,
+                           uint4* __restrict__ agg16, uint4* __restrict__ desc)
+{
+    if (plan->skip_mask & kPlanFusedKept) return;
+    uint64_t reached = static_cast<uint64_t>(ctas) + *ticket;
+    if (reached > tiles) reached = tiles;
+    const uint64_t agg_vecs = (reached + 7) / 8 * 8 * kRadix * sizeof(uint16_t) / 16;  // whole blocks of 8 tiles
+    const uint64_t desc_vecs = reached * kRadix * sizeof(uint64_t) / 16;
+    const uint64_t stride = static_cast<uint64_t>(gridDim.x) * blockDim.x;
+    for (uint64_t i = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < agg_vecs + desc_vecs; i += stride)
+        (i < agg_vecs ? agg16[i] : desc[i - agg_vecs]) = make_uint4(0, 0, 0, 0);
+}
+
+cudaError_t launch_fused_fallback_zero(const SortPlan* plan, const uint32_t* ticket, uint32_t ctas, uint64_t tiles, uint16_t* agg16,
+                                       uint64_t* desc, int sm_count, cudaStream_t stream)
+{
+    fused_fallback_zero_kernel<<<static_cast<unsigned>(sm_count) * 4, 512, 0, stream>>>(plan, ticket, ctas, tiles,
+                                                                                         reinterpret_cast<uint4*>(agg16),
+                                                                                         reinterpret_cast<uint4*>(desc));
+    return cudaGetLastError();
 }
 
 // Single digit place (the sharded path's most-significant-digit histogram): one atomic per key, same
@@ -284,13 +312,22 @@ cudaError_t launch_digit_histogram(const void* keys, uint64_t n, int key_bytes, 
 // number of executed passes before them, and a final copy moves the result home if that number is odd.
 // One CTA walks the (at most 8) places: the plan needs all of them.
 // =====================================================================================================
+// Fused sorts (DESIGN §4.12): kScanFused follows the fused first pass and adds kPlanFusedKept to the plan when that pass's
+// result stands; kScanFallback is the fallback's scan and returns at once when it does.
+enum ScanMode : int { kScanClassic = 0, kScanFused = 1, kScanFallback = 2 };
+
 __global__ void __launch_bounds__(kRadix)
 scan_kernel(const unsigned long long* __restrict__ ghist, unsigned long long* __restrict__ gbase, int places,
-            SortPlan* plan, unsigned long long n, int allow_skip, int allow_hot)
+            SortPlan* plan, unsigned long long n, int allow_skip, int allow_hot, int mode, const uint32_t* fused_abort,
+            unsigned long long region)
 {
     __shared__ unsigned long long s_warp[kRadix / 32];
+    if (mode == kScanFallback && (plan->skip_mask & kPlanFusedKept)) return;  // (read by all threads before any writes it)
     const int d = threadIdx.x, lane = d & 31, warp = d >> 5;
     uint32_t skip_mask = 0;
+    // fused: the first pass stood if no tile of it found a digit's region too small (it then scattered nothing) and no
+    // place-0 bin exceeds its region
+    const int overfull = mode == kScanFused ? __syncthreads_or(ghist[d] > region || *fused_abort != 0) : 0;
     for (int p = 0; p < places; ++p) {
         const unsigned long long c = ghist[p * kRadix + d];
         unsigned long long incl = c;
@@ -317,6 +354,10 @@ scan_kernel(const unsigned long long* __restrict__ ghist, unsigned long long* __
         pl.executed = __popc(run);
         pl.first_exec = run ? static_cast<uint32_t>(__ffs(run) - 1) : 0xffffffffu;
         pl.last_exec = run ? static_cast<uint32_t>(31 - __clz(run)) : 0xffffffffu;
+        // kept: place 0 ran in the plain pass (it cannot be skipped or hot and fit its regions, but say so) and a later
+        // place executes -- that pass reads the gapped layout and leaves it dense
+        if (mode == kScanFused && !overfull && (run & 1u) && !((skip_mask >> kPlanHotShift) & 1u) && (run & ~1u))
+            pl.skip_mask |= kPlanFusedKept;
         *plan = pl;
     }
 }
@@ -324,7 +365,17 @@ scan_kernel(const unsigned long long* __restrict__ ghist, unsigned long long* __
 cudaError_t launch_scan(const unsigned long long* ghist, unsigned long long* gbase, int places, cudaStream_t stream,
                         SortPlan* plan, uint64_t n, bool allow_skip, bool allow_hot)
 {
-    scan_kernel<<<1, kRadix, 0, stream>>>(ghist, gbase, places, plan, n, allow_skip ? 1 : 0, allow_hot ? 1 : 0);
+    scan_kernel<<<1, kRadix, 0, stream>>>(ghist, gbase, places, plan, n, allow_skip ? 1 : 0, allow_hot ? 1 : 0, kScanClassic,
+                                          nullptr, 0ull);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_scan_fused(const unsigned long long* ghist, unsigned long long* gbase, int places, cudaStream_t stream,
+                              SortPlan* plan, uint64_t n, bool allow_skip, bool allow_hot, bool fallback, const uint32_t* fused_abort,
+                              uint64_t region)
+{
+    scan_kernel<<<1, kRadix, 0, stream>>>(ghist, gbase, places, plan, n, allow_skip ? 1 : 0, allow_hot ? 1 : 0,
+                                          fallback ? kScanFallback : kScanFused, fused_abort, region);
     return cudaGetLastError();
 }
 
@@ -760,6 +811,33 @@ struct TileRereduce {
     KeyT ca, cb, cd;
 };
 
+// The stalled path's hook of lookback_wide (fused sorts, DESIGN §4.12): hook(-1) on every stalled poll -- kHookAbort stops
+// the lookback (a fused first pass that has aborted keeps nothing, and the stalled tile may never run); hook(t) when giving
+// up on tile t -- a count is the hook's own re-reduction of t (the gapped source), kHookDefault leaves it to rereduce_tile.
+// It reads what it needs where it is called, so that nothing of it is held in registers across the lookback.
+constexpr long long kHookAbort = -1, kHookDefault = -2;
+struct NoStallHook {
+    __device__ __forceinline__ long long operator()(long long) const { return kHookDefault; }
+};
+
+// rereduce_tile for the gapped source a fused sort's first pass leaves (DESIGN §4.12): logical position p of the input is
+// at p + (r * region - gap[r]) for the region r whose dense range holds p.  Cold path, like rereduce_tile.
+template <typename KeyT>
+__device__ __noinline__ uint32_t rereduce_tile_gapped(const KeyT* in, uint64_t base, uint32_t tile_keys, uint32_t shift, uint32_t mask,
+                                                      const unsigned long long* gap, unsigned long long region, uint16_t* dst,
+                                                      uint32_t d)
+{
+    uint32_t c = 0, r = 0;
+    for (uint32_t step = kRadix / 2; step; step >>= 1) if (gap[r + step] <= base) r += step;
+    for (uint32_t i = 0; i < tile_keys; ++i) {
+        const uint64_t p = base + i;
+        while (r + 1 < kRadix && gap[r + 1] <= p) ++r;
+        c += digit_of(in[p + r * region - gap[r]], shift, mask) == d;
+    }
+    st_relaxed_gpu_u16(dst, kAggReady | c);
+    return c;
+}
+
 // Forward-progress fallback (reference: EmulatedDeadlocking.cu:159-267, SweepCommon.hlsl:317-425 -- a thread block that
 // has spun too long on a predecessor's flag stops waiting and computes that tile's reduction itself).  Here every digit
 // thread that gives up on tile x counts ITS digit over the tile's keys (the whole warp reads the same key: one
@@ -805,10 +883,10 @@ __device__ __forceinline__ uint32_t agg_elem(const uint4& v, int t)
 // added by the caller, so descriptor values stay below n even when the bases are peer addresses in the sharded exchange
 // pass).  A predecessor whose reduction is still missing after spin_cap polls is re-reduced by this thread
 // (rereduce_tile): the spin is bounded.
-template <int NBLK, typename KeyT>
+template <int NBLK, typename KeyT, typename Hook = NoStallHook>
 __device__ __forceinline__ unsigned long long
 lookback_wide(uint16_t* agg16, const uint64_t* incl64, uint32_t tile, uint32_t d, uint32_t epoch, uint32_t spin_cap,
-              const TileRereduce<KeyT>& rr)
+              const TileRereduce<KeyT>& rr, Hook hook = Hook())
 {
     unsigned long long sum = 0;                       // reductions of tiles (cur, tile-1] already added
     int64_t cur = static_cast<int64_t>(tile) - 1;     // nearest predecessor not yet accounted for
@@ -849,13 +927,18 @@ lookback_wide(uint16_t* agg16, const uint64_t* incl64, uint32_t tile, uint32_t d
         }
         sum = run;
         if (stalled) {
+            if (hook(-1) == kHookAbort) return sum;
             polls = next == cur ? polls + 1 : 1;
             if (polls > spin_cap) {
                 // maybe the stalled tile has finished altogether meanwhile: its inclusive prefix settles everything
                 const uint64_t w = ld_relaxed_gpu_u64(incl64 + next * kRadix + d);
                 if (desc_epoch(w) == epoch && (w & kFlagMask) == kFlagInclusive) return sum + desc_value(w);
-                sum += rereduce_tile<KeyT>(rr.in + static_cast<uint64_t>(next) * rr.tile_keys, rr.tile_keys, rr.shift, rr.mask,
-                                           rr.encode ? 1u : 0u, rr.ca, rr.cb, rr.cd, agg16 + agg_index(next, d), d);
+                const long long h = hook(next);
+                if (h >= 0)
+                    sum += static_cast<unsigned long long>(h);
+                else
+                    sum += rereduce_tile<KeyT>(rr.in + static_cast<uint64_t>(next) * rr.tile_keys, rr.tile_keys, rr.shift, rr.mask,
+                                               rr.encode ? 1u : 0u, rr.ca, rr.cb, rr.cd, agg16 + agg_index(next, d), d);
                 --next;
                 polls = 0;
             } else {
@@ -915,11 +998,22 @@ struct PassParams {
     uint32_t stall_every;  // test hook (0 = off): tiles with tile % N == N-1 never publish their reduction
     const SortPlan* plan;  // device plan or null
     const void* keys_in = nullptr;  // argsort (INDICES): the caller's untouched keys, read by the first executed pass
+    // fused sorts (u32 keys only, DESIGN §4.12): the region capacity c (0: not a fused sort); the fused first pass's abort
+    // word and the global histogram it fills; place 0's dense digit bases, which map the gapped source to positions
+    unsigned long long region = 0;
+    uint32_t* fused_abort = nullptr;
+    unsigned long long* fused_hist = nullptr;
+    const unsigned long long* dense_base0 = nullptr;
 };
 
 // plan_bits of an argsort pass (INDICES): this is the first executed pass -- its keys come from PassParams::keys_in and its
 // payloads are the keys' own input positions
 constexpr uint32_t kPlanBitsFirstIndices = 8u;
+// plan_bits of the first executed pass after the fused first pass: its source is gapped (plan_reads_gapped)
+constexpr uint32_t kPlanBitsGapped = 16u;
+
+__device__ __forceinline__ void named_bar_arrive(uint32_t id, uint32_t threads) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
+__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t threads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
 
 // Reads a copy of a value the caller also holds in a register, kept in shared memory for this purpose: the compiler cannot
 // prove the two equal, so whatever is computed from the copy is computed again rather than taken from earlier expressions
@@ -946,20 +1040,32 @@ struct WideSmem {
     uint32_t wmax[kRadix / 32];                      // (HOT) per digit warp: max of (tile count << 8 | digit)
     uint32_t next_tile;                              // the tile this CTA works on after the current one (drawn ticket)
     uint32_t plan_bits;                              // bit 0: source is the alt buffer; bits 1-2: codec flags of this pass;
-                                                     // bit 3: first pass of an argsort (kPlanBitsFirstIndices)
+                                                     // bit 3: first pass of an argsort (kPlanBitsFirstIndices); bit 4: the
+                                                     // source is gapped (kPlanBitsGapped)
     uint32_t digit_shift, digit_mask;                // copies of the pass's digit, re-read by the rank phase (opaque_copy)
+    // u32 keys only (fused sorts): place 0's dense digit bases (gapped source); the fused first pass's counts of places
+    // 1-3 over the CTA's tiles, and whether it stops
+    static constexpr bool kFusable = sizeof(KeyT) == 4 && !PAIRS;
+    unsigned long long gap_base[kFusable ? kRadix : 1];
+    uint32_t fhist[kFusable ? 3 * kRadix : 1];
+    uint32_t fused_stop;
 };
 
 // INDICES (argsort, pairs only): buf0/val0 are the caller's output keys and indices, buf1/val1 the alt buffers.  The first
 // executed pass, which by the plan's parity would read the caller's side, reads its keys from pp.keys_in instead and makes
 // every payload from the key's position in the input; every other pass is the pairs pass as it is.
-template <typename KeyT, bool PAIRS, int K, int WARPS, int RANK_MODE, int LOOK, int MINB, bool HOT = false, bool INDICES = false>
+// FUSED (u32 keys, the fused first pass of a whole-key sort, DESIGN §4.12): runs without a plan, reads buf0 and writes
+// buf1 with digit d's keys in the region [d * c, (d + 1) * c), c = pp.region; counts places 0-3 into pp.fused_hist; a tile
+// that would overflow a region scatters nothing, sets *pp.fused_abort, and every tile after it stops as well.
+template <typename KeyT, bool PAIRS, int K, int WARPS, int RANK_MODE, int LOOK, int MINB, bool HOT = false, bool INDICES = false,
+          bool FUSED = false>
 __global__ void __launch_bounds__(WARPS * 32, HOT ? OSB_HOT_MINB : MINB)
 digit_binning_wide_kernel(KeyT* buf0, KeyT* buf1, uint32_t* val0, uint32_t* val1, uint64_t n,
                           const unsigned long long* __restrict__ gbase, uint16_t* agg16, uint64_t* incl64,
                           uint32_t* ticket, PassParams pp, KeyCodec codec)
 {
     static_assert(!INDICES || PAIRS, "the indices are the 32-bit payloads of a pairs pass");
+    static_assert(!FUSED || (sizeof(KeyT) == 4 && !PAIRS && !HOT && WARPS * 32 > kRadix), "the fused first pass: u32 keys, plain");
     using S = WideSmem<KeyT, PAIRS, K, WARPS>;
     constexpr int THREADS = S::THREADS;
     constexpr int T = S::T;
@@ -1011,6 +1117,9 @@ digit_binning_wide_kernel(KeyT* buf0, KeyT* buf1, uint32_t* val0, uint32_t* val1
         if (codec.flags & kCodecFromPlan)
             my_bits |= (pp.place == pl.first_exec ? kCodecEncodeOnLoad << 1 : 0u) | (pp.place == pl.last_exec ? kCodecDecodeOnStore << 1 : 0u);
         if constexpr (INDICES) my_bits |= pp.place == pl.first_exec ? kPlanBitsFirstIndices : 0u;
+        if constexpr (S::kFusable) my_bits |= plan_reads_gapped(pl, pp.place) ? kPlanBitsGapped : 0u;
+        // a fused sort whose fused first pass stood: the classic pass of place 0 (its fallback) has nothing to do
+        if (pp.place == 0 && (pl.skip_mask & kPlanFusedKept)) my_skip = true;
     }
     if (my_skip) return;  // all keys share this digit: nothing to move (the plan accounts for the parity)
     if (HOT != my_hot) return;  // a pass is executed by exactly one of the two instantiations the host enqueues
@@ -1024,7 +1133,45 @@ digit_binning_wide_kernel(KeyT* buf0, KeyT* buf1, uint32_t* val0, uint32_t* val1
     KeyReg key[K];
     uint32_t val[PAIRS ? K : 1];
     const uint32_t warp_off = warp * (32 * K) + lane;
+    // The gapped source (the first executed pass after a fused first pass; u32 keys): logical position p is at
+    // p + (r * c - B0[r]) of the alt buffer, r the region whose dense range [B0[r], B0[r + 1]) holds p.  A full tile inside
+    // one region takes one offset; a tile across a region boundary, and the ragged last tile, look the region up per key.
+    auto region_of = [&](uint64_t p) {
+        uint32_t r = 0;
+#pragma unroll 1
+        for (uint32_t step = kRadix / 2; step; step >>= 1) if (sm.gap_base[r + step] <= p) r += step;
+        return r;
+    };
+    auto load_gapped = [&](uint32_t t) {
+        const KeyT* __restrict__ in = buf1;
+        const unsigned long long c = pp.region;
+        const uint64_t base = static_cast<uint64_t>(t) * T;
+        if (base + T <= n) {
+            const uint32_t r0 = region_of(base);
+            if (r0 == region_of(base + T - 1)) {
+                const KeyT* __restrict__ src = in + (base + r0 * c - sm.gap_base[r0]) + warp_off;
+#pragma unroll
+                for (int i = 0; i < K; ++i) key[i] = ld_stream(src + i * 32);
+                return;
+            }
+        }
+        const uint64_t live = base < n ? n - base : 0u;
+#pragma unroll
+        for (int i = 0; i < K; ++i) {
+            const uint32_t idx = warp_off + i * 32;
+            if (idx < live) {
+                const uint64_t p = base + idx;
+                const uint32_t r = region_of(p);
+                key[i] = in[p + r * c - sm.gap_base[r]];
+            } else {
+                key[i] = static_cast<KeyT>(~static_cast<KeyT>(0));
+            }
+        }
+    };
     auto load_tile = [&](uint32_t t) {
+        if constexpr (S::kFusable) {
+            if (my_bits & kPlanBitsGapped) { load_gapped(t); return; }
+        }
         const bool swap = my_bits & 1u;
         const bool iota = INDICES && (my_bits & kPlanBitsFirstIndices);  // argsort, first pass: payload = input position
         const KeyT* __restrict__ in = iota ? static_cast<const KeyT*>(pp.keys_in) : swap ? buf1 : buf0;
@@ -1062,11 +1209,22 @@ digit_binning_wide_kernel(KeyT* buf0, KeyT* buf1, uint32_t* val0, uint32_t* val1
     // the dispatch order of the first tiles: a predecessor that is not running is re-reduced by its successors after
     // spin_cap polls (rereduce_tile), so the chained scan cannot hang.
     uint32_t tile = blockIdx.x;
+    if constexpr (S::kFusable) {
+        if (my_bits & kPlanBitsGapped) {  // (my_bits is the same in every thread)
+            for (int i = tid; i < kRadix; i += THREADS) sm.gap_base[i] = pp.dense_base0[i];
+            __syncthreads();
+        }
+    }
     load_tile(tile);
     {
         uint4* h4 = reinterpret_cast<uint4*>(sm.hist);
         for (int i = tid; i < WARPS * kRadix / 4; i += THREADS) h4[i] = make_uint4(0, 0, 0, 0);
     }
+    if constexpr (FUSED) {
+        for (int i = tid; i < 3 * kRadix; i += THREADS) sm.fhist[i] = 0;
+        if (tid == 0) sm.fused_stop = 0;
+    }
+    uint32_t fused_count = 0;  // FUSED, digit threads: this CTA's keys with digit tid in place 0
     if (tid == 0) { sm.plan_bits = my_bits; sm.digit_shift = shift; sm.digit_mask = dmask; }
     __syncthreads();  // histograms cleared, plan_bits visible (the loads above are already in flight)
     // plan_bits (direction, codec flags) is re-read from shared memory where it is needed instead of being carried in
@@ -1144,13 +1302,38 @@ digit_binning_wide_kernel(KeyT* buf0, KeyT* buf1, uint32_t* val0, uint32_t* val1
             rr.tile_keys = T; rr.shift = shift; rr.mask = dmask;
             rr.encode = (sm.plan_bits >> 1) & kCodecEncodeOnLoad;
             rr.ca = static_cast<KeyT>(codec.a); rr.cb = static_cast<KeyT>(codec.b); rr.cd = static_cast<KeyT>(codec.d);
-            const unsigned long long prior = lookback_wide<LOOK / 8, KeyT>(agg16, incl64, tile, tid, epoch, pp.spin_cap, rr);
+            auto hook = [&](long long t) -> long long {
+                if (t < 0) {
+                    if constexpr (FUSED) return *reinterpret_cast<const volatile uint32_t*>(pp.fused_abort) ? kHookAbort : kHookDefault;
+                    return kHookDefault;
+                }
+                if (S::kFusable && (sm.plan_bits & kPlanBitsGapped))
+                    return rereduce_tile_gapped<KeyT>(buf1, static_cast<uint64_t>(t) * T, T, shift, dmask, pp.dense_base0, pp.region,
+                                                      agg16 + agg_index(t, tid), tid);
+                return kHookDefault;
+            };
+            const unsigned long long prior = lookback_wide<LOOK / 8, KeyT>(agg16, incl64, tile, tid, epoch, pp.spin_cap, rr, hook);
             const bool swap = sm.plan_bits & 1u;
             KeyT* out = swap ? buf0 : buf1;
             uint32_t* out_val = swap ? val0 : val1;
             st_relaxed_gpu_u64(incl64 + static_cast<uint64_t>(tile) * kRadix + tid,
                                desc_pack(epoch, kFlagInclusive, prior + tile_count));
-            const unsigned long long first = gbase[tid] + prior - tile_excl;  // element index (relative to out) of tile slot 0
+            // FUSED: digit tid's region starts at tid * c; a digit whose keys would run past it stops the pass, as does
+            // an abort seen here (this tile's lookback may have given up on a predecessor that never ran).  So does a digit
+            // holding more than a sixteenth of the tile (uniform keys: 64 +- 8 of 16,384): such low-entropy inputs mostly
+            // overflow a region anyway, only thousands of tiles later, and stopping at once saves that part of the pass.
+            if constexpr (FUSED) {
+                const uint32_t live_d = tile_count - ((tid == kRadix - 1 && !full) ? (T - valid) : 0u);  // (padding: digit 255)
+                fused_count += live_d;
+                if (prior + live_d > pp.region || live_d > T / 16) {
+                    *reinterpret_cast<volatile uint32_t*>(pp.fused_abort) = 1u;
+                    sm.fused_stop = 1u;
+                } else if (*reinterpret_cast<const volatile uint32_t*>(pp.fused_abort)) {
+                    sm.fused_stop = 1u;
+                }
+            }
+            // element index (relative to out) of tile slot 0
+            const unsigned long long first = (FUSED ? tid * pp.region : gbase[tid]) + prior - tile_excl;
             sm.keyptr[tid] = reinterpret_cast<unsigned long long>(out) + first * sizeof(KeyT);
             if constexpr (PAIRS) sm.valptr[tid] = reinterpret_cast<unsigned long long>(out_val) + first * sizeof(uint32_t);
             if (tid < 32) {
@@ -1211,10 +1394,34 @@ digit_binning_wide_kernel(KeyT* buf0, KeyT* buf1, uint32_t* val0, uint32_t* val1
     const uint32_t next = sm.next_tile;
     if constexpr (kPersistent) { if (!HOT || warp >= kRadix / 32) load_tile(next); }
     OSB_PHASE(4);
+    // FUSED: the warps that do not look back count places 1-3 of the digit-sorted tile meanwhile (the ragged tile's padding
+    // holds its last slots), into the CTA's histogram; the digit warps only signal that their rank stores are done.
+    if constexpr (FUSED) {
+        if (warp < kRadix / 32) {
+            named_bar_arrive(1, THREADS);
+        } else {
+            named_bar_sync(1, THREADS);
+            const uint4* s4 = reinterpret_cast<const uint4*>(sm.sorted);
+#pragma unroll 1
+            for (uint32_t j = tid - kRadix; j < T / 4; j += THREADS - kRadix) {
+                const uint4 v = s4[j];
+                const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+                for (int q = 0; q < 4; ++q) {
+                    if (full || 4 * j + q < valid) {
+                        atomicAdd(&sm.fhist[(w[q] >> 8) & 255u], 1u);
+                        atomicAdd(&sm.fhist[kRadix + ((w[q] >> 16) & 255u)], 1u);
+                        atomicAdd(&sm.fhist[2 * kRadix + (w[q] >> 24)], 1u);
+                    }
+                }
+            }
+        }
+    }
     chained_scan();
     OSB_PHASE(5);
     __syncthreads();
     OSB_PHASE(8);
+    if constexpr (FUSED) { if (sm.fused_stop) break; }  // nothing of this pass is kept: leave the rest to the fallback
     if constexpr (HOT) { if (warp < kRadix / 32) load_tile(next); }
 
     // ---- scatter -----------------------------------------------------------------------------------------
@@ -1316,6 +1523,14 @@ digit_binning_wide_kernel(KeyT* buf0, KeyT* buf1, uint32_t* val0, uint32_t* val1
     // rank) and next_tile (read by every thread before the barrier above); the sorted tile, the digit pointers and the run
     // table this scatter reads are rewritten only after the next tile's count barrier.
     }  // tile loop
+    // FUSED: the CTA's counts go to the global histogram once (its last tile's were complete at the barrier after the lookback)
+    if constexpr (FUSED) {
+        if (!sm.fused_stop) {
+            if (tid < kRadix && fused_count) atomicAdd(&pp.fused_hist[tid], static_cast<unsigned long long>(fused_count));
+            for (int i = tid; i < 3 * kRadix; i += THREADS)
+                if (sm.fhist[i]) atomicAdd(&pp.fused_hist[kRadix + i], static_cast<unsigned long long>(sm.fhist[i]));
+        }
+    }
 }
 
 // =====================================================================================================
@@ -1706,6 +1921,8 @@ struct PassArgs {
         pp.stall_every = cfg.debug_stall_every;
         pp.plan = cfg.plan;
         pp.keys_in = cfg.argsort_in;
+        pp.region = cfg.fused_region;
+        pp.dense_base0 = cfg.fused_dense_base0;
         return pp;
     }
 };
@@ -1941,6 +2158,51 @@ bool binning_has_hot_twin(int key_bytes, bool pairs, bool indices, const Binning
     bool hot = false;
     with_pass_shape(key_bytes, pairs, indices, cfg.variant, [&](auto s) { hot = decltype(s)::has_hot; return cudaSuccess; });
     return hot;
+}
+
+// The fused first pass of the u32 keys pass (DESIGN §4.12), both rank modes.
+using FusedShape = WideShape<uint32_t, false>;
+template <int RANK_MODE>
+static auto fused_kernel()
+{
+    using G = FusedShape::G;
+    return digit_binning_wide_kernel<uint32_t, false, G::K, G::WARPS, RANK_MODE, G::LOOK, G::MINB, false, false, true>;
+}
+
+cudaError_t launch_fused_first_pass(const uint32_t* keys, uint32_t* alt, uint64_t n, uint64_t region, unsigned long long* ghist,
+                                    uint32_t* abort_word, uint64_t* desc, uint16_t* agg16, uint32_t* ticket, uint32_t epoch,
+                                    const BinningConfig& cfg, cudaStream_t stream, uint32_t* ctas)
+{
+    return with_rank_mode(cfg.rank_mode, [&](auto r) {
+        constexpr int RANK_MODE = decltype(r)::value;
+        const auto kern = fused_kernel<RANK_MODE>();
+        static int per_sm = 0;  // (one value per rank mode)
+        if (per_sm == 0) {
+            int b = 0;
+            if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, kern, FusedShape::S::THREADS, FusedShape::smem) != cudaSuccess || b < 1) b = 1;
+            per_sm = b;
+        }
+        const uint64_t tiles = (n + FusedShape::T - 1) / FusedShape::T;
+        uint64_t cap = static_cast<uint64_t>(cfg.sm_count) * per_sm;
+        if (cfg.debug_max_ctas && cfg.debug_max_ctas < cap) cap = cfg.debug_max_ctas;
+        PassParams pp;
+        pp.shift = 0;
+        pp.dbits = 8;
+        pp.epoch = epoch;
+        pp.place = 0;
+        pp.spin_cap = cfg.spin_cap;
+        pp.stall_every = cfg.debug_stall_every;
+        pp.plan = nullptr;
+        pp.region = region;
+        pp.fused_abort = abort_word;
+        pp.fused_hist = ghist;
+        KeyCodec codec = cfg.codec;
+        codec.flags &= kCodecEncodeOnLoad;
+        *ctas = static_cast<uint32_t>(tiles < cap ? tiles : cap);
+        kern<<<*ctas, FusedShape::S::THREADS, FusedShape::smem, stream>>>(
+            const_cast<uint32_t*>(keys), alt, nullptr, nullptr, n, nullptr, agg16, desc, ticket, pp, codec);
+        return cudaGetLastError();
+    });
 }
 
 cudaError_t launch_digit_binning(const void* in, void* out, const uint32_t* in_val, uint32_t* out_val, uint64_t n,
@@ -2364,6 +2626,8 @@ cudaError_t configure_kernels()
     if (e == cudaSuccess) e = for_each_type(RingShapes{}, shape);
     if (e == cudaSuccess) e = for_each_type(TileShapes{}, shape);
     if (e == cudaSuccess) e = for_each_type(SegShapes{}, shape);
+    if (e == cudaSuccess) e = set_smem(fused_kernel<kRankAtomic>(), FusedShape::smem);
+    if (e == cudaSuccess) e = set_smem(fused_kernel<kRankBallot>(), FusedShape::smem);
     return e;
 }
 

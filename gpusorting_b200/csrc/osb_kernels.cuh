@@ -34,6 +34,10 @@ struct BinningConfig {
     bool hot_passes = false;          // also enqueue the HOT instantiation (the plan decides which of the two runs the pass)
     const void* argsort_in = nullptr; // argsort (u32/u16/u64 pairs, needs the plan): the first executed pass reads its keys from here
                                       // and makes every payload from the key's input position (in/in_val: output keys/indices)
+    // fused sorts (u32 keys, DESIGN §4.12): the region capacity and place 0's dense digit bases, with which the first executed
+    // pass after place 0 reads the gapped layout the fused first pass leaves when the plan keeps it (0 / null: not a fused sort)
+    uint64_t fused_region = 0;
+    const unsigned long long* fused_dense_base0 = nullptr;
 };
 
 // keys per partition tile for a key width / pairs flag / variant (host needs it to size descriptors)
@@ -45,9 +49,27 @@ bool binning_has_hot_twin(int key_bytes, bool pairs, bool indices, const Binning
 cudaError_t configure_kernels();
 
 // GlobalHistogram (reference: OneSweep::GlobalHistogram, Sort/OneSweep.cu:44-123).
-// ghist[place*256 + digit] += counts; caller zeroes ghist first.
+// ghist[place*256 + digit] += counts; caller zeroes ghist first.  gate != null: the fallback of a fused sort, which returns
+// at once when the plan keeps the fused first pass.
 cudaError_t launch_global_histogram(const void* keys, uint64_t n, int key_bytes, unsigned long long* ghist,
-                                    int sm_count, cudaStream_t stream, const KeyCodec* codec = nullptr);
+                                    int sm_count, cudaStream_t stream, const KeyCodec* codec = nullptr, const SortPlan* gate = nullptr);
+
+// ---- fused sorts: whole-key u32 keys-only sorts without a GlobalHistogram in front (DESIGN §4.12) -------------------------
+// The fused first pass: reads keys (codec: encode on load), writes digit d's keys to alt[d * region, (d + 1) * region), adds
+// the histogram of places 0-3 to ghist[0..1023] (zeroed by the caller), and sets *abort_word (zeroed by the caller) instead
+// of overflowing a region.  No plan; its own ticket, place 0's epoch and reductions.  *ctas: the CTAs it launched.
+cudaError_t launch_fused_first_pass(const uint32_t* keys, uint32_t* alt, uint64_t n, uint64_t region, unsigned long long* ghist,
+                                    uint32_t* abort_word, uint64_t* desc, uint16_t* agg16, uint32_t* ticket, uint32_t epoch,
+                                    const BinningConfig& cfg, cudaStream_t stream, uint32_t* ctas);
+// The scan after the fused first pass (fallback = false): the plan of launch_scan plus kPlanFusedKept when the fused pass
+// stands.  The fallback's scan (fallback = true) returns at once when it does, else writes the classic plan.
+cudaError_t launch_scan_fused(const unsigned long long* ghist, unsigned long long* gbase, int places, cudaStream_t stream,
+                              SortPlan* plan, uint64_t n, bool allow_skip, bool allow_hot, bool fallback, const uint32_t* fused_abort,
+                              uint64_t region);
+// The fallback's clear of place 0's reductions and the descriptors of the tiles the fused pass reached (its ctas and the
+// tiles drawn from its ticket, at most tiles); returns at once when the plan keeps the fused pass.
+cudaError_t launch_fused_fallback_zero(const SortPlan* plan, const uint32_t* ticket, uint32_t ctas, uint64_t tiles, uint16_t* agg16,
+                                       uint64_t* desc, int sm_count, cudaStream_t stream);
 
 // Single-place histogram (used by the sharded path for the most significant digit): hist256[digit] += counts.
 cudaError_t launch_digit_histogram(const void* keys, uint64_t n, int key_bytes, uint32_t shift,

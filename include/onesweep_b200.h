@@ -266,9 +266,13 @@ OSB200_API int osb200_init_random_u32(uint32_t* d_keys, uint32_t* d_payload, uin
  *                    UtilityKernels.cuh:42-52) is executed by the HOT instantiation of the DigitBinningPass, which ranks
  *                    a tile's most frequent digit with one ballot per round instead of serialised same-address atomics;
  *                    decided on the device, both instantiations are enqueued for every pass; 0 = plain kernel only
+ *   "fused_histogram" 1 (default) = whole-key u32 keys-only sorts of at least 64 tiles and below 2^32 keys run no
+ *                    GlobalHistogram in front: the first digit pass counts it and scatters into fixed regions, and the
+ *                    classic histogram, scan and first pass run only when a region overflows; 0 = the classic path
  * Info keys: "tile_keys","launches_per_sort","memsets_per_sort","sm_count","rank_mode","variant","atomic_order_ok",
- * "max_n","epoch","short_circuit","spin_cap","small_path","small_path_max_n","hot_passes","last_skip_mask",
- * "last_hot_mask","last_executed_passes" (the last three read the device plan of the previous sort and synchronise). */
+ * "max_n","epoch","short_circuit","spin_cap","small_path","small_path_max_n","hot_passes","fused_histogram","last_skip_mask",
+ * "last_hot_mask","last_executed_passes","last_fused_kept" (the last four read the device plan of the previous sort and
+ * synchronise; "last_fused_kept" = 1 when its fused first pass stood). */
 OSB200_API int osb200_set_option(osb200_handle h, const char* key, int64_t value);
 OSB200_API int64_t osb200_get_info(osb200_handle h, const char* key);
 /* With option "profile"=1 every sort records CUDA events on its stream between its kernels.  Returns the number of
