@@ -18,6 +18,7 @@ from .onesweep import (  # noqa: F401
     argsort16,
     init_random,
     sort_rows,
+    sort_segments,
 )
 
 __version__ = "0.1.0"

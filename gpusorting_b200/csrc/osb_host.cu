@@ -24,10 +24,11 @@
 
 namespace {
 
-constexpr int kVersion = 1006;  // 1002: device plan, bit ranges, forward-progress fallback, hot passes, segmented sort; 1003: argsort;
+constexpr int kVersion = 1007;  // 1002: device plan, bit ranges, forward-progress fallback, hot passes, segmented sort; 1003: argsort;
                                 // 1004: 16-bit keys (osb200_sort_keys16, osb200_sort_pairs16, osb200_argsort16);
                                 // 1005: row sort (osb200_sort_rows);
-                                // 1006: 64-bit keys with uint32 payloads and their argsort (osb200_create_pairs64)
+                                // 1006: 64-bit keys with uint32 payloads and their argsort (osb200_create_pairs64);
+                                // 1007: segment sort by offsets (osb200_sort_segments)
 constexpr int kMaxPlaces = 8;
 
 inline int cuda_status(cudaError_t e) { return e == cudaSuccess ? OSB200_OK : OSB200_ERR_CUDA - static_cast<int>(e); }
@@ -44,7 +45,7 @@ struct ControlLayout {
     static constexpr size_t ticket_bytes = 64;  // 8 u32 tickets, padded
     static constexpr size_t zeroed_bytes = ghist_bytes + ticket_bytes;
     static constexpr size_t gbase_bytes = kMaxPlaces * osb::kRadix * sizeof(unsigned long long);
-    static constexpr size_t err_bytes = 64;
+    static constexpr size_t err_bytes = 64;   // scratch of the calls that clear it first: validate, osb200_sort_segments' class counts
     static constexpr size_t plan_bytes = 64;  // osb::SortPlan, written by the scan kernel of every sort
     static constexpr size_t total = zeroed_bytes + gbase_bytes + err_bytes + plan_bytes;
 };
@@ -100,6 +101,7 @@ struct osb200_sorter {
     {
         return reinterpret_cast<osb::SortPlan*>(control + ControlLayout::zeroed_bytes + ControlLayout::gbase_bytes + ControlLayout::err_bytes);
     }
+
 };
 
 namespace {
@@ -712,6 +714,45 @@ int osb200_sort_rows(osb200_handle h, const void* d_keys_in, void* d_keys_out, u
     c.flags = osb::kCodecEncodeOnLoad | osb::kCodecDecodeOnStore;
     OSB_TRY(osb::launch_row_sort(d_keys_in, d_keys_out, d_indices, num_rows, row_len, key_bytes, codec,
                                  h->cfg.rank_mode, h->debug_rows_block, h->sm_count, q));
+    return OSB200_OK;
+}
+
+// Segment sort by offsets: the row sort's kernels for ragged rows.  Workspace: one u32 per segment for the class lists, in
+// the alt key buffer (at least 4 max_n bytes for every handle shape), and the 4 u64 class counts in the control block's
+// scratch words (err()).
+int osb200_sort_segments(osb200_handle h, const void* d_keys_in, void* d_keys_out, uint32_t* d_indices, uint64_t n,
+                         const uint64_t* d_segment_offsets, uint64_t num_segments, uint32_t max_segment_len, int key_bytes,
+                         int key_type, int descending, void* stream)
+{
+    if (check_handle(h) != OSB200_OK) return OSB200_ERR_INVALID_ARG;
+    osb::KeyCodec c;
+    const osb::KeyCodec* codec = nullptr;
+    int st = key_bytes == 2 ? make_codec16(key_type, descending, &c, &codec)
+             : key_bytes == 4 || key_bytes == 8 ? make_codec(key_bytes, key_type, descending, &c, &codec)
+                                                : OSB200_ERR_INVALID_ARG;
+    if (st != OSB200_OK) return st;
+    if (n == 0 || num_segments == 0 || max_segment_len == 0) return OSB200_OK;
+    const uintptr_t in = reinterpret_cast<uintptr_t>(d_keys_in), out = reinterpret_cast<uintptr_t>(d_keys_out),
+                    idx = reinterpret_cast<uintptr_t>(d_indices), off = reinterpret_cast<uintptr_t>(d_segment_offsets);
+    if (!in || !out || !off) return OSB200_ERR_INVALID_ARG;
+    // the kernels load and store element by element: natural alignment is enough
+    if (((in | out) & static_cast<uintptr_t>(key_bytes - 1)) || (idx & 3u) || (off & 7u)) return OSB200_ERR_INVALID_ARG;
+    // the array sizes in bytes must fit in 64 bits
+    if (n > UINT64_MAX / 8 || num_segments > UINT64_MAX / 8 - 1) return OSB200_ERR_INVALID_ARG;
+    const uint64_t kb = n * static_cast<uint64_t>(key_bytes), ib = n * sizeof(uint32_t), ob = (num_segments + 1) * sizeof(uint64_t);
+    // in place (out == in) is fine: a segment is read whole before it is written; any other overlap is not, and the offsets,
+    // read by every kernel of the call, must not overlap what it writes
+    if ((in != out && overlaps(in, kb, out, kb)) || (idx && (overlaps(in, kb, idx, ib) || overlaps(out, kb, idx, ib))) ||
+        overlaps(off, ob, out, kb) || (idx && overlaps(off, ob, idx, ib)))
+        return OSB200_ERR_INVALID_ARG;
+    if (max_segment_len > osb::row_sort_capacity(key_bytes)) return OSB200_ERR_SIZE;
+    // the class lists take one u32 per segment of the alt key buffer; segment ids are u32
+    if (num_segments > h->max_n || num_segments > (1ull << 32)) return OSB200_ERR_SIZE;
+    static_assert(ControlLayout::err_bytes >= 4 * sizeof(unsigned long long), "the class counts live in the scratch words");
+    c.flags = osb::kCodecEncodeOnLoad | osb::kCodecDecodeOnStore;
+    OSB_TRY(osb::launch_sort_segments(d_keys_in, d_keys_out, d_indices, n, reinterpret_cast<const unsigned long long*>(d_segment_offsets),
+                                      num_segments, max_segment_len, key_bytes, codec, h->cfg.rank_mode, h->sm_count,
+                                      static_cast<uint32_t*>(h->alt_keys), h->err(), static_cast<cudaStream_t>(stream)));
     return OSB200_OK;
 }
 

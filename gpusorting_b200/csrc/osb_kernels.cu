@@ -2249,18 +2249,28 @@ struct SegSmem {
     uint32_t wtot[kRadix / 32];
 };
 
+// osb200_sort_segments' class counts (see segment_bin_kernel)
+enum SegCount : int { kSegCountWarp = 0, kSegCountBlock1 = 1, kSegCountBlock2 = 2, kSegCountBlockList = 3, kSegCounts = 4 };
+
 // INDICES (argsort): the keys come from keys_in, every payload is the key's position in its segment.
 // ROWS (row sort, osb200_sort_rows): segment s is row s, [s * single_n, (s + 1) * single_n) (seg_off is not read), and the
 // keys are always read from keys_in (== keys in place).  A compile-time flag rather than a runtime one, so that the
 // segmented sort's and small path's instantiations compile as before (a runtime select cost the 8,192-key u64 kernel spills).
+// LIST (osb200_sort_segments, segment_list_sort_kernel): the CTAs sort the segments whose ids the binning kernel put at the
+// back of seg_list (entry i at seg_list[num_segments - 1 - i], seg_counts[kSegCountBlockList] of them), segment s =
+// [seg_off[s], seg_off[s + 1]), reading the keys from keys_in and writing them to keys (== keys_in in place).  Both block
+// classes share that list: the 2,048-key geometry takes its segments of up to kSegBlock1Max keys and the larger geometry the
+// rest; a kernel whose own class count is 0 returns at once.  (A kernel of its own, sharing this body, so that the other
+// modes' kernels keep their names.)
 // max_len: the caller's max_segment_len (<= T); longer segments are left as they are.
-// (ROWS: one resident CTA per SM is stated, or ptxas caps some 512-thread instantiations at 64 registers and spills.)
-template <typename KeyT, bool PAIRS, int K, int WARPS, int RANK_MODE, bool INDICES = false, bool ROWS = false>
-__global__ void __launch_bounds__(WARPS * 32, ROWS ? 1 : 0)
-segment_sort_kernel(KeyT* keys, uint32_t* vals, const unsigned long long* __restrict__ seg_off, uint64_t num_segments,
-                    uint64_t single_n, uint32_t max_len, uint32_t begin_bit, uint32_t places, uint32_t last_bits, KeyCodec codec,
-                    const KeyT* __restrict__ keys_in)
+template <typename KeyT, bool PAIRS, int K, int WARPS, int RANK_MODE, bool INDICES, bool ROWS, bool LIST>
+__device__ __forceinline__ void segment_sort_body(KeyT* keys, uint32_t* vals, const unsigned long long* __restrict__ seg_off,
+                                                  uint64_t num_segments, uint64_t single_n, uint32_t max_len, uint32_t begin_bit,
+                                                  uint32_t places, uint32_t last_bits, const KeyCodec& codec,
+                                                  const KeyT* __restrict__ keys_in, const uint32_t* __restrict__ seg_list,
+                                                  const unsigned long long* __restrict__ seg_counts)
 {
+    static_assert(!(ROWS && LIST), "one addressing mode");
     static_assert(!INDICES || PAIRS, "the indices are the payloads");
     using S = SegSmem<KeyT, PAIRS, K, WARPS>;
     constexpr int THREADS = S::THREADS;
@@ -2275,32 +2285,36 @@ segment_sort_kernel(KeyT* keys, uint32_t* vals, const unsigned long long* __rest
     const KeyT ca = static_cast<KeyT>(codec.a), cb = static_cast<KeyT>(codec.b), cd = static_cast<KeyT>(codec.d);
     const bool enc = codec.flags & kCodecEncodeOnLoad, dec = codec.flags & kCodecDecodeOnStore;
 
-    for (uint64_t seg = blockIdx.x; seg < num_segments; seg += gridDim.x) {
+    const uint64_t work = !LIST ? num_segments
+                          : seg_counts[T <= kSegBlock1Max ? kSegCountBlock1 : kSegCountBlock2] ? seg_counts[kSegCountBlockList] : 0ull;
+    for (uint64_t it = blockIdx.x; it < work; it += gridDim.x) {
+        const uint64_t seg = LIST ? seg_list[num_segments - 1 - it] : it;
         const uint64_t lo = ROWS ? seg * single_n : seg_off ? seg_off[seg] : 0ull;
         const uint64_t hi = ROWS ? lo + single_n : seg_off ? seg_off[seg + 1] : single_n;
         // empty / one key / longer than max_segment_len or the geometry (both the caller's contract: left untouched)
         if (hi <= lo + 1 || hi - lo > static_cast<uint64_t>(max_len) || hi - lo > static_cast<uint64_t>(T)) continue;
         const uint32_t len = static_cast<uint32_t>(hi - lo);
+        if (LIST && (len <= kSegBlock1Max) != (T <= kSegBlock1Max)) continue;  // the other block class's segment
 
         KeyT key[K];
         uint32_t val[PAIRS ? K : 1];
 #pragma unroll
         for (int i = 0; i < K; ++i) {
             const uint32_t idx = warp_off + i * 32;
-            KeyT k = idx < len ? (INDICES || ROWS ? keys_in : keys)[lo + idx] : static_cast<KeyT>(0);
+            KeyT k = idx < len ? (INDICES || ROWS || LIST ? keys_in : keys)[lo + idx] : static_cast<KeyT>(0);
             if (enc) k = codec_encode<KeyT>(k, ca, cb, cd);
             key[i] = idx < len ? k : static_cast<KeyT>(~static_cast<KeyT>(0));  // padding ranks last in every pass
             if constexpr (PAIRS) val[i] = INDICES ? idx : idx < len ? vals[lo + idx] : 0u;
         }
 
-        // ROWS: a warp's 32 keys of step i that all lie behind the row are padding, and every padding key has digit 255 in
+        // ROWS, LIST: a warp's 32 keys of step i that all lie behind the row are padding, and every padding key has digit 255 in
         // every pass: ranking them costs one serialised same-address atomic per key.  Such chunks are neither counted nor
         // ranked (what they read back from slots nobody wrote is never used).  The padding of the one chunk that straddles
         // `len` is ranked; it follows every real key in tile order, so it takes the slots from `len` on, which are its own
         // positions.  (The condition is warp-uniform, so the ballot ranking sees full warps.)
         const uint32_t warp_lo = warp * (32 * K);  // this warp's chunks: [warp_lo + 32 i, warp_lo + 32 i + 32)
-        const uint32_t live_chunks = ROWS ? (len > warp_lo ? (len - warp_lo + 31) / 32 : 0u) : static_cast<uint32_t>(K);
-        auto live = [&](int i) { return !ROWS || static_cast<uint32_t>(i) < live_chunks; };
+        const uint32_t live_chunks = ROWS || LIST ? (len > warp_lo ? (len - warp_lo + 31) / 32 : 0u) : static_cast<uint32_t>(K);
+        auto live = [&](int i) { return !(ROWS || LIST) || static_cast<uint32_t>(i) < live_chunks; };
         for (uint32_t p = 0; p < places; ++p) {
             const uint32_t shift = begin_bit + 8u * p;
             const uint32_t dmask = p == places - 1 ? (1u << last_bits) - 1u : 255u;
@@ -2352,6 +2366,28 @@ segment_sort_kernel(KeyT* keys, uint32_t* vals, const unsigned long long* __rest
     }
 }
 
+// (ROWS, LIST: one resident CTA per SM is stated, or ptxas caps some 512-thread instantiations at 64 registers and spills.)
+template <typename KeyT, bool PAIRS, int K, int WARPS, int RANK_MODE, bool INDICES = false, bool ROWS = false>
+__global__ void __launch_bounds__(WARPS * 32, ROWS ? 1 : 0)
+segment_sort_kernel(KeyT* keys, uint32_t* vals, const unsigned long long* __restrict__ seg_off, uint64_t num_segments,
+                    uint64_t single_n, uint32_t max_len, uint32_t begin_bit, uint32_t places, uint32_t last_bits, KeyCodec codec,
+                    const KeyT* __restrict__ keys_in)
+{
+    segment_sort_body<KeyT, PAIRS, K, WARPS, RANK_MODE, INDICES, ROWS, false>(keys, vals, seg_off, num_segments, single_n, max_len,
+                                                                             begin_bit, places, last_bits, codec, keys_in, nullptr,
+                                                                             nullptr);
+}
+
+template <typename KeyT, bool PAIRS, int K, int WARPS, int RANK_MODE, bool INDICES>
+__global__ void __launch_bounds__(WARPS * 32, 1)
+segment_list_sort_kernel(KeyT* keys, uint32_t* vals, const unsigned long long* __restrict__ seg_off, uint64_t num_segments,
+                         uint32_t max_len, uint32_t places, KeyCodec codec, const KeyT* __restrict__ keys_in,
+                         const uint32_t* __restrict__ seg_list, const unsigned long long* __restrict__ seg_counts)
+{
+    segment_sort_body<KeyT, PAIRS, K, WARPS, RANK_MODE, INDICES, false, true>(keys, vals, seg_off, num_segments, 0, max_len, 0u,
+                                                                             places, 8u, codec, keys_in, seg_list, seg_counts);
+}
+
 // three geometries per key type (SIZE 0 / 1 / 2): tiny and short segments (many resident CTAs; the work per segment is
 // proportional to the geometry's capacity, padding included) and up to a DigitBinningPass tile
 template <typename KeyT, int SIZE> struct SegGeomN;
@@ -2364,19 +2400,27 @@ template <> struct SegGeomN<uint64_t, 2> { static constexpr int K = 16, WARPS = 
 // 16-bit keys: the small-n path of their sorts (one segment of up to 16,384 keys) and the row sort; no segmented sort
 template <> struct SegGeomN<uint16_t, 1> { static constexpr int K = 8,  WARPS = 8; };   //  2,048 keys (row sort only)
 template <> struct SegGeomN<uint16_t, 2> { static constexpr int K = 32, WARPS = 16; };  // 16,384 keys, 512 threads
-template <typename KeyT, bool PAIRS, int SIZE, bool INDICES = false, bool ROWS = false>
+template <typename KeyT, bool PAIRS, int SIZE, bool INDICES = false, bool ROWS = false, bool LIST = false>
 struct SegShape {
     using Key = KeyT;
-    static constexpr bool pairs = PAIRS, indices = INDICES, rows = ROWS, has_hot = false;
+    static constexpr bool pairs = PAIRS, indices = INDICES, rows = ROWS, list = LIST, has_hot = false;
     using G = SegGeomN<KeyT, SIZE>;
     using S = SegSmem<KeyT, PAIRS, G::K, G::WARPS>;
     static constexpr uint32_t T = S::T;  // the longest segment it sorts
     static constexpr size_t smem = sizeof(S);
     static constexpr int ctas_per_sm = SIZE == 2 ? 2 : 8;
     template <int RANK_MODE, bool HOT = false>
-    static auto kernel() { return segment_sort_kernel<KeyT, PAIRS, G::K, G::WARPS, RANK_MODE, INDICES, ROWS>; }
+    static auto kernel()
+    {
+        if constexpr (LIST) return segment_list_sort_kernel<KeyT, PAIRS, G::K, G::WARPS, RANK_MODE, INDICES>;
+        else return segment_sort_kernel<KeyT, PAIRS, G::K, G::WARPS, RANK_MODE, INDICES, ROWS>;
+    }
 };
 template <typename KeyT, int SIZE, bool INDICES> using RowShape = SegShape<KeyT, INDICES, SIZE, INDICES, true>;
+template <typename KeyT, int SIZE, bool INDICES> using ListShape = SegShape<KeyT, INDICES, SIZE, INDICES, false, true>;
+static_assert(SegShape<uint16_t, false, 1>::T == kSegBlock1Max && SegShape<uint32_t, false, 1>::T == kSegBlock1Max &&
+                  SegShape<uint64_t, false, 1>::T == kSegBlock1Max,
+              "the first block class of osb200_sort_segments is the 2,048-key geometry of every key width");
 
 // Each kind of sort lists its geometries smallest first: the launchers take the first one that holds the longest segment.
 using SegShapes = TypeList<
@@ -2390,7 +2434,11 @@ using SegShapes = TypeList<
     // row sort, block path: keys only and with indices
     RowShape<uint16_t, 1, false>, RowShape<uint16_t, 2, false>, RowShape<uint16_t, 1, true>, RowShape<uint16_t, 2, true>,
     RowShape<uint32_t, 1, false>, RowShape<uint32_t, 2, false>, RowShape<uint32_t, 1, true>, RowShape<uint32_t, 2, true>,
-    RowShape<uint64_t, 1, false>, RowShape<uint64_t, 2, false>, RowShape<uint64_t, 1, true>, RowShape<uint64_t, 2, true>>;
+    RowShape<uint64_t, 1, false>, RowShape<uint64_t, 2, false>, RowShape<uint64_t, 1, true>, RowShape<uint64_t, 2, true>,
+    // segment sort by offsets (osb200_sort_segments), block classes: keys only and with indices
+    ListShape<uint16_t, 1, false>, ListShape<uint16_t, 2, false>, ListShape<uint16_t, 1, true>, ListShape<uint16_t, 2, true>,
+    ListShape<uint32_t, 1, false>, ListShape<uint32_t, 2, false>, ListShape<uint32_t, 1, true>, ListShape<uint32_t, 2, true>,
+    ListShape<uint64_t, 1, false>, ListShape<uint64_t, 2, false>, ListShape<uint64_t, 1, true>, ListShape<uint64_t, 2, true>>;
 
 // the longest segment (ROWS: row) of key_bytes-wide keys that a shape of the list sorts; 0 if there is none
 template <bool ROWS>
@@ -2399,7 +2447,7 @@ static uint32_t seg_capacity(int key_bytes)
     uint32_t cap = 0;
     for_each_type(SegShapes{}, [&](auto s) {
         using S = decltype(s);
-        if (S::rows == ROWS && key_bytes == static_cast<int>(sizeof(typename S::Key)) && S::T > cap) cap = S::T;
+        if (S::rows == ROWS && !S::list && key_bytes == static_cast<int>(sizeof(typename S::Key)) && S::T > cap) cap = S::T;
         return cudaSuccess;
     });
     return cap;
@@ -2413,14 +2461,19 @@ static cudaError_t launch_seg(Shape, void* keys, uint32_t* vals, const unsigned 
                               const KeyCodec& codec, int rank_mode, int sm_count, cudaStream_t stream, const void* keys_in)
 {
     using KeyT = typename Shape::Key;
-    const uint64_t cap = static_cast<uint64_t>(sm_count) * Shape::ctas_per_sm;
-    const unsigned grid = static_cast<unsigned>(num_segments < cap ? num_segments : cap);
-    return with_rank_mode(rank_mode, [&](auto r) {
-        const auto kern = Shape::template kernel<decltype(r)::value>();
-        kern<<<grid, Shape::S::THREADS, Shape::smem, stream>>>(static_cast<KeyT*>(keys), vals, seg_off, num_segments, single_n, max_len,
-                                                              begin_bit, places, last_bits, codec, static_cast<const KeyT*>(keys_in));
-        return cudaGetLastError();
-    });
+    if constexpr (Shape::list) {
+        return cudaErrorInvalidValue;  // launch_sort_segments launches those
+    } else {
+        const uint64_t cap = static_cast<uint64_t>(sm_count) * Shape::ctas_per_sm;
+        const unsigned grid = static_cast<unsigned>(num_segments < cap ? num_segments : cap);
+        return with_rank_mode(rank_mode, [&](auto r) {
+            const auto kern = Shape::template kernel<decltype(r)::value>();
+            kern<<<grid, Shape::S::THREADS, Shape::smem, stream>>>(static_cast<KeyT*>(keys), vals, seg_off, num_segments, single_n,
+                                                                  max_len, begin_bit, places, last_bits, codec,
+                                                                  static_cast<const KeyT*>(keys_in));
+            return cudaGetLastError();
+        });
+    }
 }
 
 cudaError_t launch_segment_sort(void* keys, uint32_t* vals, int key_bytes, const unsigned long long* seg_off, uint64_t num_segments,
@@ -2436,7 +2489,8 @@ cudaError_t launch_segment_sort(void* keys, uint32_t* vals, int key_bytes, const
         SegShapes{},
         [&](auto s) {
             using S = decltype(s);
-            return !S::rows && key_bytes == static_cast<int>(sizeof(typename S::Key)) && S::pairs == pairs && S::indices == indices &&
+            return !S::rows && !S::list && key_bytes == static_cast<int>(sizeof(typename S::Key)) && S::pairs == pairs &&
+                   S::indices == indices &&
                    max_len <= S::T;
         },
         [&](auto s) {
@@ -2467,6 +2521,101 @@ struct RowWarpSmem {  // one per warp: 1 KB of bins + the staging area (at most 
     uint32_t idx[INDICES ? 32 * K : 1];
 };
 
+// What a warp keeps across the runs it sorts: its lane, lane mask, the hist of its staging area as uint4 (lane l owns bins
+// 8l .. 8l+7: h4[2l], h4[2l+1]) and the codec as key-wide words.
+template <typename KeyT>
+struct WarpSortCtx {
+    int lane;
+    uint32_t lt;
+    uint4* h4;
+    KeyT ca, cb, cd;
+    bool enc, dec;
+};
+
+template <typename KeyT>
+__device__ __forceinline__ WarpSortCtx<KeyT> warp_sort_ctx(uint32_t* hist, const KeyCodec& codec)
+{
+    return {static_cast<int>(threadIdx.x & 31), lanemask_lt(), reinterpret_cast<uint4*>(hist), static_cast<KeyT>(codec.a),
+            static_cast<KeyT>(codec.b), static_cast<KeyT>(codec.d), (codec.flags & kCodecEncodeOnLoad) != 0,
+            (codec.flags & kCodecDecodeOnStore) != 0};
+}
+
+// One warp sorts the len <= 32 K keys [base, base + len) of `in` into the same positions of `out` (and their positions within
+// the run into idx_out), in the warp's own staging area sm.  The row kernel calls it per row, the segment kernel per segment.
+template <typename KeyT, int K, int RANK_MODE, bool INDICES>
+__device__ __forceinline__ void warp_sort_run(RowWarpSmem<KeyT, K, INDICES>& sm, const WarpSortCtx<KeyT>& x, const KeyT* in, KeyT* out,
+                                              uint32_t* idx_out, uint64_t base, uint32_t len)
+{
+    const int lane = x.lane;
+    uint4* h4 = x.h4;
+    const uint32_t lt = x.lt;
+    const KeyT ca = x.ca, cb = x.cb, cd = x.cd;
+    const bool enc = x.enc, dec = x.dec;
+
+    KeyT key[K];
+    uint32_t val[INDICES ? K : 1];
+#pragma unroll
+    for (int i = 0; i < K; ++i) {
+        const uint32_t idx = i * 32 + lane;
+        KeyT k = idx < len ? in[base + idx] : static_cast<KeyT>(0);
+        if (enc) k = codec_encode<KeyT>(k, ca, cb, cd);
+        key[i] = idx < len ? k : static_cast<KeyT>(~static_cast<KeyT>(0));
+        if constexpr (INDICES) val[i] = idx;
+    }
+#pragma unroll 1
+    for (uint32_t shift = 0; shift < sizeof(KeyT) * 8; shift += 8) {
+        h4[2 * lane] = make_uint4(0, 0, 0, 0);
+        h4[2 * lane + 1] = make_uint4(0, 0, 0, 0);
+        __syncwarp();
+#pragma unroll
+        for (int i = 0; i < K; ++i)
+            if (i * 32 + lane < len) atomicAdd(&sm.hist[digit_of(key[i], shift)], 1u);
+        __syncwarp();
+        const uint4 lo4 = h4[2 * lane], hi4 = h4[2 * lane + 1];
+        const uint32_t c[8] = {lo4.x, lo4.y, lo4.z, lo4.w, hi4.x, hi4.y, hi4.z, hi4.w};
+        uint32_t sum = 0;
+        bool whole = false;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) { sum += c[j]; whole |= c[j] == len; }
+        if (__any_sync(0xffffffffu, whole)) continue;  // one digit for the whole run: this pass keeps the order
+        uint32_t incl = sum;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o);
+            if (lane >= o) incl += t;
+        }
+        uint32_t run = incl - sum, e[8];
+#pragma unroll
+        for (int j = 0; j < 8; ++j) { e[j] = run; run += c[j]; }
+        h4[2 * lane] = make_uint4(e[0], e[1], e[2], e[3]);
+        h4[2 * lane + 1] = make_uint4(e[4], e[5], e[6], e[7]);
+        __syncwarp();
+#pragma unroll
+        for (int i = 0; i < K; ++i) {
+            const uint32_t slot = warp_rank_and_count<RANK_MODE>(sm.hist, digit_of(key[i], shift), lt);
+            sm.keys[slot] = key[i];
+            if constexpr (INDICES) sm.idx[slot] = val[i];
+        }
+        __syncwarp();
+#pragma unroll
+        for (int i = 0; i < K; ++i) {
+            key[i] = sm.keys[i * 32 + lane];
+            if constexpr (INDICES) val[i] = sm.idx[i * 32 + lane];
+        }
+        __syncwarp();
+    }
+#pragma unroll
+    for (int i = 0; i < K; ++i) {
+        const uint32_t idx = i * 32 + lane;
+        if (idx < len) {
+            KeyT k = key[i];
+            if (dec) k = codec_decode<KeyT>(k, ca, cb, cd);
+            out[base + idx] = k;
+            if constexpr (INDICES) idx_out[base + idx] = val[i];
+        }
+    }
+}
+
 template <typename KeyT, int K, int RANK_MODE, bool INDICES>
 __global__ void __launch_bounds__(kRowWarps * 32)
 row_sort_warp_kernel(const KeyT* in, KeyT* out, uint32_t* __restrict__ idx_out, uint64_t num_rows, uint32_t row_len,
@@ -2474,79 +2623,12 @@ row_sort_warp_kernel(const KeyT* in, KeyT* out, uint32_t* __restrict__ idx_out, 
 {
     using W = RowWarpSmem<KeyT, K, INDICES>;
     extern __shared__ __align__(16) unsigned char s_raw[];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int warp = threadIdx.x >> 5;
     W& sm = reinterpret_cast<W*>(s_raw)[warp];
-    uint4* h4 = reinterpret_cast<uint4*>(sm.hist);  // lane l owns bins 8l .. 8l+7 (h4[2l], h4[2l+1])
-    const uint32_t lt = lanemask_lt();
-    const KeyT ca = static_cast<KeyT>(codec.a), cb = static_cast<KeyT>(codec.b), cd = static_cast<KeyT>(codec.d);
-    const bool enc = codec.flags & kCodecEncodeOnLoad, dec = codec.flags & kCodecDecodeOnStore;
-
+    const WarpSortCtx<KeyT> x = warp_sort_ctx<KeyT>(sm.hist, codec);
     for (uint64_t row = static_cast<uint64_t>(blockIdx.x) * kRowWarps + warp; row < num_rows;
-         row += static_cast<uint64_t>(gridDim.x) * kRowWarps) {
-        const uint64_t base = row * row_len;
-        KeyT key[K];
-        uint32_t val[INDICES ? K : 1];
-#pragma unroll
-        for (int i = 0; i < K; ++i) {
-            const uint32_t idx = i * 32 + lane;
-            KeyT k = idx < row_len ? in[base + idx] : static_cast<KeyT>(0);
-            if (enc) k = codec_encode<KeyT>(k, ca, cb, cd);
-            key[i] = idx < row_len ? k : static_cast<KeyT>(~static_cast<KeyT>(0));
-            if constexpr (INDICES) val[i] = idx;
-        }
-#pragma unroll 1
-        for (uint32_t shift = 0; shift < sizeof(KeyT) * 8; shift += 8) {
-            h4[2 * lane] = make_uint4(0, 0, 0, 0);
-            h4[2 * lane + 1] = make_uint4(0, 0, 0, 0);
-            __syncwarp();
-#pragma unroll
-            for (int i = 0; i < K; ++i)
-                if (i * 32 + lane < row_len) atomicAdd(&sm.hist[digit_of(key[i], shift)], 1u);
-            __syncwarp();
-            const uint4 lo4 = h4[2 * lane], hi4 = h4[2 * lane + 1];
-            const uint32_t c[8] = {lo4.x, lo4.y, lo4.z, lo4.w, hi4.x, hi4.y, hi4.z, hi4.w};
-            uint32_t sum = 0;
-            bool whole = false;
-#pragma unroll
-            for (int j = 0; j < 8; ++j) { sum += c[j]; whole |= c[j] == row_len; }
-            if (__any_sync(0xffffffffu, whole)) continue;  // one digit for the whole row: this pass keeps the order
-            uint32_t incl = sum;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o);
-                if (lane >= o) incl += t;
-            }
-            uint32_t run = incl - sum, e[8];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) { e[j] = run; run += c[j]; }
-            h4[2 * lane] = make_uint4(e[0], e[1], e[2], e[3]);
-            h4[2 * lane + 1] = make_uint4(e[4], e[5], e[6], e[7]);
-            __syncwarp();
-#pragma unroll
-            for (int i = 0; i < K; ++i) {
-                const uint32_t slot = warp_rank_and_count<RANK_MODE>(sm.hist, digit_of(key[i], shift), lt);
-                sm.keys[slot] = key[i];
-                if constexpr (INDICES) sm.idx[slot] = val[i];
-            }
-            __syncwarp();
-#pragma unroll
-            for (int i = 0; i < K; ++i) {
-                key[i] = sm.keys[i * 32 + lane];
-                if constexpr (INDICES) val[i] = sm.idx[i * 32 + lane];
-            }
-            __syncwarp();
-        }
-#pragma unroll
-        for (int i = 0; i < K; ++i) {
-            const uint32_t idx = i * 32 + lane;
-            if (idx < row_len) {
-                KeyT k = key[i];
-                if (dec) k = codec_decode<KeyT>(k, ca, cb, cd);
-                out[base + idx] = k;
-                if constexpr (INDICES) idx_out[base + idx] = val[i];
-            }
-        }
-    }
+         row += static_cast<uint64_t>(gridDim.x) * kRowWarps)
+        warp_sort_run<KeyT, K, RANK_MODE, INDICES>(sm, x, in, out, idx_out, row * row_len, row_len);
 }
 
 // CTAs of one kernel that are resident on one SM (the warp path's grid: a grid-stride loop over the rows wants every CTA
@@ -2608,6 +2690,153 @@ cudaError_t launch_row_sort(const void* keys_in, void* keys_out, uint32_t* indic
             return launch_seg(s, keys_out, indices, nullptr, num_rows, row_len, row_len, 0u, static_cast<uint32_t>(key_bytes), 8u, codec,
                               rank_mode, sm_count, stream, keys_in);
         });
+}
+
+// =====================================================================================================
+// Segment sort by offsets (osb200_sort_segments).  The host does not know the segment lengths, so a binning kernel reads
+// the offsets once and sorts each segment into a class by its length (reference: SplitSort's BinSimple,
+// SegSort/SplitSort/SplitSort.cuh:618-668, here without its host round trip):
+//   0 keys: nothing; 1 key: written here; 2-256: the warp list; 257 - kSegBlock1Max and beyond: the block list;
+//   offsets that decrease or pass n, and segments longer than max_len: skipped (never written).
+// The lists share one array of num_segments ids: the warp list grows from its front, the block list from its back, so
+// neither can overflow.  counts = [warp list, 2,048-key class, larger class, block list]; the class kernels read their
+// count on the device, so the host enqueues them without waiting, and each segment of two or more keys is in exactly one
+// list and sorted by exactly one kernel.
+// =====================================================================================================
+template <typename KeyT>
+__global__ void __launch_bounds__(256)
+segment_bin_kernel(const unsigned long long* __restrict__ off, uint64_t num_segments, uint64_t n, uint32_t max_len,
+                   uint32_t* __restrict__ list, unsigned long long* __restrict__ counts, const KeyT* keys_in, KeyT* keys_out,
+                   uint32_t* idx_out)
+{
+    const uint32_t lane = threadIdx.x & 31, lt = lanemask_lt();
+    const uint64_t stride = static_cast<uint64_t>(gridDim.x) * blockDim.x;
+    // whole warps step together, so the ballots below always see 32 lanes
+    for (uint64_t base = static_cast<uint64_t>(blockIdx.x) * blockDim.x + (threadIdx.x & ~31u); base < num_segments; base += stride) {
+        const uint64_t s = base + lane;
+        int cls = -1;  // 0: warp list, 1 / 2: block classes
+        if (s < num_segments) {
+            const unsigned long long lo = off[s], hi = off[s + 1];
+            if (lo <= hi && hi <= n && hi - lo <= max_len) {
+                const uint32_t len = static_cast<uint32_t>(hi - lo);
+                if (len == 1) {
+                    if (keys_out != keys_in) keys_out[lo] = keys_in[lo];
+                    if (idx_out) idx_out[lo] = 0u;
+                } else if (len > 1) {
+                    cls = len <= kRowWarpMaxLen ? 0 : len <= kSegBlock1Max ? 1 : 2;
+                }
+            }
+        }
+        const uint32_t w = __ballot_sync(0xffffffffu, cls == 0), b = __ballot_sync(0xffffffffu, cls > 0);
+        const uint32_t b1 = __ballot_sync(0xffffffffu, cls == 1), b2 = b & ~b1;
+        unsigned long long wpos = 0, bpos = 0;
+        if (lane == 0) {
+            if (w) wpos = atomicAdd(&counts[kSegCountWarp], static_cast<unsigned long long>(__popc(w)));
+            if (b) bpos = atomicAdd(&counts[kSegCountBlockList], static_cast<unsigned long long>(__popc(b)));
+            if (b1) atomicAdd(&counts[kSegCountBlock1], static_cast<unsigned long long>(__popc(b1)));
+            if (b2) atomicAdd(&counts[kSegCountBlock2], static_cast<unsigned long long>(__popc(b2)));
+        }
+        wpos = __shfl_sync(0xffffffffu, wpos, 0);
+        bpos = __shfl_sync(0xffffffffu, bpos, 0);
+        if (cls == 0) list[wpos + __popc(w & lt)] = static_cast<uint32_t>(s);
+        if (cls > 0) list[num_segments - 1 - (bpos + __popc(b & lt))] = static_cast<uint32_t>(s);
+    }
+}
+
+// The warp class: one warp per segment of the warp list (grid-stride), 1, 2, 4 or 8 keys per lane by the segment's length.
+// Each warp's staging area is sized for 8.
+template <typename KeyT, int RANK_MODE, bool INDICES>
+__global__ void __launch_bounds__(kRowWarps * 32)
+segment_sort_warp_kernel(const KeyT* in, KeyT* out, uint32_t* __restrict__ idx_out, const unsigned long long* __restrict__ off,
+                         const uint32_t* __restrict__ list, const unsigned long long* __restrict__ counts, KeyCodec codec)
+{
+    extern __shared__ __align__(16) unsigned char s_raw[];
+    const int warp = threadIdx.x >> 5;
+    unsigned char* wsm = s_raw + warp * sizeof(RowWarpSmem<KeyT, 8, INDICES>);  // every K's layout starts with the same hist
+    const WarpSortCtx<KeyT> x = warp_sort_ctx<KeyT>(reinterpret_cast<uint32_t*>(wsm), codec);
+    const uint64_t count = counts[kSegCountWarp];
+    for (uint64_t i = static_cast<uint64_t>(blockIdx.x) * kRowWarps + warp; i < count; i += static_cast<uint64_t>(gridDim.x) * kRowWarps) {
+        const uint32_t s = list[i];
+        const uint64_t lo = off[s];
+        const uint32_t len = static_cast<uint32_t>(off[s + 1] - lo);
+        if (len <= 32)
+            warp_sort_run<KeyT, 1, RANK_MODE, INDICES>(*reinterpret_cast<RowWarpSmem<KeyT, 1, INDICES>*>(wsm), x, in, out, idx_out, lo, len);
+        else if (len <= 64)
+            warp_sort_run<KeyT, 2, RANK_MODE, INDICES>(*reinterpret_cast<RowWarpSmem<KeyT, 2, INDICES>*>(wsm), x, in, out, idx_out, lo, len);
+        else if (len <= 128)
+            warp_sort_run<KeyT, 4, RANK_MODE, INDICES>(*reinterpret_cast<RowWarpSmem<KeyT, 4, INDICES>*>(wsm), x, in, out, idx_out, lo, len);
+        else
+            warp_sort_run<KeyT, 8, RANK_MODE, INDICES>(*reinterpret_cast<RowWarpSmem<KeyT, 8, INDICES>*>(wsm), x, in, out, idx_out, lo, len);
+    }
+}
+
+// resident CTAs of `kern` per SM (the class kernels' grid: they grid-stride over lists whose length only the device knows)
+template <typename Kern>
+static int resident_per_sm(Kern kern, int threads, size_t smem)
+{
+    int b = 0;
+    return cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, kern, threads, smem) == cudaSuccess ? b : 0;
+}
+
+cudaError_t launch_sort_segments(const void* keys_in, void* keys_out, uint32_t* indices, uint64_t n,
+                                 const unsigned long long* off, uint64_t num_segments, uint32_t max_len, int key_bytes,
+                                 const KeyCodec* codec_in, int rank_mode, int sm_count, uint32_t* list,
+                                 unsigned long long* counts, cudaStream_t stream)
+{
+    if (num_segments == 0 || max_len == 0) return cudaSuccess;
+    if (max_len > row_sort_capacity(key_bytes)) return cudaErrorInvalidValue;
+    const KeyCodec codec = codec_in ? *codec_in : KeyCodec();
+    cudaError_t e = cudaMemsetAsync(counts, 0, kSegCounts * sizeof(unsigned long long), stream);
+    if (e != cudaSuccess) return e;
+    e = with_key_type(TypeList<uint16_t, uint32_t, uint64_t>{}, key_bytes, [&](auto k) {
+        using KeyT = decltype(k);
+        segment_bin_kernel<KeyT><<<capped_grid(num_segments, 256, static_cast<uint64_t>(sm_count) * 8), 256, 0, stream>>>(
+            off, num_segments, n, max_len, list, counts, static_cast<const KeyT*>(keys_in), static_cast<KeyT*>(keys_out), indices);
+        return cudaGetLastError();
+    });
+    if (e != cudaSuccess || max_len < 2) return e;
+    e = with_key_type(TypeList<uint16_t, uint32_t, uint64_t>{}, key_bytes, [&](auto k) {
+        return with_rank_mode(rank_mode, [&](auto r) {
+            using KeyT = decltype(k);
+            constexpr int R = decltype(r)::value;
+            auto go = [&](auto kern, auto smem_of) {
+                constexpr size_t smem = kRowWarps * sizeof(decltype(smem_of));
+                static const int per_sm = resident_per_sm(kern, kRowWarps * 32, smem);
+                if (per_sm <= 0) return cudaErrorLaunchOutOfResources;
+                kern<<<per_sm * sm_count, kRowWarps * 32, smem, stream>>>(static_cast<const KeyT*>(keys_in), static_cast<KeyT*>(keys_out), indices, off,
+                                                            list, counts, codec);
+                return cudaGetLastError();
+            };
+            return indices ? go(segment_sort_warp_kernel<KeyT, R, true>, RowWarpSmem<KeyT, 8, true>{})
+                           : go(segment_sort_warp_kernel<KeyT, R, false>, RowWarpSmem<KeyT, 8, false>{});
+        });
+    });
+    // the block classes that max_len reaches: both share the block list, each takes its own lengths
+    for (int cls = 1; e == cudaSuccess && cls <= 2; ++cls) {
+        if (max_len <= (cls == 1 ? kRowWarpMaxLen : kSegBlock1Max)) break;
+        e = find_type(
+            SegShapes{},
+            [&](auto s) {
+                using S = decltype(s);
+                return S::list && key_bytes == static_cast<int>(sizeof(typename S::Key)) && S::indices == (indices != nullptr) &&
+                       (S::T == kSegBlock1Max) == (cls == 1);
+            },
+            [&](auto s) {
+                using S = decltype(s);
+                using KeyT = typename S::Key;
+                if constexpr (!S::list) return cudaErrorInvalidValue;
+                else return with_rank_mode(rank_mode, [&](auto r) {
+                    const auto kern = S::template kernel<decltype(r)::value>();
+                    static const int per_sm = resident_per_sm(kern, S::S::THREADS, S::smem);
+                    if (per_sm <= 0) return cudaErrorLaunchOutOfResources;
+                    kern<<<per_sm * sm_count, S::S::THREADS, S::smem, stream>>>(static_cast<KeyT*>(keys_out), indices, off, num_segments,
+                                                                               max_len, static_cast<uint32_t>(key_bytes), codec,
+                                                                               static_cast<const KeyT*>(keys_in), list, counts);
+                    return cudaGetLastError();
+                });
+            });
+    }
+    return e;
 }
 
 cudaError_t configure_kernels()

@@ -131,6 +131,19 @@ cudaError_t launch_row_sort(const void* keys_in, void* keys_out, uint32_t* indic
                             int key_bytes, const KeyCodec* codec, int rank_mode, bool block_only, int sm_count,
                             cudaStream_t stream);
 
+// Segment sort by offsets (osb200_sort_segments): segment s = [off[s], off[s + 1]) of keys_in, sorted stable into the same
+// positions of keys_out (== keys_in: in place); indices (may be null) receives every output key's position within its segment.
+// A binning kernel puts every segment of 2 to max_len keys that lies inside [0, n) into a class by its length -- one warp
+// (at most kRowWarpMaxLen keys), the 2,048-key block geometry (at most kSegBlock1Max) or the largest one -- and writes the
+// one-key segments itself; then one kernel per class that max_len reaches sorts its segments.  max_len in 1 ..
+// row_sort_capacity(key_bytes).  list: num_segments u32 of workspace; counts: 4 u64 of workspace, cleared here.  The codec
+// as for launch_row_sort.
+constexpr uint32_t kSegBlock1Max = 2048;
+cudaError_t launch_sort_segments(const void* keys_in, void* keys_out, uint32_t* indices, uint64_t n,
+                                 const unsigned long long* off, uint64_t num_segments, uint32_t max_len, int key_bytes,
+                                 const KeyCodec* codec, int rank_mode, int sm_count, uint32_t* list,
+                                 unsigned long long* counts, cudaStream_t stream);
+
 // Validate (reference: Validate, UtilityKernels.cuh:403-429): err_count += #(keys[i] > keys[i+1]).
 cudaError_t launch_validate(const void* keys, uint64_t n, int key_bytes, unsigned long long* err_count, int sm_count,
                             cudaStream_t stream);

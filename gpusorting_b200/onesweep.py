@@ -238,6 +238,42 @@ class OneSweepSorter:
                   "osb200_sort_rows")
         return (out, idx) if return_indices else out
 
+    # -- segment sort: ragged rows given by offsets -------------------------------------------------------------------------
+    def sort_segments(self, x: torch.Tensor, offsets: torch.Tensor, key_type: str, descending: bool = False,
+                      return_indices: bool = True, inplace: bool = False, max_segment_len: Optional[int] = None, stream=None):
+        """Stable sort of every segment [offsets[s], offsets[s+1]) of `x` into the same positions (osb200_sort_segments):
+        sort_rows for ragged rows.  `x` is a contiguous 1-D CUDA tensor of any of the ten key dtypes, key_type as in
+        sort_rows; `offsets` a contiguous int64 tensor of num_segments + 1 offsets on the same device.  Floats follow the
+        total order of their bit patterns; equal keys keep their order in both directions.
+
+        Returns (values, indices), indices as torch.int32 positions within the segment (``indices + offsets[:-1]
+        .repeat_interleave(lengths)`` makes them global), or `values` alone with return_indices=False.  The outputs are new
+        tensors allocated with torch.empty on the stream, so positions outside every segment are uninitialised;
+        inplace=True sorts `x` itself and returns it as `values`.  Segments longer than max_segment_len are not written, nor
+        are segments whose offsets decrease or pass x.numel().  max_segment_len may be at most 16,384 (8,192 for 8-byte
+        dtypes); None computes the longest segment here, with one device->host read -- pass it when capturing a CUDA graph.
+        num_segments may be at most the sorter's max_n."""
+        if not (isinstance(x, torch.Tensor) and x.is_cuda and x.is_contiguous() and x.dim() == 1 and x.dtype in _ROW_KEY_TYPES):
+            raise TypeError(f"x must be a contiguous 1-D CUDA tensor with dtype in {tuple(_ROW_KEY_TYPES)}")
+        if x.device.index != self.device:
+            raise ValueError(f"x lives on cuda:{x.device.index}, the sorter on cuda:{self.device}")
+        if not (isinstance(offsets, torch.Tensor) and offsets.dtype == torch.int64 and offsets.is_contiguous()
+                and offsets.dim() == 1 and offsets.device == x.device):
+            raise TypeError("offsets must be a contiguous 1-D int64 tensor on the device of x")
+        kb = x.element_size()
+        kt = (KEY16_TYPES if kb == 2 else KEY_TYPES)[key_type]
+        segs = max(offsets.numel() - 1, 0)
+        if max_segment_len is None:
+            max_segment_len = max(int((offsets[1:] - offsets[:-1]).max().item()), 0) if segs else 0
+        with torch.cuda.stream(stream):  # (None: the current stream) the outputs belong to the stream that writes them
+            out = x if inplace else torch.empty_like(x)
+            idx = torch.empty(x.shape, dtype=torch.int32, device=x.device) if return_indices else None
+        with torch.cuda.device(self.device):
+            check(lib.osb200_sort_segments(self._h, x.data_ptr(), out.data_ptr(), idx.data_ptr() if idx is not None else None,
+                                           x.numel(), offsets.data_ptr(), segs, int(max_segment_len), kb, kt,
+                                           1 if descending else 0, _stream_ptr(stream)), "osb200_sort_segments")
+        return (out, idx) if return_indices else out
+
     def sort_bits(self, keys: torch.Tensor, begin_bit: int, end_bit: int, values: Optional[torch.Tensor] = None,
                   n: Optional[int] = None, stream=None):
         """Stable sort on the key bits [begin_bit, end_bit) only (osb200_sort_bits).  Keys must start on a 16-byte boundary
@@ -433,6 +469,22 @@ def sort_rows(x: torch.Tensor, descending: bool = False, return_indices: bool = 
         sp = _stream_ptr(stream)
     s = _cached_sorter(x.device.index, 4, 4, 1, sp)
     return s.sort_rows(x, _ROW_KEY_TYPES[x.dtype], descending, return_indices, False, stream)
+
+
+def sort_segments(x: torch.Tensor, offsets: torch.Tensor, descending: bool = False, return_indices: bool = True,
+                  max_segment_len: Optional[int] = None, stream=None):
+    """Stable sort of every segment [offsets[s], offsets[s+1]) of a contiguous 1-D CUDA tensor of one of sort_rows' ten
+    dtypes: (values, int32 positions within the segment), or values alone.  The key type follows the dtype.
+    OneSweepSorter.sort_segments on the stream's cached (4, 4) sorter, the one argsort uses, grown to the number of segments
+    (the call keeps one uint32 per segment in the sorter's workspace); see there for max_segment_len and what is written."""
+    if not (isinstance(x, torch.Tensor) and x.is_cuda):
+        raise TypeError("x must be a CUDA tensor")
+    if x.dtype not in _ROW_KEY_TYPES:
+        raise TypeError(f"x.dtype must be one of {tuple(_ROW_KEY_TYPES)}")
+    with torch.cuda.device(x.device.index):
+        sp = _stream_ptr(stream)
+    s = _cached_sorter(x.device.index, 4, 4, max(offsets.numel() - 1, 1), sp)
+    return s.sort_segments(x, offsets, _ROW_KEY_TYPES[x.dtype], descending, return_indices, False, max_segment_len, stream)
 
 
 class OneSweepDispatcher:

@@ -82,6 +82,16 @@ class OneSweepSorterB200 {
                                stream),
               "osb200_sort_rows");
     }
+    // every segment [offsets[s], offsets[s+1]) of n keys sorted stable into the same positions of d_keys_out (ragged rows);
+    // d_indices may be null; max_segment_len <= 16,384 (8,192 for 8-byte keys); num_segments <= the handle's max_n
+    void SortSegments(const void* d_keys_in, void* d_keys_out, uint32_t* d_indices, uint64_t n, const uint64_t* d_segment_offsets,
+                      uint64_t num_segments, uint32_t max_segment_len, int key_bytes, int key_type, bool descending,
+                      void* stream = nullptr)
+    {
+        check(osb200_sort_segments(h_, d_keys_in, d_keys_out, d_indices, n, d_segment_offsets, num_segments, max_segment_len,
+                                   key_bytes, key_type, descending ? 1 : 0, stream),
+              "osb200_sort_segments");
+    }
     // every segment [offsets[i], offsets[i+1]) sorted ascending and stable in place, one thread block per segment
     // (reference: SplitSort, SegSort/SplitSort/SplitSort.cuh:702-938); d_values may be null; max_segment_len <= 16,384
     void SegmentedSort(uint32_t* d_keys, uint32_t* d_values, const uint64_t* d_segment_offsets, uint64_t num_segments,

@@ -179,6 +179,27 @@ OSB200_API int osb200_argsort16(osb200_handle h, const void* d_keys_in, void* d_
 OSB200_API int osb200_sort_rows(osb200_handle h, const void* d_keys_in, void* d_keys_out, uint32_t* d_indices, uint64_t num_rows,
                                 uint32_t row_len, int key_bytes, int key_type, int descending, void* stream);
 
+/* Segment sort: osb200_sort_rows for ragged rows given by offsets.  Segment s is [off[s], off[s+1]) of arrays of n elements
+ * (off = d_segment_offsets, num_segments + 1 of them, 8-byte aligned); it is sorted stable into the same positions of
+ * d_keys_out, ascending or descending (the complement of the encoded key: equal keys keep their order).  d_indices may be
+ * NULL; otherwise it receives every output key's position within its segment (uint32).  key_bytes / key_type, the in-place
+ * rule (d_keys_out == d_keys_in; any other overlap, and offsets overlapping an output, are OSB200_ERR_INVALID_ARG) and the
+ * alignment are those of osb200_sort_rows.
+ *   max_segment_len: the caller's bound on the segment lengths; it decides which kernels are launched.  Above 16,384 (8,192
+ *                    for 8-byte keys): OSB200_ERR_SIZE.  Segments longer than the bound are not written; 0 is a no-op.
+ * Only positions inside segments are written.  A segment whose offsets decrease (off[s+1] < off[s]) or pass n (off[s+1] > n)
+ * is not written, and nothing outside [0, n) is touched: the offsets need not be trusted.  Positions outside every segment,
+ * such as those before off[0], keep what they held.
+ * A binning kernel reads the offsets once and writes one-key segments itself; segments of 2-256 keys are sorted one per
+ * warp, 257-2,048 keys one per 256-thread block and longer ones one per 512-thread block, each class by one kernel that
+ * returns at once when it has no segment.  At most four launches and one memset: asynchronous, no host synchronisation,
+ * graph-capturable.  Workspace: one uint32 per segment of the handle's alternate key buffer, so num_segments above
+ * min(max_n, 2^32) is OSB200_ERR_SIZE (any key or value width of handle will do); one call in flight per handle.
+ * n == 0 or num_segments == 0 is a no-op. */
+OSB200_API int osb200_sort_segments(osb200_handle h, const void* d_keys_in, void* d_keys_out, uint32_t* d_indices, uint64_t n,
+                                    const uint64_t* d_segment_offsets, uint64_t num_segments, uint32_t max_segment_len,
+                                    int key_bytes, int key_type, int descending, void* stream);
+
 /* Sort on a bit range [begin_bit, end_bit) of the (unsigned) key only, CUB-style: keys that agree on those bits keep their
  * input order (stable).  ceil((end_bit-begin_bit)/8) digit passes instead of key_bytes; the last digit may be narrower
  * than 8 bits; an odd pass count is handled inside (the result is always returned in the caller's buffers).  d_values may
