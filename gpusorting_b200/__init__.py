@@ -19,6 +19,7 @@ from .onesweep import (  # noqa: F401
     init_random,
     sort_rows,
     sort_segments,
+    topk,
 )
 
 __version__ = "0.1.0"

@@ -37,6 +37,8 @@ SIGNATURES = {
     "osb200_argsort16": (c_int, [c_vp, c_vp, c_vp, c_vp, c_u64, c_int, c_int, c_vp]),
     "osb200_sort_rows": (c_int, [c_vp, c_vp, c_vp, c_vp, c_u64, ctypes.c_uint32, c_int, c_int, c_int, c_vp]),
     "osb200_sort_segments": (c_int, [c_vp, c_vp, c_vp, c_vp, c_u64, c_vp, c_u64, ctypes.c_uint32, c_int, c_int, c_int, c_vp]),
+    "osb200_topk_rows": (c_int, [c_vp, c_vp, c_vp, c_vp, c_u64, ctypes.c_uint32, ctypes.c_uint32, c_int, c_int, c_int, c_int,
+                                 c_vp]),
     "osb200_sort_bits": (c_int, [c_vp, c_vp, c_vp, c_u64, c_int, c_int, c_vp]),
     "osb200_segmented_sort_u32": (c_int, [c_vp, c_vp, c_vp, c_vp, c_u64, ctypes.c_uint32, c_vp]),
     "osb200_sort_host_keys_u32": (c_int, [c_vp, c_vp, c_u64]),

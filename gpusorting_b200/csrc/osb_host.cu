@@ -24,11 +24,12 @@
 
 namespace {
 
-constexpr int kVersion = 1007;  // 1002: device plan, bit ranges, forward-progress fallback, hot passes, segmented sort; 1003: argsort;
+constexpr int kVersion = 1008;  // 1002: device plan, bit ranges, forward-progress fallback, hot passes, segmented sort; 1003: argsort;
                                 // 1004: 16-bit keys (osb200_sort_keys16, osb200_sort_pairs16, osb200_argsort16);
                                 // 1005: row sort (osb200_sort_rows);
                                 // 1006: 64-bit keys with uint32 payloads and their argsort (osb200_create_pairs64);
-                                // 1007: segment sort by offsets (osb200_sort_segments)
+                                // 1007: segment sort by offsets (osb200_sort_segments);
+                                // 1008: row top-k (osb200_topk_rows)
 constexpr int kMaxPlaces = 8;
 
 inline int cuda_status(cudaError_t e) { return e == cudaSuccess ? OSB200_OK : OSB200_ERR_CUDA - static_cast<int>(e); }
@@ -64,6 +65,7 @@ struct osb200_sorter {
     bool small_path = true;      // n <= one tile: the single-CTA shared-memory sort (one launch)
     bool hot_passes = true;      // low-entropy digit places run in the HOT instantiation of the pass (decided on the device)
     bool debug_rows_block = false;  // test hook: osb200_sort_rows sorts rows of <= 256 keys on the block path, not the warp path
+    uint32_t debug_topk_capacity = 0;  // test hook: N > 0 holds at most N candidates of osb200_topk_rows in shared memory
     bool fused_histogram = true;    // whole-key u32 keys-only sorts of >= kFusedMinTiles tiles: the fused first pass (§4.12)
 
     void* alt_keys = nullptr;
@@ -756,6 +758,39 @@ int osb200_sort_segments(osb200_handle h, const void* d_keys_in, void* d_keys_ou
     return OSB200_OK;
 }
 
+// Row top-k: at most two launches, no workspace -- like the row sort, any handle will do.
+int osb200_topk_rows(osb200_handle h, const void* d_keys_in, void* d_values_out, uint32_t* d_indices, uint64_t num_rows,
+                     uint32_t row_len, uint32_t k, int key_bytes, int key_type, int largest, int sorted, void* stream)
+{
+    if (check_handle(h) != OSB200_OK) return OSB200_ERR_INVALID_ARG;
+    osb::KeyCodec c;
+    const osb::KeyCodec* codec = nullptr;
+    int st = key_bytes == 2 ? make_codec16(key_type, largest, &c, &codec)
+             : key_bytes == 4 || key_bytes == 8 ? make_codec(key_bytes, key_type, largest, &c, &codec)
+                                                : OSB200_ERR_INVALID_ARG;
+    if (st != OSB200_OK) return st;
+    if (num_rows == 0 || row_len == 0 || k == 0) return OSB200_OK;
+    if (k > row_len) return OSB200_ERR_INVALID_ARG;
+    const uintptr_t in = reinterpret_cast<uintptr_t>(d_keys_in), out = reinterpret_cast<uintptr_t>(d_values_out),
+                    idx = reinterpret_cast<uintptr_t>(d_indices);
+    if (!in || !out || !idx) return OSB200_ERR_INVALID_ARG;
+    // the kernels load and store element by element: natural alignment is enough
+    if (((in | out) & static_cast<uintptr_t>(key_bytes - 1)) || (idx & 3u)) return OSB200_ERR_INVALID_ARG;
+    // the array sizes in bytes must fit in 64 bits (the outputs are smaller than the input: k <= row_len)
+    if (num_rows > UINT64_MAX / row_len) return OSB200_ERR_INVALID_ARG;
+    const uint64_t n = num_rows * row_len, m = num_rows * k;
+    if (n > UINT64_MAX / 8) return OSB200_ERR_INVALID_ARG;
+    const uint64_t kb = n * static_cast<uint64_t>(key_bytes), ob = m * static_cast<uint64_t>(key_bytes), ib = m * sizeof(uint32_t);
+    // the outputs have another shape than the input: no in-place form, and no overlap at all
+    if (overlaps(in, kb, out, ob) || overlaps(in, kb, idx, ib) || overlaps(out, ob, idx, ib)) return OSB200_ERR_INVALID_ARG;
+    if (k > osb::row_sort_capacity(key_bytes)) return OSB200_ERR_SIZE;
+    c.flags = osb::kCodecEncodeOnLoad | osb::kCodecDecodeOnStore;
+    OSB_TRY(osb::launch_topk_rows(d_keys_in, d_values_out, d_indices, num_rows, row_len, k, key_bytes, codec, sorted != 0,
+                                  h->debug_topk_capacity, h->cfg.rank_mode, h->debug_rows_block, h->sm_count,
+                                  static_cast<cudaStream_t>(stream)));
+    return OSB200_OK;
+}
+
 int osb200_sort_host_keys_u32(osb200_handle h, uint32_t* h_keys, uint64_t n)
 {
     if (check_handle(h) != OSB200_OK || h->key_bytes != 4) return OSB200_ERR_INVALID_ARG;
@@ -907,6 +942,11 @@ int osb200_set_option(osb200_handle h, const char* key, int64_t value)
         return OSB200_OK;
     }
     if (!std::strcmp(key, "debug_rows_block")) { h->debug_rows_block = value != 0; return OSB200_OK; }
+    if (!std::strcmp(key, "debug_topk_capacity")) {  // test hook of osb200_topk_rows' shared-memory candidates (0 = off)
+        if (value < 0 || value > (1ll << 30)) return OSB200_ERR_INVALID_ARG;
+        h->debug_topk_capacity = static_cast<uint32_t>(value);
+        return OSB200_OK;
+    }
     if (!std::strcmp(key, "debug_epoch")) {  // test hook: the epoch counter, to reach the wrap-around or reuse epochs
         if (value < 0 || value > osb::kEpochMax) return OSB200_ERR_INVALID_ARG;
         h->epoch = static_cast<uint32_t>(value);

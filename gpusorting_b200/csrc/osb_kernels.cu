@@ -2542,10 +2542,15 @@ __device__ __forceinline__ WarpSortCtx<KeyT> warp_sort_ctx(uint32_t* hist, const
 
 // One warp sorts the len <= 32 K keys [base, base + len) of `in` into the same positions of `out` (and their positions within
 // the run into idx_out), in the warp's own staging area sm.  The row kernel calls it per row, the segment kernel per segment.
-template <typename KeyT, int K, int RANK_MODE, bool INDICES>
+// TOPK (top-k, topk_warp_kernel; with INDICES): only the first `keep` sorted keys and payloads are stored, at
+// [obase, obase + keep) of out and idx_out; the payloads are loaded from idx_in[base ..] when idx_in is not null, else
+// they are the positions in the run.  (A compile-time flag, so that the other kernels' instantiations compile as before.)
+template <typename KeyT, int K, int RANK_MODE, bool INDICES, bool TOPK = false>
 __device__ __forceinline__ void warp_sort_run(RowWarpSmem<KeyT, K, INDICES>& sm, const WarpSortCtx<KeyT>& x, const KeyT* in, KeyT* out,
-                                              uint32_t* idx_out, uint64_t base, uint32_t len)
+                                              uint32_t* idx_out, uint64_t base, uint32_t len, const uint32_t* idx_in = nullptr,
+                                              uint64_t obase = 0, uint32_t keep = 0)
 {
+    static_assert(!TOPK || INDICES, "top-k stores positions");
     const int lane = x.lane;
     uint4* h4 = x.h4;
     const uint32_t lt = x.lt;
@@ -2560,7 +2565,8 @@ __device__ __forceinline__ void warp_sort_run(RowWarpSmem<KeyT, K, INDICES>& sm,
         KeyT k = idx < len ? in[base + idx] : static_cast<KeyT>(0);
         if (enc) k = codec_encode<KeyT>(k, ca, cb, cd);
         key[i] = idx < len ? k : static_cast<KeyT>(~static_cast<KeyT>(0));
-        if constexpr (INDICES) val[i] = idx;
+        if constexpr (TOPK) val[i] = idx_in && idx < len ? idx_in[base + idx] : idx;
+        else if constexpr (INDICES) val[i] = idx;
     }
 #pragma unroll 1
     for (uint32_t shift = 0; shift < sizeof(KeyT) * 8; shift += 8) {
@@ -2607,7 +2613,14 @@ __device__ __forceinline__ void warp_sort_run(RowWarpSmem<KeyT, K, INDICES>& sm,
 #pragma unroll
     for (int i = 0; i < K; ++i) {
         const uint32_t idx = i * 32 + lane;
-        if (idx < len) {
+        if constexpr (TOPK) {
+            if (idx < keep) {
+                KeyT k = key[i];
+                if (dec) k = codec_decode<KeyT>(k, ca, cb, cd);
+                out[obase + idx] = k;
+                idx_out[obase + idx] = val[i];
+            }
+        } else if (idx < len) {
             KeyT k = key[i];
             if (dec) k = codec_decode<KeyT>(k, ca, cb, cd);
             out[base + idx] = k;
@@ -2839,6 +2852,271 @@ cudaError_t launch_sort_segments(const void* keys_in, void* keys_out, uint32_t* 
     return e;
 }
 
+// =====================================================================================================
+// Row top-k (osb200_topk_rows): the first k keys of every row in the stable row sort, with their positions.
+//
+// Rows of at most kRowWarpMaxLen keys: one warp sorts the row (warp_sort_run, TOPK) and stores its first k keys.
+// Longer rows: one CTA per row (grid-stride over the rows on the resident CTAs) runs a radix select from the most significant
+// digit over the encoded keys.  Pass t (t = 0 .. D, D digit places) reads the candidates S_t -- the keys whose t top digits
+// are the prefix V_t chosen so far -- and
+//   * selects the keys of S_{t-1} whose t top digits are below V_t (the buckets below the one chosen at level t - 1);
+//   * counts digit t of S_t in per-warp bins; the scan picks the bucket b holding the k'-th candidate (k' = the keys still
+//     needed), k' drops by the keys below b and b is appended to V.
+// When b holds exactly k' keys, or after the last digit, the next pass is the final one: it also selects the keys equal to
+// the prefix, the first k' of them in position order.  Every selection is an ordered compaction (per-warp ballots, a scan
+// of the chunk's warp counts) in row order, so equal keys -- always selected in the same pass -- reach the output in position
+// order, and the ties at the boundary are the lowest positions.
+// The candidates are read from the row in global memory until their count fits `cap` (row_sort_capacity keys, or less as a
+// test hook): the pass that reads S_t then also compacts it, in row order, into shared memory, and later passes read only
+// that.  So a row of at most cap keys is read once, and a row is never read more than D + 1 times.
+// The selected keys leave in pass order, not key order; `sorted` sorts the [num_rows, k] output in place afterwards
+// (topk_warp_kernel for k <= 256, else topk_sort_kernel: the row sort's block body with the payloads loaded).
+// =====================================================================================================
+constexpr int kTopkWarps = 16, kTopkThreads = kTopkWarps * 32;
+constexpr int kTopkE = 8;  // keys per thread and chunk: a chunk is 4,096 keys, one block barrier
+
+template <typename KeyT>
+struct TopkSmem {
+    static constexpr uint32_t C = SegGeomN<KeyT, 2>::K * SegGeomN<KeyT, 2>::WARPS * 32;  // row_sort_capacity
+    alignas(16) KeyT keys[C];
+    alignas(16) uint32_t pos[C];
+    alignas(16) uint32_t hist[kTopkWarps * kRadix];
+    uint32_t cnt[2][kTopkE * kTopkWarps];  // per chunk (double-buffered): selected | candidates << 16 of each (e, warp)
+    uint32_t wtot[kRadix / 32];
+    uint32_t pick[3];  // the chosen bucket, the candidates below it, the candidates in it
+};
+
+template <typename KeyT>
+__global__ void __launch_bounds__(kTopkThreads, 1)
+topk_select_kernel(const KeyT* __restrict__ in, KeyT* __restrict__ out, uint32_t* __restrict__ idx_out, uint64_t num_rows,
+                   uint32_t row_len, uint32_t k, uint32_t cap, KeyCodec codec)
+{
+    using S = TopkSmem<KeyT>;
+    using U = std::conditional_t<sizeof(KeyT) == 8, uint64_t, uint32_t>;
+    constexpr uint32_t BITS = sizeof(KeyT) * 8, D = sizeof(KeyT);
+    constexpr uint32_t CHUNK = kTopkE * kTopkThreads;
+    extern __shared__ __align__(128) unsigned char s_raw[];
+    S& sm = *reinterpret_cast<S*>(s_raw);
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const uint32_t lt = lanemask_lt();
+    uint32_t* wh = sm.hist + warp * kRadix;
+    const KeyT ca = static_cast<KeyT>(codec.a), cb = static_cast<KeyT>(codec.b), cd = static_cast<KeyT>(codec.d);
+    const bool enc = codec.flags & kCodecEncodeOnLoad, dec = codec.flags & kCodecDecodeOnStore;
+
+    for (int i = tid; i < kTopkWarps * kRadix; i += kTopkThreads) sm.hist[i] = 0;
+    __syncthreads();
+    for (uint64_t row = blockIdx.x; row < num_rows; row += gridDim.x) {
+        const KeyT* src = in + row * row_len;
+        KeyT* dst = out + row * k;
+        uint32_t* dst_idx = idx_out + row * k;
+        // S_{t-1} = {x : (x & mprev) == vprev}; selected this pass: x in S_{t-1} with (x & mcur) < vcur; S_t: (x & mcur) == vcur
+        U mprev = 0, vprev = 0, mcur = 0, vcur = 0;
+        uint32_t need = k, cand = row_len, written = 0, in_smem = 0;  // in_smem: 0, or the number of candidates held there
+        bool last = false;
+        for (uint32_t t = 0;; ++t) {
+            const bool compact = !last && !in_smem && cand <= cap;
+            const bool order = t > 0 || compact;  // anything to place in row order this pass
+            const uint32_t shift = last ? 0u : BITS - 8u * (t + 1);
+            const uint64_t n_src = in_smem ? in_smem : row_len;
+            uint32_t sel_run = 0, eq_run = 0, chunk = 0;
+            for (uint64_t c0 = 0; c0 < n_src; c0 += CHUNK, ++chunk) {
+                U x[kTopkE];
+                uint32_t p[kTopkE];
+                bool sel[kTopkE], eq[kTopkE];
+#pragma unroll
+                for (int e = 0; e < kTopkE; ++e) {
+                    const uint64_t i = c0 + static_cast<uint32_t>(e * kTopkThreads + tid);
+                    const bool valid = i < n_src;
+                    KeyT v = 0;
+                    if (valid) v = in_smem ? sm.keys[i] : src[i];
+                    if (valid && !in_smem && enc) v = codec_encode<KeyT>(v, ca, cb, cd);
+                    x[e] = static_cast<U>(v);
+                    p[e] = in_smem && valid ? sm.pos[i] : static_cast<uint32_t>(i);
+                    sel[e] = valid && (x[e] & mprev) == vprev && (x[e] & mcur) < vcur;
+                    eq[e] = valid && (x[e] & mcur) == vcur;
+                    if (!last && eq[e]) atomicAdd(&wh[static_cast<uint32_t>(x[e] >> shift) & 0xffu], 1u);
+                }
+                if (!order) continue;
+                uint32_t bsel[kTopkE], beq[kTopkE];
+                uint32_t* cnt = sm.cnt[chunk & 1];
+#pragma unroll
+                for (int e = 0; e < kTopkE; ++e) {
+                    bsel[e] = __ballot_sync(0xffffffffu, sel[e]);
+                    beq[e] = __ballot_sync(0xffffffffu, eq[e]);
+                    if (lane == 0) cnt[e * kTopkWarps + warp] = __popc(bsel[e]) | (__popc(beq[e]) << 16);
+                }
+                __syncthreads();
+                // exclusive prefix of the (e, warp) counts in row order: lane l scans entries 4l .. 4l + 3
+                const uint4 c4 = reinterpret_cast<const uint4*>(cnt)[lane];
+                const uint32_t s4 = c4.x + c4.y + c4.z + c4.w;
+                uint32_t incl = s4;
+#pragma unroll
+                for (int o = 1; o < 32; o <<= 1) {
+                    const uint32_t v = __shfl_up_sync(0xffffffffu, incl, o);
+                    if (lane >= o) incl += v;
+                }
+                const uint32_t total = __shfl_sync(0xffffffffu, incl, 31);
+                const uint32_t sub = warp & 3;
+                const uint32_t mine = incl - s4 + (sub > 0 ? c4.x : 0u) + (sub > 1 ? c4.y : 0u) + (sub > 2 ? c4.z : 0u);
+#pragma unroll
+                for (int e = 0; e < kTopkE; ++e) {
+                    const uint32_t pre = __shfl_sync(0xffffffffu, mine, 4 * e + (warp >> 2));
+                    const uint32_t s_before = sel_run + (pre & 0xffffu) + __popc(bsel[e] & lt);
+                    const uint32_t e_before = eq_run + (pre >> 16) + __popc(beq[e] & lt);
+                    if (sel[e] || (last && eq[e] && e_before < need)) {
+                        const uint32_t o = written + s_before + (last ? min(e_before, need) : 0u);
+                        KeyT v = static_cast<KeyT>(x[e]);
+                        if (dec) v = codec_decode<KeyT>(v, ca, cb, cd);
+                        dst[o] = v;
+                        dst_idx[o] = p[e];
+                    }
+                    if (compact && eq[e]) {
+                        sm.keys[e_before] = static_cast<KeyT>(x[e]);
+                        sm.pos[e_before] = p[e];
+                    }
+                }
+                sel_run += total & 0xffffu;
+                eq_run += total >> 16;
+            }
+            if (last) break;
+            written += sel_run;
+            if (compact) in_smem = cand;
+            // the bucket of digit t that holds the need-th candidate
+            __syncthreads();
+            uint32_t c = 0;
+            if (tid < kRadix) {
+#pragma unroll
+                for (int w = 0; w < kTopkWarps; ++w) { c += sm.hist[w * kRadix + tid]; sm.hist[w * kRadix + tid] = 0; }
+            }
+            const uint32_t excl = block_excl_scan_256<kTopkThreads>(c, sm.wtot);
+            if (tid < kRadix && c && excl < need && need <= excl + c) {
+                sm.pick[0] = tid;
+                sm.pick[1] = excl;
+                sm.pick[2] = c;
+            }
+            __syncthreads();
+            const uint32_t b = sm.pick[0];
+            need -= sm.pick[1];
+            cand = sm.pick[2];
+            mprev = mcur;
+            vprev = vcur;
+            mcur |= static_cast<U>(0xffu) << shift;
+            vcur |= static_cast<U>(b) << shift;
+            last = cand == need || t + 1 == D;
+        }
+        __syncthreads();  // the next row's pass 0 may compact into the buffer this row's last pass read
+    }
+}
+
+// topk_warp_kernel: rows of row_len <= 32 K keys of `in`; the first k of each sorted row go to row r * k of out / idx_out.
+// With idx_in (the in-place sort of a block-path result: in == out, idx_in == idx_out, row_len == k) the payloads are loaded.
+template <typename KeyT, int K, int RANK_MODE>
+__global__ void __launch_bounds__(kRowWarps * 32)
+topk_warp_kernel(const KeyT* in, KeyT* out, const uint32_t* idx_in, uint32_t* idx_out, uint64_t num_rows, uint32_t row_len,
+                 uint32_t k, KeyCodec codec)
+{
+    using W = RowWarpSmem<KeyT, K, true>;
+    extern __shared__ __align__(16) unsigned char s_raw[];
+    const int warp = threadIdx.x >> 5;
+    W& sm = reinterpret_cast<W*>(s_raw)[warp];
+    const WarpSortCtx<KeyT> x = warp_sort_ctx<KeyT>(sm.hist, codec);
+    for (uint64_t row = static_cast<uint64_t>(blockIdx.x) * kRowWarps + warp; row < num_rows;
+         row += static_cast<uint64_t>(gridDim.x) * kRowWarps)
+        warp_sort_run<KeyT, K, RANK_MODE, true, true>(sm, x, in, out, idx_out, row * row_len, row_len, idx_in, row * k, k);
+}
+
+// topk_sort_kernel: the row sort's block body (ROWS) on the [num_rows, k] block-path result, in place, with the gathered
+// positions as payloads.  A kernel of its own, so that segment_sort_kernel keeps its instantiations.
+template <typename KeyT, int K, int WARPS, int RANK_MODE>
+__global__ void __launch_bounds__(WARPS * 32, 1)
+topk_sort_kernel(KeyT* keys, uint32_t* vals, uint64_t num_rows, uint32_t k, KeyCodec codec)
+{
+    segment_sort_body<KeyT, true, K, WARPS, RANK_MODE, false, true, false>(keys, vals, nullptr, num_rows, k, k, 0u, sizeof(KeyT),
+                                                                          8u, codec, keys, nullptr, nullptr);
+}
+
+template <typename KeyT, int SIZE>
+struct TopkSortShape {
+    using Key = KeyT;
+    static constexpr bool has_hot = false;
+    using G = SegGeomN<KeyT, SIZE>;
+    using S = SegSmem<KeyT, true, G::K, G::WARPS>;
+    static constexpr uint32_t T = S::T;
+    static constexpr size_t smem = sizeof(S);
+    template <int RANK_MODE, bool HOT = false>
+    static auto kernel() { return topk_sort_kernel<KeyT, G::K, G::WARPS, RANK_MODE>; }
+};
+using TopkSortShapes = TypeList<TopkSortShape<uint16_t, 1>, TopkSortShape<uint16_t, 2>, TopkSortShape<uint32_t, 1>,
+                                TopkSortShape<uint32_t, 2>, TopkSortShape<uint64_t, 1>, TopkSortShape<uint64_t, 2>>;
+using TopkKeys = TypeList<uint16_t, uint32_t, uint64_t>;
+
+template <typename KeyT, int K, int RANK_MODE>
+static cudaError_t launch_topk_warp(const KeyT* in, KeyT* out, const uint32_t* idx_in, uint32_t* idx_out, uint64_t num_rows,
+                                    uint32_t row_len, uint32_t k, const KeyCodec& codec, int sm_count, cudaStream_t stream)
+{
+    auto kern = topk_warp_kernel<KeyT, K, RANK_MODE>;
+    constexpr size_t smem = kRowWarps * sizeof(RowWarpSmem<KeyT, K, true>);
+    static const int per_sm = resident_per_sm(kern, kRowWarps * 32, smem);
+    if (per_sm <= 0) return cudaErrorLaunchOutOfResources;
+    const uint64_t need = (num_rows + kRowWarps - 1) / kRowWarps, cap = static_cast<uint64_t>(sm_count) * per_sm;
+    kern<<<static_cast<unsigned>(need < cap ? need : cap), kRowWarps * 32, smem, stream>>>(in, out, idx_in, idx_out, num_rows, row_len,
+                                                                                          k, codec);
+    return cudaGetLastError();
+}
+
+template <typename KeyT, int RANK_MODE>
+static cudaError_t launch_topk_warp_k(const KeyT* in, KeyT* out, const uint32_t* idx_in, uint32_t* idx_out, uint64_t num_rows,
+                                      uint32_t row_len, uint32_t k, const KeyCodec& codec, int sm_count, cudaStream_t stream)
+{
+    if (row_len <= 32) return launch_topk_warp<KeyT, 1, RANK_MODE>(in, out, idx_in, idx_out, num_rows, row_len, k, codec, sm_count, stream);
+    if (row_len <= 64) return launch_topk_warp<KeyT, 2, RANK_MODE>(in, out, idx_in, idx_out, num_rows, row_len, k, codec, sm_count, stream);
+    if (row_len <= 128) return launch_topk_warp<KeyT, 4, RANK_MODE>(in, out, idx_in, idx_out, num_rows, row_len, k, codec, sm_count, stream);
+    return launch_topk_warp<KeyT, 8, RANK_MODE>(in, out, idx_in, idx_out, num_rows, row_len, k, codec, sm_count, stream);
+}
+
+cudaError_t launch_topk_rows(const void* keys_in, void* values_out, uint32_t* indices, uint64_t num_rows, uint32_t row_len,
+                             uint32_t k, int key_bytes, const KeyCodec* codec_in, bool sorted, uint32_t capacity, int rank_mode,
+                             bool block_only, int sm_count, cudaStream_t stream)
+{
+    if (num_rows == 0 || row_len == 0 || k == 0) return cudaSuccess;
+    if (k > row_len || k > row_sort_capacity(key_bytes)) return cudaErrorInvalidValue;
+    const uint32_t cap = capacity && capacity < row_sort_capacity(key_bytes) ? capacity : row_sort_capacity(key_bytes);
+    const KeyCodec codec = codec_in ? *codec_in : KeyCodec();
+    return with_key_type(TopkKeys{}, key_bytes, [&](auto kt) {
+        using KeyT = decltype(kt);
+        const KeyT* in = static_cast<const KeyT*>(keys_in);
+        KeyT* out = static_cast<KeyT*>(values_out);
+        return with_rank_mode(rank_mode, [&](auto r) {
+            constexpr int R = decltype(r)::value;
+            if (row_len <= kRowWarpMaxLen && !block_only)  // sorted already
+                return launch_topk_warp_k<KeyT, R>(in, out, nullptr, indices, num_rows, row_len, k, codec, sm_count, stream);
+            auto kern = topk_select_kernel<KeyT>;
+            static const int per_sm = resident_per_sm(kern, kTopkThreads, sizeof(TopkSmem<KeyT>));
+            if (per_sm <= 0) return cudaErrorLaunchOutOfResources;
+            const uint64_t ctas = static_cast<uint64_t>(per_sm) * sm_count;
+            kern<<<static_cast<unsigned>(num_rows < ctas ? num_rows : ctas), kTopkThreads, sizeof(TopkSmem<KeyT>), stream>>>(
+                in, out, indices, num_rows, row_len, k, cap, codec);
+            cudaError_t e = cudaGetLastError();
+            if (e != cudaSuccess || !sorted || k == 1) return e;
+            if (k <= kRowWarpMaxLen)
+                return launch_topk_warp_k<KeyT, R>(out, out, indices, indices, num_rows, k, k, codec, sm_count, stream);
+            return find_type(
+                TopkSortShapes{},
+                [&](auto s) { using Sh = decltype(s); return std::is_same_v<typename Sh::Key, KeyT> && k <= Sh::T; },
+                [&](auto s) {
+                    using Sh = decltype(s);
+                    const auto sk = Sh::template kernel<R>();
+                    static const int sort_per_sm = resident_per_sm(sk, Sh::S::THREADS, Sh::smem);
+                    if (sort_per_sm <= 0) return cudaErrorLaunchOutOfResources;
+                    const uint64_t sort_ctas = static_cast<uint64_t>(sort_per_sm) * sm_count;
+                    sk<<<static_cast<unsigned>(num_rows < sort_ctas ? num_rows : sort_ctas), Sh::S::THREADS, Sh::smem, stream>>>(
+                        reinterpret_cast<typename Sh::Key*>(out), indices, num_rows, k, codec);
+                    return cudaGetLastError();
+                });
+        });
+    });
+}
+
 cudaError_t configure_kernels()
 {
     cudaError_t e = for_each_type(HistKeys{}, [](auto k) {
@@ -2855,6 +3133,11 @@ cudaError_t configure_kernels()
     if (e == cudaSuccess) e = for_each_type(RingShapes{}, shape);
     if (e == cudaSuccess) e = for_each_type(TileShapes{}, shape);
     if (e == cudaSuccess) e = for_each_type(SegShapes{}, shape);
+    if (e == cudaSuccess) e = for_each_type(TopkSortShapes{}, shape);
+    if (e == cudaSuccess) e = for_each_type(TopkKeys{}, [](auto k) {
+        using KeyT = decltype(k);
+        return set_smem(topk_select_kernel<KeyT>, sizeof(TopkSmem<KeyT>));
+    });
     if (e == cudaSuccess) e = set_smem(fused_kernel<kRankAtomic>(), FusedShape::smem);
     if (e == cudaSuccess) e = set_smem(fused_kernel<kRankBallot>(), FusedShape::smem);
     return e;

@@ -144,6 +144,16 @@ cudaError_t launch_sort_segments(const void* keys_in, void* keys_out, uint32_t* 
                                  const KeyCodec* codec, int rank_mode, int sm_count, uint32_t* list,
                                  unsigned long long* counts, cudaStream_t stream);
 
+// Row top-k (osb200_topk_rows): the first k keys of row r = [r * row_len, (r + 1) * row_len) of keys_in in its stable sort, and
+// their positions within the row, into [r * k, (r + 1) * k) of values_out and indices.  Rows of at most kRowWarpMaxLen keys are
+// sorted one per warp unless block_only; longer rows are radix-selected one per CTA (topk_select_kernel), the candidates held
+// in shared memory once at most `capacity` of them are left (0: row_sort_capacity(key_bytes)).  sorted: the block path's
+// result is then sorted in place (a second launch); without it the k pairs of a row are in an unspecified order.
+// k in 1 .. min(row_len, row_sort_capacity(key_bytes)); the codec as for launch_row_sort.
+cudaError_t launch_topk_rows(const void* keys_in, void* values_out, uint32_t* indices, uint64_t num_rows, uint32_t row_len,
+                             uint32_t k, int key_bytes, const KeyCodec* codec, bool sorted, uint32_t capacity, int rank_mode,
+                             bool block_only, int sm_count, cudaStream_t stream);
+
 // Validate (reference: Validate, UtilityKernels.cuh:403-429): err_count += #(keys[i] > keys[i+1]).
 cudaError_t launch_validate(const void* keys, uint64_t n, int key_bytes, unsigned long long* err_count, int sm_count,
                             cudaStream_t stream);

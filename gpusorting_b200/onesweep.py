@@ -238,6 +238,35 @@ class OneSweepSorter:
                   "osb200_sort_rows")
         return (out, idx) if return_indices else out
 
+    # -- row top-k: the first k keys of every row's stable sort, no workspace (any sorter will do) ------------------------
+    def topk_rows(self, x: torch.Tensor, k: int, key_type: str, largest: bool = True, sorted: bool = True, stream=None):
+        """The k largest (or smallest) keys of every row of `x` along its last dimension and their positions
+        (osb200_topk_rows), the shape of ``torch.topk(x, k, dim=-1, largest, sorted)``.  `x` and key_type as in sort_rows.
+        The selected set is exactly the first k columns of the stable row sort (descending for largest): of equal keys at
+        the boundary the lowest positions are taken.  sorted=True returns them in that order, bit-identical to
+        ``sort_rows(x, descending=largest)`` cut to k; sorted=False returns the same pairs in an unspecified order.
+
+        Returns (values, indices) shaped ``x.shape[:-1] + (k,)``, indices as torch.int32 positions within the row, allocated
+        with torch.empty on the stream.  The rows may be of any length; k may be at most 16,384 (8,192 for 8-byte dtypes)
+        and at most the row length."""
+        if not (isinstance(x, torch.Tensor) and x.is_cuda and x.is_contiguous() and x.dim() >= 1 and x.dtype in _ROW_KEY_TYPES):
+            raise TypeError(f"x must be a contiguous CUDA tensor of rank >= 1 with dtype in {tuple(_ROW_KEY_TYPES)}")
+        if x.device.index != self.device:
+            raise ValueError(f"x lives on cuda:{x.device.index}, the sorter on cuda:{self.device}")
+        kb = x.element_size()
+        kt = (KEY16_TYPES if kb == 2 else KEY_TYPES)[key_type]
+        k = int(k)
+        row_len = x.shape[-1]
+        num_rows = x.numel() // row_len if row_len else 0
+        shape = tuple(x.shape[:-1]) + (k,)
+        with torch.cuda.stream(stream):  # (None: the current stream) the outputs belong to the stream that writes them
+            out = torch.empty(shape, dtype=x.dtype, device=x.device)
+            idx = torch.empty(shape, dtype=torch.int32, device=x.device)
+        with torch.cuda.device(self.device):
+            check(lib.osb200_topk_rows(self._h, x.data_ptr(), out.data_ptr(), idx.data_ptr(), num_rows, row_len, k, kb, kt,
+                                       1 if largest else 0, 1 if sorted else 0, _stream_ptr(stream)), "osb200_topk_rows")
+        return out, idx
+
     # -- segment sort: ragged rows given by offsets -------------------------------------------------------------------------
     def sort_segments(self, x: torch.Tensor, offsets: torch.Tensor, key_type: str, descending: bool = False,
                       return_indices: bool = True, inplace: bool = False, max_segment_len: Optional[int] = None, stream=None):
@@ -469,6 +498,21 @@ def sort_rows(x: torch.Tensor, descending: bool = False, return_indices: bool = 
         sp = _stream_ptr(stream)
     s = _cached_sorter(x.device.index, 4, 4, 1, sp)
     return s.sort_rows(x, _ROW_KEY_TYPES[x.dtype], descending, return_indices, False, stream)
+
+
+def topk(x: torch.Tensor, k: int, largest: bool = True, sorted: bool = True, stream=None):
+    """``torch.topk(x, k, dim=-1, largest, sorted)`` for a contiguous CUDA tensor of one of sort_rows' ten dtypes: (values,
+    int32 positions within the row), with ties taken in input order -- exactly the first k columns of the stable row sort.
+    The key type follows the dtype.  OneSweepSorter.topk_rows on the stream's cached (4, 4) sorter, the one argsort uses
+    (the top-k needs no workspace)."""
+    if not (isinstance(x, torch.Tensor) and x.is_cuda):
+        raise TypeError("x must be a CUDA tensor")
+    if x.dtype not in _ROW_KEY_TYPES:
+        raise TypeError(f"x.dtype must be one of {tuple(_ROW_KEY_TYPES)}")
+    with torch.cuda.device(x.device.index):
+        sp = _stream_ptr(stream)
+    s = _cached_sorter(x.device.index, 4, 4, 1, sp)
+    return s.topk_rows(x, k, _ROW_KEY_TYPES[x.dtype], largest, sorted, stream)
 
 
 def sort_segments(x: torch.Tensor, offsets: torch.Tensor, descending: bool = False, return_indices: bool = True,

@@ -82,6 +82,16 @@ class OneSweepSorterB200 {
                                stream),
               "osb200_sort_rows");
     }
+    // the first k keys of every row [r*row_len, (r+1)*row_len) in its stable sort (ascending, or descending for largest) and
+    // their positions within the row, into [r*k, (r+1)*k) of d_values_out and d_indices; sorted = false leaves each row's k
+    // pairs in an unspecified order; any row_len, k <= 16,384 (8,192 for 8-byte keys); any sorter
+    void TopkRows(const void* d_keys_in, void* d_values_out, uint32_t* d_indices, uint64_t num_rows, uint32_t row_len, uint32_t k,
+                  int key_bytes, int key_type, bool largest, bool sorted, void* stream = nullptr)
+    {
+        check(osb200_topk_rows(h_, d_keys_in, d_values_out, d_indices, num_rows, row_len, k, key_bytes, key_type, largest ? 1 : 0,
+                               sorted ? 1 : 0, stream),
+              "osb200_topk_rows");
+    }
     // every segment [offsets[s], offsets[s+1]) of n keys sorted stable into the same positions of d_keys_out (ragged rows);
     // d_indices may be null; max_segment_len <= 16,384 (8,192 for 8-byte keys); num_segments <= the handle's max_n
     void SortSegments(const void* d_keys_in, void* d_keys_out, uint32_t* d_indices, uint64_t n, const uint64_t* d_segment_offsets,

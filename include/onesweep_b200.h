@@ -200,6 +200,27 @@ OSB200_API int osb200_sort_segments(osb200_handle h, const void* d_keys_in, void
                                     const uint64_t* d_segment_offsets, uint64_t num_segments, uint32_t max_segment_len,
                                     int key_bytes, int key_type, int descending, void* stream);
 
+/* Row top-k: the k smallest (largest = 0) or largest (largest = 1) keys of every row and their positions, the shape of
+ * torch.topk(x, k, dim=-1, largest, sorted).  Row r of d_keys_in is elements [r*row_len, (r+1)*row_len); its result is
+ * [r*k, (r+1)*k) of d_values_out and d_indices (uint32 positions within the row, required).
+ *   key_bytes / key_type: those of osb200_sort_rows.  largest = 1 selects through the descending codec, as descending does there.
+ *   The selected set is exactly the first k keys of the row's stable sort (ascending, or descending for largest = 1): of equal
+ *   keys at the boundary the lowest positions are taken.  sorted = 1 writes them in that order, bit-identical to the first k
+ *   columns of osb200_sort_rows with descending = largest; sorted = 0 writes the same k (key, position) pairs in an
+ *   unspecified order.
+ * row_len may be any uint32; k may be at most 16,384 (2- and 4-byte keys) or 8,192 (8-byte keys): OSB200_ERR_SIZE above.
+ * k > row_len is OSB200_ERR_INVALID_ARG; num_rows == 0, row_len == 0 or k == 0 is a no-op.  Natural alignment of the keys and
+ * 4-byte alignment of the indices are required; array sizes that overflow 64 bits, a null pointer and any overlap between the
+ * input and either output or between the two outputs are OSB200_ERR_INVALID_ARG (there is no in-place form).
+ * Any handle will do: the call uses only the handle's device, rank mode, SM count and the test hooks "debug_rows_block" and
+ * "debug_topk_capacity", and allocates nothing.  Rows of at most 256 keys are sorted one per warp and cut to k; longer rows
+ * are radix-selected one per thread block, from the most significant digit, with the candidates in shared memory once at
+ * most 16,384 (8,192) of them are left.  sorted = 1 then sorts the [num_rows, k] result in place.  At most two launches:
+ * asynchronous, no host synchronisation, graph-capturable. */
+OSB200_API int osb200_topk_rows(osb200_handle h, const void* d_keys_in, void* d_values_out, uint32_t* d_indices,
+                                uint64_t num_rows, uint32_t row_len, uint32_t k, int key_bytes, int key_type,
+                                int largest, int sorted, void* stream);
+
 /* Sort on a bit range [begin_bit, end_bit) of the (unsigned) key only, CUB-style: keys that agree on those bits keep their
  * input order (stable).  ceil((end_bit-begin_bit)/8) digit passes instead of key_bytes; the last digit may be narrower
  * than 8 bits; an odd pass count is handled inside (the result is always returned in the caller's buffers).  d_values may
@@ -275,7 +296,11 @@ OSB200_API int osb200_init_random_u32(uint32_t* d_keys, uint32_t* d_payload, uin
  *   "debug_max_ctas" test hook of the persistent DigitBinningPass (uint32 keys, HOT passes): N > 0 runs it on at most N CTAs (the tiles after
  *                    each CTA's first are handed out by an atomic ticket); 0 (default) = as many as can be resident
  *   "debug_rows_block"  test hook of osb200_sort_rows: 1 = rows of at most 256 keys go through the block path (2,048-key
- *                    geometry) instead of one warp per row, to compare the two paths; 0 (default) = the warp path
+ *                    geometry) instead of one warp per row, to compare the two paths; 0 (default) = the warp path.
+ *                    osb200_topk_rows honours it too: its rows of at most 256 keys are then radix-selected one per block
+ *   "debug_topk_capacity"  test hook of osb200_topk_rows: N > 0 keeps at most N candidates of a row in shared memory (instead
+ *                    of 16,384, or 8,192 for 8-byte keys), so that short rows exercise the passes that read global memory
+ *                    and the switch to shared memory; 0 (default) = the full capacity
  *   "debug_epoch"    test hook of the descriptor epochs: sets the handle's epoch counter (0 .. 2^24 - 1; info "epoch"), so
  *                    that the next passes cross the wrap-around (which clears every descriptor) or reuse the epochs of a
  *                    captured sort
