@@ -3,11 +3,13 @@
 
 Keys are compared through their radix image: the unsigned key whose ascending order is the requested order of the typed
 value (tests.oraclelib.to_radix and tests.test_gpu_keys16.radix16, restated here in torch so they run on the device).  A
-64-bit image is kept in an int64 container and a 16-bit one in int32 (0 .. 65535); ordered() turns either into a tensor
-whose signed order is the key order.  Every checker reads keys as raw bits (float NaNs compare unequal to themselves)."""
+64-bit image is kept in an int64 container, a 32-bit one in int64 (0 .. 2^32 - 1) and a 16-bit one in int32 (0 .. 65535);
+ordered() turns any of them into a tensor whose signed order is the key order.  Every checker reads keys as raw bits
+(float NaNs compare unequal to themselves)."""
 import torch
 
 SIGN64 = -(1 << 63)
+MASK32 = 0xFFFFFFFF
 _INT_OF_WIDTH = {2: torch.int16, 4: torch.int32, 8: torch.int64}
 
 
@@ -37,6 +39,31 @@ def from_radix64(r: torch.Tensor, kind: str, descending: bool = False) -> torch.
     return u
 
 
+def as_int32(u: torch.Tensor) -> torch.Tensor:
+    """32-bit patterns held as int64 0 .. 2^32 - 1, as the int32 container of the same bits"""
+    return ((u ^ 0x80000000) - 0x80000000).to(torch.int32)
+
+
+def to_radix32(bits: torch.Tensor, kind: str, descending: bool = False) -> torch.Tensor:
+    """oraclelib.to_radix for 32-bit containers: kind "u", "i" or "f"; the uint32 image as int64 (0 .. 2^32 - 1)"""
+    u = bits_of(bits).to(torch.int64) & MASK32
+    if kind == "i":
+        u = u ^ 0x80000000
+    elif kind == "f":
+        u = torch.where(u >= 0x80000000, u ^ MASK32, u | 0x80000000)
+    return u ^ MASK32 if descending else u
+
+
+def from_radix32(r: torch.Tensor, kind: str, descending: bool = False) -> torch.Tensor:
+    """inverse of to_radix32: the int32 bits whose radix image is `r` (int64, 0 .. 2^32 - 1)"""
+    u = r ^ MASK32 if descending else r
+    if kind == "i":
+        u = u ^ 0x80000000
+    elif kind == "f":
+        u = torch.where(u >= 0x80000000, u ^ 0x80000000, u ^ MASK32)
+    return as_int32(u)
+
+
 def radix16(bits: torch.Tensor, key_type: str, descending: bool = False) -> torch.Tensor:
     """test_gpu_keys16.radix16 for 16-bit containers (key_type "u16", "i16", "f16" or "bf16"): the image as int32"""
     u = bits_of(bits).to(torch.int32) & 0xFFFF
@@ -58,15 +85,47 @@ def from_radix16(r: torch.Tensor, key_type: str, descending: bool = False) -> to
 
 
 def key_radix(key_type: str, descending: bool = False):
-    """the radix image function of a key type of 16 or 64 bits ("u16" .. "bf16", "u64", "i64", "f64")"""
+    """the radix image function of a key type ("u16" .. "bf16", "u32", "i32", "f32", "u64", "i64", "f64")"""
     if key_type in ("u64", "i64", "f64"):
         return lambda bits: to_radix64(bits, key_type[0], descending)
+    if key_type in ("u32", "i32", "f32"):
+        return lambda bits: to_radix32(bits, key_type[0], descending)
     return lambda bits: radix16(bits, key_type, descending)
 
 
 def ordered(r: torch.Tensor) -> torch.Tensor:
-    """a radix image as a tensor whose signed order is its unsigned order (16-bit images in int32 already are)"""
+    """a radix image as a tensor whose signed order is its unsigned order (16-bit images in int32 already are, and 32-bit
+    ones in int64 keep their order with the sign bit set)"""
     return r ^ SIGN64 if r.dtype == torch.int64 else r
+
+
+# ---- an affine permutation of 32-bit keys and its sort ---------------------------------------------------------------------
+# key[i] = (a i + b) mod 2^bits, a odd, for i < n <= 2^bits: n distinct keys, and the keys of consecutive positions run
+# through every residue of the low byte, so every 256 aligned positions hold each low byte once.  The ascending sort is
+# known without a sort: with M the m = 2^bits - n values left out (those of i = n .. 2^bits - 1), sorted, output position
+# p holds the p-th value not in M, which is p + #{j : M[j] - j <= p}.
+def affine_keys(a: int, b: int, lo: int, hi: int, bits: int = 32, device=None) -> torch.Tensor:
+    """the keys of positions [lo, hi) as int64 (0 .. 2^bits - 1); a < 2^31, so that a i fits int64 for every i < 2^32"""
+    assert a % 2 == 1 and 0 < a < (1 << 31)
+    i = torch.arange(lo, hi, dtype=torch.int64, device=device)
+    return (a * i + b) & ((1 << bits) - 1)
+
+
+def affine_gaps(a: int, b: int, n: int, bits: int = 32, device=None) -> torch.Tensor:
+    """M[j] - j (non-decreasing) for the sorted values M that the n keys leave out"""
+    m = torch.sort(affine_keys(a, b, n, 1 << bits, bits, device)).values
+    return m - torch.arange(m.numel(), dtype=torch.int64, device=device)
+
+
+def affine_sorted(gaps: torch.Tensor, lo: int, hi: int) -> torch.Tensor:
+    """positions [lo, hi) of the ascending sort of the n keys, as int64"""
+    p = torch.arange(lo, hi, dtype=torch.int64, device=gaps.device)
+    return p + torch.searchsorted(gaps, p, right=True)
+
+
+def sort_by_low_byte(t: torch.Tensor) -> None:
+    """reorders the keys of `t` in place, stable, by their low byte: a window of such keys concentrates each digit of place 0"""
+    t.copy_(t[torch.sort(t & 0xFF, stable=True).indices])
 
 
 # ---- checkers ------------------------------------------------------------------------------------------------------------
@@ -125,6 +184,31 @@ def check_sorted_keys16(out: torch.Tensor, src: torch.Tensor, radix, chunk: int)
         v = int(bad[0, 0])
         raise AssertionError(f"radix value {v:#06x}: {int(h_in[v])} in the input, {int(h_out[v])} in the output "
                              f"({bad.numel()} values differ)")
+
+
+def check_topk_rows(vals: torch.Tensor, idx: torch.Tensor, src: torch.Tensor, radix, k: int, sorted: bool,
+                    chunk: int) -> None:
+    """`vals` and `idx` ([rows, k]) must be the first k columns of torch.sort(stable=True) of every row's radix image in `src`
+    ([rows, row_len]): the positions in that order when `sorted`, else the same positions in any order (each row's pairs
+    are sorted by position first, and compared with the reference's first k sorted by position); and every key must be the
+    bits of src at its position.  Whole rows at a time (at least one row per step)."""
+    row_len = src.shape[-1]
+    s2 = bits_of(src).reshape(-1, row_len)
+    v2, i2 = bits_of(vals).reshape(-1, k), idx.reshape(-1, k)
+    assert k <= row_len and v2.shape == i2.shape == (s2.shape[0], k), f"shapes {vals.shape}, {idx.shape} and {src.shape}"
+    rows = s2.shape[0]
+    step = max(1, chunk // row_len)
+    for a in range(0, rows, step):
+        b = min(a + step, rows)
+        want = torch.sort(ordered(radix(s2[a:b])), dim=-1, stable=True).indices[:, :k]
+        got_i, got_v = positions(i2[a:b]), v2[a:b]
+        if not sorted:
+            got_i, by_pos = torch.sort(got_i, dim=-1)
+            got_v = torch.gather(got_v, 1, by_pos)
+            want = torch.sort(want, dim=-1).values
+        _require(got_i == want, "positions differ from the stable sort of the row cut to k", a * k, k)
+        _require(got_v == torch.gather(s2[a:b], 1, want), "keys differ from the row's keys at those positions", a * k, k)
+        del want, got_i, got_v
 
 
 def check_rows(out: torch.Tensor, idx, src: torch.Tensor, radix, chunk: int) -> None:

@@ -103,3 +103,29 @@ def test_workspace_holds_the_regions():
         rest = tiles * RADIX * 8 + (tiles + 8) * RADIX * 2 * 4 + control
         assert g.lib.osb200_workspace_bytes(n, 4, 0) == 4 * alt + rest, n
         assert g.lib.osb200_workspace_bytes(n, 4, 4) == 4 * alt + 4 * n + rest, n
+
+
+WINDOW_N = (1 << 32) - (1 << 20) - 3  # the fused sort of tests/test_gpu_large_n_new_paths.py
+
+
+def test_regions_reach_past_element_2pow32():
+    """the largest fused sorts put their last regions beyond element 2^32 of the alt buffer: at WINDOW_N keys element 2^32
+    falls inside region 248, and regions 249-255 start past it"""
+    n = WINDOW_N
+    c = region_keys(n)
+    assert fused_eligible(n) and (n + TILE - 1) // TILE == 262_080 and c == 17_298_304
+    assert RADIX * c > 1 << 32 and (1 << 32) // c == 248
+    assert 248 * c < (1 << 32) < 249 * c
+    # the smallest n whose regions pass element 2^32
+    assert RADIX * region_keys(4_164_562_689) > 1 << 32 >= RADIX * region_keys(4_164_562_688)
+
+
+def test_workspace_holds_the_regions_past_2pow32():
+    import gpusorting_b200 as g
+
+    n = WINDOW_N
+    alt = RADIX * region_keys(n)
+    assert alt > n  # the alt buffer is sized for the regions, not for the n keys
+    tiles = (n + 8191) // 8192  # as in test_workspace_holds_the_regions
+    rest = tiles * RADIX * 8 + (tiles + 8) * RADIX * 2 * 4 + 2 * 8 * RADIX * 8 + 64 + 64 + 64
+    assert g.lib.osb200_workspace_bytes(n, 4, 0) == 4 * alt + rest

@@ -1,7 +1,10 @@
 """The chunked checkers of tests/bigcheck.py, on CPU tensors: their torch radix images equal the numpy ones the other tests
 use, they accept the stable sort, and they reject each way a large sort could be subtly wrong -- payloads of equal keys
 swapped, a payload off by 2^32 or past n, a key changed, an inversion exactly at a chunk border, a value replaced by its
-neighbour (still sorted, but not a permutation), and a row whose indices are unstable.  No GPU needed."""
+neighbour (still sorted, but not a permutation), and a row whose indices are unstable.  The affine permutation's known
+sort equals np.sort at a small modulus, and the top-k checker names the first bad row of each planted defect: a swapped
+pair, a tie taken at a higher position, an index off by one, a key that is not src[idx], an unsorted output passed as
+sorted and a pair missing from an unsorted output.  No GPU needed."""
 import numpy as np
 import pytest
 import torch
@@ -216,3 +219,157 @@ def test_check_rows(key_type, descending, row_len):
     o[r, c] = out[r, c + 1]
     rejects(o, idx, f"keys differ .*: first at output row {r}, column {c}")
     rejects(out[:-1], idx[:-1], "shapes")
+
+
+# ---- 32-bit radix images -------------------------------------------------------------------------------------------------
+SPECIALS32 = np.array([0, 1, 0x7FFFFFFF, 0x80000000, 0x80000001, 0xFFFFFFFF, 0x7F800000, 0xFF800000, 0x7FC00000,
+                       0xFFC00000, 0x7F800001, 0xFF800001, 0x00000001, 0x80000001, 0x3F800000, 0xBF800000], dtype=np.uint32)
+
+
+@pytest.mark.parametrize("descending", [False, True])
+@pytest.mark.parametrize("kind", ["u", "i", "f"])
+def test_radix32_images_match_numpy(kind, descending):
+    """NaNs of both signs, +-0, +-inf and the extremes of every kind included"""
+    rng = np.random.default_rng(5)
+    bits = np.concatenate([rng.integers(0, 1 << 32, 4096, dtype=np.uint64).astype(np.uint32), SPECIALS32])
+    got = bc.to_radix32(torch.from_numpy(bits.view(np.int32).copy()), kind, descending)
+    assert got.dtype == torch.int64 and int(got.min()) >= 0 and int(got.max()) <= 0xFFFFFFFF
+    want = to_radix(bits, kind, descending)
+    np.testing.assert_array_equal(got.numpy().astype(np.uint32), want)
+    back = bc.from_radix32(got, kind, descending)
+    assert back.dtype == torch.int32
+    np.testing.assert_array_equal(back.numpy().view(np.uint32), bits)
+    back = bc.from_radix32(torch.from_numpy(want.astype(np.int64)), kind, descending)
+    np.testing.assert_array_equal(back.numpy().view(np.uint32), from_radix(want, kind, descending))
+    # the images sort like numpy's, through ordered() and through key_radix
+    order = torch.sort(bc.ordered(bc.key_radix(kind + "32", descending)(torch.from_numpy(bits.view(np.int32).copy()))),
+                       stable=True).indices
+    np.testing.assert_array_equal(order.numpy(), np.argsort(want, kind="stable"))
+
+
+# ---- the affine permutation's sort -----------------------------------------------------------------------------------------
+@pytest.mark.parametrize("window", [False, True])
+@pytest.mark.parametrize("a,b", [(0x2545F491, 0x9E3779B9), (1, 0), (0x7FFFFFFF, 12345)])
+def test_affine_sorted_is_the_sort(a, b, window):
+    """at modulus 2^20 with n = 2^20 - 37 (37 values left out), with and without a window of keys sorted by their low byte"""
+    bits, n = 20, (1 << 20) - 37
+    keys = bc.affine_keys(a, b, 0, n, bits)
+    assert torch.unique(keys).numel() == n
+    assert bool((torch.bincount((keys[:n // 256 * 256] & 0xFF).reshape(-1, 256)[7], minlength=256) == 1).all())
+    if window:
+        lo, hi = 8192, 8192 + 4096
+        bc.sort_by_low_byte(keys[lo:hi])
+        assert bool((keys[lo:lo + 16] & 0xFF == 0).all()) and bool((keys[hi - 16:hi] & 0xFF == 255).all())
+        assert torch.equal(torch.sort(keys).values, torch.sort(bc.affine_keys(a, b, 0, n, bits)).values)
+    gaps = bc.affine_gaps(a, b, n, bits)
+    assert gaps.numel() == 37 and bool((gaps[1:] >= gaps[:-1]).all())
+    want = np.sort(keys.numpy())
+    np.testing.assert_array_equal(bc.affine_sorted(gaps, 0, n).numpy(), want)
+    for lo, hi in ((0, 1), (1000, 5000), (n - 77, n)):  # any chunk
+        np.testing.assert_array_equal(bc.affine_sorted(gaps, lo, hi).numpy(), want[lo:hi])
+
+
+def test_affine_gaps_names_the_left_out_values():
+    a, b, bits, n = 0x2545F491, 77, 12, 4000
+    gaps = bc.affine_gaps(a, b, n, bits)
+    left_out = np.setdiff1d(np.arange(1 << bits), bc.affine_keys(a, b, 0, n, bits).numpy())
+    np.testing.assert_array_equal(gaps.numpy() + np.arange(left_out.size), left_out)
+
+
+# ---- row top-k -----------------------------------------------------------------------------------------------------------
+def topk_case(key_type, largest, rows, row_len, k, seed=6):
+    """(src, vals, idx) of the stable top k, sorted; a third of the keys come from 8 values, and every row has equal keys on
+    both sides of its boundary"""
+    rng = np.random.default_rng(seed)
+    if key_type == "f32":
+        bits = rng.integers(0, 1 << 32, rows * row_len, dtype=np.uint64).astype(np.uint32)
+        tied = rng.random(bits.size) < 0.35
+        bits[tied] = bits[rng.integers(0, 8, int(tied.sum()))]
+        bits[rng.choice(bits.size, SPECIALS32.size, replace=False)] = SPECIALS32
+    else:
+        bits = random_bits(rng, rows * row_len, key_type)
+
+    def image(bits):
+        return to_radix(bits, "f", largest) if key_type == "f32" else np_radix(bits, key_type, largest)
+
+    # a tie across the boundary of every row: the first key left out becomes a copy of the last one taken
+    b2 = bits.reshape(rows, row_len)
+    order = np.argsort(image(bits).reshape(rows, row_len), axis=-1, kind="stable")
+    b2[np.arange(rows), order[:, k]] = b2[np.arange(rows), order[:, k - 1]]
+    order = np.argsort(image(bits).reshape(rows, row_len), axis=-1, kind="stable")[:, :k]
+    src = (torch.from_numpy(bits.view(np.int32).copy()) if key_type == "f32" else as_torch(bits)).reshape(rows, row_len)
+    vals = torch.gather(src, 1, torch.from_numpy(order))
+    return src, vals, torch.from_numpy(order.astype(np.int32))
+
+
+def shuffled_rows(vals, idx, seed=7):
+    """every row's pairs in another order (the same one for keys and positions)"""
+    perm = torch.argsort(torch.from_numpy(np.random.default_rng(seed).random(tuple(idx.shape))), dim=-1)
+    return torch.gather(vals, 1, perm), torch.gather(idx, 1, perm)
+
+
+@pytest.mark.parametrize("key_type,largest", [("f32", True), ("f32", False), ("bf16", True), ("u16", False),
+                                              ("f64", True), ("i64", False)])
+@pytest.mark.parametrize("row_len,k", [(4, 2), (300, 50)])
+def test_check_topk_rows(key_type, largest, row_len, k):
+    radix = bc.key_radix(key_type, largest)
+    rows = 3 * CHUNK // row_len + 7 if row_len < CHUNK else 9
+    src, vals, idx = topk_case(key_type, largest, rows, row_len, k)
+    uv, ui = shuffled_rows(vals, idx)
+    for chunk in (CHUNK, 1, rows * row_len):
+        bc.check_topk_rows(vals, idx, src, radix, k, True, chunk)
+        bc.check_topk_rows(vals, idx, src, radix, k, False, chunk)
+        bc.check_topk_rows(uv, ui, src, radix, k, False, chunk)
+    r0 = rows - 2  # the planted defects go into a row of a later step than the first
+
+    def rejects(v, i, srt, match):
+        with pytest.raises(AssertionError, match=match):
+            bc.check_topk_rows(v, i, src, radix, k, srt, CHUNK)
+
+    bits = bc.bits_of(src)
+    img = bc.ordered(radix(src))
+    # a swapped pair: two columns of different keys exchanged, keys and positions
+    vb = bc.bits_of(vals)
+    r = next(r for r in range(r0, rows) if bool((vb[r, 1:] != vb[r, :-1]).any()))
+    c = int(torch.nonzero(vb[r, 1:] != vb[r, :-1])[0, 0])
+    v, i = vals.clone(), idx.clone()
+    v[r, c], v[r, c + 1] = vals[r, c + 1], vals[r, c]
+    i[r, c], i[r, c + 1] = idx[r, c + 1], idx[r, c]
+    rejects(v, i, True, f"positions differ .*: first at output row {r}, column {c}")
+    # a tie taken at a higher position: the last key taken has an equal key behind the first k, which replaces it
+    found = None
+    for r in range(r0, rows):
+        last = img[r, int(idx[r, k - 1])]
+        later = torch.nonzero(img[r] == last).reshape(-1)
+        later = later[later > int(idx[r, k - 1])]
+        taken = set(idx[r].tolist())
+        later = [p for p in later.tolist() if p not in taken]
+        if later:
+            found = (r, later[0])
+            break
+    assert found is not None, "no row of the last step has a tie at its boundary"
+    r, p = found
+    for srt, (v0, i0) in ((True, (vals, idx)), (False, (uv, ui))):
+        v, i = v0.clone(), i0.clone()
+        c = int(torch.nonzero(i0[r] == idx[r, k - 1])[0, 0])
+        i[r, c] = p
+        bc.bits_of(v)[r, c] = bits[r, p]
+        rejects(v, i, srt, f"positions differ .*: first at output row {r}")
+    # an index off by one
+    for srt, (v0, i0) in ((True, (vals, idx)), (False, (uv, ui))):
+        i = i0.clone()
+        i[r0, k // 2] += 1 if int(i0[r0, k // 2]) + 1 < row_len else -1
+        rejects(v0, i, srt, f"positions differ .*: first at output row {r0}")
+    # a key that is not src[idx]
+    for srt, (v0, i0) in ((True, (vals, idx)), (False, (uv, ui))):
+        v = v0.clone()
+        bc.bits_of(v)[r0, k - 1] ^= 1
+        rejects(v, i0, srt, f"keys differ .*: first at output row {r0}")
+    # an unsorted output passed as sorted: the first row whose order the shuffle changed is named
+    r = next(r for r in range(rows) if not torch.equal(ui[r], idx[r]))
+    rejects(uv, ui, True, f"positions differ .*: first at output row {r},")
+    # one element missing from an unsorted output: a pair of the row written twice
+    v, i = uv.clone(), ui.clone()
+    v[r0, 0], i[r0, 0] = uv[r0, 1], ui[r0, 1]
+    rejects(v, i, False, f"positions differ .*: first at output row {r0}")
+    rejects(vals[:-1], idx[:-1], True, "shapes")
