@@ -20,6 +20,7 @@ from .onesweep import (  # noqa: F401
     sort_rows,
     sort_segments,
     topk,
+    topk_segments,
 )
 
 __version__ = "0.1.0"

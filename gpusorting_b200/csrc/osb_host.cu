@@ -24,12 +24,13 @@
 
 namespace {
 
-constexpr int kVersion = 1008;  // 1002: device plan, bit ranges, forward-progress fallback, hot passes, segmented sort; 1003: argsort;
+constexpr int kVersion = 1009;  // 1002: device plan, bit ranges, forward-progress fallback, hot passes, segmented sort; 1003: argsort;
                                 // 1004: 16-bit keys (osb200_sort_keys16, osb200_sort_pairs16, osb200_argsort16);
                                 // 1005: row sort (osb200_sort_rows);
                                 // 1006: 64-bit keys with uint32 payloads and their argsort (osb200_create_pairs64);
                                 // 1007: segment sort by offsets (osb200_sort_segments);
-                                // 1008: row top-k (osb200_topk_rows)
+                                // 1008: row top-k (osb200_topk_rows);
+                                // 1009: segment top-k (osb200_topk_segments)
 constexpr int kMaxPlaces = 8;
 
 inline int cuda_status(cudaError_t e) { return e == cudaSuccess ? OSB200_OK : OSB200_ERR_CUDA - static_cast<int>(e); }
@@ -788,6 +789,47 @@ int osb200_topk_rows(osb200_handle h, const void* d_keys_in, void* d_values_out,
     OSB_TRY(osb::launch_topk_rows(d_keys_in, d_values_out, d_indices, num_rows, row_len, k, key_bytes, codec, sorted != 0,
                                   h->debug_topk_capacity, h->cfg.rank_mode, h->debug_rows_block, h->sm_count,
                                   static_cast<cudaStream_t>(stream)));
+    return OSB200_OK;
+}
+
+// Segment top-k: row top-k for ragged segments.  Workspace as for osb200_sort_segments: one u32 per segment of the alt key
+// buffer for the class lists and the 4 u64 class counts in the control block's scratch words.
+int osb200_topk_segments(osb200_handle h, const void* d_keys_in, void* d_values_out, uint32_t* d_indices, uint64_t n,
+                         const uint64_t* d_segment_offsets, uint64_t num_segments, uint32_t k, int key_bytes, int key_type,
+                         int largest, int sorted, void* stream)
+{
+    if (check_handle(h) != OSB200_OK) return OSB200_ERR_INVALID_ARG;
+    osb::KeyCodec c;
+    const osb::KeyCodec* codec = nullptr;
+    int st = key_bytes == 2 ? make_codec16(key_type, largest, &c, &codec)
+             : key_bytes == 4 || key_bytes == 8 ? make_codec(key_bytes, key_type, largest, &c, &codec)
+                                                : OSB200_ERR_INVALID_ARG;
+    if (st != OSB200_OK) return st;
+    // (n == 0 is not a no-op: every row is then padding)
+    if (num_segments == 0 || k == 0) return OSB200_OK;
+    const uintptr_t in = reinterpret_cast<uintptr_t>(d_keys_in), out = reinterpret_cast<uintptr_t>(d_values_out),
+                    idx = reinterpret_cast<uintptr_t>(d_indices), off = reinterpret_cast<uintptr_t>(d_segment_offsets);
+    if ((!in && n) || !out || !idx || !off) return OSB200_ERR_INVALID_ARG;
+    // the kernels load and store element by element: natural alignment is enough
+    if (((in | out) & static_cast<uintptr_t>(key_bytes - 1)) || (idx & 3u) || (off & 7u)) return OSB200_ERR_INVALID_ARG;
+    // the array sizes in bytes must fit in 64 bits
+    if (n > UINT64_MAX / 8 || num_segments > UINT64_MAX / 8 - 1 || num_segments > UINT64_MAX / 8 / k) return OSB200_ERR_INVALID_ARG;
+    const uint64_t m = num_segments * k;
+    const uint64_t kb = n * static_cast<uint64_t>(key_bytes), ob = m * static_cast<uint64_t>(key_bytes), ib = m * sizeof(uint32_t),
+                   fb = (num_segments + 1) * sizeof(uint64_t);
+    // the outputs have another shape than the input: no in-place form, and no overlap between any two of the four arrays
+    if ((in && (overlaps(in, kb, out, ob) || overlaps(in, kb, idx, ib) || overlaps(in, kb, off, fb))) || overlaps(out, ob, idx, ib) ||
+        overlaps(off, fb, out, ob) || overlaps(off, fb, idx, ib))
+        return OSB200_ERR_INVALID_ARG;
+    if (k > osb::row_sort_capacity(key_bytes)) return OSB200_ERR_SIZE;
+    // the class lists take one u32 per segment of the alt key buffer; segment ids are u32
+    if (num_segments > h->max_n || num_segments > (1ull << 32)) return OSB200_ERR_SIZE;
+    static_assert(ControlLayout::err_bytes >= 4 * sizeof(unsigned long long), "the class counts live in the scratch words");
+    c.flags = osb::kCodecEncodeOnLoad | osb::kCodecDecodeOnStore;
+    OSB_TRY(osb::launch_topk_segments(d_keys_in, d_values_out, d_indices, n, reinterpret_cast<const unsigned long long*>(d_segment_offsets),
+                                      num_segments, k, key_bytes, codec, sorted != 0, h->debug_topk_capacity, h->cfg.rank_mode,
+                                      h->debug_rows_block, h->sm_count, static_cast<uint32_t*>(h->alt_keys), h->err(),
+                                      static_cast<cudaStream_t>(stream)));
     return OSB200_OK;
 }
 

@@ -2262,15 +2262,21 @@ enum SegCount : int { kSegCountWarp = 0, kSegCountBlock1 = 1, kSegCountBlock2 = 
 // classes share that list: the 2,048-key geometry takes its segments of up to kSegBlock1Max keys and the larger geometry the
 // rest; a kernel whose own class count is 0 returns at once.  (A kernel of its own, sharing this body, so that the other
 // modes' kernels keep their names.)
+// ROW_SEL (with ROWS; osb200_topk_segments' sorted pass, topk_segment_sort_kernel): row s is sorted only if segment s =
+// [seg_off[s], seg_off[s + 1]) is one the radix select wrote: inside [0, sel_n), longer than sel_min and shorter than 2^32
+// keys (the binning kernel's test).  (Not its block list: with the list and its device-side count the 16,384-key
+// instantiations spill; the row count is a kernel parameter, as for ROWS.)
 // max_len: the caller's max_segment_len (<= T); longer segments are left as they are.
-template <typename KeyT, bool PAIRS, int K, int WARPS, int RANK_MODE, bool INDICES, bool ROWS, bool LIST>
+template <typename KeyT, bool PAIRS, int K, int WARPS, int RANK_MODE, bool INDICES, bool ROWS, bool LIST, bool ROW_SEL = false>
 __device__ __forceinline__ void segment_sort_body(KeyT* keys, uint32_t* vals, const unsigned long long* __restrict__ seg_off,
                                                   uint64_t num_segments, uint64_t single_n, uint32_t max_len, uint32_t begin_bit,
                                                   uint32_t places, uint32_t last_bits, const KeyCodec& codec,
                                                   const KeyT* __restrict__ keys_in, const uint32_t* __restrict__ seg_list,
-                                                  const unsigned long long* __restrict__ seg_counts)
+                                                  const unsigned long long* __restrict__ seg_counts, uint64_t sel_n = 0,
+                                                  uint32_t sel_min = 0)
 {
     static_assert(!(ROWS && LIST), "one addressing mode");
+    static_assert(!ROW_SEL || ROWS, "a selection of rows");
     static_assert(!INDICES || PAIRS, "the indices are the payloads");
     using S = SegSmem<KeyT, PAIRS, K, WARPS>;
     constexpr int THREADS = S::THREADS;
@@ -2288,6 +2294,10 @@ __device__ __forceinline__ void segment_sort_body(KeyT* keys, uint32_t* vals, co
     const uint64_t work = !LIST ? num_segments
                           : seg_counts[T <= kSegBlock1Max ? kSegCountBlock1 : kSegCountBlock2] ? seg_counts[kSegCountBlockList] : 0ull;
     for (uint64_t it = blockIdx.x; it < work; it += gridDim.x) {
+        if constexpr (ROW_SEL) {
+            const unsigned long long slo = seg_off[it], shi = seg_off[it + 1];
+            if (!(slo <= shi && shi <= sel_n && shi - slo > sel_min && shi - slo <= 0xFFFFFFFFull)) continue;
+        }
         const uint64_t seg = LIST ? seg_list[num_segments - 1 - it] : it;
         const uint64_t lo = ROWS ? seg * single_n : seg_off ? seg_off[seg] : 0ull;
         const uint64_t hi = ROWS ? lo + single_n : seg_off ? seg_off[seg + 1] : single_n;
@@ -2545,12 +2555,15 @@ __device__ __forceinline__ WarpSortCtx<KeyT> warp_sort_ctx(uint32_t* hist, const
 // TOPK (top-k, topk_warp_kernel; with INDICES): only the first `keep` sorted keys and payloads are stored, at
 // [obase, obase + keep) of out and idx_out; the payloads are loaded from idx_in[base ..] when idx_in is not null, else
 // they are the positions in the run.  (A compile-time flag, so that the other kernels' instantiations compile as before.)
-template <typename KeyT, int K, int RANK_MODE, bool INDICES, bool TOPK = false>
+// PAD (with TOPK; osb200_topk_segments, whose keep may pass len): the stored columns at or past len are padding, the decoded
+// all-ones key that the padding carries through the sort and the position 0xFFFFFFFF.
+template <typename KeyT, int K, int RANK_MODE, bool INDICES, bool TOPK = false, bool PAD = false>
 __device__ __forceinline__ void warp_sort_run(RowWarpSmem<KeyT, K, INDICES>& sm, const WarpSortCtx<KeyT>& x, const KeyT* in, KeyT* out,
                                               uint32_t* idx_out, uint64_t base, uint32_t len, const uint32_t* idx_in = nullptr,
                                               uint64_t obase = 0, uint32_t keep = 0)
 {
     static_assert(!TOPK || INDICES, "top-k stores positions");
+    static_assert(!PAD || TOPK, "padding is a top-k store");
     const int lane = x.lane;
     uint4* h4 = x.h4;
     const uint32_t lt = x.lt;
@@ -2618,7 +2631,7 @@ __device__ __forceinline__ void warp_sort_run(RowWarpSmem<KeyT, K, INDICES>& sm,
                 KeyT k = key[i];
                 if (dec) k = codec_decode<KeyT>(k, ca, cb, cd);
                 out[obase + idx] = k;
-                idx_out[obase + idx] = val[i];
+                idx_out[obase + idx] = PAD && idx >= len ? 0xFFFFFFFFu : val[i];
             }
         } else if (idx < len) {
             KeyT k = key[i];
@@ -2715,12 +2728,16 @@ cudaError_t launch_row_sort(const void* keys_in, void* keys_out, uint32_t* indic
 // neither can overflow.  counts = [warp list, 2,048-key class, larger class, block list]; the class kernels read their
 // count on the device, so the host enqueues them without waiting, and each segment of two or more keys is in exactly one
 // list and sorted by exactly one kernel.
+// TOPK (osb200_topk_segments, topk_segment_bin_kernel): every segment is listed, for every one has k output columns to
+// fill.  Segments of warp_max + 1 to 2^32 - 1 keys inside [0, n) go to the block list (counted as the 2,048-key class);
+// all others -- up to warp_max keys, empty, and invalid ones, which the warp class treats as empty -- to the warp list.
+// Nothing is written here but the lists and counts (keys_in, keys_out, idx_out and max_len are not used).
 // =====================================================================================================
-template <typename KeyT>
-__global__ void __launch_bounds__(256)
-segment_bin_kernel(const unsigned long long* __restrict__ off, uint64_t num_segments, uint64_t n, uint32_t max_len,
-                   uint32_t* __restrict__ list, unsigned long long* __restrict__ counts, const KeyT* keys_in, KeyT* keys_out,
-                   uint32_t* idx_out)
+template <typename KeyT, bool TOPK>
+__device__ __forceinline__ void segment_bin_body(const unsigned long long* __restrict__ off, uint64_t num_segments, uint64_t n,
+                                                 uint32_t max_len, uint32_t* __restrict__ list,
+                                                 unsigned long long* __restrict__ counts, const KeyT* keys_in, KeyT* keys_out,
+                                                 uint32_t* idx_out, uint32_t warp_max)
 {
     const uint32_t lane = threadIdx.x & 31, lt = lanemask_lt();
     const uint64_t stride = static_cast<uint64_t>(gridDim.x) * blockDim.x;
@@ -2728,7 +2745,10 @@ segment_bin_kernel(const unsigned long long* __restrict__ off, uint64_t num_segm
     for (uint64_t base = static_cast<uint64_t>(blockIdx.x) * blockDim.x + (threadIdx.x & ~31u); base < num_segments; base += stride) {
         const uint64_t s = base + lane;
         int cls = -1;  // 0: warp list, 1 / 2: block classes
-        if (s < num_segments) {
+        if (TOPK && s < num_segments) {
+            const unsigned long long lo = off[s], hi = off[s + 1];
+            cls = lo <= hi && hi <= n && hi - lo > warp_max && hi - lo <= 0xFFFFFFFFull ? 1 : 0;
+        } else if (s < num_segments) {
             const unsigned long long lo = off[s], hi = off[s + 1];
             if (lo <= hi && hi <= n && hi - lo <= max_len) {
                 const uint32_t len = static_cast<uint32_t>(hi - lo);
@@ -2754,6 +2774,15 @@ segment_bin_kernel(const unsigned long long* __restrict__ off, uint64_t num_segm
         if (cls == 0) list[wpos + __popc(w & lt)] = static_cast<uint32_t>(s);
         if (cls > 0) list[num_segments - 1 - (bpos + __popc(b & lt))] = static_cast<uint32_t>(s);
     }
+}
+
+template <typename KeyT>
+__global__ void __launch_bounds__(256)
+segment_bin_kernel(const unsigned long long* __restrict__ off, uint64_t num_segments, uint64_t n, uint32_t max_len,
+                   uint32_t* __restrict__ list, unsigned long long* __restrict__ counts, const KeyT* keys_in, KeyT* keys_out,
+                   uint32_t* idx_out)
+{
+    segment_bin_body<KeyT, false>(off, num_segments, n, max_len, list, counts, keys_in, keys_out, idx_out, kRowWarpMaxLen);
 }
 
 // The warp class: one warp per segment of the warp list (grid-stride), 1, 2, 4 or 8 keys per lane by the segment's length.
@@ -2886,10 +2915,15 @@ struct TopkSmem {
     uint32_t pick[3];  // the chosen bucket, the candidates below it, the candidates in it
 };
 
-template <typename KeyT>
-__global__ void __launch_bounds__(kTopkThreads, 1)
-topk_select_kernel(const KeyT* __restrict__ in, KeyT* __restrict__ out, uint32_t* __restrict__ idx_out, uint64_t num_rows,
-                   uint32_t row_len, uint32_t k, uint32_t cap, KeyCodec codec)
+// LIST (osb200_topk_segments, topk_segment_select_kernel): the rows are the segments whose ids the binning kernel put at the
+// back of `list` (entry i at list[num_rows - 1 - i], counts[kSegCountBlockList] of them), row s = [off[s], off[s + 1]) of
+// `in`, with k' = m = min(length, k) and its result at row s * k; columns m .. k - 1 are padding (the decoded all-ones key,
+// position 0xFFFFFFFF).  A segment of at most k keys starts with `last` set: one ordered pass selects all of it.
+template <typename KeyT, bool LIST>
+__device__ __forceinline__ void topk_select_body(const KeyT* __restrict__ in, KeyT* __restrict__ out, uint32_t* __restrict__ idx_out,
+                                                 uint64_t num_rows, uint32_t row_len, uint32_t k, uint32_t cap, const KeyCodec& codec,
+                                                 const unsigned long long* __restrict__ off, const uint32_t* __restrict__ list,
+                                                 const unsigned long long* __restrict__ counts)
 {
     using S = TopkSmem<KeyT>;
     using U = std::conditional_t<sizeof(KeyT) == 8, uint64_t, uint32_t>;
@@ -2903,21 +2937,27 @@ topk_select_kernel(const KeyT* __restrict__ in, KeyT* __restrict__ out, uint32_t
     const KeyT ca = static_cast<KeyT>(codec.a), cb = static_cast<KeyT>(codec.b), cd = static_cast<KeyT>(codec.d);
     const bool enc = codec.flags & kCodecEncodeOnLoad, dec = codec.flags & kCodecDecodeOnStore;
 
+    const uint64_t work = LIST ? counts[kSegCountBlockList] : num_rows;
+    if (LIST && work == 0) return;
     for (int i = tid; i < kTopkWarps * kRadix; i += kTopkThreads) sm.hist[i] = 0;
     __syncthreads();
-    for (uint64_t row = blockIdx.x; row < num_rows; row += gridDim.x) {
-        const KeyT* src = in + row * row_len;
+    for (uint64_t it = blockIdx.x; it < work; it += gridDim.x) {
+        const uint64_t row = LIST ? list[num_rows - 1 - it] : it;
+        const uint64_t lo = LIST ? off[row] : row * row_len;
+        const uint32_t len = LIST ? static_cast<uint32_t>(off[row + 1] - lo) : row_len;  // (LIST: binned as 257 .. 2^32 - 1)
+        const KeyT* src = in + lo;
         KeyT* dst = out + row * k;
         uint32_t* dst_idx = idx_out + row * k;
+        const uint32_t m = LIST ? min(len, k) : k;
         // S_{t-1} = {x : (x & mprev) == vprev}; selected this pass: x in S_{t-1} with (x & mcur) < vcur; S_t: (x & mcur) == vcur
         U mprev = 0, vprev = 0, mcur = 0, vcur = 0;
-        uint32_t need = k, cand = row_len, written = 0, in_smem = 0;  // in_smem: 0, or the number of candidates held there
-        bool last = false;
+        uint32_t need = m, cand = len, written = 0, in_smem = 0;  // in_smem: 0, or the number of candidates held there
+        bool last = LIST && len <= k;
         for (uint32_t t = 0;; ++t) {
             const bool compact = !last && !in_smem && cand <= cap;
-            const bool order = t > 0 || compact;  // anything to place in row order this pass
+            const bool order = t > 0 || compact || (LIST && last);  // anything to place in row order this pass
             const uint32_t shift = last ? 0u : BITS - 8u * (t + 1);
-            const uint64_t n_src = in_smem ? in_smem : row_len;
+            const uint64_t n_src = in_smem ? in_smem : len;
             uint32_t sel_run = 0, eq_run = 0, chunk = 0;
             for (uint64_t c0 = 0; c0 < n_src; c0 += CHUNK, ++chunk) {
                 U x[kTopkE];
@@ -3004,8 +3044,23 @@ topk_select_kernel(const KeyT* __restrict__ in, KeyT* __restrict__ out, uint32_t
             vcur |= static_cast<U>(b) << shift;
             last = cand == need || t + 1 == D;
         }
+        if constexpr (LIST) {
+            const KeyT pad = dec ? codec_decode<KeyT>(static_cast<KeyT>(~static_cast<KeyT>(0)), ca, cb, cd) : static_cast<KeyT>(~static_cast<KeyT>(0));
+            for (uint32_t c = m + tid; c < k; c += kTopkThreads) {
+                dst[c] = pad;
+                dst_idx[c] = 0xFFFFFFFFu;
+            }
+        }
         __syncthreads();  // the next row's pass 0 may compact into the buffer this row's last pass read
     }
+}
+
+template <typename KeyT>
+__global__ void __launch_bounds__(kTopkThreads, 1)
+topk_select_kernel(const KeyT* __restrict__ in, KeyT* __restrict__ out, uint32_t* __restrict__ idx_out, uint64_t num_rows,
+                   uint32_t row_len, uint32_t k, uint32_t cap, KeyCodec codec)
+{
+    topk_select_body<KeyT, false>(in, out, idx_out, num_rows, row_len, k, cap, codec, nullptr, nullptr, nullptr);
 }
 
 // topk_warp_kernel: rows of row_len <= 32 K keys of `in`; the first k of each sorted row go to row r * k of out / idx_out.
@@ -3035,6 +3090,108 @@ topk_sort_kernel(KeyT* keys, uint32_t* vals, uint64_t num_rows, uint32_t k, KeyC
                                                                           8u, codec, keys, nullptr, nullptr);
 }
 
+// =====================================================================================================
+// Segment top-k (osb200_topk_segments): row top-k for ragged segments given by offsets.  Segment s's result is row s of a
+// [num_segments, k] output: its first m = min(length, k) keys in the stable sort and their positions, then k - m columns of
+// padding -- the key whose radix image is all ones (it sorts last) and the position 0xFFFFFFFF.
+//   * topk_segment_bin_kernel (segment_bin_body, TOPK) lists every segment: up to 256 keys, and the empty and invalid ones,
+//     on the warp list, longer ones on the block list.
+//   * topk_segment_warp_kernel: one warp per segment of the warp list (warp_sort_run, TOPK and PAD), then the padding past
+//     the warp's 32 K columns, coalesced.
+//   * topk_segment_select_kernel: topk_select_body in list mode, one CTA per segment of the block list.
+//   * sorted: only the radix select's rows are sorted in place, whole k-wide rows -- the padding's image is all ones and the
+//     sort is stable, so it stays at the tail: topk_segment_sort_warp_kernel (over the block list) for k <= 256, else
+//     topk_segment_sort_kernel (over all rows, skipping the warp class's by their offsets).
+// Every class kernel runs on the resident CTAs and reads its count on the device, so nothing waits on the host.
+// =====================================================================================================
+__global__ void __launch_bounds__(256)
+topk_segment_bin_kernel(const unsigned long long* __restrict__ off, uint64_t num_segments, uint64_t n, uint32_t warp_max,
+                        uint32_t* __restrict__ list, unsigned long long* __restrict__ counts)
+{
+    segment_bin_body<uint32_t, true>(off, num_segments, n, 0u, list, counts, nullptr, nullptr, nullptr, warp_max);
+}
+
+template <typename KeyT, int RANK_MODE>
+__global__ void __launch_bounds__(kRowWarps * 32)
+topk_segment_warp_kernel(const KeyT* in, KeyT* out, uint32_t* __restrict__ idx_out, uint64_t n,
+                         const unsigned long long* __restrict__ off, const uint32_t* __restrict__ list,
+                         const unsigned long long* __restrict__ counts, uint32_t k, KeyCodec codec)
+{
+    extern __shared__ __align__(16) unsigned char s_raw[];
+    const int warp = threadIdx.x >> 5;
+    unsigned char* wsm = s_raw + warp * sizeof(RowWarpSmem<KeyT, 8, true>);  // every K's layout starts with the same hist
+    const WarpSortCtx<KeyT> x = warp_sort_ctx<KeyT>(reinterpret_cast<uint32_t*>(wsm), codec);
+    const KeyT ones = static_cast<KeyT>(~static_cast<KeyT>(0));
+    const KeyT pad = x.dec ? codec_decode<KeyT>(ones, x.ca, x.cb, x.cd) : ones;
+    const uint64_t count = counts[kSegCountWarp];
+    for (uint64_t i = static_cast<uint64_t>(blockIdx.x) * kRowWarps + warp; i < count; i += static_cast<uint64_t>(gridDim.x) * kRowWarps) {
+        const uint32_t s = list[i];
+        const unsigned long long lo = off[s], hi = off[s + 1];
+        // offsets that decrease, pass n or span 2^32 keys or more: the binning kernel listed it here as empty
+        const uint32_t len = lo <= hi && hi <= n && hi - lo <= kRowWarpMaxLen ? static_cast<uint32_t>(hi - lo) : 0u;
+        const uint64_t obase = static_cast<uint64_t>(s) * k;
+        uint32_t stored;  // the columns warp_sort_run stores: min(k, 32 K)
+        if (len <= 32) {
+            stored = min(k, 32u);
+            warp_sort_run<KeyT, 1, RANK_MODE, true, true, true>(*reinterpret_cast<RowWarpSmem<KeyT, 1, true>*>(wsm), x, in, out, idx_out,
+                                                                lo, len, nullptr, obase, stored);
+        } else if (len <= 64) {
+            stored = min(k, 64u);
+            warp_sort_run<KeyT, 2, RANK_MODE, true, true, true>(*reinterpret_cast<RowWarpSmem<KeyT, 2, true>*>(wsm), x, in, out, idx_out,
+                                                                lo, len, nullptr, obase, stored);
+        } else if (len <= 128) {
+            stored = min(k, 128u);
+            warp_sort_run<KeyT, 4, RANK_MODE, true, true, true>(*reinterpret_cast<RowWarpSmem<KeyT, 4, true>*>(wsm), x, in, out, idx_out,
+                                                                lo, len, nullptr, obase, stored);
+        } else {
+            stored = min(k, 256u);
+            warp_sort_run<KeyT, 8, RANK_MODE, true, true, true>(*reinterpret_cast<RowWarpSmem<KeyT, 8, true>*>(wsm), x, in, out, idx_out,
+                                                                lo, len, nullptr, obase, stored);
+        }
+        for (uint32_t c = stored + x.lane; c < k; c += 32) {
+            out[obase + c] = pad;
+            idx_out[obase + c] = 0xFFFFFFFFu;
+        }
+    }
+}
+
+template <typename KeyT>
+__global__ void __launch_bounds__(kTopkThreads, 1)
+topk_segment_select_kernel(const KeyT* __restrict__ in, KeyT* __restrict__ out, uint32_t* __restrict__ idx_out, uint64_t num_segments,
+                           uint32_t k, uint32_t cap, KeyCodec codec, const unsigned long long* __restrict__ off,
+                           const uint32_t* __restrict__ list, const unsigned long long* __restrict__ counts)
+{
+    topk_select_body<KeyT, true>(in, out, idx_out, num_segments, 0u, k, cap, codec, off, list, counts);
+}
+
+// the sorted pass of the block list's rows (k <= 32 K), in place, the positions loaded as payloads
+template <typename KeyT, int K, int RANK_MODE>
+__global__ void __launch_bounds__(kRowWarps * 32)
+topk_segment_sort_warp_kernel(KeyT* keys, uint32_t* idx, uint64_t num_segments, uint32_t k, const uint32_t* __restrict__ list,
+                              const unsigned long long* __restrict__ counts, KeyCodec codec)
+{
+    using W = RowWarpSmem<KeyT, K, true>;
+    extern __shared__ __align__(16) unsigned char s_raw[];
+    const int warp = threadIdx.x >> 5;
+    W& sm = reinterpret_cast<W*>(s_raw)[warp];
+    const WarpSortCtx<KeyT> x = warp_sort_ctx<KeyT>(sm.hist, codec);
+    const uint64_t count = counts[kSegCountBlockList];
+    for (uint64_t i = static_cast<uint64_t>(blockIdx.x) * kRowWarps + warp; i < count; i += static_cast<uint64_t>(gridDim.x) * kRowWarps) {
+        const uint64_t row = static_cast<uint64_t>(list[num_segments - 1 - i]) * k;
+        warp_sort_run<KeyT, K, RANK_MODE, true, true>(sm, x, keys, keys, idx, row, k, idx, row, k);
+    }
+}
+
+// the sorted pass of the radix select's rows for k > 256: the row sort's block body (ROWS, ROW_SEL), in place
+template <typename KeyT, int K, int WARPS, int RANK_MODE>
+__global__ void __launch_bounds__(WARPS * 32, 1)
+topk_segment_sort_kernel(KeyT* keys, uint32_t* vals, uint64_t num_segments, uint32_t k, KeyCodec codec,
+                         const unsigned long long* __restrict__ off, uint64_t n, uint32_t warp_max)
+{
+    segment_sort_body<KeyT, true, K, WARPS, RANK_MODE, false, true, false, true>(keys, vals, off, num_segments, k, k, 0u, sizeof(KeyT),
+                                                                                8u, codec, keys, nullptr, nullptr, n, warp_max);
+}
+
 template <typename KeyT, int SIZE>
 struct TopkSortShape {
     using Key = KeyT;
@@ -3045,6 +3202,8 @@ struct TopkSortShape {
     static constexpr size_t smem = sizeof(S);
     template <int RANK_MODE, bool HOT = false>
     static auto kernel() { return topk_sort_kernel<KeyT, G::K, G::WARPS, RANK_MODE>; }
+    template <int RANK_MODE>
+    static auto list_kernel() { return topk_segment_sort_kernel<KeyT, G::K, G::WARPS, RANK_MODE>; }
 };
 using TopkSortShapes = TypeList<TopkSortShape<uint16_t, 1>, TopkSortShape<uint16_t, 2>, TopkSortShape<uint32_t, 1>,
                                 TopkSortShape<uint32_t, 2>, TopkSortShape<uint64_t, 1>, TopkSortShape<uint64_t, 2>>;
@@ -3117,6 +3276,81 @@ cudaError_t launch_topk_rows(const void* keys_in, void* values_out, uint32_t* in
     });
 }
 
+template <typename KeyT, int K, int RANK_MODE>
+static cudaError_t launch_topk_segment_sort_warp(KeyT* keys, uint32_t* idx, uint64_t num_segments, uint32_t k, const uint32_t* list,
+                                                 const unsigned long long* counts, const KeyCodec& codec, int sm_count,
+                                                 cudaStream_t stream)
+{
+    auto kern = topk_segment_sort_warp_kernel<KeyT, K, RANK_MODE>;
+    constexpr size_t smem = kRowWarps * sizeof(RowWarpSmem<KeyT, K, true>);
+    static const int per_sm = resident_per_sm(kern, kRowWarps * 32, smem);
+    if (per_sm <= 0) return cudaErrorLaunchOutOfResources;
+    kern<<<per_sm * sm_count, kRowWarps * 32, smem, stream>>>(keys, idx, num_segments, k, list, counts, codec);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_topk_segments(const void* keys_in, void* values_out, uint32_t* indices, uint64_t n, const unsigned long long* off,
+                                 uint64_t num_segments, uint32_t k, int key_bytes, const KeyCodec* codec_in, bool sorted,
+                                 uint32_t capacity, int rank_mode, bool block_only, int sm_count, uint32_t* list,
+                                 unsigned long long* counts, cudaStream_t stream)
+{
+    if (num_segments == 0 || k == 0) return cudaSuccess;
+    if (k > row_sort_capacity(key_bytes)) return cudaErrorInvalidValue;
+    const uint32_t cap = capacity && capacity < row_sort_capacity(key_bytes) ? capacity : row_sort_capacity(key_bytes);
+    const KeyCodec codec = codec_in ? *codec_in : KeyCodec();
+    cudaError_t e = cudaMemsetAsync(counts, 0, kSegCounts * sizeof(unsigned long long), stream);
+    if (e != cudaSuccess) return e;
+    const uint32_t warp_max = block_only ? 0u : kRowWarpMaxLen;
+    topk_segment_bin_kernel<<<capped_grid(num_segments, 256, static_cast<uint64_t>(sm_count) * 8), 256, 0, stream>>>(
+        off, num_segments, n, warp_max, list, counts);
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    return with_key_type(TopkKeys{}, key_bytes, [&](auto kt) {
+        using KeyT = decltype(kt);
+        const KeyT* in = static_cast<const KeyT*>(keys_in);
+        KeyT* out = static_cast<KeyT*>(values_out);
+        return with_rank_mode(rank_mode, [&](auto r) {
+            constexpr int R = decltype(r)::value;
+            {
+                auto kern = topk_segment_warp_kernel<KeyT, R>;
+                constexpr size_t smem = kRowWarps * sizeof(RowWarpSmem<KeyT, 8, true>);
+                static const int per_sm = resident_per_sm(kern, kRowWarps * 32, smem);
+                if (per_sm <= 0) return cudaErrorLaunchOutOfResources;
+                kern<<<per_sm * sm_count, kRowWarps * 32, smem, stream>>>(in, out, indices, n, off, list, counts, k, codec);
+                cudaError_t le = cudaGetLastError();
+                if (le != cudaSuccess) return le;
+            }
+            {
+                auto kern = topk_segment_select_kernel<KeyT>;
+                static const int per_sm = resident_per_sm(kern, kTopkThreads, sizeof(TopkSmem<KeyT>));
+                if (per_sm <= 0) return cudaErrorLaunchOutOfResources;
+                kern<<<per_sm * sm_count, kTopkThreads, sizeof(TopkSmem<KeyT>), stream>>>(in, out, indices, num_segments, k, cap, codec,
+                                                                                          off, list, counts);
+                cudaError_t le = cudaGetLastError();
+                if (le != cudaSuccess || !sorted || k == 1) return le;
+            }
+            // sorted: the block list's rows, in place (the warp list's are sorted already)
+            if (k <= 32) return launch_topk_segment_sort_warp<KeyT, 1, R>(out, indices, num_segments, k, list, counts, codec, sm_count, stream);
+            if (k <= 64) return launch_topk_segment_sort_warp<KeyT, 2, R>(out, indices, num_segments, k, list, counts, codec, sm_count, stream);
+            if (k <= 128) return launch_topk_segment_sort_warp<KeyT, 4, R>(out, indices, num_segments, k, list, counts, codec, sm_count, stream);
+            if (k <= kRowWarpMaxLen)
+                return launch_topk_segment_sort_warp<KeyT, 8, R>(out, indices, num_segments, k, list, counts, codec, sm_count, stream);
+            return find_type(
+                TopkSortShapes{},
+                [&](auto s) { using Sh = decltype(s); return std::is_same_v<typename Sh::Key, KeyT> && k <= Sh::T; },
+                [&](auto s) {
+                    using Sh = decltype(s);
+                    const auto sk = Sh::template list_kernel<R>();
+                    static const int sort_per_sm = resident_per_sm(sk, Sh::S::THREADS, Sh::smem);
+                    if (sort_per_sm <= 0) return cudaErrorLaunchOutOfResources;
+                    const uint64_t sort_ctas = static_cast<uint64_t>(sort_per_sm) * sm_count;
+                    sk<<<static_cast<unsigned>(num_segments < sort_ctas ? num_segments : sort_ctas), Sh::S::THREADS, Sh::smem, stream>>>(
+                        reinterpret_cast<typename Sh::Key*>(out), indices, num_segments, k, codec, off, n, warp_max);
+                    return cudaGetLastError();
+                });
+        });
+    });
+}
+
 cudaError_t configure_kernels()
 {
     cudaError_t e = for_each_type(HistKeys{}, [](auto k) {
@@ -3136,7 +3370,13 @@ cudaError_t configure_kernels()
     if (e == cudaSuccess) e = for_each_type(TopkSortShapes{}, shape);
     if (e == cudaSuccess) e = for_each_type(TopkKeys{}, [](auto k) {
         using KeyT = decltype(k);
-        return set_smem(topk_select_kernel<KeyT>, sizeof(TopkSmem<KeyT>));
+        const cudaError_t m = set_smem(topk_select_kernel<KeyT>, sizeof(TopkSmem<KeyT>));
+        return m != cudaSuccess ? m : set_smem(topk_segment_select_kernel<KeyT>, sizeof(TopkSmem<KeyT>));
+    });
+    if (e == cudaSuccess) e = for_each_type(TopkSortShapes{}, [](auto s) {
+        using Sh = decltype(s);
+        const cudaError_t m = set_smem(Sh::template list_kernel<kRankAtomic>(), Sh::smem);
+        return m != cudaSuccess ? m : set_smem(Sh::template list_kernel<kRankBallot>(), Sh::smem);
     });
     if (e == cudaSuccess) e = set_smem(fused_kernel<kRankAtomic>(), FusedShape::smem);
     if (e == cudaSuccess) e = set_smem(fused_kernel<kRankBallot>(), FusedShape::smem);

@@ -154,6 +154,19 @@ cudaError_t launch_topk_rows(const void* keys_in, void* values_out, uint32_t* in
                              uint32_t k, int key_bytes, const KeyCodec* codec, bool sorted, uint32_t capacity, int rank_mode,
                              bool block_only, int sm_count, cudaStream_t stream);
 
+// Segment top-k (osb200_topk_segments): segment s = [off[s], off[s + 1]) of keys_in; its first m = min(length, k) keys in the
+// stable sort and their positions within the segment go to [s * k, s * k + m) of values_out and indices, and columns m .. k - 1
+// are padding (the decoded all-ones key, position 0xFFFFFFFF).  Segments whose offsets decrease, pass n or span 2^32 keys or
+// more are all padding.  A binning kernel lists segments of at most kRowWarpMaxLen keys (0 with block_only), and the empty and
+// invalid ones, for one warp each and the longer ones for the radix select, one CTA each, the candidates held in shared
+// memory once at most `capacity` are left (0: row_sort_capacity(key_bytes)); sorted then sorts the select's rows in place.
+// k in 0 .. row_sort_capacity(key_bytes); list: num_segments u32 of workspace; counts: 4 u64 of workspace, cleared here.  The
+// codec as for launch_row_sort.
+cudaError_t launch_topk_segments(const void* keys_in, void* values_out, uint32_t* indices, uint64_t n, const unsigned long long* off,
+                                 uint64_t num_segments, uint32_t k, int key_bytes, const KeyCodec* codec, bool sorted,
+                                 uint32_t capacity, int rank_mode, bool block_only, int sm_count, uint32_t* list,
+                                 unsigned long long* counts, cudaStream_t stream);
+
 // Validate (reference: Validate, UtilityKernels.cuh:403-429): err_count += #(keys[i] > keys[i+1]).
 cudaError_t launch_validate(const void* keys, uint64_t n, int key_bytes, unsigned long long* err_count, int sm_count,
                             cudaStream_t stream);

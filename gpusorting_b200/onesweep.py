@@ -303,6 +303,43 @@ class OneSweepSorter:
                                            1 if descending else 0, _stream_ptr(stream)), "osb200_sort_segments")
         return (out, idx) if return_indices else out
 
+    # -- segment top-k: row top-k for ragged rows given by offsets -----------------------------------------------------------
+    def topk_segments(self, x: torch.Tensor, offsets: torch.Tensor, k: int, key_type: str, largest: bool = True,
+                      sorted: bool = True, stream=None):
+        """The k largest (or smallest) keys of every segment [offsets[s], offsets[s+1]) of `x` and their positions within
+        the segment (osb200_topk_segments): topk_rows for ragged rows.  `x`, `offsets` and key_type as in sort_segments.
+        Segment s's result is row s of a [num_segments, k] output.  Its first m = min(length, k) columns hold the first m keys
+        of the segment's stable sort (descending for largest); of equal keys at the boundary the lowest positions are taken.
+        sorted=True returns them in that order, sorted=False the same pairs in an unspecified order.  Columns m .. k-1 are
+        padding: index -1 and the key that sorts last -- for largest=True 0, the minimum of a signed dtype or the float of
+        all-ones bits (a NaN), for largest=False the maximum of an integer dtype or the NaN 0x7F..F.  Segments whose offsets
+        decrease or pass x.numel() are all padding.
+
+        Returns (values, indices) of shape [num_segments, k], indices as torch.int32, allocated with torch.empty on the
+        stream.  k may be at most 16,384 (8,192 for 8-byte dtypes) and may exceed a segment's length; num_segments may be
+        at most the sorter's max_n."""
+        if not (isinstance(x, torch.Tensor) and x.is_cuda and x.is_contiguous() and x.dim() == 1 and x.dtype in _ROW_KEY_TYPES):
+            raise TypeError(f"x must be a contiguous 1-D CUDA tensor with dtype in {tuple(_ROW_KEY_TYPES)}")
+        if x.device.index != self.device:
+            raise ValueError(f"x lives on cuda:{x.device.index}, the sorter on cuda:{self.device}")
+        if not (isinstance(offsets, torch.Tensor) and offsets.dtype == torch.int64 and offsets.is_contiguous()
+                and offsets.dim() == 1 and offsets.device == x.device):
+            raise TypeError("offsets must be a contiguous 1-D int64 tensor on the device of x")
+        kb = x.element_size()
+        kt = (KEY16_TYPES if kb == 2 else KEY_TYPES)[key_type]
+        k = int(k)
+        if k < 0:
+            raise ValueError(f"k must be >= 0, got {k}")
+        segs = max(offsets.numel() - 1, 0)
+        with torch.cuda.stream(stream):  # (None: the current stream) the outputs belong to the stream that writes them
+            out = torch.empty((segs, k), dtype=x.dtype, device=x.device)
+            idx = torch.empty((segs, k), dtype=torch.int32, device=x.device)
+        with torch.cuda.device(self.device):
+            check(lib.osb200_topk_segments(self._h, x.data_ptr() if x.numel() else None, out.data_ptr(), idx.data_ptr(),
+                                           x.numel(), offsets.data_ptr(), segs, k, kb, kt, 1 if largest else 0,
+                                           1 if sorted else 0, _stream_ptr(stream)), "osb200_topk_segments")
+        return out, idx
+
     def sort_bits(self, keys: torch.Tensor, begin_bit: int, end_bit: int, values: Optional[torch.Tensor] = None,
                   n: Optional[int] = None, stream=None):
         """Stable sort on the key bits [begin_bit, end_bit) only (osb200_sort_bits).  Keys must start on a 16-byte boundary
@@ -529,6 +566,22 @@ def sort_segments(x: torch.Tensor, offsets: torch.Tensor, descending: bool = Fal
         sp = _stream_ptr(stream)
     s = _cached_sorter(x.device.index, 4, 4, max(offsets.numel() - 1, 1), sp)
     return s.sort_segments(x, offsets, _ROW_KEY_TYPES[x.dtype], descending, return_indices, False, max_segment_len, stream)
+
+
+def topk_segments(x: torch.Tensor, offsets: torch.Tensor, k: int, largest: bool = True, sorted: bool = True, stream=None):
+    """The k largest (or smallest) keys of every segment [offsets[s], offsets[s+1]) of a contiguous 1-D CUDA tensor of one of
+    sort_rows' ten dtypes, and their int32 positions within the segment: (values, indices) of shape [num_segments, k],
+    padded past each segment's length with index -1 and the key that sorts last.  The key type follows the dtype.
+    OneSweepSorter.topk_segments on the stream's cached (4, 4) sorter, the one argsort uses, grown to the number of segments
+    (the call keeps one uint32 per segment in the sorter's workspace)."""
+    if not (isinstance(x, torch.Tensor) and x.is_cuda):
+        raise TypeError("x must be a CUDA tensor")
+    if x.dtype not in _ROW_KEY_TYPES:
+        raise TypeError(f"x.dtype must be one of {tuple(_ROW_KEY_TYPES)}")
+    with torch.cuda.device(x.device.index):
+        sp = _stream_ptr(stream)
+    s = _cached_sorter(x.device.index, 4, 4, max(offsets.numel() - 1, 1), sp)
+    return s.topk_segments(x, offsets, k, _ROW_KEY_TYPES[x.dtype], largest, sorted, stream)
 
 
 class OneSweepDispatcher:

@@ -92,6 +92,17 @@ class OneSweepSorterB200 {
                                sorted ? 1 : 0, stream),
               "osb200_topk_rows");
     }
+    // the first m = min(length, k) keys of every segment [offsets[s], offsets[s+1]) in its stable sort (ascending, or descending
+    // for largest) and their positions within the segment, into row s of [num_segments, k] outputs; columns m .. k-1 are
+    // padding (position 0xFFFFFFFF, the key that sorts last); segments whose offsets decrease or pass n are all padding;
+    // k <= 16,384 (8,192 for 8-byte keys); num_segments <= the handle's max_n
+    void TopkSegments(const void* d_keys_in, void* d_values_out, uint32_t* d_indices, uint64_t n, const uint64_t* d_segment_offsets,
+                      uint64_t num_segments, uint32_t k, int key_bytes, int key_type, bool largest, bool sorted, void* stream = nullptr)
+    {
+        check(osb200_topk_segments(h_, d_keys_in, d_values_out, d_indices, n, d_segment_offsets, num_segments, k, key_bytes, key_type,
+                                   largest ? 1 : 0, sorted ? 1 : 0, stream),
+              "osb200_topk_segments");
+    }
     // every segment [offsets[s], offsets[s+1]) of n keys sorted stable into the same positions of d_keys_out (ragged rows);
     // d_indices may be null; max_segment_len <= 16,384 (8,192 for 8-byte keys); num_segments <= the handle's max_n
     void SortSegments(const void* d_keys_in, void* d_keys_out, uint32_t* d_indices, uint64_t n, const uint64_t* d_segment_offsets,

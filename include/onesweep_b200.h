@@ -221,6 +221,36 @@ OSB200_API int osb200_topk_rows(osb200_handle h, const void* d_keys_in, void* d_
                                 uint64_t num_rows, uint32_t row_len, uint32_t k, int key_bytes, int key_type,
                                 int largest, int sorted, void* stream);
 
+/* Segment top-k: osb200_topk_rows for ragged segments given by offsets.  Segment s is [off[s], off[s+1]) of n keys (off =
+ * d_segment_offsets, num_segments + 1 of them, 8-byte aligned, as for osb200_sort_segments).  With L its length and
+ * m = min(L, k), its result is row s of a [num_segments, k] output, elements [s*k, s*k + k) of d_values_out and d_indices:
+ *   columns 0 .. m-1: the first m keys of the segment's stable sort (ascending, or descending for largest = 1; the codec of
+ *   osb200_topk_rows) and their uint32 positions within the segment.  Of equal keys at the boundary the lowest positions are
+ *   taken.  sorted = 1 writes them in sort order, bit-identical to the first m keys and indices osb200_sort_segments writes
+ *   for the segment (descending = largest) wherever that call accepts it; sorted = 0 writes the same m pairs in an
+ *   unspecified order.
+ *   columns m .. k-1: padding, position 0xFFFFFFFF (-1 as int32) and the key that sorts last in the selection order, the
+ *   decode of the all-ones radix image: UINT_MAX, INT_MAX or the NaN 0x7F..F for largest = 0; 0, INT_MIN or the NaN 0xF..F
+ *   for largest = 1.
+ * A segment whose offsets decrease, whose end passes n, or that is longer than 2^32 - 1 keys is empty: its row is all padding.
+ * Nothing outside [0, n) is read and nothing outside [0, num_segments*k) of either output is written: the offsets need not
+ * be trusted.
+ * k may be at most 16,384 (2- and 4-byte keys) or 8,192 (8-byte keys): OSB200_ERR_SIZE above; k larger than a segment is
+ * fine.  k == 0 or num_segments == 0 is a no-op; n == 0 is not (every row is padding), and d_keys_in may be NULL only then.
+ * key_bytes / key_type are those of osb200_sort_rows.  d_indices is required.  Natural alignment of the keys, 4-byte alignment
+ * of the indices, a null handle, output or offsets pointer, array sizes that overflow 64 bits and any overlap between the
+ * input, the offsets and the two outputs are OSB200_ERR_INVALID_ARG (there is no in-place form).
+ * Workspace: one uint32 per segment of the handle's alternate key buffer and the class counts in its control block, so
+ * num_segments above min(max_n, 2^32) is OSB200_ERR_SIZE (any key or value width of handle will do); one call in flight per
+ * handle.  A binning kernel reads the offsets once; segments of at most 256 keys, and the empty and invalid ones, are sorted
+ * and padded one per warp, longer ones radix-selected one per thread block as in osb200_topk_rows, a segment of at most k
+ * keys in one pass.  sorted = 1 then sorts the block-selected rows in place.  The test hooks "debug_rows_block" (every
+ * non-empty segment to the radix select) and "debug_topk_capacity" apply.  At most one memset and four launches:
+ * asynchronous, no host synchronisation, graph-capturable. */
+OSB200_API int osb200_topk_segments(osb200_handle h, const void* d_keys_in, void* d_values_out, uint32_t* d_indices, uint64_t n,
+                                    const uint64_t* d_segment_offsets, uint64_t num_segments, uint32_t k, int key_bytes,
+                                    int key_type, int largest, int sorted, void* stream);
+
 /* Sort on a bit range [begin_bit, end_bit) of the (unsigned) key only, CUB-style: keys that agree on those bits keep their
  * input order (stable).  ceil((end_bit-begin_bit)/8) digit passes instead of key_bytes; the last digit may be narrower
  * than 8 bits; an odd pass count is handled inside (the result is always returned in the caller's buffers).  d_values may
