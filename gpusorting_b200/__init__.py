@@ -17,6 +17,7 @@ from .onesweep import (  # noqa: F401
     argsort,
     argsort16,
     init_random,
+    release_cached_sorters,
     sort_rows,
     sort_segments,
     topk,

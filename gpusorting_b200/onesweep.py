@@ -471,6 +471,9 @@ def init_random(keys: torch.Tensor, and_count: int, seed: int, n: Optional[int] 
 # (device, key width, pairs) and grown on demand, so repeated calls do not re-allocate.
 # --------------------------------------------------------------------------------------------------
 _CACHE: dict = {}
+# Sorters the cache has replaced with larger ones.  They stay open: a CUDA graph that captured a module call holds their
+# buffers, and closing them would leave its replays reading and writing freed device memory.
+_RETIRED: list = []
 
 
 def _cached_sorter(device: int, key_bytes: int, value_bytes: int, n: int, stream_ptr: int) -> OneSweepSorter:
@@ -479,10 +482,20 @@ def _cached_sorter(device: int, key_bytes: int, value_bytes: int, n: int, stream
     s = _CACHE.get(k)
     if s is None or s.max_n < n:
         if s is not None:
-            s.close()
+            _RETIRED.append(s)
         s = OneSweepSorter(max(n, 1), key_bytes, value_bytes, device)
         _CACHE[k] = s
     return s
+
+
+def release_cached_sorters() -> None:
+    """Frees the sorters the module calls' cache has replaced with larger ones, after synchronizing every device they live
+    on.  Safe only when no live CUDA graph uses them: a graph that captured a module call before its cached sorter grew
+    keeps that sorter's buffers, so destroy such graphs first.  The sorters in use stay cached."""
+    for d in sorted({s.device for s in _RETIRED}):
+        torch.cuda.synchronize(d)
+    while _RETIRED:
+        _RETIRED.pop().close()
 
 
 def Sort(keys: torch.Tensor, values: Optional[torch.Tensor] = None, n: Optional[int] = None, stream=None):
