@@ -176,6 +176,39 @@ int check_handle(const osb200_sorter* s) { return s ? OSB200_OK : OSB200_ERR_INV
 
 bool overlaps(uintptr_t a, uint64_t alen, uintptr_t b, uint64_t blen) { return a < b + blen && b < a + alen; }
 
+// An array argument of the row and segment sorts and top-k: its address, size in bytes and natural alignment, whether null
+// is an error (else a null array is absent), and whether the call writes it.
+struct ArrayArg { const void* p; uint64_t bytes; int align; bool required, written; };
+
+// The argument checks of osb200_sort_rows, osb200_sort_segments, osb200_topk_rows and osb200_topk_segments, in order:
+// every required array is given; every array is naturally aligned (the kernels load and store element by element); the
+// byte sizes fit in 64 bits (sizes_fit); no array the call writes overlaps another one -- except a[1] == a[0] (out == in)
+// where the call sorts in place, since a row or segment is read whole before it is written.
+template <size_t N>
+int check_arrays(const ArrayArg (&a)[N], bool sizes_fit, bool in_place)
+{
+    for (const ArrayArg& x : a)
+        if ((x.required && !x.p) || (reinterpret_cast<uintptr_t>(x.p) & static_cast<uintptr_t>(x.align - 1)))
+            return OSB200_ERR_INVALID_ARG;
+    if (!sizes_fit) return OSB200_ERR_INVALID_ARG;
+    for (size_t i = 0; i < N; ++i)
+        for (size_t j = i + 1; j < N; ++j) {
+            const ArrayArg &x = a[i], &y = a[j];
+            if (!x.p || !y.p || !(x.written || y.written) || (in_place && i == 0 && j == 1 && x.p == y.p)) continue;
+            if (overlaps(reinterpret_cast<uintptr_t>(x.p), x.bytes, reinterpret_cast<uintptr_t>(y.p), y.bytes))
+                return OSB200_ERR_INVALID_ARG;
+        }
+    return OSB200_OK;
+}
+
+// The workspace of the segment calls: one u32 per segment of the alt key buffer for the class lists (at least 4 max_n bytes
+// for every handle shape; segment ids are u32) and the 4 u64 class counts in the control block's scratch words (err()).
+int check_segment_workspace(const osb200_sorter* h, uint64_t num_segments)
+{
+    static_assert(ControlLayout::err_bytes >= 4 * sizeof(unsigned long long), "the class counts live in the scratch words");
+    return num_segments > h->max_n || num_segments > (1ull << 32) ? OSB200_ERR_SIZE : OSB200_OK;
+}
+
 // The launch plan (reference: OneSweepDispatcher.cuh:311-363): GlobalHistogram, Scan, one DigitBinningPass per digit
 // place of [begin_bit, end_bit), then the (normally empty) copy-back.  Everything is enqueued on `stream`; which passes
 // actually move data is decided on the device (osb::SortPlan): the host never waits for the histogram.
@@ -535,40 +568,36 @@ int osb200_sort_keys_u64(osb200_handle h, uint64_t* d_keys, uint64_t n, void* st
     return sort_impl(h, h->key_bytes, d_keys, nullptr, n, static_cast<cudaStream_t>(stream));
 }
 
-// Typed keys (SURVEY 8f rank 1).  key_type must match the key width (the handle's, or the row sort's key_bytes).  *codec is
-// c, or null for plain unsigned ascending keys, which the kernels sort as they are.
-static int make_codec(int key_bytes, int key_type, int descending, osb::KeyCodec* c, const osb::KeyCodec** codec)
+// Typed keys (SURVEY 8f rank 1).  The codec of key_type for keys of key_bytes: 2 (osb200_key16_type, on a 4-byte handle
+// the same driver with a key width of 2 -- two digit passes; F16 and BF16 share the float codec, sign bit 15, and differ
+// only in the dtype the caller keeps them in), 4 or 8 (osb200_key_type of that width).  A type of another width, or
+// another key_bytes: INVALID_ARG.  *codec is c with `flags`, or null for plain unsigned ascending keys, which the kernels
+// sort as they are.
+static int codec_for(int key_bytes, int key_type, int descending, uint32_t flags, osb::KeyCodec* c, const osb::KeyCodec** codec)
 {
     const bool wide64 = key_bytes == 8;
-    const unsigned long long all = wide64 ? ~0ull : 0xffffffffull, sign = wide64 ? (1ull << 63) : (1ull << 31);
-    switch (key_type) {
-        case OSB200_KEY_U32: if (wide64) return OSB200_ERR_INVALID_ARG; c->a = 0; c->b = 0; break;
-        case OSB200_KEY_I32: if (wide64) return OSB200_ERR_INVALID_ARG; c->a = 0; c->b = sign; break;
-        case OSB200_KEY_F32: if (wide64) return OSB200_ERR_INVALID_ARG; c->a = all; c->b = sign; break;
-        case OSB200_KEY_U64: if (!wide64) return OSB200_ERR_INVALID_ARG; c->a = 0; c->b = 0; break;
-        case OSB200_KEY_I64: if (!wide64) return OSB200_ERR_INVALID_ARG; c->a = 0; c->b = sign; break;
-        case OSB200_KEY_F64: if (!wide64) return OSB200_ERR_INVALID_ARG; c->a = all; c->b = sign; break;
-        default: return OSB200_ERR_INVALID_ARG;
+    const unsigned long long all = wide64 ? ~0ull : key_bytes == 4 ? 0xffffffffull : 0xffffull, sign = all ^ (all >> 1);
+    if (key_bytes == 2) {
+        switch (key_type) {
+            case OSB200_KEY16_U16: c->a = 0; c->b = 0; break;
+            case OSB200_KEY16_I16: c->a = 0; c->b = sign; break;
+            case OSB200_KEY16_F16:
+            case OSB200_KEY16_BF16: c->a = all; c->b = sign; break;
+            default: return OSB200_ERR_INVALID_ARG;
+        }
+    } else if (key_bytes == 4 || key_bytes == 8) {
+        switch (key_type) {
+            case OSB200_KEY_U32: case OSB200_KEY_U64: c->a = 0; c->b = 0; break;
+            case OSB200_KEY_I32: case OSB200_KEY_I64: c->a = 0; c->b = sign; break;
+            case OSB200_KEY_F32: case OSB200_KEY_F64: c->a = all; c->b = sign; break;
+            default: return OSB200_ERR_INVALID_ARG;
+        }
+        if ((key_type >= OSB200_KEY_U64) != wide64) return OSB200_ERR_INVALID_ARG;  // a type of the other width
+    } else {
+        return OSB200_ERR_INVALID_ARG;
     }
     c->d = descending ? all : 0;
-    c->flags = 0;
-    *codec = c->a == 0 && c->b == 0 && c->d == 0 ? nullptr : c;
-    return OSB200_OK;
-}
-
-// 16-bit keys (osb200_key16_type) on a 4-byte handle: the same driver with a key width of 2 -- two digit passes.  F16 and
-// BF16 share the float codec (sign bit 15); they differ only in the dtype the caller keeps them in.
-static int make_codec16(int key_type, int descending, osb::KeyCodec* c, const osb::KeyCodec** codec)
-{
-    switch (key_type) {
-        case OSB200_KEY16_U16: c->a = 0; c->b = 0; break;
-        case OSB200_KEY16_I16: c->a = 0; c->b = 0x8000u; break;
-        case OSB200_KEY16_F16:
-        case OSB200_KEY16_BF16: c->a = 0xFFFFu; c->b = 0x8000u; break;
-        default: return OSB200_ERR_INVALID_ARG;
-    }
-    c->d = descending ? 0xFFFFu : 0;
-    c->flags = 0;
+    c->flags = flags;
     *codec = c->a == 0 && c->b == 0 && c->d == 0 ? nullptr : c;
     return OSB200_OK;
 }
@@ -577,7 +606,7 @@ static int make_codec16(int key_type, int descending, osb::KeyCodec* c, const os
 // INVALID_ARG), then the variant (typed keys and the indices mode live in the default pass's device plan).
 static int typed_codec(const osb200_sorter* h, int key_bytes, int key_type, int descending, osb::KeyCodec* c, const osb::KeyCodec** codec)
 {
-    const int st = key_bytes == 2 ? make_codec16(key_type, descending, c, codec) : make_codec(key_bytes, key_type, descending, c, codec);
+    const int st = codec_for(key_bytes, key_type, descending, 0u, c, codec);
     if (st != OSB200_OK) return st;
     return h->cfg.variant == osb::kVariantWide ? OSB200_OK : OSB200_ERR_UNSUPPORTED;
 }
@@ -682,6 +711,10 @@ int osb200_argsort16(osb200_handle h, const void* d_keys_in, void* d_keys_out, u
     return argsort_impl(h, 2, d_keys_in, d_keys_out, d_indices, n, key_type, descending, stream);
 }
 
+// The row and segment sorts and top-k take 2-, 4- or 8-byte keys of any handle; their kernels encode every key they load and
+// decode every key they store.
+static constexpr uint32_t kRaggedCodecFlags = osb::kCodecEncodeOnLoad | osb::kCodecDecodeOnStore;
+
 // Row sort: one launch, no workspace -- only the handle's device, rank mode and SM count are used, so any handle will do.
 int osb200_sort_rows(osb200_handle h, const void* d_keys_in, void* d_keys_out, uint32_t* d_indices, uint64_t num_rows,
                      uint32_t row_len, int key_bytes, int key_type, int descending, void* stream)
@@ -689,40 +722,27 @@ int osb200_sort_rows(osb200_handle h, const void* d_keys_in, void* d_keys_out, u
     if (check_handle(h) != OSB200_OK) return OSB200_ERR_INVALID_ARG;
     osb::KeyCodec c;
     const osb::KeyCodec* codec = nullptr;
-    int st = key_bytes == 2 ? make_codec16(key_type, descending, &c, &codec)
-             : key_bytes == 4 || key_bytes == 8 ? make_codec(key_bytes, key_type, descending, &c, &codec)
-                                                : OSB200_ERR_INVALID_ARG;
+    int st = codec_for(key_bytes, key_type, descending, kRaggedCodecFlags, &c, &codec);
     if (st != OSB200_OK) return st;
     if (num_rows == 0 || row_len == 0) return OSB200_OK;
-    const uintptr_t in = reinterpret_cast<uintptr_t>(d_keys_in), out = reinterpret_cast<uintptr_t>(d_keys_out),
-                    idx = reinterpret_cast<uintptr_t>(d_indices);
-    if (!in || !out) return OSB200_ERR_INVALID_ARG;
-    // the kernels load and store element by element: natural alignment is enough
-    if (((in | out) & static_cast<uintptr_t>(key_bytes - 1)) || (idx & 3u)) return OSB200_ERR_INVALID_ARG;
-    // the array sizes in bytes must fit in 64 bits
-    if (num_rows > UINT64_MAX / row_len) return OSB200_ERR_INVALID_ARG;
-    const uint64_t n = num_rows * row_len;
-    if (n > UINT64_MAX / 8) return OSB200_ERR_INVALID_ARG;
-    const uint64_t kb = n * static_cast<uint64_t>(key_bytes), ib = n * sizeof(uint32_t);
-    // in place (out == in) is fine: a row is read whole before it is written; any other overlap is not
-    if ((in != out && overlaps(in, kb, out, kb)) || (idx && (overlaps(in, kb, idx, ib) || overlaps(out, kb, idx, ib))))
-        return OSB200_ERR_INVALID_ARG;
+    const uint64_t n = num_rows * row_len, kb = n * static_cast<uint64_t>(key_bytes), ib = n * sizeof(uint32_t);
+    const ArrayArg arrays[] = {{d_keys_in, kb, key_bytes, true, false}, {d_keys_out, kb, key_bytes, true, true},
+                               {d_indices, ib, 4, false, true}};
+    st = check_arrays(arrays, num_rows <= UINT64_MAX / row_len && n <= UINT64_MAX / 8, true);
+    if (st != OSB200_OK) return st;
     if (row_len > osb::row_sort_capacity(key_bytes)) return OSB200_ERR_SIZE;
     cudaStream_t q = static_cast<cudaStream_t>(stream);
     if (row_len == 1) {  // every row is sorted already
-        if (in != out) OSB_TRY(cudaMemcpyAsync(d_keys_out, d_keys_in, kb, cudaMemcpyDeviceToDevice, q));
-        if (idx) OSB_TRY(cudaMemsetAsync(d_indices, 0, ib, q));
+        if (d_keys_in != d_keys_out) OSB_TRY(cudaMemcpyAsync(d_keys_out, d_keys_in, kb, cudaMemcpyDeviceToDevice, q));
+        if (d_indices) OSB_TRY(cudaMemsetAsync(d_indices, 0, ib, q));
         return OSB200_OK;
     }
-    c.flags = osb::kCodecEncodeOnLoad | osb::kCodecDecodeOnStore;
     OSB_TRY(osb::launch_row_sort(d_keys_in, d_keys_out, d_indices, num_rows, row_len, key_bytes, codec,
                                  h->cfg.rank_mode, h->debug_rows_block, h->sm_count, q));
     return OSB200_OK;
 }
 
-// Segment sort by offsets: the row sort's kernels for ragged rows.  Workspace: one u32 per segment for the class lists, in
-// the alt key buffer (at least 4 max_n bytes for every handle shape), and the 4 u64 class counts in the control block's
-// scratch words (err()).
+// Segment sort by offsets: the row sort's kernels for ragged rows, with the workspace of check_segment_workspace.
 int osb200_sort_segments(osb200_handle h, const void* d_keys_in, void* d_keys_out, uint32_t* d_indices, uint64_t n,
                          const uint64_t* d_segment_offsets, uint64_t num_segments, uint32_t max_segment_len, int key_bytes,
                          int key_type, int descending, void* stream)
@@ -730,29 +750,17 @@ int osb200_sort_segments(osb200_handle h, const void* d_keys_in, void* d_keys_ou
     if (check_handle(h) != OSB200_OK) return OSB200_ERR_INVALID_ARG;
     osb::KeyCodec c;
     const osb::KeyCodec* codec = nullptr;
-    int st = key_bytes == 2 ? make_codec16(key_type, descending, &c, &codec)
-             : key_bytes == 4 || key_bytes == 8 ? make_codec(key_bytes, key_type, descending, &c, &codec)
-                                                : OSB200_ERR_INVALID_ARG;
+    int st = codec_for(key_bytes, key_type, descending, kRaggedCodecFlags, &c, &codec);
     if (st != OSB200_OK) return st;
     if (n == 0 || num_segments == 0 || max_segment_len == 0) return OSB200_OK;
-    const uintptr_t in = reinterpret_cast<uintptr_t>(d_keys_in), out = reinterpret_cast<uintptr_t>(d_keys_out),
-                    idx = reinterpret_cast<uintptr_t>(d_indices), off = reinterpret_cast<uintptr_t>(d_segment_offsets);
-    if (!in || !out || !off) return OSB200_ERR_INVALID_ARG;
-    // the kernels load and store element by element: natural alignment is enough
-    if (((in | out) & static_cast<uintptr_t>(key_bytes - 1)) || (idx & 3u) || (off & 7u)) return OSB200_ERR_INVALID_ARG;
-    // the array sizes in bytes must fit in 64 bits
-    if (n > UINT64_MAX / 8 || num_segments > UINT64_MAX / 8 - 1) return OSB200_ERR_INVALID_ARG;
     const uint64_t kb = n * static_cast<uint64_t>(key_bytes), ib = n * sizeof(uint32_t), ob = (num_segments + 1) * sizeof(uint64_t);
-    // in place (out == in) is fine: a segment is read whole before it is written; any other overlap is not, and the offsets,
-    // read by every kernel of the call, must not overlap what it writes
-    if ((in != out && overlaps(in, kb, out, kb)) || (idx && (overlaps(in, kb, idx, ib) || overlaps(out, kb, idx, ib))) ||
-        overlaps(off, ob, out, kb) || (idx && overlaps(off, ob, idx, ib)))
-        return OSB200_ERR_INVALID_ARG;
+    // the offsets are read by every kernel of the call
+    const ArrayArg arrays[] = {{d_keys_in, kb, key_bytes, true, false}, {d_keys_out, kb, key_bytes, true, true},
+                               {d_indices, ib, 4, false, true}, {d_segment_offsets, ob, 8, true, false}};
+    st = check_arrays(arrays, n <= UINT64_MAX / 8 && num_segments <= UINT64_MAX / 8 - 1, true);
+    if (st != OSB200_OK) return st;
     if (max_segment_len > osb::row_sort_capacity(key_bytes)) return OSB200_ERR_SIZE;
-    // the class lists take one u32 per segment of the alt key buffer; segment ids are u32
-    if (num_segments > h->max_n || num_segments > (1ull << 32)) return OSB200_ERR_SIZE;
-    static_assert(ControlLayout::err_bytes >= 4 * sizeof(unsigned long long), "the class counts live in the scratch words");
-    c.flags = osb::kCodecEncodeOnLoad | osb::kCodecDecodeOnStore;
+    if ((st = check_segment_workspace(h, num_segments)) != OSB200_OK) return st;
     OSB_TRY(osb::launch_sort_segments(d_keys_in, d_keys_out, d_indices, n, reinterpret_cast<const unsigned long long*>(d_segment_offsets),
                                       num_segments, max_segment_len, key_bytes, codec, h->cfg.rank_mode, h->sm_count,
                                       static_cast<uint32_t*>(h->alt_keys), h->err(), static_cast<cudaStream_t>(stream)));
@@ -766,34 +774,26 @@ int osb200_topk_rows(osb200_handle h, const void* d_keys_in, void* d_values_out,
     if (check_handle(h) != OSB200_OK) return OSB200_ERR_INVALID_ARG;
     osb::KeyCodec c;
     const osb::KeyCodec* codec = nullptr;
-    int st = key_bytes == 2 ? make_codec16(key_type, largest, &c, &codec)
-             : key_bytes == 4 || key_bytes == 8 ? make_codec(key_bytes, key_type, largest, &c, &codec)
-                                                : OSB200_ERR_INVALID_ARG;
+    int st = codec_for(key_bytes, key_type, largest, kRaggedCodecFlags, &c, &codec);
     if (st != OSB200_OK) return st;
     if (num_rows == 0 || row_len == 0 || k == 0) return OSB200_OK;
     if (k > row_len) return OSB200_ERR_INVALID_ARG;
-    const uintptr_t in = reinterpret_cast<uintptr_t>(d_keys_in), out = reinterpret_cast<uintptr_t>(d_values_out),
-                    idx = reinterpret_cast<uintptr_t>(d_indices);
-    if (!in || !out || !idx) return OSB200_ERR_INVALID_ARG;
-    // the kernels load and store element by element: natural alignment is enough
-    if (((in | out) & static_cast<uintptr_t>(key_bytes - 1)) || (idx & 3u)) return OSB200_ERR_INVALID_ARG;
-    // the array sizes in bytes must fit in 64 bits (the outputs are smaller than the input: k <= row_len)
-    if (num_rows > UINT64_MAX / row_len) return OSB200_ERR_INVALID_ARG;
+    // (the outputs are smaller than the input: k <= row_len)
     const uint64_t n = num_rows * row_len, m = num_rows * k;
-    if (n > UINT64_MAX / 8) return OSB200_ERR_INVALID_ARG;
     const uint64_t kb = n * static_cast<uint64_t>(key_bytes), ob = m * static_cast<uint64_t>(key_bytes), ib = m * sizeof(uint32_t);
-    // the outputs have another shape than the input: no in-place form, and no overlap at all
-    if (overlaps(in, kb, out, ob) || overlaps(in, kb, idx, ib) || overlaps(out, ob, idx, ib)) return OSB200_ERR_INVALID_ARG;
+    // the outputs have another shape than the input: no in-place form
+    const ArrayArg arrays[] = {{d_keys_in, kb, key_bytes, true, false}, {d_values_out, ob, key_bytes, true, true},
+                               {d_indices, ib, 4, true, true}};
+    st = check_arrays(arrays, num_rows <= UINT64_MAX / row_len && n <= UINT64_MAX / 8, false);
+    if (st != OSB200_OK) return st;
     if (k > osb::row_sort_capacity(key_bytes)) return OSB200_ERR_SIZE;
-    c.flags = osb::kCodecEncodeOnLoad | osb::kCodecDecodeOnStore;
     OSB_TRY(osb::launch_topk_rows(d_keys_in, d_values_out, d_indices, num_rows, row_len, k, key_bytes, codec, sorted != 0,
                                   h->debug_topk_capacity, h->cfg.rank_mode, h->debug_rows_block, h->sm_count,
                                   static_cast<cudaStream_t>(stream)));
     return OSB200_OK;
 }
 
-// Segment top-k: row top-k for ragged segments.  Workspace as for osb200_sort_segments: one u32 per segment of the alt key
-// buffer for the class lists and the 4 u64 class counts in the control block's scratch words.
+// Segment top-k: row top-k for ragged segments, with the workspace of check_segment_workspace.
 int osb200_topk_segments(osb200_handle h, const void* d_keys_in, void* d_values_out, uint32_t* d_indices, uint64_t n,
                          const uint64_t* d_segment_offsets, uint64_t num_segments, uint32_t k, int key_bytes, int key_type,
                          int largest, int sorted, void* stream)
@@ -801,31 +801,23 @@ int osb200_topk_segments(osb200_handle h, const void* d_keys_in, void* d_values_
     if (check_handle(h) != OSB200_OK) return OSB200_ERR_INVALID_ARG;
     osb::KeyCodec c;
     const osb::KeyCodec* codec = nullptr;
-    int st = key_bytes == 2 ? make_codec16(key_type, largest, &c, &codec)
-             : key_bytes == 4 || key_bytes == 8 ? make_codec(key_bytes, key_type, largest, &c, &codec)
-                                                : OSB200_ERR_INVALID_ARG;
+    int st = codec_for(key_bytes, key_type, largest, kRaggedCodecFlags, &c, &codec);
     if (st != OSB200_OK) return st;
     // (n == 0 is not a no-op: every row is then padding)
     if (num_segments == 0 || k == 0) return OSB200_OK;
-    const uintptr_t in = reinterpret_cast<uintptr_t>(d_keys_in), out = reinterpret_cast<uintptr_t>(d_values_out),
-                    idx = reinterpret_cast<uintptr_t>(d_indices), off = reinterpret_cast<uintptr_t>(d_segment_offsets);
-    if ((!in && n) || !out || !idx || !off) return OSB200_ERR_INVALID_ARG;
-    // the kernels load and store element by element: natural alignment is enough
-    if (((in | out) & static_cast<uintptr_t>(key_bytes - 1)) || (idx & 3u) || (off & 7u)) return OSB200_ERR_INVALID_ARG;
-    // the array sizes in bytes must fit in 64 bits
-    if (n > UINT64_MAX / 8 || num_segments > UINT64_MAX / 8 - 1 || num_segments > UINT64_MAX / 8 / k) return OSB200_ERR_INVALID_ARG;
     const uint64_t m = num_segments * k;
     const uint64_t kb = n * static_cast<uint64_t>(key_bytes), ob = m * static_cast<uint64_t>(key_bytes), ib = m * sizeof(uint32_t),
                    fb = (num_segments + 1) * sizeof(uint64_t);
-    // the outputs have another shape than the input: no in-place form, and no overlap between any two of the four arrays
-    if ((in && (overlaps(in, kb, out, ob) || overlaps(in, kb, idx, ib) || overlaps(in, kb, off, fb))) || overlaps(out, ob, idx, ib) ||
-        overlaps(off, fb, out, ob) || overlaps(off, fb, idx, ib))
+    // the outputs have another shape than the input: no in-place form
+    const ArrayArg arrays[] = {{d_keys_in, kb, key_bytes, n != 0, false}, {d_values_out, ob, key_bytes, true, true},
+                               {d_indices, ib, 4, true, true}, {d_segment_offsets, fb, 8, true, false}};
+    st = check_arrays(arrays, n <= UINT64_MAX / 8 && num_segments <= UINT64_MAX / 8 - 1 && num_segments <= UINT64_MAX / 8 / k, false);
+    if (st != OSB200_OK) return st;
+    // unlike osb200_sort_segments, input keys that overlap the offsets are refused too, though the call only reads both
+    if (overlaps(reinterpret_cast<uintptr_t>(d_keys_in), kb, reinterpret_cast<uintptr_t>(d_segment_offsets), fb))
         return OSB200_ERR_INVALID_ARG;
     if (k > osb::row_sort_capacity(key_bytes)) return OSB200_ERR_SIZE;
-    // the class lists take one u32 per segment of the alt key buffer; segment ids are u32
-    if (num_segments > h->max_n || num_segments > (1ull << 32)) return OSB200_ERR_SIZE;
-    static_assert(ControlLayout::err_bytes >= 4 * sizeof(unsigned long long), "the class counts live in the scratch words");
-    c.flags = osb::kCodecEncodeOnLoad | osb::kCodecDecodeOnStore;
+    if ((st = check_segment_workspace(h, num_segments)) != OSB200_OK) return st;
     OSB_TRY(osb::launch_topk_segments(d_keys_in, d_values_out, d_indices, n, reinterpret_cast<const unsigned long long*>(d_segment_offsets),
                                       num_segments, k, key_bytes, codec, sorted != 0, h->debug_topk_capacity, h->cfg.rank_mode,
                                       h->debug_rows_block, h->sm_count, static_cast<uint32_t*>(h->alt_keys), h->err(),

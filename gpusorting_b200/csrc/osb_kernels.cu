@@ -66,6 +66,24 @@ static unsigned capped_grid(uint64_t work, uint64_t per_cta, uint64_t cap)
     return static_cast<unsigned>(want < cap ? want : cap);
 }
 
+// Kern<<<grid, THREADS, SMEM, stream>>>(args...) on the CTAs that are resident on the device at once, at most max_ctas of
+// them: kernels that grid-stride over their work (or over lists whose length only the device knows) want every CTA
+// resident from the start.  The occupancy is queried once per process and kernel: the static belongs to this
+// instantiation, and kernels with the same signature are still different template arguments.
+constexpr uint64_t kAllResident = ~0ull;
+template <auto Kern, int THREADS, size_t SMEM, typename... Args>
+static cudaError_t launch_resident(uint64_t max_ctas, int sm_count, cudaStream_t stream, Args... args)
+{
+    static const int per_sm = [] {
+        int b = 0;
+        return cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, Kern, THREADS, SMEM) == cudaSuccess ? b : 0;
+    }();
+    if (per_sm <= 0) return cudaErrorLaunchOutOfResources;
+    const uint64_t ctas = static_cast<uint64_t>(per_sm) * sm_count;
+    Kern<<<static_cast<unsigned>(max_ctas < ctas ? max_ctas : ctas), THREADS, SMEM, stream>>>(args...);
+    return cudaGetLastError();
+}
+
 template <typename K>
 static cudaError_t set_smem(K* kernel, size_t bytes)
 {
@@ -2413,14 +2431,14 @@ template <> struct SegGeomN<uint16_t, 2> { static constexpr int K = 32, WARPS = 
 template <typename KeyT, bool PAIRS, int SIZE, bool INDICES = false, bool ROWS = false, bool LIST = false>
 struct SegShape {
     using Key = KeyT;
-    static constexpr bool pairs = PAIRS, indices = INDICES, rows = ROWS, list = LIST, has_hot = false;
+    static constexpr bool pairs = PAIRS, indices = INDICES, has_hot = false;
     using G = SegGeomN<KeyT, SIZE>;
     using S = SegSmem<KeyT, PAIRS, G::K, G::WARPS>;
     static constexpr uint32_t T = S::T;  // the longest segment it sorts
     static constexpr size_t smem = sizeof(S);
     static constexpr int ctas_per_sm = SIZE == 2 ? 2 : 8;
     template <int RANK_MODE, bool HOT = false>
-    static auto kernel()
+    static constexpr auto kernel()
     {
         if constexpr (LIST) return segment_list_sort_kernel<KeyT, PAIRS, G::K, G::WARPS, RANK_MODE, INDICES>;
         else return segment_sort_kernel<KeyT, PAIRS, G::K, G::WARPS, RANK_MODE, INDICES, ROWS>;
@@ -2433,6 +2451,7 @@ static_assert(SegShape<uint16_t, false, 1>::T == kSegBlock1Max && SegShape<uint3
               "the first block class of osb200_sort_segments is the 2,048-key geometry of every key width");
 
 // Each kind of sort lists its geometries smallest first: the launchers take the first one that holds the longest segment.
+// Segmented sort and small path (launch_segment_sort).
 using SegShapes = TypeList<
     // segmented sort and small path: 32-bit keys and pairs, 64-bit keys
     SegShape<uint32_t, false, 0>, SegShape<uint32_t, false, 1>, SegShape<uint32_t, false, 2>,
@@ -2440,30 +2459,33 @@ using SegShapes = TypeList<
     SegShape<uint64_t, false, 0>, SegShape<uint64_t, false, 1>, SegShape<uint64_t, false, 2>,
     // small path only (the single segment of a sort of at most one tile): 16-bit keys and pairs, 64-bit pairs, every argsort
     SegShape<uint16_t, false, 2>, SegShape<uint16_t, true, 2>, SegShape<uint64_t, true, 2>,
-    SegShape<uint16_t, true, 2, true>, SegShape<uint32_t, true, 2, true>, SegShape<uint64_t, true, 2, true>,
-    // row sort, block path: keys only and with indices
+    SegShape<uint16_t, true, 2, true>, SegShape<uint32_t, true, 2, true>, SegShape<uint64_t, true, 2, true>>;
+// Row sort, block path (launch_row_sort): keys only and with indices.
+using RowShapes = TypeList<
     RowShape<uint16_t, 1, false>, RowShape<uint16_t, 2, false>, RowShape<uint16_t, 1, true>, RowShape<uint16_t, 2, true>,
     RowShape<uint32_t, 1, false>, RowShape<uint32_t, 2, false>, RowShape<uint32_t, 1, true>, RowShape<uint32_t, 2, true>,
-    RowShape<uint64_t, 1, false>, RowShape<uint64_t, 2, false>, RowShape<uint64_t, 1, true>, RowShape<uint64_t, 2, true>,
-    // segment sort by offsets (osb200_sort_segments), block classes: keys only and with indices
+    RowShape<uint64_t, 1, false>, RowShape<uint64_t, 2, false>, RowShape<uint64_t, 1, true>, RowShape<uint64_t, 2, true>>;
+// Segment sort by offsets (launch_sort_segments), block classes: keys only and with indices.
+using ListShapes = TypeList<
     ListShape<uint16_t, 1, false>, ListShape<uint16_t, 2, false>, ListShape<uint16_t, 1, true>, ListShape<uint16_t, 2, true>,
     ListShape<uint32_t, 1, false>, ListShape<uint32_t, 2, false>, ListShape<uint32_t, 1, true>, ListShape<uint32_t, 2, true>,
     ListShape<uint64_t, 1, false>, ListShape<uint64_t, 2, false>, ListShape<uint64_t, 1, true>, ListShape<uint64_t, 2, true>>;
 
-// the longest segment (ROWS: row) of key_bytes-wide keys that a shape of the list sorts; 0 if there is none
-template <bool ROWS>
-static uint32_t seg_capacity(int key_bytes)
+// the longest segment of key_bytes-wide keys that a shape of the list sorts; 0 if there is none
+template <typename... Shapes>
+static uint32_t capacity_of(TypeList<Shapes...> shapes, int key_bytes)
 {
     uint32_t cap = 0;
-    for_each_type(SegShapes{}, [&](auto s) {
+    for_each_type(shapes, [&](auto s) {
         using S = decltype(s);
-        if (S::rows == ROWS && !S::list && key_bytes == static_cast<int>(sizeof(typename S::Key)) && S::T > cap) cap = S::T;
+        if (key_bytes == static_cast<int>(sizeof(typename S::Key)) && S::T > cap) cap = S::T;
         return cudaSuccess;
     });
     return cap;
 }
 
-uint32_t segment_sort_capacity(int key_bytes) { return seg_capacity<false>(key_bytes); }
+uint32_t segment_sort_capacity(int key_bytes) { return capacity_of(SegShapes{}, key_bytes); }
+uint32_t row_sort_capacity(int key_bytes) { return capacity_of(RowShapes{}, key_bytes); }
 
 template <typename Shape>
 static cudaError_t launch_seg(Shape, void* keys, uint32_t* vals, const unsigned long long* seg_off, uint64_t num_segments,
@@ -2471,19 +2493,15 @@ static cudaError_t launch_seg(Shape, void* keys, uint32_t* vals, const unsigned 
                               const KeyCodec& codec, int rank_mode, int sm_count, cudaStream_t stream, const void* keys_in)
 {
     using KeyT = typename Shape::Key;
-    if constexpr (Shape::list) {
-        return cudaErrorInvalidValue;  // launch_sort_segments launches those
-    } else {
-        const uint64_t cap = static_cast<uint64_t>(sm_count) * Shape::ctas_per_sm;
-        const unsigned grid = static_cast<unsigned>(num_segments < cap ? num_segments : cap);
-        return with_rank_mode(rank_mode, [&](auto r) {
-            const auto kern = Shape::template kernel<decltype(r)::value>();
-            kern<<<grid, Shape::S::THREADS, Shape::smem, stream>>>(static_cast<KeyT*>(keys), vals, seg_off, num_segments, single_n,
-                                                                  max_len, begin_bit, places, last_bits, codec,
-                                                                  static_cast<const KeyT*>(keys_in));
-            return cudaGetLastError();
-        });
-    }
+    const uint64_t cap = static_cast<uint64_t>(sm_count) * Shape::ctas_per_sm;
+    const unsigned grid = static_cast<unsigned>(num_segments < cap ? num_segments : cap);
+    return with_rank_mode(rank_mode, [&](auto r) {
+        const auto kern = Shape::template kernel<decltype(r)::value>();
+        kern<<<grid, Shape::S::THREADS, Shape::smem, stream>>>(static_cast<KeyT*>(keys), vals, seg_off, num_segments, single_n,
+                                                              max_len, begin_bit, places, last_bits, codec,
+                                                              static_cast<const KeyT*>(keys_in));
+        return cudaGetLastError();
+    });
 }
 
 cudaError_t launch_segment_sort(void* keys, uint32_t* vals, int key_bytes, const unsigned long long* seg_off, uint64_t num_segments,
@@ -2499,8 +2517,7 @@ cudaError_t launch_segment_sort(void* keys, uint32_t* vals, int key_bytes, const
         SegShapes{},
         [&](auto s) {
             using S = decltype(s);
-            return !S::rows && !S::list && key_bytes == static_cast<int>(sizeof(typename S::Key)) && S::pairs == pairs &&
-                   S::indices == indices &&
+            return key_bytes == static_cast<int>(sizeof(typename S::Key)) && S::pairs == pairs && S::indices == indices &&
                    max_len <= S::T;
         },
         [&](auto s) {
@@ -2530,6 +2547,19 @@ struct RowWarpSmem {  // one per warp: 1 KB of bins + the staging area (at most 
     alignas(16) KeyT keys[32 * K];
     uint32_t idx[INDICES ? 32 * K : 1];
 };
+template <typename KeyT, int K, bool INDICES>
+constexpr size_t kRowWarpSmemBytes = kRowWarps * sizeof(RowWarpSmem<KeyT, K, INDICES>);  // a CTA's dynamic shared memory
+
+// The keys per lane of a warp that sorts a run of len <= kRowWarpMaxLen keys: f(std::integral_constant<int, K>{}), K = 1, 2,
+// 4 or 8.
+template <typename F>
+static cudaError_t with_warp_k(uint32_t len, F&& f)
+{
+    if (len <= 32) return f(std::integral_constant<int, 1>{});
+    if (len <= 64) return f(std::integral_constant<int, 2>{});
+    if (len <= 128) return f(std::integral_constant<int, 4>{});
+    return f(std::integral_constant<int, 8>{});
+}
 
 // What a warp keeps across the runs it sorts: its lane, lane mask, the hist of its staging area as uint4 (lane l owns bins
 // 8l .. 8l+7: h4[2l], h4[2l+1]) and the codec as key-wide words.
@@ -2657,37 +2687,6 @@ row_sort_warp_kernel(const KeyT* in, KeyT* out, uint32_t* __restrict__ idx_out, 
         warp_sort_run<KeyT, K, RANK_MODE, INDICES>(sm, x, in, out, idx_out, row * row_len, row_len);
 }
 
-// CTAs of one kernel that are resident on one SM (the warp path's grid: a grid-stride loop over the rows wants every CTA
-// resident from the start)
-template <typename KeyT, int K, int RANK_MODE, bool INDICES>
-static cudaError_t launch_row_warp(const void* in, void* out, uint32_t* idx, uint64_t num_rows, uint32_t row_len,
-                                   const KeyCodec& codec, int sm_count, cudaStream_t stream)
-{
-    auto kern = row_sort_warp_kernel<KeyT, K, RANK_MODE, INDICES>;
-    constexpr size_t smem = kRowWarps * sizeof(RowWarpSmem<KeyT, K, INDICES>);
-    static const int per_sm = [&] {
-        int b = 0;
-        return cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, kern, kRowWarps * 32, smem) == cudaSuccess ? b : 0;
-    }();
-    if (per_sm <= 0) return cudaErrorLaunchOutOfResources;
-    const uint64_t need = (num_rows + kRowWarps - 1) / kRowWarps, cap = static_cast<uint64_t>(sm_count) * per_sm;
-    kern<<<static_cast<unsigned>(need < cap ? need : cap), kRowWarps * 32, smem, stream>>>(
-        static_cast<const KeyT*>(in), static_cast<KeyT*>(out), idx, num_rows, row_len, codec);
-    return cudaGetLastError();
-}
-
-template <typename KeyT, int RANK_MODE, bool INDICES>
-static cudaError_t launch_row_warp_k(const void* in, void* out, uint32_t* idx, uint64_t num_rows, uint32_t row_len,
-                                     const KeyCodec& codec, int sm_count, cudaStream_t stream)
-{
-    if (row_len <= 32) return launch_row_warp<KeyT, 1, RANK_MODE, INDICES>(in, out, idx, num_rows, row_len, codec, sm_count, stream);
-    if (row_len <= 64) return launch_row_warp<KeyT, 2, RANK_MODE, INDICES>(in, out, idx, num_rows, row_len, codec, sm_count, stream);
-    if (row_len <= 128) return launch_row_warp<KeyT, 4, RANK_MODE, INDICES>(in, out, idx, num_rows, row_len, codec, sm_count, stream);
-    return launch_row_warp<KeyT, 8, RANK_MODE, INDICES>(in, out, idx, num_rows, row_len, codec, sm_count, stream);
-}
-
-uint32_t row_sort_capacity(int key_bytes) { return seg_capacity<true>(key_bytes); }
-
 cudaError_t launch_row_sort(const void* keys_in, void* keys_out, uint32_t* indices, uint64_t num_rows, uint32_t row_len,
                             int key_bytes, const KeyCodec* codec_in, int rank_mode, bool block_only, int sm_count,
                             cudaStream_t stream)
@@ -2698,19 +2697,26 @@ cudaError_t launch_row_sort(const void* keys_in, void* keys_out, uint32_t* indic
     if (row_len <= kRowWarpMaxLen && !block_only) {
         return with_key_type(TypeList<uint16_t, uint32_t, uint64_t>{}, key_bytes, [&](auto k) {
             return with_rank_mode(rank_mode, [&](auto r) {
-                using KeyT = decltype(k);
-                constexpr int R = decltype(r)::value;
-                return indices ? launch_row_warp_k<KeyT, R, true>(keys_in, keys_out, indices, num_rows, row_len, codec, sm_count, stream)
-                               : launch_row_warp_k<KeyT, R, false>(keys_in, keys_out, indices, num_rows, row_len, codec, sm_count, stream);
+                return with_warp_k(row_len, [&](auto kk) {
+                    using KeyT = decltype(k);
+                    constexpr int R = decltype(r)::value, K = decltype(kk)::value;
+                    auto go = [&](auto ind) {
+                        constexpr bool I = decltype(ind)::value;
+                        return launch_resident<row_sort_warp_kernel<KeyT, K, R, I>, kRowWarps * 32, kRowWarpSmemBytes<KeyT, K, I>>(
+                            (num_rows + kRowWarps - 1) / kRowWarps, sm_count, stream, static_cast<const KeyT*>(keys_in),
+                            static_cast<KeyT*>(keys_out), indices, num_rows, row_len, codec);
+                    };
+                    return indices ? go(std::true_type{}) : go(std::false_type{});
+                });
             });
         });
     }
     // block path: segment s of segment_sort_kernel is row s
     return find_type(
-        SegShapes{},
+        RowShapes{},
         [&](auto s) {
             using S = decltype(s);
-            return S::rows && key_bytes == static_cast<int>(sizeof(typename S::Key)) && S::indices == (indices != nullptr) && row_len <= S::T;
+            return key_bytes == static_cast<int>(sizeof(typename S::Key)) && S::indices == (indices != nullptr) && row_len <= S::T;
         },
         [&](auto s) {
             return launch_seg(s, keys_out, indices, nullptr, num_rows, row_len, row_len, 0u, static_cast<uint32_t>(key_bytes), 8u, codec,
@@ -2812,14 +2818,6 @@ segment_sort_warp_kernel(const KeyT* in, KeyT* out, uint32_t* __restrict__ idx_o
     }
 }
 
-// resident CTAs of `kern` per SM (the class kernels' grid: they grid-stride over lists whose length only the device knows)
-template <typename Kern>
-static int resident_per_sm(Kern kern, int threads, size_t smem)
-{
-    int b = 0;
-    return cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, kern, threads, smem) == cudaSuccess ? b : 0;
-}
-
 cudaError_t launch_sort_segments(const void* keys_in, void* keys_out, uint32_t* indices, uint64_t n,
                                  const unsigned long long* off, uint64_t num_segments, uint32_t max_len, int key_bytes,
                                  const KeyCodec* codec_in, int rank_mode, int sm_count, uint32_t* list,
@@ -2841,40 +2839,32 @@ cudaError_t launch_sort_segments(const void* keys_in, void* keys_out, uint32_t* 
         return with_rank_mode(rank_mode, [&](auto r) {
             using KeyT = decltype(k);
             constexpr int R = decltype(r)::value;
-            auto go = [&](auto kern, auto smem_of) {
-                constexpr size_t smem = kRowWarps * sizeof(decltype(smem_of));
-                static const int per_sm = resident_per_sm(kern, kRowWarps * 32, smem);
-                if (per_sm <= 0) return cudaErrorLaunchOutOfResources;
-                kern<<<per_sm * sm_count, kRowWarps * 32, smem, stream>>>(static_cast<const KeyT*>(keys_in), static_cast<KeyT*>(keys_out), indices, off,
-                                                            list, counts, codec);
-                return cudaGetLastError();
+            auto go = [&](auto ind) {  // each warp's staging area is sized for 8 keys per lane
+                constexpr bool I = decltype(ind)::value;
+                return launch_resident<segment_sort_warp_kernel<KeyT, R, I>, kRowWarps * 32, kRowWarpSmemBytes<KeyT, 8, I>>(
+                    kAllResident, sm_count, stream, static_cast<const KeyT*>(keys_in), static_cast<KeyT*>(keys_out), indices, off,
+                    list, counts, codec);
             };
-            return indices ? go(segment_sort_warp_kernel<KeyT, R, true>, RowWarpSmem<KeyT, 8, true>{})
-                           : go(segment_sort_warp_kernel<KeyT, R, false>, RowWarpSmem<KeyT, 8, false>{});
+            return indices ? go(std::true_type{}) : go(std::false_type{});
         });
     });
     // the block classes that max_len reaches: both share the block list, each takes its own lengths
     for (int cls = 1; e == cudaSuccess && cls <= 2; ++cls) {
         if (max_len <= (cls == 1 ? kRowWarpMaxLen : kSegBlock1Max)) break;
         e = find_type(
-            SegShapes{},
+            ListShapes{},
             [&](auto s) {
                 using S = decltype(s);
-                return S::list && key_bytes == static_cast<int>(sizeof(typename S::Key)) && S::indices == (indices != nullptr) &&
+                return key_bytes == static_cast<int>(sizeof(typename S::Key)) && S::indices == (indices != nullptr) &&
                        (S::T == kSegBlock1Max) == (cls == 1);
             },
             [&](auto s) {
                 using S = decltype(s);
                 using KeyT = typename S::Key;
-                if constexpr (!S::list) return cudaErrorInvalidValue;
-                else return with_rank_mode(rank_mode, [&](auto r) {
-                    const auto kern = S::template kernel<decltype(r)::value>();
-                    static const int per_sm = resident_per_sm(kern, S::S::THREADS, S::smem);
-                    if (per_sm <= 0) return cudaErrorLaunchOutOfResources;
-                    kern<<<per_sm * sm_count, S::S::THREADS, S::smem, stream>>>(static_cast<KeyT*>(keys_out), indices, off, num_segments,
-                                                                               max_len, static_cast<uint32_t>(key_bytes), codec,
-                                                                               static_cast<const KeyT*>(keys_in), list, counts);
-                    return cudaGetLastError();
+                return with_rank_mode(rank_mode, [&](auto r) {
+                    return launch_resident<S::template kernel<decltype(r)::value>(), S::S::THREADS, S::smem>(
+                        kAllResident, sm_count, stream, static_cast<KeyT*>(keys_out), indices, off, num_segments, max_len,
+                        static_cast<uint32_t>(key_bytes), codec, static_cast<const KeyT*>(keys_in), list, counts);
                 });
             });
     }
@@ -3201,37 +3191,13 @@ struct TopkSortShape {
     static constexpr uint32_t T = S::T;
     static constexpr size_t smem = sizeof(S);
     template <int RANK_MODE, bool HOT = false>
-    static auto kernel() { return topk_sort_kernel<KeyT, G::K, G::WARPS, RANK_MODE>; }
+    static constexpr auto kernel() { return topk_sort_kernel<KeyT, G::K, G::WARPS, RANK_MODE>; }
     template <int RANK_MODE>
-    static auto list_kernel() { return topk_segment_sort_kernel<KeyT, G::K, G::WARPS, RANK_MODE>; }
+    static constexpr auto list_kernel() { return topk_segment_sort_kernel<KeyT, G::K, G::WARPS, RANK_MODE>; }
 };
 using TopkSortShapes = TypeList<TopkSortShape<uint16_t, 1>, TopkSortShape<uint16_t, 2>, TopkSortShape<uint32_t, 1>,
                                 TopkSortShape<uint32_t, 2>, TopkSortShape<uint64_t, 1>, TopkSortShape<uint64_t, 2>>;
 using TopkKeys = TypeList<uint16_t, uint32_t, uint64_t>;
-
-template <typename KeyT, int K, int RANK_MODE>
-static cudaError_t launch_topk_warp(const KeyT* in, KeyT* out, const uint32_t* idx_in, uint32_t* idx_out, uint64_t num_rows,
-                                    uint32_t row_len, uint32_t k, const KeyCodec& codec, int sm_count, cudaStream_t stream)
-{
-    auto kern = topk_warp_kernel<KeyT, K, RANK_MODE>;
-    constexpr size_t smem = kRowWarps * sizeof(RowWarpSmem<KeyT, K, true>);
-    static const int per_sm = resident_per_sm(kern, kRowWarps * 32, smem);
-    if (per_sm <= 0) return cudaErrorLaunchOutOfResources;
-    const uint64_t need = (num_rows + kRowWarps - 1) / kRowWarps, cap = static_cast<uint64_t>(sm_count) * per_sm;
-    kern<<<static_cast<unsigned>(need < cap ? need : cap), kRowWarps * 32, smem, stream>>>(in, out, idx_in, idx_out, num_rows, row_len,
-                                                                                          k, codec);
-    return cudaGetLastError();
-}
-
-template <typename KeyT, int RANK_MODE>
-static cudaError_t launch_topk_warp_k(const KeyT* in, KeyT* out, const uint32_t* idx_in, uint32_t* idx_out, uint64_t num_rows,
-                                      uint32_t row_len, uint32_t k, const KeyCodec& codec, int sm_count, cudaStream_t stream)
-{
-    if (row_len <= 32) return launch_topk_warp<KeyT, 1, RANK_MODE>(in, out, idx_in, idx_out, num_rows, row_len, k, codec, sm_count, stream);
-    if (row_len <= 64) return launch_topk_warp<KeyT, 2, RANK_MODE>(in, out, idx_in, idx_out, num_rows, row_len, k, codec, sm_count, stream);
-    if (row_len <= 128) return launch_topk_warp<KeyT, 4, RANK_MODE>(in, out, idx_in, idx_out, num_rows, row_len, k, codec, sm_count, stream);
-    return launch_topk_warp<KeyT, 8, RANK_MODE>(in, out, idx_in, idx_out, num_rows, row_len, k, codec, sm_count, stream);
-}
 
 cudaError_t launch_topk_rows(const void* keys_in, void* values_out, uint32_t* indices, uint64_t num_rows, uint32_t row_len,
                              uint32_t k, int key_bytes, const KeyCodec* codec_in, bool sorted, uint32_t capacity, int rank_mode,
@@ -3247,46 +3213,29 @@ cudaError_t launch_topk_rows(const void* keys_in, void* values_out, uint32_t* in
         KeyT* out = static_cast<KeyT*>(values_out);
         return with_rank_mode(rank_mode, [&](auto r) {
             constexpr int R = decltype(r)::value;
-            if (row_len <= kRowWarpMaxLen && !block_only)  // sorted already
-                return launch_topk_warp_k<KeyT, R>(in, out, nullptr, indices, num_rows, row_len, k, codec, sm_count, stream);
-            auto kern = topk_select_kernel<KeyT>;
-            static const int per_sm = resident_per_sm(kern, kTopkThreads, sizeof(TopkSmem<KeyT>));
-            if (per_sm <= 0) return cudaErrorLaunchOutOfResources;
-            const uint64_t ctas = static_cast<uint64_t>(per_sm) * sm_count;
-            kern<<<static_cast<unsigned>(num_rows < ctas ? num_rows : ctas), kTopkThreads, sizeof(TopkSmem<KeyT>), stream>>>(
-                in, out, indices, num_rows, row_len, k, cap, codec);
-            cudaError_t e = cudaGetLastError();
+            // one warp per row of `src`: its first k sorted keys go to row r * k of out
+            auto warp_rows = [&](const KeyT* src, const uint32_t* idx_in, uint32_t len) {
+                return with_warp_k(len, [&](auto kk) {
+                    constexpr int K = decltype(kk)::value;
+                    return launch_resident<topk_warp_kernel<KeyT, K, R>, kRowWarps * 32, kRowWarpSmemBytes<KeyT, K, true>>(
+                        (num_rows + kRowWarps - 1) / kRowWarps, sm_count, stream, src, out, idx_in, indices, num_rows, len, k, codec);
+                });
+            };
+            if (row_len <= kRowWarpMaxLen && !block_only) return warp_rows(in, nullptr, row_len);  // sorted already
+            const cudaError_t e = launch_resident<topk_select_kernel<KeyT>, kTopkThreads, sizeof(TopkSmem<KeyT>)>(
+                num_rows, sm_count, stream, in, out, indices, num_rows, row_len, k, cap, codec);
             if (e != cudaSuccess || !sorted || k == 1) return e;
-            if (k <= kRowWarpMaxLen)
-                return launch_topk_warp_k<KeyT, R>(out, out, indices, indices, num_rows, k, k, codec, sm_count, stream);
+            if (k <= kRowWarpMaxLen) return warp_rows(out, indices, k);
             return find_type(
                 TopkSortShapes{},
                 [&](auto s) { using Sh = decltype(s); return std::is_same_v<typename Sh::Key, KeyT> && k <= Sh::T; },
                 [&](auto s) {
                     using Sh = decltype(s);
-                    const auto sk = Sh::template kernel<R>();
-                    static const int sort_per_sm = resident_per_sm(sk, Sh::S::THREADS, Sh::smem);
-                    if (sort_per_sm <= 0) return cudaErrorLaunchOutOfResources;
-                    const uint64_t sort_ctas = static_cast<uint64_t>(sort_per_sm) * sm_count;
-                    sk<<<static_cast<unsigned>(num_rows < sort_ctas ? num_rows : sort_ctas), Sh::S::THREADS, Sh::smem, stream>>>(
-                        reinterpret_cast<typename Sh::Key*>(out), indices, num_rows, k, codec);
-                    return cudaGetLastError();
+                    return launch_resident<Sh::template kernel<R>(), Sh::S::THREADS, Sh::smem>(
+                        num_rows, sm_count, stream, static_cast<typename Sh::Key*>(values_out), indices, num_rows, k, codec);
                 });
         });
     });
-}
-
-template <typename KeyT, int K, int RANK_MODE>
-static cudaError_t launch_topk_segment_sort_warp(KeyT* keys, uint32_t* idx, uint64_t num_segments, uint32_t k, const uint32_t* list,
-                                                 const unsigned long long* counts, const KeyCodec& codec, int sm_count,
-                                                 cudaStream_t stream)
-{
-    auto kern = topk_segment_sort_warp_kernel<KeyT, K, RANK_MODE>;
-    constexpr size_t smem = kRowWarps * sizeof(RowWarpSmem<KeyT, K, true>);
-    static const int per_sm = resident_per_sm(kern, kRowWarps * 32, smem);
-    if (per_sm <= 0) return cudaErrorLaunchOutOfResources;
-    kern<<<per_sm * sm_count, kRowWarps * 32, smem, stream>>>(keys, idx, num_segments, k, list, counts, codec);
-    return cudaGetLastError();
 }
 
 cudaError_t launch_topk_segments(const void* keys_in, void* values_out, uint32_t* indices, uint64_t n, const unsigned long long* off,
@@ -3310,42 +3259,27 @@ cudaError_t launch_topk_segments(const void* keys_in, void* values_out, uint32_t
         KeyT* out = static_cast<KeyT*>(values_out);
         return with_rank_mode(rank_mode, [&](auto r) {
             constexpr int R = decltype(r)::value;
-            {
-                auto kern = topk_segment_warp_kernel<KeyT, R>;
-                constexpr size_t smem = kRowWarps * sizeof(RowWarpSmem<KeyT, 8, true>);
-                static const int per_sm = resident_per_sm(kern, kRowWarps * 32, smem);
-                if (per_sm <= 0) return cudaErrorLaunchOutOfResources;
-                kern<<<per_sm * sm_count, kRowWarps * 32, smem, stream>>>(in, out, indices, n, off, list, counts, k, codec);
-                cudaError_t le = cudaGetLastError();
-                if (le != cudaSuccess) return le;
-            }
-            {
-                auto kern = topk_segment_select_kernel<KeyT>;
-                static const int per_sm = resident_per_sm(kern, kTopkThreads, sizeof(TopkSmem<KeyT>));
-                if (per_sm <= 0) return cudaErrorLaunchOutOfResources;
-                kern<<<per_sm * sm_count, kTopkThreads, sizeof(TopkSmem<KeyT>), stream>>>(in, out, indices, num_segments, k, cap, codec,
-                                                                                          off, list, counts);
-                cudaError_t le = cudaGetLastError();
-                if (le != cudaSuccess || !sorted || k == 1) return le;
-            }
+            cudaError_t le = launch_resident<topk_segment_warp_kernel<KeyT, R>, kRowWarps * 32, kRowWarpSmemBytes<KeyT, 8, true>>(
+                kAllResident, sm_count, stream, in, out, indices, n, off, list, counts, k, codec);
+            if (le == cudaSuccess)
+                le = launch_resident<topk_segment_select_kernel<KeyT>, kTopkThreads, sizeof(TopkSmem<KeyT>)>(
+                    kAllResident, sm_count, stream, in, out, indices, num_segments, k, cap, codec, off, list, counts);
+            if (le != cudaSuccess || !sorted || k == 1) return le;
             // sorted: the block list's rows, in place (the warp list's are sorted already)
-            if (k <= 32) return launch_topk_segment_sort_warp<KeyT, 1, R>(out, indices, num_segments, k, list, counts, codec, sm_count, stream);
-            if (k <= 64) return launch_topk_segment_sort_warp<KeyT, 2, R>(out, indices, num_segments, k, list, counts, codec, sm_count, stream);
-            if (k <= 128) return launch_topk_segment_sort_warp<KeyT, 4, R>(out, indices, num_segments, k, list, counts, codec, sm_count, stream);
             if (k <= kRowWarpMaxLen)
-                return launch_topk_segment_sort_warp<KeyT, 8, R>(out, indices, num_segments, k, list, counts, codec, sm_count, stream);
+                return with_warp_k(k, [&](auto kk) {
+                    constexpr int K = decltype(kk)::value;
+                    return launch_resident<topk_segment_sort_warp_kernel<KeyT, K, R>, kRowWarps * 32, kRowWarpSmemBytes<KeyT, K, true>>(
+                        kAllResident, sm_count, stream, out, indices, num_segments, k, list, counts, codec);
+                });
             return find_type(
                 TopkSortShapes{},
                 [&](auto s) { using Sh = decltype(s); return std::is_same_v<typename Sh::Key, KeyT> && k <= Sh::T; },
                 [&](auto s) {
                     using Sh = decltype(s);
-                    const auto sk = Sh::template list_kernel<R>();
-                    static const int sort_per_sm = resident_per_sm(sk, Sh::S::THREADS, Sh::smem);
-                    if (sort_per_sm <= 0) return cudaErrorLaunchOutOfResources;
-                    const uint64_t sort_ctas = static_cast<uint64_t>(sort_per_sm) * sm_count;
-                    sk<<<static_cast<unsigned>(num_segments < sort_ctas ? num_segments : sort_ctas), Sh::S::THREADS, Sh::smem, stream>>>(
-                        reinterpret_cast<typename Sh::Key*>(out), indices, num_segments, k, codec, off, n, warp_max);
-                    return cudaGetLastError();
+                    return launch_resident<Sh::template list_kernel<R>(), Sh::S::THREADS, Sh::smem>(
+                        num_segments, sm_count, stream, static_cast<typename Sh::Key*>(values_out), indices, num_segments, k, codec,
+                        off, n, warp_max);
                 });
         });
     });
@@ -3367,6 +3301,8 @@ cudaError_t configure_kernels()
     if (e == cudaSuccess) e = for_each_type(RingShapes{}, shape);
     if (e == cudaSuccess) e = for_each_type(TileShapes{}, shape);
     if (e == cudaSuccess) e = for_each_type(SegShapes{}, shape);
+    if (e == cudaSuccess) e = for_each_type(RowShapes{}, shape);
+    if (e == cudaSuccess) e = for_each_type(ListShapes{}, shape);
     if (e == cudaSuccess) e = for_each_type(TopkSortShapes{}, shape);
     if (e == cudaSuccess) e = for_each_type(TopkKeys{}, [](auto k) {
         using KeyT = decltype(k);

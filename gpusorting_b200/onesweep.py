@@ -53,6 +53,17 @@ def _check_dev_tensor(t: torch.Tensor, dtypes, name: str, n: Optional[int] = Non
         raise ValueError(f"n={n} is outside 0..{name}.numel()={t.numel()}")
 
 
+def _new_outputs(stream, x: torch.Tensor, shape, indices: bool = True, out: Optional[torch.Tensor] = None):
+    """(keys, int32 indices) of `shape` on x's device, the keys in x's dtype, allocated with torch.empty on the stream
+    (None: the current stream): the outputs belong to the stream that writes them.  out: the keys to write instead of new
+    ones; indices=False: no indices (None)."""
+    with torch.cuda.stream(stream):
+        if out is None:
+            out = torch.empty(shape, dtype=x.dtype, device=x.device)
+        idx = torch.empty(shape, dtype=torch.int32, device=x.device) if indices else None
+    return out, idx
+
+
 class OneSweepSorter:
     """Owns one C-ABI sorter handle (alt buffers, tile descriptors) for up to ``max_n`` elements.
 
@@ -119,13 +130,32 @@ class OneSweepSorter:
     def _typed(self):
         return _TYPED_DTYPES_4 if self.key_bytes == 4 else _TYPED_DTYPES_8
 
+    def _call(self, fn, *args, stream=None) -> None:
+        """fn(handle, *args, stream pointer) on the sorter's device; a failing status raises OneSweepError naming fn."""
+        with torch.cuda.device(self.device):
+            check(fn(self._h, *args, _stream_ptr(stream)), fn.__name__)
+
+    def _ragged_keys(self, x: torch.Tensor, key_type: str, offsets: Optional[torch.Tensor] = None):
+        """The checks of the row calls (x of rank >= 1) and, given offsets, of the segment calls (1-D x and its offsets);
+        returns x's key width and the C key type."""
+        if offsets is None:
+            if not (isinstance(x, torch.Tensor) and x.is_cuda and x.is_contiguous() and x.dim() >= 1 and x.dtype in _ROW_KEY_TYPES):
+                raise TypeError(f"x must be a contiguous CUDA tensor of rank >= 1 with dtype in {tuple(_ROW_KEY_TYPES)}")
+        elif not (isinstance(x, torch.Tensor) and x.is_cuda and x.is_contiguous() and x.dim() == 1 and x.dtype in _ROW_KEY_TYPES):
+            raise TypeError(f"x must be a contiguous 1-D CUDA tensor with dtype in {tuple(_ROW_KEY_TYPES)}")
+        if x.device.index != self.device:
+            raise ValueError(f"x lives on cuda:{x.device.index}, the sorter on cuda:{self.device}")
+        if offsets is not None and not (isinstance(offsets, torch.Tensor) and offsets.dtype == torch.int64
+                                        and offsets.is_contiguous() and offsets.dim() == 1 and offsets.device == x.device):
+            raise TypeError("offsets must be a contiguous 1-D int64 tensor on the device of x")
+        kb = x.element_size()
+        return kb, (KEY16_TYPES if kb == 2 else KEY_TYPES)[key_type]
+
     def sort_keys(self, keys: torch.Tensor, n: Optional[int] = None, stream=None) -> torch.Tensor:
         n = keys.numel() if n is None else int(n)
         _check_dev_tensor(keys, self._raw(), "keys", n, self.device)
-        fn, what = ((lib.osb200_sort_keys_u32, "osb200_sort_keys_u32") if self.key_bytes == 4
-                    else (lib.osb200_sort_keys_u64, "osb200_sort_keys_u64"))
-        with torch.cuda.device(self.device):
-            check(fn(self._h, keys.data_ptr(), n, _stream_ptr(stream)), what)
+        fn = lib.osb200_sort_keys_u32 if self.key_bytes == 4 else lib.osb200_sort_keys_u64
+        self._call(fn, keys.data_ptr(), n, stream=stream)
         return keys
 
     def sort_keys_typed(self, keys: torch.Tensor, key_type: str, descending: bool = False, n: Optional[int] = None,
@@ -134,9 +164,7 @@ class OneSweepSorter:
         KEY_TYPES; it states how the bits are ordered, whatever the tensor dtype (which only has to have the width)."""
         n = keys.numel() if n is None else int(n)
         _check_dev_tensor(keys, self._typed(), "keys", n, self.device)
-        with torch.cuda.device(self.device):
-            check(lib.osb200_sort_keys_typed(self._h, keys.data_ptr(), n, KEY_TYPES[key_type], 1 if descending else 0,
-                                             _stream_ptr(stream)), "osb200_sort_keys_typed")
+        self._call(lib.osb200_sort_keys_typed, keys.data_ptr(), n, KEY_TYPES[key_type], 1 if descending else 0, stream=stream)
         return keys
 
     def sort_pairs_typed(self, keys: torch.Tensor, values: torch.Tensor, key_type: str, descending: bool = False,
@@ -147,9 +175,8 @@ class OneSweepSorter:
         n = keys.numel() if n is None else int(n)
         _check_dev_tensor(keys, self._typed(), "keys", n, self.device)
         _check_dev_tensor(values, _TYPED_DTYPES_4, "values", n, self.device)
-        with torch.cuda.device(self.device):
-            check(lib.osb200_sort_pairs_typed(self._h, keys.data_ptr(), values.data_ptr(), n, KEY_TYPES[key_type],
-                                              1 if descending else 0, _stream_ptr(stream)), "osb200_sort_pairs_typed")
+        self._call(lib.osb200_sort_pairs_typed, keys.data_ptr(), values.data_ptr(), n, KEY_TYPES[key_type],
+                   1 if descending else 0, stream=stream)
         return keys, values
 
     def argsort(self, keys: torch.Tensor, key_type: str, descending: bool = False, n: Optional[int] = None, stream=None):
@@ -163,12 +190,9 @@ class OneSweepSorter:
         both directions."""
         n = keys.numel() if n is None else int(n)
         _check_dev_tensor(keys, self._typed(), "keys", n, self.device)
-        with torch.cuda.stream(stream):  # (None: the current stream) the outputs belong to the stream that writes them
-            out = torch.empty(n, dtype=keys.dtype, device=keys.device)
-            idx = torch.empty(n, dtype=torch.int32, device=keys.device)
-        with torch.cuda.device(self.device):
-            check(lib.osb200_argsort(self._h, keys.data_ptr(), out.data_ptr(), idx.data_ptr(), n, KEY_TYPES[key_type],
-                                     1 if descending else 0, _stream_ptr(stream)), "osb200_argsort")
+        out, idx = _new_outputs(stream, keys, n)
+        self._call(lib.osb200_argsort, keys.data_ptr(), out.data_ptr(), idx.data_ptr(), n, KEY_TYPES[key_type],
+                   1 if descending else 0, stream=stream)
         return out, idx
 
     # -- 16-bit keys: two digit passes over 2-byte keys, on this (4-byte) sorter's workspace --------------------------
@@ -179,9 +203,7 @@ class OneSweepSorter:
         Keys must start on a 16-byte boundary (OneSweepError status -1 otherwise).  Needs a sorter with key_bytes == 4."""
         n = keys.numel() if n is None else int(n)
         _check_dev_tensor(keys, _TYPED_DTYPES_2, "keys", n, self.device)
-        with torch.cuda.device(self.device):
-            check(lib.osb200_sort_keys16(self._h, keys.data_ptr(), n, KEY16_TYPES[key_type], 1 if descending else 0,
-                                         _stream_ptr(stream)), "osb200_sort_keys16")
+        self._call(lib.osb200_sort_keys16, keys.data_ptr(), n, KEY16_TYPES[key_type], 1 if descending else 0, stream=stream)
         return keys
 
     def sort_pairs16(self, keys: torch.Tensor, values: torch.Tensor, key_type: str, descending: bool = False,
@@ -191,9 +213,8 @@ class OneSweepSorter:
         n = keys.numel() if n is None else int(n)
         _check_dev_tensor(keys, _TYPED_DTYPES_2, "keys", n, self.device)
         _check_dev_tensor(values, _TYPED_DTYPES_4, "values", n, self.device)
-        with torch.cuda.device(self.device):
-            check(lib.osb200_sort_pairs16(self._h, keys.data_ptr(), values.data_ptr(), n, KEY16_TYPES[key_type],
-                                          1 if descending else 0, _stream_ptr(stream)), "osb200_sort_pairs16")
+        self._call(lib.osb200_sort_pairs16, keys.data_ptr(), values.data_ptr(), n, KEY16_TYPES[key_type],
+                   1 if descending else 0, stream=stream)
         return keys, values
 
     def argsort16(self, keys: torch.Tensor, key_type: str, descending: bool = False, n: Optional[int] = None, stream=None):
@@ -202,12 +223,9 @@ class OneSweepSorter:
         `keys` is left untouched.  Needs a (4, 4) sorter."""
         n = keys.numel() if n is None else int(n)
         _check_dev_tensor(keys, _TYPED_DTYPES_2, "keys", n, self.device)
-        with torch.cuda.stream(stream):  # (None: the current stream) the outputs belong to the stream that writes them
-            out = torch.empty(n, dtype=keys.dtype, device=keys.device)
-            idx = torch.empty(n, dtype=torch.int32, device=keys.device)
-        with torch.cuda.device(self.device):
-            check(lib.osb200_argsort16(self._h, keys.data_ptr(), out.data_ptr(), idx.data_ptr(), n, KEY16_TYPES[key_type],
-                                       1 if descending else 0, _stream_ptr(stream)), "osb200_argsort16")
+        out, idx = _new_outputs(stream, keys, n)
+        self._call(lib.osb200_argsort16, keys.data_ptr(), out.data_ptr(), idx.data_ptr(), n, KEY16_TYPES[key_type],
+                   1 if descending else 0, stream=stream)
         return out, idx
 
     # -- row sort: every row of a batch along its last dimension, no workspace (any sorter will do) -------------------
@@ -221,21 +239,12 @@ class OneSweepSorter:
         Returns (values, indices) shaped like `x`, indices as torch.int32 positions within the row, or `values` alone with
         return_indices=False.  The outputs are new tensors allocated with torch.empty on the stream; inplace=True sorts `x`
         itself and returns it as `values`.  The last dimension may hold at most 16,384 keys (8,192 for 8-byte dtypes)."""
-        if not (isinstance(x, torch.Tensor) and x.is_cuda and x.is_contiguous() and x.dim() >= 1 and x.dtype in _ROW_KEY_TYPES):
-            raise TypeError(f"x must be a contiguous CUDA tensor of rank >= 1 with dtype in {tuple(_ROW_KEY_TYPES)}")
-        if x.device.index != self.device:
-            raise ValueError(f"x lives on cuda:{x.device.index}, the sorter on cuda:{self.device}")
-        kb = x.element_size()
-        kt = (KEY16_TYPES if kb == 2 else KEY_TYPES)[key_type]
+        kb, kt = self._ragged_keys(x, key_type)
         row_len = x.shape[-1]
         num_rows = x.numel() // row_len if row_len else 0
-        with torch.cuda.stream(stream):  # (None: the current stream) the outputs belong to the stream that writes them
-            out = x if inplace else torch.empty_like(x)
-            idx = torch.empty(x.shape, dtype=torch.int32, device=x.device) if return_indices else None
-        with torch.cuda.device(self.device):
-            check(lib.osb200_sort_rows(self._h, x.data_ptr(), out.data_ptr(), idx.data_ptr() if idx is not None else None,
-                                       num_rows, row_len, kb, kt, 1 if descending else 0, _stream_ptr(stream)),
-                  "osb200_sort_rows")
+        out, idx = _new_outputs(stream, x, x.shape, return_indices, x if inplace else None)
+        self._call(lib.osb200_sort_rows, x.data_ptr(), out.data_ptr(), idx.data_ptr() if idx is not None else None, num_rows,
+                   row_len, kb, kt, 1 if descending else 0, stream=stream)
         return (out, idx) if return_indices else out
 
     # -- row top-k: the first k keys of every row's stable sort, no workspace (any sorter will do) ------------------------
@@ -249,22 +258,14 @@ class OneSweepSorter:
         Returns (values, indices) shaped ``x.shape[:-1] + (k,)``, indices as torch.int32 positions within the row, allocated
         with torch.empty on the stream.  The rows may be of any length; k may be at most 16,384 (8,192 for 8-byte dtypes)
         and at most the row length."""
-        if not (isinstance(x, torch.Tensor) and x.is_cuda and x.is_contiguous() and x.dim() >= 1 and x.dtype in _ROW_KEY_TYPES):
-            raise TypeError(f"x must be a contiguous CUDA tensor of rank >= 1 with dtype in {tuple(_ROW_KEY_TYPES)}")
-        if x.device.index != self.device:
-            raise ValueError(f"x lives on cuda:{x.device.index}, the sorter on cuda:{self.device}")
-        kb = x.element_size()
-        kt = (KEY16_TYPES if kb == 2 else KEY_TYPES)[key_type]
+        kb, kt = self._ragged_keys(x, key_type)
         k = int(k)
         row_len = x.shape[-1]
         num_rows = x.numel() // row_len if row_len else 0
         shape = tuple(x.shape[:-1]) + (k,)
-        with torch.cuda.stream(stream):  # (None: the current stream) the outputs belong to the stream that writes them
-            out = torch.empty(shape, dtype=x.dtype, device=x.device)
-            idx = torch.empty(shape, dtype=torch.int32, device=x.device)
-        with torch.cuda.device(self.device):
-            check(lib.osb200_topk_rows(self._h, x.data_ptr(), out.data_ptr(), idx.data_ptr(), num_rows, row_len, k, kb, kt,
-                                       1 if largest else 0, 1 if sorted else 0, _stream_ptr(stream)), "osb200_topk_rows")
+        out, idx = _new_outputs(stream, x, shape)
+        self._call(lib.osb200_topk_rows, x.data_ptr(), out.data_ptr(), idx.data_ptr(), num_rows, row_len, k, kb, kt,
+                   1 if largest else 0, 1 if sorted else 0, stream=stream)
         return out, idx
 
     # -- segment sort: ragged rows given by offsets -------------------------------------------------------------------------
@@ -282,25 +283,13 @@ class OneSweepSorter:
         are segments whose offsets decrease or pass x.numel().  max_segment_len may be at most 16,384 (8,192 for 8-byte
         dtypes); None computes the longest segment here, with one device->host read -- pass it when capturing a CUDA graph.
         num_segments may be at most the sorter's max_n."""
-        if not (isinstance(x, torch.Tensor) and x.is_cuda and x.is_contiguous() and x.dim() == 1 and x.dtype in _ROW_KEY_TYPES):
-            raise TypeError(f"x must be a contiguous 1-D CUDA tensor with dtype in {tuple(_ROW_KEY_TYPES)}")
-        if x.device.index != self.device:
-            raise ValueError(f"x lives on cuda:{x.device.index}, the sorter on cuda:{self.device}")
-        if not (isinstance(offsets, torch.Tensor) and offsets.dtype == torch.int64 and offsets.is_contiguous()
-                and offsets.dim() == 1 and offsets.device == x.device):
-            raise TypeError("offsets must be a contiguous 1-D int64 tensor on the device of x")
-        kb = x.element_size()
-        kt = (KEY16_TYPES if kb == 2 else KEY_TYPES)[key_type]
+        kb, kt = self._ragged_keys(x, key_type, offsets)
         segs = max(offsets.numel() - 1, 0)
         if max_segment_len is None:
             max_segment_len = max(int((offsets[1:] - offsets[:-1]).max().item()), 0) if segs else 0
-        with torch.cuda.stream(stream):  # (None: the current stream) the outputs belong to the stream that writes them
-            out = x if inplace else torch.empty_like(x)
-            idx = torch.empty(x.shape, dtype=torch.int32, device=x.device) if return_indices else None
-        with torch.cuda.device(self.device):
-            check(lib.osb200_sort_segments(self._h, x.data_ptr(), out.data_ptr(), idx.data_ptr() if idx is not None else None,
-                                           x.numel(), offsets.data_ptr(), segs, int(max_segment_len), kb, kt,
-                                           1 if descending else 0, _stream_ptr(stream)), "osb200_sort_segments")
+        out, idx = _new_outputs(stream, x, x.shape, return_indices, x if inplace else None)
+        self._call(lib.osb200_sort_segments, x.data_ptr(), out.data_ptr(), idx.data_ptr() if idx is not None else None,
+                   x.numel(), offsets.data_ptr(), segs, int(max_segment_len), kb, kt, 1 if descending else 0, stream=stream)
         return (out, idx) if return_indices else out
 
     # -- segment top-k: row top-k for ragged rows given by offsets -----------------------------------------------------------
@@ -318,26 +307,14 @@ class OneSweepSorter:
         Returns (values, indices) of shape [num_segments, k], indices as torch.int32, allocated with torch.empty on the
         stream.  k may be at most 16,384 (8,192 for 8-byte dtypes) and may exceed a segment's length; num_segments may be
         at most the sorter's max_n."""
-        if not (isinstance(x, torch.Tensor) and x.is_cuda and x.is_contiguous() and x.dim() == 1 and x.dtype in _ROW_KEY_TYPES):
-            raise TypeError(f"x must be a contiguous 1-D CUDA tensor with dtype in {tuple(_ROW_KEY_TYPES)}")
-        if x.device.index != self.device:
-            raise ValueError(f"x lives on cuda:{x.device.index}, the sorter on cuda:{self.device}")
-        if not (isinstance(offsets, torch.Tensor) and offsets.dtype == torch.int64 and offsets.is_contiguous()
-                and offsets.dim() == 1 and offsets.device == x.device):
-            raise TypeError("offsets must be a contiguous 1-D int64 tensor on the device of x")
-        kb = x.element_size()
-        kt = (KEY16_TYPES if kb == 2 else KEY_TYPES)[key_type]
+        kb, kt = self._ragged_keys(x, key_type, offsets)
         k = int(k)
         if k < 0:
             raise ValueError(f"k must be >= 0, got {k}")
         segs = max(offsets.numel() - 1, 0)
-        with torch.cuda.stream(stream):  # (None: the current stream) the outputs belong to the stream that writes them
-            out = torch.empty((segs, k), dtype=x.dtype, device=x.device)
-            idx = torch.empty((segs, k), dtype=torch.int32, device=x.device)
-        with torch.cuda.device(self.device):
-            check(lib.osb200_topk_segments(self._h, x.data_ptr() if x.numel() else None, out.data_ptr(), idx.data_ptr(),
-                                           x.numel(), offsets.data_ptr(), segs, k, kb, kt, 1 if largest else 0,
-                                           1 if sorted else 0, _stream_ptr(stream)), "osb200_topk_segments")
+        out, idx = _new_outputs(stream, x, (segs, k))
+        self._call(lib.osb200_topk_segments, x.data_ptr() if x.numel() else None, out.data_ptr(), idx.data_ptr(), x.numel(),
+                   offsets.data_ptr(), segs, k, kb, kt, 1 if largest else 0, 1 if sorted else 0, stream=stream)
         return out, idx
 
     def sort_bits(self, keys: torch.Tensor, begin_bit: int, end_bit: int, values: Optional[torch.Tensor] = None,
@@ -348,9 +325,8 @@ class OneSweepSorter:
         _check_dev_tensor(keys, self._raw(), "keys", n, self.device)
         if values is not None:
             _check_dev_tensor(values, _TYPED_DTYPES_4, "values", n, self.device)
-        with torch.cuda.device(self.device):
-            check(lib.osb200_sort_bits(self._h, keys.data_ptr(), values.data_ptr() if values is not None else None, n,
-                                       int(begin_bit), int(end_bit), _stream_ptr(stream)), "osb200_sort_bits")
+        self._call(lib.osb200_sort_bits, keys.data_ptr(), values.data_ptr() if values is not None else None, n, int(begin_bit),
+                   int(end_bit), stream=stream)
         return keys if values is None else (keys, values)
 
     def segmented_sort(self, keys: torch.Tensor, segment_offsets: torch.Tensor, values: Optional[torch.Tensor] = None,
@@ -369,10 +345,8 @@ class OneSweepSorter:
             return keys if values is None else (keys, values)
         if max_segment_len is None:
             max_segment_len = int((segment_offsets[1:] - segment_offsets[:-1]).max().item())
-        with torch.cuda.device(self.device):
-            check(lib.osb200_segmented_sort_u32(self._h, keys.data_ptr(), values.data_ptr() if values is not None else None,
-                                                segment_offsets.data_ptr(), segs, int(max_segment_len), _stream_ptr(stream)),
-                  "osb200_segmented_sort_u32")
+        self._call(lib.osb200_segmented_sort_u32, keys.data_ptr(), values.data_ptr() if values is not None else None,
+                   segment_offsets.data_ptr(), segs, int(max_segment_len), stream=stream)
         return keys if values is None else (keys, values)
 
     def sort_pairs(self, keys: torch.Tensor, values: torch.Tensor, n: Optional[int] = None, stream=None):
@@ -384,12 +358,9 @@ class OneSweepSorter:
         _check_dev_tensor(values, _TYPED_DTYPES_4, "values", n, self.device)  # payloads are opaque 32-bit words
         if self.key_bytes == 8:
             return self.sort_pairs_typed(keys, values, "u64", False, n, stream)
-        with torch.cuda.device(self.device):
-            check(lib.osb200_sort_pairs_u32(self._h, keys.data_ptr(), values.data_ptr(), n, _stream_ptr(stream)),
-                  "osb200_sort_pairs_u32")
+        self._call(lib.osb200_sort_pairs_u32, keys.data_ptr(), values.data_ptr(), n, stream=stream)
         return keys, values
 
-    # -- host-buffer sorts (end-to-end: H2D + sort + D2H inside the call) ---------------------------
     def sort_host(self, keys, values=None, n: Optional[int] = None):
         """keys/values: numpy arrays or CPU torch tensors (pinned or pageable), sorted in place."""
         kp, kn, kb = _host_ptr(keys)
@@ -411,9 +382,7 @@ class OneSweepSorter:
         n = keys.numel() if n is None else int(n)
         _check_dev_tensor(keys, self._typed(), "keys", n, self.device)
         hist = torch.empty(self.key_bytes * 256, dtype=torch.int64, device=keys.device)
-        with torch.cuda.device(self.device):
-            check(lib.osb200_global_histogram(self._h, keys.data_ptr(), n, hist.data_ptr(), _stream_ptr(stream)),
-                  "osb200_global_histogram")
+        self._call(lib.osb200_global_histogram, keys.data_ptr(), n, hist.data_ptr(), stream=stream)
         return hist.view(self.key_bytes, 256)
 
     def digit_binning_pass(self, src: torch.Tensor, dst: torch.Tensor, radix_shift: int, src_values=None,
@@ -428,17 +397,14 @@ class OneSweepSorter:
             _check_dev_tensor(dst_values, _TYPED_DTYPES_4, "dst_values", n, self.device)
         sv = src_values.data_ptr() if src_values is not None else None
         dv = dst_values.data_ptr() if dst_values is not None else None
-        with torch.cuda.device(self.device):
-            check(lib.osb200_digit_binning_pass(self._h, src.data_ptr(), dst.data_ptr(), sv, dv, n, int(radix_shift),
-                                                _stream_ptr(stream)), "osb200_digit_binning_pass")
+        self._call(lib.osb200_digit_binning_pass, src.data_ptr(), dst.data_ptr(), sv, dv, n, int(radix_shift), stream=stream)
 
     def validate(self, keys: torch.Tensor, n: Optional[int] = None, stream=None) -> int:
         """Number of adjacent inversions (reference Validate, UtilityKernels.cuh:403-429); 0 == sorted."""
         n = keys.numel() if n is None else int(n)
         _check_dev_tensor(keys, self._typed(), "keys", n, self.device)
         err = ctypes.c_uint64(0)
-        with torch.cuda.device(self.device):
-            check(lib.osb200_validate(self._h, keys.data_ptr(), n, ctypes.byref(err), _stream_ptr(stream)), "osb200_validate")
+        self._call(lib.osb200_validate, keys.data_ptr(), n, ctypes.byref(err), stream=stream)
         return int(err.value)
 
 
@@ -498,15 +464,22 @@ def release_cached_sorters() -> None:
         _RETIRED.pop().close()
 
 
+def _module_sorter(t, name: str, key_bytes: int, n: int, stream, dtypes=None, value_bytes: int = 4) -> OneSweepSorter:
+    """The cached sorter of t's device and the stream for a module call on t, which must be a CUDA tensor (with a dtype of
+    `dtypes`, if given).  The stream is read with t's device current."""
+    if not (isinstance(t, torch.Tensor) and t.is_cuda):
+        raise TypeError(f"{name} must be a CUDA tensor")
+    if dtypes is not None and t.dtype not in dtypes:
+        raise TypeError(f"{name}.dtype must be one of {tuple(dtypes)}")
+    with torch.cuda.device(t.device.index):
+        sp = _stream_ptr(stream)
+    return _cached_sorter(t.device.index, key_bytes, value_bytes, n, sp)
+
+
 def Sort(keys: torch.Tensor, values: Optional[torch.Tensor] = None, n: Optional[int] = None, stream=None):
     """OneSweep::Sort(keys[, values], n): ascending, stable, in place; returns its arguments."""
     n = keys.numel() if n is None else int(n)
-    kb = keys.element_size()
-    if not (isinstance(keys, torch.Tensor) and keys.is_cuda):
-        raise TypeError("keys must be a CUDA tensor")
-    with torch.cuda.device(keys.device.index):
-        sp = _stream_ptr(stream)
-    s = _cached_sorter(keys.device.index, kb, 0 if values is None else 4, n, sp)
+    s = _module_sorter(keys, "keys", keys.element_size(), n, stream, value_bytes=0 if values is None else 4)
     if values is None:
         return s.sort_keys(keys, n, stream)
     return s.sort_pairs(keys, values, n, stream)
@@ -516,11 +489,8 @@ def argsort(keys: torch.Tensor, key_type: str, descending: bool = False, n: Opti
     """Stable (sorted_keys, indices) of 32- or 64-bit keys, input untouched: OneSweepSorter.argsort on the stream's cached
     (4, 4) sorter, or its (8, 4) sorter for int64 / uint64 / float64 keys (one handle per stream, as for Sort)."""
     n = keys.numel() if n is None else int(n)
-    if not (isinstance(keys, torch.Tensor) and keys.is_cuda):
-        raise TypeError("keys must be a CUDA tensor")
-    with torch.cuda.device(keys.device.index):
-        sp = _stream_ptr(stream)
-    s = _cached_sorter(keys.device.index, 8 if keys.element_size() == 8 else 4, 4, n, sp)
+    wide = isinstance(keys, torch.Tensor) and keys.element_size() == 8
+    s = _module_sorter(keys, "keys", 8 if wide else 4, n, stream)
     return s.argsort(keys, key_type, descending, n, stream)
 
 
@@ -528,25 +498,14 @@ def argsort16(keys: torch.Tensor, key_type: str, descending: bool = False, n: Op
     """Stable (sorted_keys, indices) of 16-bit keys (int16, uint16, float16, bfloat16; key_type "u16", "i16", "f16" or
     "bf16"), input untouched: OneSweepSorter.argsort16 on the stream's cached (4, 4) sorter, the one argsort uses."""
     n = keys.numel() if n is None else int(n)
-    if not (isinstance(keys, torch.Tensor) and keys.is_cuda):
-        raise TypeError("keys must be a CUDA tensor")
-    with torch.cuda.device(keys.device.index):
-        sp = _stream_ptr(stream)
-    s = _cached_sorter(keys.device.index, 4, 4, n, sp)
-    return s.argsort16(keys, key_type, descending, n, stream)
+    return _module_sorter(keys, "keys", 4, n, stream).argsort16(keys, key_type, descending, n, stream)
 
 
 def sort_rows(x: torch.Tensor, descending: bool = False, return_indices: bool = True, stream=None):
     """``torch.sort(x, dim=-1, stable=True)`` for a contiguous CUDA tensor of int16, uint16, float16, bfloat16, int32, uint32,
     float32, int64, uint64 or float64: (values, int32 indices), or values alone.  The key type follows the dtype.
     OneSweepSorter.sort_rows on the stream's cached (4, 4) sorter, the one argsort uses (the row sort needs no workspace)."""
-    if not (isinstance(x, torch.Tensor) and x.is_cuda):
-        raise TypeError("x must be a CUDA tensor")
-    if x.dtype not in _ROW_KEY_TYPES:
-        raise TypeError(f"x.dtype must be one of {tuple(_ROW_KEY_TYPES)}")
-    with torch.cuda.device(x.device.index):
-        sp = _stream_ptr(stream)
-    s = _cached_sorter(x.device.index, 4, 4, 1, sp)
+    s = _module_sorter(x, "x", 4, 1, stream, _ROW_KEY_TYPES)
     return s.sort_rows(x, _ROW_KEY_TYPES[x.dtype], descending, return_indices, False, stream)
 
 
@@ -555,13 +514,7 @@ def topk(x: torch.Tensor, k: int, largest: bool = True, sorted: bool = True, str
     int32 positions within the row), with ties taken in input order -- exactly the first k columns of the stable row sort.
     The key type follows the dtype.  OneSweepSorter.topk_rows on the stream's cached (4, 4) sorter, the one argsort uses
     (the top-k needs no workspace)."""
-    if not (isinstance(x, torch.Tensor) and x.is_cuda):
-        raise TypeError("x must be a CUDA tensor")
-    if x.dtype not in _ROW_KEY_TYPES:
-        raise TypeError(f"x.dtype must be one of {tuple(_ROW_KEY_TYPES)}")
-    with torch.cuda.device(x.device.index):
-        sp = _stream_ptr(stream)
-    s = _cached_sorter(x.device.index, 4, 4, 1, sp)
+    s = _module_sorter(x, "x", 4, 1, stream, _ROW_KEY_TYPES)
     return s.topk_rows(x, k, _ROW_KEY_TYPES[x.dtype], largest, sorted, stream)
 
 
@@ -571,13 +524,7 @@ def sort_segments(x: torch.Tensor, offsets: torch.Tensor, descending: bool = Fal
     dtypes: (values, int32 positions within the segment), or values alone.  The key type follows the dtype.
     OneSweepSorter.sort_segments on the stream's cached (4, 4) sorter, the one argsort uses, grown to the number of segments
     (the call keeps one uint32 per segment in the sorter's workspace); see there for max_segment_len and what is written."""
-    if not (isinstance(x, torch.Tensor) and x.is_cuda):
-        raise TypeError("x must be a CUDA tensor")
-    if x.dtype not in _ROW_KEY_TYPES:
-        raise TypeError(f"x.dtype must be one of {tuple(_ROW_KEY_TYPES)}")
-    with torch.cuda.device(x.device.index):
-        sp = _stream_ptr(stream)
-    s = _cached_sorter(x.device.index, 4, 4, max(offsets.numel() - 1, 1), sp)
+    s = _module_sorter(x, "x", 4, max(offsets.numel() - 1, 1), stream, _ROW_KEY_TYPES)
     return s.sort_segments(x, offsets, _ROW_KEY_TYPES[x.dtype], descending, return_indices, False, max_segment_len, stream)
 
 
@@ -587,13 +534,7 @@ def topk_segments(x: torch.Tensor, offsets: torch.Tensor, k: int, largest: bool 
     padded past each segment's length with index -1 and the key that sorts last.  The key type follows the dtype.
     OneSweepSorter.topk_segments on the stream's cached (4, 4) sorter, the one argsort uses, grown to the number of segments
     (the call keeps one uint32 per segment in the sorter's workspace)."""
-    if not (isinstance(x, torch.Tensor) and x.is_cuda):
-        raise TypeError("x must be a CUDA tensor")
-    if x.dtype not in _ROW_KEY_TYPES:
-        raise TypeError(f"x.dtype must be one of {tuple(_ROW_KEY_TYPES)}")
-    with torch.cuda.device(x.device.index):
-        sp = _stream_ptr(stream)
-    s = _cached_sorter(x.device.index, 4, 4, max(offsets.numel() - 1, 1), sp)
+    s = _module_sorter(x, "x", 4, max(offsets.numel() - 1, 1), stream, _ROW_KEY_TYPES)
     return s.topk_segments(x, offsets, k, _ROW_KEY_TYPES[x.dtype], largest, sorted, stream)
 
 
