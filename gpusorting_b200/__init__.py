@@ -18,6 +18,7 @@ from .onesweep import (  # noqa: F401
     argsort16,
     init_random,
     release_cached_sorters,
+    sort_long_rows,
     sort_rows,
     sort_segments,
     topk,

@@ -24,13 +24,14 @@
 
 namespace {
 
-constexpr int kVersion = 1009;  // 1002: device plan, bit ranges, forward-progress fallback, hot passes, segmented sort; 1003: argsort;
+constexpr int kVersion = 1010;  // 1002: device plan, bit ranges, forward-progress fallback, hot passes, segmented sort; 1003: argsort;
                                 // 1004: 16-bit keys (osb200_sort_keys16, osb200_sort_pairs16, osb200_argsort16);
                                 // 1005: row sort (osb200_sort_rows);
                                 // 1006: 64-bit keys with uint32 payloads and their argsort (osb200_create_pairs64);
                                 // 1007: segment sort by offsets (osb200_sort_segments);
                                 // 1008: row top-k (osb200_topk_rows);
-                                // 1009: segment top-k (osb200_topk_segments)
+                                // 1009: segment top-k (osb200_topk_segments);
+                                // 1010: rows of any length (osb200_sort_long_rows)
 constexpr int kMaxPlaces = 8;
 
 inline int cuda_status(cudaError_t e) { return e == cudaSuccess ? OSB200_OK : OSB200_ERR_CUDA - static_cast<int>(e); }
@@ -67,6 +68,7 @@ struct osb200_sorter {
     bool hot_passes = true;      // low-entropy digit places run in the HOT instantiation of the pass (decided on the device)
     bool debug_rows_block = false;  // test hook: osb200_sort_rows sorts rows of <= 256 keys on the block path, not the warp path
     uint32_t debug_topk_capacity = 0;  // test hook: N > 0 holds at most N candidates of osb200_topk_rows in shared memory
+    bool debug_long_rows = false;   // test hook: osb200_sort_long_rows sorts rows of 2 .. row_sort_capacity keys on the long path
     bool fused_histogram = true;    // whole-key u32 keys-only sorts of >= kFusedMinTiles tiles: the fused first pass (§4.12)
 
     void* alt_keys = nullptr;
@@ -75,6 +77,7 @@ struct osb200_sorter {
     unsigned char* control = nullptr;  // ControlLayout
     uint64_t* desc = nullptr;          // [tiles][256] 64-bit descriptors (epoch-stamped, cleared only by captured sorts)
     uint16_t* agg16 = nullptr;         // [places][tiles][256] compact reductions (zeroed once per sort)
+    uint64_t agg16_bytes = 0;
     uint64_t desc_tiles = 0;
     uint32_t epoch = 0;
 
@@ -497,7 +500,8 @@ int create_impl(osb200_handle* out, uint64_t max_n, int key_bytes, int value_byt
     if (ok && value_bytes) ok = cudaMalloc(&s->alt_vals, max_n * sizeof(uint32_t)) == cudaSuccess;
     ok = ok && cudaMalloc(&s->control, ControlLayout::total) == cudaSuccess;
     ok = ok && cudaMalloc(&s->desc, s->desc_tiles * osb::kRadix * sizeof(uint64_t)) == cudaSuccess;
-    ok = ok && cudaMalloc(&s->agg16, (s->desc_tiles + 8) * osb::kRadix * sizeof(uint16_t) * key_bytes) == cudaSuccess;
+    s->agg16_bytes = (s->desc_tiles + 8) * osb::kRadix * sizeof(uint16_t) * key_bytes;
+    ok = ok && cudaMalloc(&s->agg16, s->agg16_bytes) == cudaSuccess;
     if (!ok) { cudaGetLastError(); osb200_destroy(s); return OSB200_ERR_ALLOC; }
     e = cudaMemset(s->desc, 0, s->desc_tiles * osb::kRadix * sizeof(uint64_t));  // epoch 0 == never valid
     if (e == cudaSuccess) e = cudaMemset(s->control, 0, ControlLayout::total);
@@ -715,9 +719,12 @@ int osb200_argsort16(osb200_handle h, const void* d_keys_in, void* d_keys_out, u
 // decode every key they store.
 static constexpr uint32_t kRaggedCodecFlags = osb::kCodecEncodeOnLoad | osb::kCodecDecodeOnStore;
 
-// Row sort: one launch, no workspace -- only the handle's device, rank mode and SM count are used, so any handle will do.
-int osb200_sort_rows(osb200_handle h, const void* d_keys_in, void* d_keys_out, uint32_t* d_indices, uint64_t num_rows,
-                     uint32_t row_len, int key_bytes, int key_type, int descending, void* stream)
+// The row sorts.  Rows of at most row_sort_capacity keys: one launch of osb::launch_row_sort, no workspace -- only the handle's
+// device, rank mode and SM count are used, so any handle will do.  long_rows (osb200_sort_long_rows): longer rows, and with the
+// test hook debug_long_rows every row of two or more keys, take the long path on the handle's alternate buffers, control
+// block and reductions (agg16: the tile counts and chunk sums, which every other call clears or overwrites before reading).
+static int sort_rows_impl(osb200_sorter* h, const void* d_keys_in, void* d_keys_out, uint32_t* d_indices, uint64_t num_rows,
+                          uint32_t row_len, int key_bytes, int key_type, int descending, void* stream, bool long_rows)
 {
     if (check_handle(h) != OSB200_OK) return OSB200_ERR_INVALID_ARG;
     osb::KeyCodec c;
@@ -730,16 +737,40 @@ int osb200_sort_rows(osb200_handle h, const void* d_keys_in, void* d_keys_out, u
                                {d_indices, ib, 4, false, true}};
     st = check_arrays(arrays, num_rows <= UINT64_MAX / row_len && n <= UINT64_MAX / 8, true);
     if (st != OSB200_OK) return st;
-    if (row_len > osb::row_sort_capacity(key_bytes)) return OSB200_ERR_SIZE;
+    const bool fits = row_len <= osb::row_sort_capacity(key_bytes);
+    if (!long_rows && !fits) return OSB200_ERR_SIZE;
     cudaStream_t q = static_cast<cudaStream_t>(stream);
     if (row_len == 1) {  // every row is sorted already
         if (d_keys_in != d_keys_out) OSB_TRY(cudaMemcpyAsync(d_keys_out, d_keys_in, kb, cudaMemcpyDeviceToDevice, q));
         if (d_indices) OSB_TRY(cudaMemsetAsync(d_indices, 0, ib, q));
         return OSB200_OK;
     }
-    OSB_TRY(osb::launch_row_sort(d_keys_in, d_keys_out, d_indices, num_rows, row_len, key_bytes, codec,
-                                 h->cfg.rank_mode, h->debug_rows_block, h->sm_count, q));
+    if (!long_rows || (fits && !h->debug_long_rows)) {
+        OSB_TRY(osb::launch_row_sort(d_keys_in, d_keys_out, d_indices, num_rows, row_len, key_bytes, codec,
+                                     h->cfg.rank_mode, h->debug_rows_block, h->sm_count, q));
+        return OSB200_OK;
+    }
+    // the long path's workspace: alternate keys at least as wide as the row's, payloads for the indices, n <= max_n, and the
+    // tile counts and chunk sums inside the reductions
+    if (h->key_bytes < key_bytes || (d_indices && h->value_bytes != 4)) return OSB200_ERR_INVALID_ARG;
+    if (n > h->max_n || osb::long_rows_scratch_bytes(num_rows, row_len) > h->agg16_bytes) return OSB200_ERR_SIZE;
+    OSB_TRY(cudaMemsetAsync(h->control, 0, ControlLayout::zeroed_bytes, q));
+    OSB_TRY(osb::launch_long_rows(d_keys_in, d_keys_out, d_indices, h->alt_keys, d_indices ? h->alt_vals : nullptr, num_rows, row_len,
+                                  key_bytes, codec, h->cfg.rank_mode, h->short_circuit, h->ghist(), h->gbase(), h->plan(),
+                                  reinterpret_cast<uint32_t*>(h->agg16), h->sm_count, q));
     return OSB200_OK;
+}
+
+int osb200_sort_rows(osb200_handle h, const void* d_keys_in, void* d_keys_out, uint32_t* d_indices, uint64_t num_rows,
+                     uint32_t row_len, int key_bytes, int key_type, int descending, void* stream)
+{
+    return sort_rows_impl(h, d_keys_in, d_keys_out, d_indices, num_rows, row_len, key_bytes, key_type, descending, stream, false);
+}
+
+int osb200_sort_long_rows(osb200_handle h, const void* d_keys_in, void* d_keys_out, uint32_t* d_indices, uint64_t num_rows,
+                          uint32_t row_len, int key_bytes, int key_type, int descending, void* stream)
+{
+    return sort_rows_impl(h, d_keys_in, d_keys_out, d_indices, num_rows, row_len, key_bytes, key_type, descending, stream, true);
 }
 
 // Segment sort by offsets: the row sort's kernels for ragged rows, with the workspace of check_segment_workspace.
@@ -976,6 +1007,7 @@ int osb200_set_option(osb200_handle h, const char* key, int64_t value)
         return OSB200_OK;
     }
     if (!std::strcmp(key, "debug_rows_block")) { h->debug_rows_block = value != 0; return OSB200_OK; }
+    if (!std::strcmp(key, "debug_long_rows")) { h->debug_long_rows = value != 0; return OSB200_OK; }
     if (!std::strcmp(key, "debug_topk_capacity")) {  // test hook of osb200_topk_rows' shared-memory candidates (0 = off)
         if (value < 0 || value > (1ll << 30)) return OSB200_ERR_INVALID_ARG;
         h->debug_topk_capacity = static_cast<uint32_t>(value);

@@ -2872,6 +2872,354 @@ cudaError_t launch_sort_segments(const void* keys_in, void* keys_out, uint32_t* 
 }
 
 // =====================================================================================================
+// Long rows (osb200_sort_long_rows): an LSD radix sort of every row, reduce-then-scan within the row, so no tile ever
+// waits on another one (DESIGN §4.16).
+//
+// Row r is cut into tpr = ceil(row_len / kLongRowTile) tiles that never straddle rows; the last one is ragged.  The plan is
+// the DigitBinningPass's (GlobalHistogram over all n keys, the scan's SortPlan: a place on which every key of the call agrees
+// is skipped, and the parity / first_exec / last_exec of the executed places give every pass its source, destination and
+// codec).  Per executed place p:
+//   count    each tile counts digit p of its keys into cnt[row][digit][tile] (digit-major within the row);
+//   scan     a segmented exclusive scan of each row's 256 * tpr counts, in place: chunk sums, a scan of the chunk sums within
+//            the row, then the chunks with their prefixes (one level when a row's counts fit one chunk).  A long row is
+//            spread over as many CTAs as it has chunks;
+//   scatter  each tile ranks its keys stably in shared memory (the DigitBinningPass's warp ranking, both rank modes), stages
+//            them in digit order and writes key j of digit d to row base + cnt[row][d][tile] + (j - the tile's first slot of
+//            d): a warp's stores are consecutive within a digit run.  Indices move with their keys; the first executed pass
+//            reads keys_in and makes each index from the key's position within the row.
+// Every kernel returns at once when the plan skips its place.  copy home: an odd number of executed passes leaves the rows
+// in the alternate buffers; none leaves keys_in sorted as it is (indices 0 .. row_len - 1 per row).
+// =====================================================================================================
+constexpr int kLongWarps = 16, kLongThreads = kLongWarps * 32, kLongK = static_cast<int>(kLongRowTile) / kLongThreads;
+static_assert(kLongK * kLongThreads == static_cast<int>(kLongRowTile), "a tile is kLongK keys per thread");
+constexpr int kLongScanPer = 8;                                         // counts per thread of a scan chunk
+constexpr uint32_t kLongChunk = kLongThreads * kLongScanPer;            // counts per scan chunk
+static_assert(kRadix % kLongScanPer == 0, "a row's counts are whole threads' worth");
+
+uint64_t long_rows_scratch_bytes(uint64_t num_rows, uint32_t row_len)
+{
+    const uint64_t tpr = (static_cast<uint64_t>(row_len) + kLongRowTile - 1) / kLongRowTile;
+    const uint64_t cpr = (tpr * kRadix + kLongChunk - 1) / kLongChunk;
+    // the tile counts, then (when a row has more than one chunk) the chunk sums, 16-byte aligned
+    return (num_rows * tpr * kRadix + (cpr > 1 ? num_rows * cpr + 3 : 0)) / 4 * 4 * sizeof(uint32_t);
+}
+
+// What an executed pass of the plan reads and writes: keys_in on the first executed place, else the buffer an even
+// number of earlier executed passes left the keys in (keys_out, or alt when odd).
+struct LongPass { bool skip, first, last, from_alt; };
+__device__ __forceinline__ LongPass long_pass(const SortPlan* plan, uint32_t place)
+{
+    const SortPlan pl = *plan;
+    return {((pl.skip_mask >> place) & 1u) != 0, place == pl.first_exec, place == pl.last_exec, plan_src_is_alt(pl, place)};
+}
+
+// The GlobalHistogram reads 16-byte vectors; the keys before the first 16-byte boundary of a naturally aligned input are
+// counted here (at most 7 of them).
+template <typename KeyT>
+__global__ void __launch_bounds__(32)
+long_rows_head_hist_kernel(const KeyT* __restrict__ keys, uint32_t head, unsigned long long* __restrict__ ghist, KeyCodec codec)
+{
+    if (threadIdx.x >= head) return;
+    KeyT k = keys[threadIdx.x];
+    if (codec.flags & kCodecEncodeOnLoad)
+        k = codec_encode<KeyT>(k, static_cast<KeyT>(codec.a), static_cast<KeyT>(codec.b), static_cast<KeyT>(codec.d));
+#pragma unroll
+    for (int p = 0; p < static_cast<int>(sizeof(KeyT)); ++p) atomicAdd(&ghist[p * kRadix + digit_of(k, 8u * p)], 1ull);
+}
+
+template <typename KeyT>
+__global__ void __launch_bounds__(kLongThreads)
+long_rows_count_kernel(const SortPlan* __restrict__ plan, uint32_t place, const KeyT* keys_in, const KeyT* keys_out, const KeyT* alt,
+                       uint64_t num_rows, uint32_t row_len, uint32_t tpr, uint32_t* __restrict__ cnt, KeyCodec codec)
+{
+    const LongPass ps = long_pass(plan, place);
+    if (ps.skip) return;
+    const KeyT* src = ps.first ? keys_in : ps.from_alt ? alt : keys_out;
+    const bool enc = ps.first && (codec.flags & kCodecEncodeOnLoad);
+    const KeyT ca = static_cast<KeyT>(codec.a), cb = static_cast<KeyT>(codec.b), cd = static_cast<KeyT>(codec.d);
+    const uint32_t shift = 8u * place;
+    // bank-private columns, as in the GlobalHistogram: every lane of a warp instruction hits its own bank
+    __shared__ uint32_t s_hist[kRadix * 32];
+    uint32_t* s_col = s_hist + (threadIdx.x & 31);
+    const uint64_t tiles = num_rows * tpr;
+    for (uint64_t g = blockIdx.x; g < tiles; g += gridDim.x) {
+        const uint64_t r = g / tpr;
+        const uint32_t t = static_cast<uint32_t>(g - r * tpr), t0 = t * kLongRowTile;
+        const uint32_t len = row_len - t0 < kLongRowTile ? row_len - t0 : kLongRowTile;
+        const KeyT* tile = src + r * row_len + t0;
+        for (int i = threadIdx.x; i < kRadix * 32; i += kLongThreads) s_hist[i] = 0;
+        __syncthreads();
+        KeyT key[kLongK];
+#pragma unroll
+        for (int i = 0; i < kLongK; ++i) {
+            const uint32_t j = threadIdx.x + i * kLongThreads;
+            key[i] = j < len ? tile[j] : static_cast<KeyT>(0);
+        }
+#pragma unroll
+        for (int i = 0; i < kLongK; ++i) {
+            if (threadIdx.x + i * kLongThreads >= len) break;
+            const KeyT k = enc ? codec_encode<KeyT>(key[i], ca, cb, cd) : key[i];
+            atomicAdd(&s_col[digit_of(k, shift) * 32], 1u);
+        }
+        __syncthreads();
+        if (threadIdx.x < kRadix) {
+            uint32_t sum = 0;
+#pragma unroll 8
+            for (int c = 0; c < 32; ++c) sum += s_hist[threadIdx.x * 32 + ((c + threadIdx.x) & 31)];
+            cnt[(r * kRadix + threadIdx.x) * tpr + t] = sum;
+        }
+        __syncthreads();  // the fold has read s_hist
+    }
+}
+
+// The m <= kLongChunk counts at p, thread i holding counts 8i .. 8i+7: their sum (to every thread), and with SCAN their
+// exclusive prefix plus carry written back in place.  All kLongThreads threads call it.
+template <bool SCAN>
+__device__ __forceinline__ uint32_t long_chunk(uint32_t* p, uint32_t m, uint32_t carry, uint32_t* s_w /*[kLongWarps]*/)
+{
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const uint32_t b = static_cast<uint32_t>(tid) * kLongScanPer;
+    uint32_t v[kLongScanPer], sum = 0;
+#pragma unroll
+    for (int j = 0; j < kLongScanPer; ++j) { v[j] = b + j < m ? p[b + j] : 0u; sum += v[j]; }
+    uint32_t incl = sum;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o);
+        if (lane >= o) incl += t;
+    }
+    if (lane == 31) s_w[warp] = incl;
+    __syncthreads();
+    uint32_t pre = 0, total = 0;
+#pragma unroll
+    for (int w = 0; w < kLongWarps; ++w) { const uint32_t x = s_w[w]; pre += w < warp ? x : 0u; total += x; }
+    __syncthreads();  // s_w is reused by the next chunk
+    if constexpr (SCAN) {
+        uint32_t run = carry + pre + incl - sum;
+#pragma unroll
+        for (int j = 0; j < kLongScanPer; ++j) {
+            if (b + j < m) p[b + j] = run;
+            run += v[j];
+        }
+    }
+    return total;
+}
+
+// Chunk c of row r: counts [c * kLongChunk, min((c + 1) * kLongChunk, row_counts)) of the row's row_counts = 256 * tpr.
+// csum[r * cpr + c] = the chunk's sum.
+__global__ void __launch_bounds__(kLongThreads)
+long_rows_chunk_sum_kernel(const SortPlan* __restrict__ plan, uint32_t place, uint32_t* cnt, uint32_t* __restrict__ csum,
+                           uint64_t num_rows, uint64_t row_counts, uint32_t cpr)
+{
+    if (long_pass(plan, place).skip) return;
+    __shared__ uint32_t s_w[kLongWarps];
+    for (uint64_t g = blockIdx.x; g < num_rows * cpr; g += gridDim.x) {
+        const uint64_t r = g / cpr, c0 = (g - r * cpr) * kLongChunk;
+        const uint32_t m = static_cast<uint32_t>(row_counts - c0 < kLongChunk ? row_counts - c0 : kLongChunk);
+        const uint32_t s = long_chunk<false>(cnt + r * row_counts + c0, m, 0u, s_w);
+        if (threadIdx.x == 0) csum[g] = s;
+    }
+}
+
+// The exclusive scan of each row's cpr chunk sums, in place; one CTA per row at a time.
+__global__ void __launch_bounds__(kLongThreads)
+long_rows_chunk_scan_kernel(const SortPlan* __restrict__ plan, uint32_t place, uint32_t* csum, uint64_t num_rows, uint32_t cpr)
+{
+    if (long_pass(plan, place).skip) return;
+    __shared__ uint32_t s_w[kLongWarps];
+    for (uint64_t r = blockIdx.x; r < num_rows; r += gridDim.x) {
+        uint32_t carry = 0;
+        for (uint32_t c0 = 0; c0 < cpr; c0 += kLongChunk)
+            carry += long_chunk<true>(csum + r * cpr + c0, cpr - c0 < kLongChunk ? cpr - c0 : kLongChunk, carry, s_w);
+    }
+}
+
+// Every chunk's counts become their exclusive prefix within the row: the chunk's own scan plus its chunk prefix (csum null:
+// a row is one chunk).
+__global__ void __launch_bounds__(kLongThreads)
+long_rows_scan_kernel(const SortPlan* __restrict__ plan, uint32_t place, uint32_t* cnt, const uint32_t* __restrict__ csum,
+                      uint64_t num_rows, uint64_t row_counts, uint32_t cpr)
+{
+    if (long_pass(plan, place).skip) return;
+    __shared__ uint32_t s_w[kLongWarps];
+    for (uint64_t g = blockIdx.x; g < num_rows * cpr; g += gridDim.x) {
+        const uint64_t r = g / cpr, c0 = (g - r * cpr) * kLongChunk;
+        const uint32_t m = static_cast<uint32_t>(row_counts - c0 < kLongChunk ? row_counts - c0 : kLongChunk);
+        long_chunk<true>(cnt + r * row_counts + c0, m, csum ? csum[g] : 0u, s_w);
+    }
+}
+
+template <typename KeyT, bool INDICES>
+struct LongRowsSmem {
+    alignas(16) KeyT sorted[kLongRowTile];
+    alignas(16) uint32_t sorted_idx[INDICES ? kLongRowTile : 4];
+    alignas(16) uint32_t hist[kLongWarps * kRadix];
+    uint32_t first[kRadix];  // the tile's first slot of every digit
+    uint32_t base[kRadix];   // the row-relative output position of the tile's first key of every digit
+    uint32_t wtot[kRadix / 32];
+};
+
+// (Two resident CTAs per SM are stated for 16- and 32-bit keys only: with indices they spill at 64 registers.)
+template <typename KeyT, int RANK_MODE, bool INDICES>
+__global__ void __launch_bounds__(kLongThreads, sizeof(KeyT) == 8 || INDICES ? 1 : 2)
+long_rows_scatter_kernel(const SortPlan* __restrict__ plan, uint32_t place, const KeyT* keys_in, KeyT* keys_out, KeyT* alt,
+                         uint32_t* idx_out, uint32_t* alt_idx, uint64_t num_rows, uint32_t row_len, uint32_t tpr,
+                         const uint32_t* __restrict__ base, KeyCodec codec)
+{
+    const LongPass ps = long_pass(plan, place);
+    if (ps.skip) return;
+    const KeyT* src = ps.first ? keys_in : ps.from_alt ? alt : keys_out;
+    KeyT* dst = ps.from_alt ? keys_out : alt;
+    const uint32_t* src_idx = ps.from_alt ? alt_idx : idx_out;
+    uint32_t* dst_idx = ps.from_alt ? idx_out : alt_idx;
+    const bool enc = ps.first && (codec.flags & kCodecEncodeOnLoad), dec = ps.last && (codec.flags & kCodecDecodeOnStore);
+    const KeyT ca = static_cast<KeyT>(codec.a), cb = static_cast<KeyT>(codec.b), cd = static_cast<KeyT>(codec.d);
+    const uint32_t shift = 8u * place;
+
+    using S = LongRowsSmem<KeyT, INDICES>;
+    extern __shared__ __align__(128) unsigned char s_raw[];
+    S& sm = *reinterpret_cast<S*>(s_raw);
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const uint32_t lt = lanemask_lt();
+    uint32_t* wh = sm.hist + warp * kRadix;
+    const uint32_t warp_lo = warp * (32 * kLongK), warp_off = warp_lo + lane;
+    const uint64_t tiles = num_rows * tpr;
+    for (uint64_t g = blockIdx.x; g < tiles; g += gridDim.x) {
+        const uint64_t r = g / tpr, row_lo = r * row_len;
+        const uint32_t t = static_cast<uint32_t>(g - r * tpr), t0 = t * kLongRowTile;
+        const uint32_t len = row_len - t0 < kLongRowTile ? row_len - t0 : kLongRowTile;
+        __syncthreads();  // the previous tile has been stored from shared memory
+        {
+            uint4* h4 = reinterpret_cast<uint4*>(sm.hist);
+            for (int i = tid; i < kLongWarps * kRadix / 4; i += kLongThreads) h4[i] = make_uint4(0, 0, 0, 0);
+        }
+        // tile order: key i of a lane is warp_lo + 32 i + lane; the padding (all ones) ranks after every real key
+        KeyT key[kLongK];
+        uint32_t val[INDICES ? kLongK : 1];
+#pragma unroll
+        for (int i = 0; i < kLongK; ++i) {
+            const uint32_t j = warp_off + i * 32;
+            KeyT k = j < len ? src[row_lo + t0 + j] : static_cast<KeyT>(0);
+            if (enc) k = codec_encode<KeyT>(k, ca, cb, cd);
+            key[i] = j < len ? k : static_cast<KeyT>(~static_cast<KeyT>(0));
+            if constexpr (INDICES) val[i] = ps.first ? t0 + j : j < len ? src_idx[row_lo + t0 + j] : 0u;
+        }
+        // a warp's chunks of 32 keys that lie wholly behind the tile are neither counted nor ranked (as in segment_sort_body)
+        const uint32_t live_chunks = len > warp_lo ? (len - warp_lo + 31) / 32 : 0u;
+        __syncthreads();
+#pragma unroll
+        for (int i = 0; i < kLongK; ++i)
+            if (static_cast<uint32_t>(i) < live_chunks) atomicAdd(&wh[digit_of(key[i], shift)], 1u);
+        __syncthreads();
+        uint32_t tile_count = 0;
+        if (tid < kRadix) {
+#pragma unroll
+            for (int w = 0; w < kLongWarps; ++w) tile_count += sm.hist[w * kRadix + tid];
+        }
+        const uint32_t tile_excl = block_excl_scan_256<kLongThreads>(tile_count, sm.wtot);
+        if (tid < kRadix) {
+            uint32_t run = tile_excl;
+#pragma unroll
+            for (int w = 0; w < kLongWarps; ++w) { const uint32_t c = sm.hist[w * kRadix + tid]; sm.hist[w * kRadix + tid] = run; run += c; }
+            sm.first[tid] = tile_excl;
+            sm.base[tid] = base[(r * kRadix + tid) * tpr + t];
+        }
+        __syncthreads();
+#pragma unroll
+        for (int i = 0; i < kLongK; ++i) {
+            if (static_cast<uint32_t>(i) >= live_chunks) continue;
+            const uint32_t slot = warp_rank_and_count<RANK_MODE>(wh, digit_of(key[i], shift), lt);
+            sm.sorted[slot] = key[i];
+            if constexpr (INDICES) sm.sorted_idx[slot] = val[i];
+        }
+        __syncthreads();
+        for (uint32_t j = tid; j < len; j += kLongThreads) {
+            KeyT k = sm.sorted[j];
+            const uint32_t d = digit_of(k, shift);
+            const uint64_t o = row_lo + (sm.base[d] + (j - sm.first[d]));
+            if (dec) k = codec_decode<KeyT>(k, ca, cb, cd);
+            st_scatter(dst + o, k);
+            if constexpr (INDICES) st_scatter(dst_idx + o, sm.sorted_idx[j]);
+        }
+    }
+}
+
+// Odd executed passes: keys and indices from the alternate buffers.  None: keys_in is its own stable sort -- its keys (not
+// copied in place) and the positions 0 .. row_len - 1 of every row.
+template <typename KeyT>
+__global__ void __launch_bounds__(512)
+long_rows_copy_home_kernel(const SortPlan* __restrict__ plan, const KeyT* keys_in, const KeyT* __restrict__ alt, KeyT* keys_out,
+                           const uint32_t* __restrict__ alt_idx, uint32_t* __restrict__ idx_out, uint64_t n, uint32_t row_len)
+{
+    const uint32_t ex = plan->executed;
+    if (ex != 0 && !(ex & 1u)) return;
+    const KeyT* src = ex ? alt : keys_in;
+    const bool keys = src != keys_out;
+    const uint64_t stride = static_cast<uint64_t>(gridDim.x) * blockDim.x;
+    for (uint64_t i = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += stride) {
+        if (keys) __stcs(keys_out + i, __ldcs(src + i));
+        if (idx_out) __stcs(idx_out + i, ex ? __ldcs(alt_idx + i) : static_cast<uint32_t>(i % row_len));
+    }
+}
+
+using LongRowKeys = TypeList<uint16_t, uint32_t, uint64_t>;
+
+cudaError_t launch_long_rows(const void* keys_in, void* keys_out, uint32_t* indices, void* alt_keys, uint32_t* alt_idx,
+                             uint64_t num_rows, uint32_t row_len, int key_bytes, const KeyCodec* codec_in, int rank_mode,
+                             bool allow_skip, unsigned long long* ghist, unsigned long long* gbase, SortPlan* plan,
+                             uint32_t* scratch, int sm_count, cudaStream_t stream)
+{
+    if (num_rows == 0 || row_len < 2) return cudaErrorInvalidValue;
+    const uint64_t n = num_rows * row_len;
+    const uint32_t tpr = (row_len + kLongRowTile - 1) / kLongRowTile;
+    const uint64_t row_counts = static_cast<uint64_t>(tpr) * kRadix;
+    const uint32_t cpr = static_cast<uint32_t>((row_counts + kLongChunk - 1) / kLongChunk);
+    uint32_t* cnt = scratch;
+    uint32_t* csum = cpr > 1 ? scratch + (num_rows * row_counts + 3) / 4 * 4 : nullptr;
+    const KeyCodec codec = codec_in ? *codec_in : KeyCodec();
+    KeyCodec enc = codec;
+    enc.flags &= kCodecEncodeOnLoad;
+    return with_key_type(LongRowKeys{}, key_bytes, [&](auto kt) {
+        using KeyT = decltype(kt);
+        const KeyT* in = static_cast<const KeyT*>(keys_in);
+        KeyT* out = static_cast<KeyT*>(keys_out);
+        KeyT* alt = static_cast<KeyT*>(alt_keys);
+        // the plan: keys before the first 16-byte boundary here, the rest in the GlobalHistogram, then the scan
+        const uint32_t head = static_cast<uint32_t>(((16u - (reinterpret_cast<uintptr_t>(in) & 15u)) & 15u) / sizeof(KeyT));
+        if (head) long_rows_head_hist_kernel<KeyT><<<1, 32, 0, stream>>>(in, head, ghist, enc);
+        cudaError_t e = launch_global_histogram(in + head, n - head, key_bytes, ghist, sm_count, stream, codec_in ? &enc : nullptr);
+        if (e == cudaSuccess) e = launch_scan(ghist, gbase, key_bytes, stream, plan, n, allow_skip, false);
+        const unsigned scan_grid = capped_grid(num_rows * cpr, 1, static_cast<uint64_t>(sm_count) * 4);
+        for (uint32_t p = 0; e == cudaSuccess && p < sizeof(KeyT); ++p) {
+            e = launch_resident<long_rows_count_kernel<KeyT>, kLongThreads, 0>(num_rows * tpr, sm_count, stream, plan, p, in, out, alt,
+                                                                               num_rows, row_len, tpr, cnt, codec);
+            if (e == cudaSuccess && csum) {
+                long_rows_chunk_sum_kernel<<<scan_grid, kLongThreads, 0, stream>>>(plan, p, cnt, csum, num_rows, row_counts, cpr);
+                long_rows_chunk_scan_kernel<<<capped_grid(num_rows, 1, static_cast<uint64_t>(sm_count) * 4), kLongThreads, 0, stream>>>(
+                    plan, p, csum, num_rows, cpr);
+            }
+            if (e == cudaSuccess) {
+                long_rows_scan_kernel<<<scan_grid, kLongThreads, 0, stream>>>(plan, p, cnt, csum, num_rows, row_counts, cpr);
+                e = cudaGetLastError();
+            }
+            if (e == cudaSuccess) e = with_rank_mode(rank_mode, [&](auto rm) {
+                auto go = [&](auto ind) {
+                    constexpr bool I = decltype(ind)::value;
+                    return launch_resident<long_rows_scatter_kernel<KeyT, decltype(rm)::value, I>, kLongThreads, sizeof(LongRowsSmem<KeyT, I>)>(
+                        num_rows * tpr, sm_count, stream, plan, p, in, out, alt, indices, alt_idx, num_rows, row_len, tpr,
+                        static_cast<const uint32_t*>(cnt), codec);
+                };
+                return indices ? go(std::true_type{}) : go(std::false_type{});
+            });
+        }
+        if (e != cudaSuccess) return e;
+        long_rows_copy_home_kernel<KeyT><<<capped_grid(n, 512, static_cast<uint64_t>(sm_count) * 4), 512, 0, stream>>>(
+            plan, in, alt, out, alt_idx, indices, n, row_len);
+        return cudaGetLastError();
+    });
+}
+
+// =====================================================================================================
 // Row top-k (osb200_topk_rows): the first k keys of every row in the stable row sort, with their positions.
 //
 // Rows of at most kRowWarpMaxLen keys: one warp sorts the row (warp_sort_run, TOPK) and stores its first k keys.
@@ -3316,6 +3664,13 @@ cudaError_t configure_kernels()
     });
     if (e == cudaSuccess) e = set_smem(fused_kernel<kRankAtomic>(), FusedShape::smem);
     if (e == cudaSuccess) e = set_smem(fused_kernel<kRankBallot>(), FusedShape::smem);
+    if (e == cudaSuccess) e = for_each_type(LongRowKeys{}, [](auto k) {
+        using KeyT = decltype(k);
+        cudaError_t m = set_smem(long_rows_scatter_kernel<KeyT, kRankAtomic, false>, sizeof(LongRowsSmem<KeyT, false>));
+        if (m == cudaSuccess) m = set_smem(long_rows_scatter_kernel<KeyT, kRankBallot, false>, sizeof(LongRowsSmem<KeyT, false>));
+        if (m == cudaSuccess) m = set_smem(long_rows_scatter_kernel<KeyT, kRankAtomic, true>, sizeof(LongRowsSmem<KeyT, true>));
+        return m != cudaSuccess ? m : set_smem(long_rows_scatter_kernel<KeyT, kRankBallot, true>, sizeof(LongRowsSmem<KeyT, true>));
+    });
     return e;
 }
 

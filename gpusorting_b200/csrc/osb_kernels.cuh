@@ -131,6 +131,19 @@ cudaError_t launch_row_sort(const void* keys_in, void* keys_out, uint32_t* indic
                             int key_bytes, const KeyCodec* codec, int rank_mode, bool block_only, int sm_count,
                             cudaStream_t stream);
 
+// Long rows (osb200_sort_long_rows): rows of any length >= 2, LSD radix sort over tiles of kLongRowTile keys that never straddle
+// rows, reduce-then-scan within each row (no tile waits on another).  Enqueues the GlobalHistogram over all n = num_rows *
+// row_len keys into ghist (zeroed by the caller), the scan that writes `plan` (gbase is written too, and not used), per digit
+// place a count, a scan of each row's tile counts and a scatter, then the copy home.  alt_keys: n keys of key_bytes;
+// alt_idx: n u32 when indices is not null; scratch: long_rows_scratch_bytes(num_rows, row_len) bytes, 16-byte aligned, which
+// the call overwrites before it reads them.  The codec as for launch_row_sort.
+constexpr uint32_t kLongRowTile = 8192;
+uint64_t long_rows_scratch_bytes(uint64_t num_rows, uint32_t row_len);
+cudaError_t launch_long_rows(const void* keys_in, void* keys_out, uint32_t* indices, void* alt_keys, uint32_t* alt_idx,
+                             uint64_t num_rows, uint32_t row_len, int key_bytes, const KeyCodec* codec, int rank_mode,
+                             bool allow_skip, unsigned long long* ghist, unsigned long long* gbase, SortPlan* plan,
+                             uint32_t* scratch, int sm_count, cudaStream_t stream);
+
 // Segment sort by offsets (osb200_sort_segments): segment s = [off[s], off[s + 1]) of keys_in, sorted stable into the same
 // positions of keys_out (== keys_in: in place); indices (may be null) receives every output key's position within its segment.
 // A binning kernel puts every segment of 2 to max_len keys that lies inside [0, n) into a class by its length -- one warp

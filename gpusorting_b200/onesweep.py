@@ -247,6 +247,20 @@ class OneSweepSorter:
                    row_len, kb, kt, 1 if descending else 0, stream=stream)
         return (out, idx) if return_indices else out
 
+    def sort_long_rows(self, x: torch.Tensor, key_type: str, descending: bool = False, return_indices: bool = True,
+                       inplace: bool = False, stream=None):
+        """sort_rows for rows of any length (osb200_sort_long_rows): the same arguments, shapes and results.  Rows of at most
+        16,384 keys (8,192 for 8-byte dtypes) are sorted by sort_rows' own kernels on any sorter.  Longer rows use this
+        sorter's workspace: x.numel() may be at most max_n, the sorter's key_bytes must be at least x's element size, and
+        return_indices=True needs value_bytes == 4 -- a (4, 4) sorter for 2- and 4-byte dtypes, a (8, 4) one for any."""
+        kb, kt = self._ragged_keys(x, key_type)
+        row_len = x.shape[-1]
+        num_rows = x.numel() // row_len if row_len else 0
+        out, idx = _new_outputs(stream, x, x.shape, return_indices, x if inplace else None)
+        self._call(lib.osb200_sort_long_rows, x.data_ptr(), out.data_ptr(), idx.data_ptr() if idx is not None else None,
+                   num_rows, row_len, kb, kt, 1 if descending else 0, stream=stream)
+        return (out, idx) if return_indices else out
+
     # -- row top-k: the first k keys of every row's stable sort, no workspace (any sorter will do) ------------------------
     def topk_rows(self, x: torch.Tensor, k: int, key_type: str, largest: bool = True, sorted: bool = True, stream=None):
         """The k largest (or smallest) keys of every row of `x` along its last dimension and their positions
@@ -507,6 +521,24 @@ def sort_rows(x: torch.Tensor, descending: bool = False, return_indices: bool = 
     OneSweepSorter.sort_rows on the stream's cached (4, 4) sorter, the one argsort uses (the row sort needs no workspace)."""
     s = _module_sorter(x, "x", 4, 1, stream, _ROW_KEY_TYPES)
     return s.sort_rows(x, _ROW_KEY_TYPES[x.dtype], descending, return_indices, False, stream)
+
+
+# the longest row sort_rows takes, by element size: sort_long_rows needs a sorter's workspace only above it
+_ROW_CAPACITY = {2: 16384, 4: 16384, 8: 8192}
+
+
+def sort_long_rows(x: torch.Tensor, descending: bool = False, return_indices: bool = True, stream=None):
+    """sort_rows for rows of any length: ``torch.sort(x, dim=-1, stable=True)`` for a contiguous CUDA tensor of one of
+    sort_rows' ten dtypes, returning (values, int32 positions within the row) or values alone.  Rows above sort_rows' limit
+    run on the stream's cached (4, 4) sorter, the one argsort uses, or its (8, 4) sorter for 8-byte dtypes, grown to
+    x.numel(); shorter rows on the (4, 4) one as in sort_rows."""
+    kb = x.element_size() if isinstance(x, torch.Tensor) else 4
+    row_len = x.shape[-1] if isinstance(x, torch.Tensor) and x.dim() else 0
+    if row_len > _ROW_CAPACITY.get(kb, 16384):
+        s = _module_sorter(x, "x", 8 if kb == 8 else 4, x.numel(), stream, _ROW_KEY_TYPES)
+    else:
+        s = _module_sorter(x, "x", 4, 1, stream, _ROW_KEY_TYPES)
+    return s.sort_long_rows(x, _ROW_KEY_TYPES[x.dtype], descending, return_indices, False, stream)
 
 
 def topk(x: torch.Tensor, k: int, largest: bool = True, sorted: bool = True, stream=None):

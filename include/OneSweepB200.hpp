@@ -82,6 +82,15 @@ class OneSweepSorterB200 {
                                stream),
               "osb200_sort_rows");
     }
+    // SortRows for rows of any length: rows above SortRows' limit use this handle's workspace (num_rows * row_len <= max_n, a
+    // key width of at least key_bytes, and value_bytes 4 with indices)
+    void SortLongRows(const void* d_keys_in, void* d_keys_out, uint32_t* d_indices, uint64_t num_rows, uint32_t row_len, int key_bytes,
+                      int key_type, bool descending, void* stream = nullptr)
+    {
+        check(osb200_sort_long_rows(h_, d_keys_in, d_keys_out, d_indices, num_rows, row_len, key_bytes, key_type, descending ? 1 : 0,
+                                    stream),
+              "osb200_sort_long_rows");
+    }
     // the first k keys of every row [r*row_len, (r+1)*row_len) in its stable sort (ascending, or descending for largest) and
     // their positions within the row, into [r*k, (r+1)*k) of d_values_out and d_indices; sorted = false leaves each row's k
     // pairs in an unspecified order; any row_len, k <= 16,384 (8,192 for 8-byte keys); any sorter

@@ -179,6 +179,31 @@ OSB200_API int osb200_argsort16(osb200_handle h, const void* d_keys_in, void* d_
 OSB200_API int osb200_sort_rows(osb200_handle h, const void* d_keys_in, void* d_keys_out, uint32_t* d_indices, uint64_t num_rows,
                                 uint32_t row_len, int key_bytes, int key_type, int descending, void* stream);
 
+/* Long-row sort: osb200_sort_rows for every row_len from 1 to 2^32 - 1, with the same semantics -- key_bytes / key_type and
+ * codec, stable in both directions, d_indices NULL or uint32 positions within the row, d_keys_out == d_keys_in in place (any
+ * other overlap OSB200_ERR_INVALID_ARG), natural alignment only, num_rows == 0 or row_len == 0 a no-op and row_len == 1 a copy
+ * with zero indices.  The argument errors of osb200_sort_rows come first.
+ * Rows of at most 16,384 keys (8,192 for 8-byte keys) are sorted by osb200_sort_rows' own launch, on any handle and with no
+ * workspace.  Longer rows take the long path, which uses the handle's workspace and allocates nothing.  It needs:
+ *   - num_rows * row_len <= max_n, else OSB200_ERR_SIZE;
+ *   - a handle key width of at least key_bytes -- a (4, 0) or (4, 4) handle for 2- and 4-byte keys, a (8, 0) or (8, 4) handle
+ *     for any width -- else OSB200_ERR_INVALID_ARG;
+ *   - value_bytes == 4 when d_indices is given (a (4, 4) handle, or osb200_create_pairs64's (8, 4)), else
+ *     OSB200_ERR_INVALID_ARG;
+ *   - room in the handle's reductions for 1 KiB per tile of 8,192 keys (a ragged last tile per row included) and the chunk
+ *     sums: a handle of max_n >= num_rows * row_len always has it for rows above the limit; else OSB200_ERR_SIZE.
+ * The long path writes the handle's alternate key buffer (key_bytes * n bytes), its alternate payloads (4n, with indices),
+ * its control block (histogram and plan: info "last_executed_passes" / "last_skip_mask" read this call's plan) and its
+ * compact reductions.  It never writes the chained-scan descriptors.
+ * It is an LSD radix sort per row over tiles that never straddle rows: a GlobalHistogram over all keys decides, as for
+ * osb200_sort_keys_typed, which digit places every key shares (skipped; option "short_circuit"); per executed place a count
+ * of each tile's digits, a scan of each row's tile counts and a stable scatter, and a copy home when an odd number of places
+ * ran.  No tile waits on another.  One memset and a fixed sequence of launches: asynchronous, no host synchronisation,
+ * graph-capturable; one call in flight per handle.  Option "debug_long_rows" = 1 (a test hook) sends rows of 2 .. 16,384
+ * (8,192) keys to the long path too, with its workspace rules. */
+OSB200_API int osb200_sort_long_rows(osb200_handle h, const void* d_keys_in, void* d_keys_out, uint32_t* d_indices,
+                                     uint64_t num_rows, uint32_t row_len, int key_bytes, int key_type, int descending, void* stream);
+
 /* Segment sort: osb200_sort_rows for ragged rows given by offsets.  Segment s is [off[s], off[s+1]) of arrays of n elements
  * (off = d_segment_offsets, num_segments + 1 of them, 8-byte aligned); it is sorted stable into the same positions of
  * d_keys_out, ascending or descending (the complement of the encoded key: equal keys keep their order).  d_indices may be
@@ -328,6 +353,9 @@ OSB200_API int osb200_init_random_u32(uint32_t* d_keys, uint32_t* d_payload, uin
  *   "debug_rows_block"  test hook of osb200_sort_rows: 1 = rows of at most 256 keys go through the block path (2,048-key
  *                    geometry) instead of one warp per row, to compare the two paths; 0 (default) = the warp path.
  *                    osb200_topk_rows honours it too: its rows of at most 256 keys are then radix-selected one per block
+ *   "debug_long_rows"  test hook of osb200_sort_long_rows: 1 = rows of 2 .. 16,384 keys (8,192 for 8-byte keys) take the long
+ *                    path too, with its workspace rules (short rows have a tile each, so many of them may need more room
+ *                    than max_n gives: OSB200_ERR_SIZE), to compare it with osb200_sort_rows; 0 (default) = osb200_sort_rows' launch
  *   "debug_topk_capacity"  test hook of osb200_topk_rows: N > 0 keeps at most N candidates of a row in shared memory (instead
  *                    of 16,384, or 8,192 for 8-byte keys), so that short rows exercise the passes that read global memory
  *                    and the switch to shared memory; 0 (default) = the full capacity
