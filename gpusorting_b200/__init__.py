@@ -19,6 +19,7 @@ from .onesweep import (  # noqa: F401
     init_random,
     release_cached_sorters,
     sort_long_rows,
+    sort_long_segments,
     sort_rows,
     sort_segments,
     topk,

@@ -38,6 +38,7 @@ SIGNATURES = {
     "osb200_sort_rows": (c_int, [c_vp, c_vp, c_vp, c_vp, c_u64, ctypes.c_uint32, c_int, c_int, c_int, c_vp]),
     "osb200_sort_long_rows": (c_int, [c_vp, c_vp, c_vp, c_vp, c_u64, ctypes.c_uint32, c_int, c_int, c_int, c_vp]),
     "osb200_sort_segments": (c_int, [c_vp, c_vp, c_vp, c_vp, c_u64, c_vp, c_u64, ctypes.c_uint32, c_int, c_int, c_int, c_vp]),
+    "osb200_sort_long_segments": (c_int, [c_vp, c_vp, c_vp, c_vp, c_u64, c_vp, c_u64, ctypes.c_uint32, c_int, c_int, c_int, c_vp]),
     "osb200_topk_rows": (c_int, [c_vp, c_vp, c_vp, c_vp, c_u64, ctypes.c_uint32, ctypes.c_uint32, c_int, c_int, c_int, c_int,
                                  c_vp]),
     "osb200_topk_segments": (c_int, [c_vp, c_vp, c_vp, c_vp, c_u64, c_vp, c_u64, ctypes.c_uint32, c_int, c_int, c_int, c_int,

@@ -24,14 +24,15 @@
 
 namespace {
 
-constexpr int kVersion = 1010;  // 1002: device plan, bit ranges, forward-progress fallback, hot passes, segmented sort; 1003: argsort;
+constexpr int kVersion = 1011;  // 1002: device plan, bit ranges, forward-progress fallback, hot passes, segmented sort; 1003: argsort;
                                 // 1004: 16-bit keys (osb200_sort_keys16, osb200_sort_pairs16, osb200_argsort16);
                                 // 1005: row sort (osb200_sort_rows);
                                 // 1006: 64-bit keys with uint32 payloads and their argsort (osb200_create_pairs64);
                                 // 1007: segment sort by offsets (osb200_sort_segments);
                                 // 1008: row top-k (osb200_topk_rows);
                                 // 1009: segment top-k (osb200_topk_segments);
-                                // 1010: rows of any length (osb200_sort_long_rows)
+                                // 1010: rows of any length (osb200_sort_long_rows);
+                                // 1011: segments of any length (osb200_sort_long_segments)
 constexpr int kMaxPlaces = 8;
 
 inline int cuda_status(cudaError_t e) { return e == cudaSuccess ? OSB200_OK : OSB200_ERR_CUDA - static_cast<int>(e); }
@@ -48,7 +49,7 @@ struct ControlLayout {
     static constexpr size_t ticket_bytes = 64;  // 8 u32 tickets, padded
     static constexpr size_t zeroed_bytes = ghist_bytes + ticket_bytes;
     static constexpr size_t gbase_bytes = kMaxPlaces * osb::kRadix * sizeof(unsigned long long);
-    static constexpr size_t err_bytes = 64;   // scratch of the calls that clear it first: validate, osb200_sort_segments' class counts
+    static constexpr size_t err_bytes = 64;   // scratch of the calls that clear it first: validate, the segment calls' counts
     static constexpr size_t plan_bytes = 64;  // osb::SortPlan, written by the scan kernel of every sort
     static constexpr size_t total = zeroed_bytes + gbase_bytes + err_bytes + plan_bytes;
 };
@@ -68,7 +69,8 @@ struct osb200_sorter {
     bool hot_passes = true;      // low-entropy digit places run in the HOT instantiation of the pass (decided on the device)
     bool debug_rows_block = false;  // test hook: osb200_sort_rows sorts rows of <= 256 keys on the block path, not the warp path
     uint32_t debug_topk_capacity = 0;  // test hook: N > 0 holds at most N candidates of osb200_topk_rows in shared memory
-    bool debug_long_rows = false;   // test hook: osb200_sort_long_rows sorts rows of 2 .. row_sort_capacity keys on the long path
+    bool debug_long_rows = false;   // test hook: osb200_sort_long_rows and osb200_sort_long_segments sort rows and segments of
+                                    // 2 .. row_sort_capacity keys on the long path
     bool fused_histogram = true;    // whole-key u32 keys-only sorts of >= kFusedMinTiles tiles: the fused first pass (§4.12)
 
     void* alt_keys = nullptr;
@@ -773,10 +775,15 @@ int osb200_sort_long_rows(osb200_handle h, const void* d_keys_in, void* d_keys_o
     return sort_rows_impl(h, d_keys_in, d_keys_out, d_indices, num_rows, row_len, key_bytes, key_type, descending, stream, true);
 }
 
-// Segment sort by offsets: the row sort's kernels for ragged rows, with the workspace of check_segment_workspace.
-int osb200_sort_segments(osb200_handle h, const void* d_keys_in, void* d_keys_out, uint32_t* d_indices, uint64_t n,
-                         const uint64_t* d_segment_offsets, uint64_t num_segments, uint32_t max_segment_len, int key_bytes,
-                         int key_type, int descending, void* stream)
+// The segment sorts.  Segments of at most row_sort_capacity keys: the row sort's kernels for ragged rows, with the workspace
+// of check_segment_workspace.  long_segments (osb200_sort_long_segments) with a larger max_segment_len, or with the test hook
+// debug_long_rows: segments longer than row_sort_capacity (with the hook, every segment of two or more keys) take the long
+// path, with the long rows' handle rules: the alternate buffers, the control block's scratch words and the reductions
+// (agg16: the tile counts, chunk sums and tile map, which every other call clears or overwrites before reading).  The room
+// the long path needs is bounded by n and the shortest long segment only (long_segments_layout), never by the offsets.
+static int sort_segments_impl(osb200_sorter* h, const void* d_keys_in, void* d_keys_out, uint32_t* d_indices, uint64_t n,
+                              const uint64_t* d_segment_offsets, uint64_t num_segments, uint32_t max_segment_len, int key_bytes,
+                              int key_type, int descending, void* stream, bool long_segments)
 {
     if (check_handle(h) != OSB200_OK) return OSB200_ERR_INVALID_ARG;
     osb::KeyCodec c;
@@ -790,12 +797,44 @@ int osb200_sort_segments(osb200_handle h, const void* d_keys_in, void* d_keys_ou
                                {d_indices, ib, 4, false, true}, {d_segment_offsets, ob, 8, true, false}};
     st = check_arrays(arrays, n <= UINT64_MAX / 8 && num_segments <= UINT64_MAX / 8 - 1, true);
     if (st != OSB200_OK) return st;
-    if (max_segment_len > osb::row_sort_capacity(key_bytes)) return OSB200_ERR_SIZE;
+    const uint32_t cap = osb::row_sort_capacity(key_bytes);
+    if (!long_segments && max_segment_len > cap) return OSB200_ERR_SIZE;
     if ((st = check_segment_workspace(h, num_segments)) != OSB200_OK) return st;
-    OSB_TRY(osb::launch_sort_segments(d_keys_in, d_keys_out, d_indices, n, reinterpret_cast<const unsigned long long*>(d_segment_offsets),
-                                      num_segments, max_segment_len, key_bytes, codec, h->cfg.rank_mode, h->sm_count,
-                                      static_cast<uint32_t*>(h->alt_keys), h->err(), static_cast<cudaStream_t>(stream)));
+    const auto* off = reinterpret_cast<const unsigned long long*>(d_segment_offsets);
+    cudaStream_t q = static_cast<cudaStream_t>(stream);
+    const uint32_t long_min = h->debug_long_rows ? 2u : cap + 1;
+    if (!long_segments || max_segment_len < long_min) {
+        OSB_TRY(osb::launch_sort_segments(d_keys_in, d_keys_out, d_indices, n, off, num_segments, max_segment_len, key_bytes, codec,
+                                          h->cfg.rank_mode, h->sm_count, static_cast<uint32_t*>(h->alt_keys), h->err(), q));
+        return OSB200_OK;
+    }
+    static_assert(ControlLayout::err_bytes >= 7 * sizeof(unsigned long long), "the long path's counts live in the scratch words");
+    if (h->key_bytes < key_bytes || (d_indices && h->value_bytes != 4)) return OSB200_ERR_INVALID_ARG;
+    const osb::LongSegLayout l = osb::long_segments_layout(n, long_min);
+    if (n > h->max_n || l.words * sizeof(uint32_t) > h->agg16_bytes || l.tile_cap > UINT32_MAX || l.chunk_cap > UINT32_MAX)
+        return OSB200_ERR_SIZE;
+    OSB_TRY(cudaMemsetAsync(h->control, 0, ControlLayout::zeroed_bytes, q));
+    OSB_TRY(osb::launch_long_segments(d_keys_in, d_keys_out, d_indices, h->alt_keys, d_indices ? h->alt_vals : nullptr, n, off,
+                                      num_segments, max_segment_len, long_min, key_bytes, codec, h->cfg.rank_mode, h->short_circuit,
+                                      h->ghist(), h->gbase(), h->plan(), static_cast<uint32_t*>(h->alt_keys), h->err(),
+                                      reinterpret_cast<uint32_t*>(h->agg16), h->sm_count, q));
     return OSB200_OK;
+}
+
+int osb200_sort_segments(osb200_handle h, const void* d_keys_in, void* d_keys_out, uint32_t* d_indices, uint64_t n,
+                         const uint64_t* d_segment_offsets, uint64_t num_segments, uint32_t max_segment_len, int key_bytes,
+                         int key_type, int descending, void* stream)
+{
+    return sort_segments_impl(h, d_keys_in, d_keys_out, d_indices, n, d_segment_offsets, num_segments, max_segment_len, key_bytes,
+                              key_type, descending, stream, false);
+}
+
+int osb200_sort_long_segments(osb200_handle h, const void* d_keys_in, void* d_keys_out, uint32_t* d_indices, uint64_t n,
+                              const uint64_t* d_segment_offsets, uint64_t num_segments, uint32_t max_segment_len, int key_bytes,
+                              int key_type, int descending, void* stream)
+{
+    return sort_segments_impl(h, d_keys_in, d_keys_out, d_indices, n, d_segment_offsets, num_segments, max_segment_len, key_bytes,
+                              key_type, descending, stream, true);
 }
 
 // Row top-k: at most two launches, no workspace -- like the row sort, any handle will do.

@@ -2269,6 +2269,8 @@ struct SegSmem {
 
 // osb200_sort_segments' class counts (see segment_bin_kernel)
 enum SegCount : int { kSegCountWarp = 0, kSegCountBlock1 = 1, kSegCountBlock2 = 2, kSegCountBlockList = 3, kSegCounts = 4 };
+// osb200_sort_long_segments' counts after them: the long list's length, then its tiles and scan chunks (see launch_long_segments)
+enum LongSegCount : int { kSegCountLong = 4, kSegCountLongTiles = 5, kSegCountLongChunks = 6, kLongSegCounts = 7 };
 
 // INDICES (argsort): the keys come from keys_in, every payload is the key's position in its segment.
 // ROWS (row sort, osb200_sort_rows): segment s is row s, [s * single_n, (s + 1) * single_n) (seg_off is not read), and the
@@ -2738,12 +2740,16 @@ cudaError_t launch_row_sort(const void* keys_in, void* keys_out, uint32_t* indic
 // fill.  Segments of warp_max + 1 to 2^32 - 1 keys inside [0, n) go to the block list (counted as the 2,048-key class);
 // all others -- up to warp_max keys, empty, and invalid ones, which the warp class treats as empty -- to the warp list.
 // Nothing is written here but the lists and counts (keys_in, keys_out, idx_out and max_len are not used).
+// LONG (osb200_sort_long_segments, long_segment_bin_kernel): segments of long_min to max_len keys go to the long list
+// instead (ids in arrival order, at most long_cap of them; counts[kSegCountLong] counts them all), the shorter ones to the
+// classes as above.
 // =====================================================================================================
-template <typename KeyT, bool TOPK>
+template <typename KeyT, bool TOPK, bool LONG = false>
 __device__ __forceinline__ void segment_bin_body(const unsigned long long* __restrict__ off, uint64_t num_segments, uint64_t n,
                                                  uint32_t max_len, uint32_t* __restrict__ list,
                                                  unsigned long long* __restrict__ counts, const KeyT* keys_in, KeyT* keys_out,
-                                                 uint32_t* idx_out, uint32_t warp_max)
+                                                 uint32_t* idx_out, uint32_t warp_max, uint32_t long_min = 0,
+                                                 uint32_t* __restrict__ long_list = nullptr, uint64_t long_cap = 0)
 {
     const uint32_t lane = threadIdx.x & 31, lt = lanemask_lt();
     const uint64_t stride = static_cast<uint64_t>(gridDim.x) * blockDim.x;
@@ -2761,12 +2767,21 @@ __device__ __forceinline__ void segment_bin_body(const unsigned long long* __res
                 if (len == 1) {
                     if (keys_out != keys_in) keys_out[lo] = keys_in[lo];
                     if (idx_out) idx_out[lo] = 0u;
+                } else if (LONG && len >= long_min) {
+                    cls = 3;
                 } else if (len > 1) {
                     cls = len <= kRowWarpMaxLen ? 0 : len <= kSegBlock1Max ? 1 : 2;
                 }
             }
         }
-        const uint32_t w = __ballot_sync(0xffffffffu, cls == 0), b = __ballot_sync(0xffffffffu, cls > 0);
+        if constexpr (LONG) {
+            const uint32_t l = __ballot_sync(0xffffffffu, cls == 3);
+            unsigned long long lpos = 0;
+            if (lane == 0 && l) lpos = atomicAdd(&counts[kSegCountLong], static_cast<unsigned long long>(__popc(l)));
+            lpos = __shfl_sync(0xffffffffu, lpos, 0) + __popc(l & lt);
+            if (cls == 3 && lpos < long_cap) long_list[lpos] = static_cast<uint32_t>(s);
+        }
+        const uint32_t w = __ballot_sync(0xffffffffu, cls == 0), b = __ballot_sync(0xffffffffu, cls > 0 && (!LONG || cls < 3));
         const uint32_t b1 = __ballot_sync(0xffffffffu, cls == 1), b2 = b & ~b1;
         unsigned long long wpos = 0, bpos = 0;
         if (lane == 0) {
@@ -2778,7 +2793,7 @@ __device__ __forceinline__ void segment_bin_body(const unsigned long long* __res
         wpos = __shfl_sync(0xffffffffu, wpos, 0);
         bpos = __shfl_sync(0xffffffffu, bpos, 0);
         if (cls == 0) list[wpos + __popc(w & lt)] = static_cast<uint32_t>(s);
-        if (cls > 0) list[num_segments - 1 - (bpos + __popc(b & lt))] = static_cast<uint32_t>(s);
+        if (cls > 0 && (!LONG || cls < 3)) list[num_segments - 1 - (bpos + __popc(b & lt))] = static_cast<uint32_t>(s);
     }
 }
 
@@ -2818,6 +2833,11 @@ segment_sort_warp_kernel(const KeyT* in, KeyT* out, uint32_t* __restrict__ idx_o
     }
 }
 
+static cudaError_t launch_segment_classes(const void* keys_in, void* keys_out, uint32_t* indices, const unsigned long long* off,
+                                          uint64_t num_segments, uint32_t max_len, int key_bytes, const KeyCodec& codec,
+                                          int rank_mode, int sm_count, uint32_t* list, unsigned long long* counts,
+                                          cudaStream_t stream);
+
 cudaError_t launch_sort_segments(const void* keys_in, void* keys_out, uint32_t* indices, uint64_t n,
                                  const unsigned long long* off, uint64_t num_segments, uint32_t max_len, int key_bytes,
                                  const KeyCodec* codec_in, int rank_mode, int sm_count, uint32_t* list,
@@ -2835,7 +2855,18 @@ cudaError_t launch_sort_segments(const void* keys_in, void* keys_out, uint32_t* 
         return cudaGetLastError();
     });
     if (e != cudaSuccess || max_len < 2) return e;
-    e = with_key_type(TypeList<uint16_t, uint32_t, uint64_t>{}, key_bytes, [&](auto k) {
+    return launch_segment_classes(keys_in, keys_out, indices, off, num_segments, max_len, key_bytes, codec, rank_mode, sm_count,
+                                  list, counts, stream);
+}
+
+// The class kernels of the binned segments of 2 to max_len <= row_sort_capacity keys: the warp list, then the block classes
+// that max_len reaches.
+static cudaError_t launch_segment_classes(const void* keys_in, void* keys_out, uint32_t* indices, const unsigned long long* off,
+                                          uint64_t num_segments, uint32_t max_len, int key_bytes, const KeyCodec& codec,
+                                          int rank_mode, int sm_count, uint32_t* list, unsigned long long* counts,
+                                          cudaStream_t stream)
+{
+    cudaError_t e = with_key_type(TypeList<uint16_t, uint32_t, uint64_t>{}, key_bytes, [&](auto k) {
         return with_rank_mode(rank_mode, [&](auto r) {
             using KeyT = decltype(k);
             constexpr int R = decltype(r)::value;
@@ -2927,10 +2958,90 @@ long_rows_head_hist_kernel(const KeyT* __restrict__ keys, uint32_t head, unsigne
     for (int p = 0; p < static_cast<int>(sizeof(KeyT)); ++p) atomicAdd(&ghist[p * kRadix + digit_of(k, 8u * p)], 1ull);
 }
 
-template <typename KeyT>
-__global__ void __launch_bounds__(kLongThreads)
-long_rows_count_kernel(const SortPlan* __restrict__ plan, uint32_t place, const KeyT* keys_in, const KeyT* keys_out, const KeyT* alt,
-                       uint64_t num_rows, uint32_t row_len, uint32_t tpr, uint32_t* __restrict__ cnt, KeyCodec codec)
+// Where the long path's tiles are.  LongRowGeo: row r is tiles r * tpr .. (r + 1) * tpr - 1, its counts start at
+// r * 256 * tpr, its scan chunks at r * cpr.  LongSegGeo (osb200_sort_long_segments) finds a tile's segment on the device.
+// Both give: tiles() and tile(g) (the start lo of g's row or segment, g's tile t in it, its first key t0 and length len),
+// cnt_index(tile, d) (where the tile's count of digit d is), chunks() and chunk(g) (the counts of the row or segment that
+// chunk g covers, and its first count c0), groups() and group(i) (the chunk sums of row or segment i).
+struct LongRowGeo {
+    uint64_t num_rows;
+    uint32_t row_len, tpr;
+    uint64_t row_counts;
+    uint32_t cpr;
+    struct Tile { uint64_t r, lo; uint32_t t, t0, len; };
+    struct Chunk { uint64_t base, c0, row_counts; };
+    struct Group { uint64_t first; uint32_t count; };
+    __device__ __forceinline__ uint64_t tiles() const { return num_rows * tpr; }
+    __device__ __forceinline__ Tile tile(uint64_t g) const
+    {
+        const uint64_t r = g / tpr;
+        const uint32_t t = static_cast<uint32_t>(g - r * tpr), t0 = t * kLongRowTile;
+        const uint32_t len = row_len - t0 < kLongRowTile ? row_len - t0 : kLongRowTile;
+        return {r, r * row_len, t, t0, len};
+    }
+    template <typename D>  // the digit as the caller holds it (a thread index): the row kernels' arithmetic as it was
+    __device__ __forceinline__ uint64_t cnt_index(const Tile& x, D d) const { return (x.r * kRadix + d) * tpr + x.t; }
+    __device__ __forceinline__ uint64_t chunks() const { return num_rows * cpr; }
+    __device__ __forceinline__ Chunk chunk(uint64_t g) const
+    {
+        const uint64_t r = g / cpr, c0 = (g - r * cpr) * kLongChunk;
+        return {r * row_counts, c0, row_counts};
+    }
+    __device__ __forceinline__ uint64_t groups() const { return num_rows; }
+    __device__ __forceinline__ Group group(uint64_t r) const { return {r * cpr, cpr}; }
+};
+
+// The largest j < m with pre[j] <= g, for pre increasing from pre[0] = 0.  All threads of the CTA call it; each round reads
+// kLongThreads entries at once and narrows the range as many times, so a list of up to 2^18 entries takes two rounds.
+__device__ __forceinline__ uint32_t cta_find(const uint32_t* __restrict__ pre, uint32_t m, uint64_t g)
+{
+    uint32_t lo = 0, hi = m;
+    while (hi - lo > 1) {
+        const uint32_t step = (hi - lo + kLongThreads - 1) / kLongThreads, i = lo + threadIdx.x * step;
+        lo += step * static_cast<uint32_t>(__syncthreads_count(threadIdx.x > 0 && i < hi && pre[i] <= g));
+        hi = lo + step < hi ? lo + step : hi;
+    }
+    return lo;
+}
+
+// The long segments: the tile map of long_segments_map_kernel.  list[j] is the j-th listed segment, tfirst[j] and cfirst[j]
+// its first tile and first scan chunk (tfirst[m], cfirst[m]: the totals), counts[kSegCountLong...] the list's length and
+// totals.  A tile's counts are digit-major within its segment, as within a row.
+struct LongSegGeo {
+    const unsigned long long* off;
+    const uint32_t* list;
+    const uint32_t* tfirst;
+    const uint32_t* cfirst;
+    const unsigned long long* counts;
+    struct Tile { uint64_t cb, lo; uint32_t t, t0, len, tpr; };
+    struct Chunk { uint64_t base, c0, row_counts; };
+    struct Group { uint64_t first; uint32_t count; };
+    __device__ __forceinline__ uint32_t listed() const { return static_cast<uint32_t>(counts[kSegCountLong]); }
+    __device__ __forceinline__ uint64_t tiles() const { return counts[kSegCountLongTiles]; }
+    __device__ __forceinline__ Tile tile(uint64_t g) const
+    {
+        const uint32_t j = cta_find(tfirst, listed(), g), f = tfirst[j], s = list[j];
+        const uint64_t lo = off[s];
+        const uint32_t seg_len = static_cast<uint32_t>(off[s + 1] - lo);
+        const uint32_t t = static_cast<uint32_t>(g - f), t0 = t * kLongRowTile;
+        const uint32_t len = seg_len - t0 < kLongRowTile ? seg_len - t0 : kLongRowTile;
+        return {static_cast<uint64_t>(f) * kRadix, lo, t, t0, len, tfirst[j + 1] - f};
+    }
+    template <typename D>
+    __device__ __forceinline__ uint64_t cnt_index(const Tile& x, D d) const { return x.cb + static_cast<uint64_t>(d) * x.tpr + x.t; }
+    __device__ __forceinline__ uint64_t chunks() const { return counts[kSegCountLongChunks]; }
+    __device__ __forceinline__ Chunk chunk(uint64_t g) const
+    {
+        const uint32_t j = cta_find(cfirst, listed(), g), f = tfirst[j];
+        return {static_cast<uint64_t>(f) * kRadix, (g - cfirst[j]) * kLongChunk, static_cast<uint64_t>(tfirst[j + 1] - f) * kRadix};
+    }
+    __device__ __forceinline__ uint64_t groups() const { return listed(); }
+    __device__ __forceinline__ Group group(uint64_t j) const { return {cfirst[j], cfirst[j + 1] - cfirst[j]}; }
+};
+
+template <typename KeyT, typename Geo>
+__device__ __forceinline__ void long_count_body(const Geo& geo, const SortPlan* __restrict__ plan, uint32_t place, const KeyT* keys_in,
+                                                const KeyT* keys_out, const KeyT* alt, uint32_t* __restrict__ cnt, KeyCodec codec)
 {
     const LongPass ps = long_pass(plan, place);
     if (ps.skip) return;
@@ -2941,12 +3052,11 @@ long_rows_count_kernel(const SortPlan* __restrict__ plan, uint32_t place, const 
     // bank-private columns, as in the GlobalHistogram: every lane of a warp instruction hits its own bank
     __shared__ uint32_t s_hist[kRadix * 32];
     uint32_t* s_col = s_hist + (threadIdx.x & 31);
-    const uint64_t tiles = num_rows * tpr;
+    const uint64_t tiles = geo.tiles();
     for (uint64_t g = blockIdx.x; g < tiles; g += gridDim.x) {
-        const uint64_t r = g / tpr;
-        const uint32_t t = static_cast<uint32_t>(g - r * tpr), t0 = t * kLongRowTile;
-        const uint32_t len = row_len - t0 < kLongRowTile ? row_len - t0 : kLongRowTile;
-        const KeyT* tile = src + r * row_len + t0;
+        const auto x = geo.tile(g);
+        const uint32_t len = x.len;
+        const KeyT* tile = src + x.lo + x.t0;
         for (int i = threadIdx.x; i < kRadix * 32; i += kLongThreads) s_hist[i] = 0;
         __syncthreads();
         KeyT key[kLongK];
@@ -2966,10 +3076,26 @@ long_rows_count_kernel(const SortPlan* __restrict__ plan, uint32_t place, const 
             uint32_t sum = 0;
 #pragma unroll 8
             for (int c = 0; c < 32; ++c) sum += s_hist[threadIdx.x * 32 + ((c + threadIdx.x) & 31)];
-            cnt[(r * kRadix + threadIdx.x) * tpr + t] = sum;
+            cnt[geo.cnt_index(x, threadIdx.x)] = sum;
         }
         __syncthreads();  // the fold has read s_hist
     }
+}
+
+template <typename KeyT>
+__global__ void __launch_bounds__(kLongThreads)
+long_rows_count_kernel(const SortPlan* __restrict__ plan, uint32_t place, const KeyT* keys_in, const KeyT* keys_out, const KeyT* alt,
+                       uint64_t num_rows, uint32_t row_len, uint32_t tpr, uint32_t* __restrict__ cnt, KeyCodec codec)
+{
+    long_count_body<KeyT>(LongRowGeo{num_rows, row_len, tpr, 0, 0}, plan, place, keys_in, keys_out, alt, cnt, codec);
+}
+
+template <typename KeyT>
+__global__ void __launch_bounds__(kLongThreads)
+long_segments_count_kernel(const SortPlan* __restrict__ plan, uint32_t place, const KeyT* keys_in, const KeyT* keys_out, const KeyT* alt,
+                           LongSegGeo geo, uint32_t* __restrict__ cnt, KeyCodec codec)
+{
+    long_count_body<KeyT>(geo, plan, place, keys_in, keys_out, alt, cnt, codec);
 }
 
 // The m <= kLongChunk counts at p, thread i holding counts 8i .. 8i+7: their sum (to every thread), and with SCAN their
@@ -3005,48 +3131,88 @@ __device__ __forceinline__ uint32_t long_chunk(uint32_t* p, uint32_t m, uint32_t
     return total;
 }
 
-// Chunk c of row r: counts [c * kLongChunk, min((c + 1) * kLongChunk, row_counts)) of the row's row_counts = 256 * tpr.
-// csum[r * cpr + c] = the chunk's sum.
-__global__ void __launch_bounds__(kLongThreads)
-long_rows_chunk_sum_kernel(const SortPlan* __restrict__ plan, uint32_t place, uint32_t* cnt, uint32_t* __restrict__ csum,
-                           uint64_t num_rows, uint64_t row_counts, uint32_t cpr)
+// Chunk g covers counts [c0, min(c0 + kLongChunk, row_counts)) of its row's or segment's row_counts = 256 * tiles:
+// csum[g] = their sum.
+template <typename Geo>
+__device__ __forceinline__ void long_chunk_sum_body(const Geo& geo, const SortPlan* __restrict__ plan, uint32_t place, uint32_t* cnt,
+                                                    uint32_t* __restrict__ csum)
 {
     if (long_pass(plan, place).skip) return;
     __shared__ uint32_t s_w[kLongWarps];
-    for (uint64_t g = blockIdx.x; g < num_rows * cpr; g += gridDim.x) {
-        const uint64_t r = g / cpr, c0 = (g - r * cpr) * kLongChunk;
-        const uint32_t m = static_cast<uint32_t>(row_counts - c0 < kLongChunk ? row_counts - c0 : kLongChunk);
-        const uint32_t s = long_chunk<false>(cnt + r * row_counts + c0, m, 0u, s_w);
+    for (uint64_t g = blockIdx.x; g < geo.chunks(); g += gridDim.x) {
+        const auto x = geo.chunk(g);
+        const uint32_t m = static_cast<uint32_t>(x.row_counts - x.c0 < kLongChunk ? x.row_counts - x.c0 : kLongChunk);
+        const uint32_t s = long_chunk<false>(cnt + x.base + x.c0, m, 0u, s_w);
         if (threadIdx.x == 0) csum[g] = s;
     }
 }
 
-// The exclusive scan of each row's cpr chunk sums, in place; one CTA per row at a time.
 __global__ void __launch_bounds__(kLongThreads)
-long_rows_chunk_scan_kernel(const SortPlan* __restrict__ plan, uint32_t place, uint32_t* csum, uint64_t num_rows, uint32_t cpr)
+long_rows_chunk_sum_kernel(const SortPlan* __restrict__ plan, uint32_t place, uint32_t* cnt, uint32_t* __restrict__ csum,
+                           uint64_t num_rows, uint64_t row_counts, uint32_t cpr)
+{
+    long_chunk_sum_body(LongRowGeo{num_rows, 0, 0, row_counts, cpr}, plan, place, cnt, csum);
+}
+
+__global__ void __launch_bounds__(kLongThreads)
+long_segments_chunk_sum_kernel(const SortPlan* __restrict__ plan, uint32_t place, uint32_t* cnt, uint32_t* __restrict__ csum, LongSegGeo geo)
+{
+    long_chunk_sum_body(geo, plan, place, cnt, csum);
+}
+
+// The exclusive scan of each row's or segment's chunk sums, in place; one CTA per row or segment at a time.
+template <typename Geo>
+__device__ __forceinline__ void long_chunk_scan_body(const Geo& geo, const SortPlan* __restrict__ plan, uint32_t place, uint32_t* csum)
 {
     if (long_pass(plan, place).skip) return;
     __shared__ uint32_t s_w[kLongWarps];
-    for (uint64_t r = blockIdx.x; r < num_rows; r += gridDim.x) {
+    for (uint64_t r = blockIdx.x; r < geo.groups(); r += gridDim.x) {
+        const auto x = geo.group(r);
         uint32_t carry = 0;
-        for (uint32_t c0 = 0; c0 < cpr; c0 += kLongChunk)
-            carry += long_chunk<true>(csum + r * cpr + c0, cpr - c0 < kLongChunk ? cpr - c0 : kLongChunk, carry, s_w);
+        for (uint32_t c0 = 0; c0 < x.count; c0 += kLongChunk)
+            carry += long_chunk<true>(csum + x.first + c0, x.count - c0 < kLongChunk ? x.count - c0 : kLongChunk, carry, s_w);
     }
 }
 
-// Every chunk's counts become their exclusive prefix within the row: the chunk's own scan plus its chunk prefix (csum null:
-// a row is one chunk).
+__global__ void __launch_bounds__(kLongThreads)
+long_rows_chunk_scan_kernel(const SortPlan* __restrict__ plan, uint32_t place, uint32_t* csum, uint64_t num_rows, uint32_t cpr)
+{
+    long_chunk_scan_body(LongRowGeo{num_rows, 0, 0, 0, cpr}, plan, place, csum);
+}
+
+__global__ void __launch_bounds__(kLongThreads)
+long_segments_chunk_scan_kernel(const SortPlan* __restrict__ plan, uint32_t place, uint32_t* csum, LongSegGeo geo)
+{
+    long_chunk_scan_body(geo, plan, place, csum);
+}
+
+// Every chunk's counts become their exclusive prefix within the row or segment: the chunk's own scan plus its chunk prefix
+// (csum null: every row or segment is one chunk).
+template <typename Geo>
+__device__ __forceinline__ void long_scan_body(const Geo& geo, const SortPlan* __restrict__ plan, uint32_t place, uint32_t* cnt,
+                                               const uint32_t* __restrict__ csum)
+{
+    if (long_pass(plan, place).skip) return;
+    __shared__ uint32_t s_w[kLongWarps];
+    for (uint64_t g = blockIdx.x; g < geo.chunks(); g += gridDim.x) {
+        const auto x = geo.chunk(g);
+        const uint32_t m = static_cast<uint32_t>(x.row_counts - x.c0 < kLongChunk ? x.row_counts - x.c0 : kLongChunk);
+        long_chunk<true>(cnt + x.base + x.c0, m, csum ? csum[g] : 0u, s_w);
+    }
+}
+
 __global__ void __launch_bounds__(kLongThreads)
 long_rows_scan_kernel(const SortPlan* __restrict__ plan, uint32_t place, uint32_t* cnt, const uint32_t* __restrict__ csum,
                       uint64_t num_rows, uint64_t row_counts, uint32_t cpr)
 {
-    if (long_pass(plan, place).skip) return;
-    __shared__ uint32_t s_w[kLongWarps];
-    for (uint64_t g = blockIdx.x; g < num_rows * cpr; g += gridDim.x) {
-        const uint64_t r = g / cpr, c0 = (g - r * cpr) * kLongChunk;
-        const uint32_t m = static_cast<uint32_t>(row_counts - c0 < kLongChunk ? row_counts - c0 : kLongChunk);
-        long_chunk<true>(cnt + r * row_counts + c0, m, csum ? csum[g] : 0u, s_w);
-    }
+    long_scan_body(LongRowGeo{num_rows, 0, 0, row_counts, cpr}, plan, place, cnt, csum);
+}
+
+__global__ void __launch_bounds__(kLongThreads)
+long_segments_scan_kernel(const SortPlan* __restrict__ plan, uint32_t place, uint32_t* cnt, const uint32_t* __restrict__ csum,
+                          LongSegGeo geo)
+{
+    long_scan_body(geo, plan, place, cnt, csum);
 }
 
 template <typename KeyT, bool INDICES>
@@ -3059,12 +3225,10 @@ struct LongRowsSmem {
     uint32_t wtot[kRadix / 32];
 };
 
-// (Two resident CTAs per SM are stated for 16- and 32-bit keys only: with indices they spill at 64 registers.)
-template <typename KeyT, int RANK_MODE, bool INDICES>
-__global__ void __launch_bounds__(kLongThreads, sizeof(KeyT) == 8 || INDICES ? 1 : 2)
-long_rows_scatter_kernel(const SortPlan* __restrict__ plan, uint32_t place, const KeyT* keys_in, KeyT* keys_out, KeyT* alt,
-                         uint32_t* idx_out, uint32_t* alt_idx, uint64_t num_rows, uint32_t row_len, uint32_t tpr,
-                         const uint32_t* __restrict__ base, KeyCodec codec)
+template <typename KeyT, int RANK_MODE, bool INDICES, typename Geo>
+__device__ __forceinline__ void long_scatter_body(const Geo& geo, const SortPlan* __restrict__ plan, uint32_t place, const KeyT* keys_in,
+                                                  KeyT* keys_out, KeyT* alt, uint32_t* idx_out, uint32_t* alt_idx,
+                                                  const uint32_t* __restrict__ base, KeyCodec codec)
 {
     const LongPass ps = long_pass(plan, place);
     if (ps.skip) return;
@@ -3083,11 +3247,11 @@ long_rows_scatter_kernel(const SortPlan* __restrict__ plan, uint32_t place, cons
     const uint32_t lt = lanemask_lt();
     uint32_t* wh = sm.hist + warp * kRadix;
     const uint32_t warp_lo = warp * (32 * kLongK), warp_off = warp_lo + lane;
-    const uint64_t tiles = num_rows * tpr;
+    const uint64_t tiles = geo.tiles();
     for (uint64_t g = blockIdx.x; g < tiles; g += gridDim.x) {
-        const uint64_t r = g / tpr, row_lo = r * row_len;
-        const uint32_t t = static_cast<uint32_t>(g - r * tpr), t0 = t * kLongRowTile;
-        const uint32_t len = row_len - t0 < kLongRowTile ? row_len - t0 : kLongRowTile;
+        const auto x = geo.tile(g);
+        const uint64_t row_lo = x.lo;
+        const uint32_t t0 = x.t0, len = x.len;
         __syncthreads();  // the previous tile has been stored from shared memory
         {
             uint4* h4 = reinterpret_cast<uint4*>(sm.hist);
@@ -3122,7 +3286,7 @@ long_rows_scatter_kernel(const SortPlan* __restrict__ plan, uint32_t place, cons
 #pragma unroll
             for (int w = 0; w < kLongWarps; ++w) { const uint32_t c = sm.hist[w * kRadix + tid]; sm.hist[w * kRadix + tid] = run; run += c; }
             sm.first[tid] = tile_excl;
-            sm.base[tid] = base[(r * kRadix + tid) * tpr + t];
+            sm.base[tid] = base[geo.cnt_index(x, tid)];
         }
         __syncthreads();
 #pragma unroll
@@ -3144,6 +3308,25 @@ long_rows_scatter_kernel(const SortPlan* __restrict__ plan, uint32_t place, cons
     }
 }
 
+// (Two resident CTAs per SM are stated for 16- and 32-bit keys only: with indices they spill at 64 registers.)
+template <typename KeyT, int RANK_MODE, bool INDICES>
+__global__ void __launch_bounds__(kLongThreads, sizeof(KeyT) == 8 || INDICES ? 1 : 2)
+long_rows_scatter_kernel(const SortPlan* __restrict__ plan, uint32_t place, const KeyT* keys_in, KeyT* keys_out, KeyT* alt,
+                         uint32_t* idx_out, uint32_t* alt_idx, uint64_t num_rows, uint32_t row_len, uint32_t tpr,
+                         const uint32_t* __restrict__ base, KeyCodec codec)
+{
+    long_scatter_body<KeyT, RANK_MODE, INDICES>(LongRowGeo{num_rows, row_len, tpr, 0, 0}, plan, place, keys_in, keys_out, alt, idx_out,
+                                                alt_idx, base, codec);
+}
+
+template <typename KeyT, int RANK_MODE, bool INDICES>
+__global__ void __launch_bounds__(kLongThreads, sizeof(KeyT) == 8 || INDICES ? 1 : 2)
+long_segments_scatter_kernel(const SortPlan* __restrict__ plan, uint32_t place, const KeyT* keys_in, KeyT* keys_out, KeyT* alt,
+                             uint32_t* idx_out, uint32_t* alt_idx, LongSegGeo geo, const uint32_t* __restrict__ base, KeyCodec codec)
+{
+    long_scatter_body<KeyT, RANK_MODE, INDICES>(geo, plan, place, keys_in, keys_out, alt, idx_out, alt_idx, base, codec);
+}
+
 // Odd executed passes: keys and indices from the alternate buffers.  None: keys_in is its own stable sort -- its keys (not
 // copied in place) and the positions 0 .. row_len - 1 of every row.
 template <typename KeyT>
@@ -3162,7 +3345,84 @@ long_rows_copy_home_kernel(const SortPlan* __restrict__ plan, const KeyT* keys_i
     }
 }
 
+// The long segments' copy home, tile by tile so that nothing outside them is written: as long_rows_copy_home_kernel, with
+// positions 0 .. L - 1 within each segment when no pass executes.
+template <typename KeyT>
+__global__ void __launch_bounds__(kLongThreads)
+long_segments_copy_home_kernel(const SortPlan* __restrict__ plan, const KeyT* keys_in, const KeyT* __restrict__ alt, KeyT* keys_out,
+                               const uint32_t* __restrict__ alt_idx, uint32_t* __restrict__ idx_out, LongSegGeo geo)
+{
+    const uint32_t ex = plan->executed;
+    if (ex != 0 && !(ex & 1u)) return;
+    const KeyT* src = ex ? alt : keys_in;
+    const bool keys = src != keys_out;
+    const uint64_t tiles = geo.tiles();
+    for (uint64_t g = blockIdx.x; g < tiles; g += gridDim.x) {
+        const auto x = geo.tile(g);
+        for (uint32_t j = threadIdx.x; j < x.len; j += kLongThreads) {
+            const uint64_t i = x.lo + x.t0 + j;
+            if (keys) __stcs(keys_out + i, __ldcs(src + i));
+            if (idx_out) __stcs(idx_out + i, ex ? __ldcs(alt_idx + i) : x.t0 + j);
+        }
+    }
+}
+
+// The tile map of the long list, one CTA: the tiles ceil(L / kLongRowTile) and scan chunks ceil(256 tiles / kLongChunk) of
+// every listed segment become exclusive prefixes in list order (tfirst, cfirst), with the totals at [m] and in counts.
+// Listed segments are disjoint unless the offsets make valid segments overlap; only then can the list or its totals pass
+// the workspace's bounds, and the long path is left empty.
+__global__ void __launch_bounds__(kLongThreads)
+long_segments_map_kernel(const unsigned long long* __restrict__ off, const uint32_t* __restrict__ list, uint32_t* tfirst,
+                         uint32_t* cfirst, unsigned long long* counts, uint64_t list_cap, uint64_t tile_cap, uint64_t chunk_cap)
+{
+    __shared__ uint32_t s_w[kLongWarps];
+    __shared__ unsigned long long s_tiles, s_chunks;
+    const unsigned long long listed = counts[kSegCountLong];
+    const uint32_t m = static_cast<uint32_t>(listed < list_cap ? listed : list_cap);
+    if (threadIdx.x == 0) s_tiles = s_chunks = 0;
+    __syncthreads();
+    for (uint32_t j = threadIdx.x; j < m; j += kLongThreads) {
+        const uint32_t s = list[j];
+        const unsigned long long tiles = (off[s + 1] - off[s] + kLongRowTile - 1) / kLongRowTile;
+        const unsigned long long chunks = (tiles * kRadix + kLongChunk - 1) / kLongChunk;
+        tfirst[j] = static_cast<uint32_t>(tiles);
+        cfirst[j] = static_cast<uint32_t>(chunks);
+        atomicAdd(&s_tiles, tiles);
+        atomicAdd(&s_chunks, chunks);
+    }
+    __syncthreads();
+    const bool fits = listed <= list_cap && s_tiles <= tile_cap && s_chunks <= chunk_cap;
+    uint32_t tc = 0, cc = 0;
+    for (uint32_t c0 = 0; fits && c0 < m; c0 += kLongChunk) {
+        const uint32_t k = m - c0 < kLongChunk ? m - c0 : kLongChunk;
+        tc += long_chunk<true>(tfirst + c0, k, tc, s_w);
+        cc += long_chunk<true>(cfirst + c0, k, cc, s_w);
+    }
+    if (threadIdx.x == 0) {
+        if (fits) { tfirst[m] = tc; cfirst[m] = cc; }
+        counts[kSegCountLong] = fits ? m : 0u;
+        counts[kSegCountLongTiles] = tc;
+        counts[kSegCountLongChunks] = cc;
+    }
+}
+
 using LongRowKeys = TypeList<uint16_t, uint32_t, uint64_t>;
+
+// The long paths' plan over keys[0, n): the keys before the first 16-byte boundary of a naturally aligned input (at most
+// 7, and never more than n) by the one-warp head kernel, the rest by the GlobalHistogram, which reads 16-byte vectors;
+// then the scan that writes `plan`.  enc: the codec's encode only (null: plain unsigned keys).
+template <typename KeyT>
+static cudaError_t launch_long_plan(const KeyT* in, uint64_t n, int key_bytes, const KeyCodec* enc, bool allow_skip,
+                                   unsigned long long* ghist, unsigned long long* gbase, SortPlan* plan, int sm_count,
+                                   cudaStream_t stream)
+{
+    uint64_t head = ((16u - (reinterpret_cast<uintptr_t>(in) & 15u)) & 15u) / sizeof(KeyT);
+    if (head > n) head = n;
+    if (head) long_rows_head_hist_kernel<KeyT><<<1, 32, 0, stream>>>(in, static_cast<uint32_t>(head), ghist, enc ? *enc : KeyCodec());
+    cudaError_t e = launch_global_histogram(in + head, n - head, key_bytes, ghist, sm_count, stream, enc);
+    return e == cudaSuccess ? launch_scan(ghist, gbase, key_bytes, stream, plan, n, allow_skip, false) : e;
+}
+
 
 cudaError_t launch_long_rows(const void* keys_in, void* keys_out, uint32_t* indices, void* alt_keys, uint32_t* alt_idx,
                              uint64_t num_rows, uint32_t row_len, int key_bytes, const KeyCodec* codec_in, int rank_mode,
@@ -3184,11 +3444,7 @@ cudaError_t launch_long_rows(const void* keys_in, void* keys_out, uint32_t* indi
         const KeyT* in = static_cast<const KeyT*>(keys_in);
         KeyT* out = static_cast<KeyT*>(keys_out);
         KeyT* alt = static_cast<KeyT*>(alt_keys);
-        // the plan: keys before the first 16-byte boundary here, the rest in the GlobalHistogram, then the scan
-        const uint32_t head = static_cast<uint32_t>(((16u - (reinterpret_cast<uintptr_t>(in) & 15u)) & 15u) / sizeof(KeyT));
-        if (head) long_rows_head_hist_kernel<KeyT><<<1, 32, 0, stream>>>(in, head, ghist, enc);
-        cudaError_t e = launch_global_histogram(in + head, n - head, key_bytes, ghist, sm_count, stream, codec_in ? &enc : nullptr);
-        if (e == cudaSuccess) e = launch_scan(ghist, gbase, key_bytes, stream, plan, n, allow_skip, false);
+        cudaError_t e = launch_long_plan(in, n, key_bytes, codec_in ? &enc : nullptr, allow_skip, ghist, gbase, plan, sm_count, stream);
         const unsigned scan_grid = capped_grid(num_rows * cpr, 1, static_cast<uint64_t>(sm_count) * 4);
         for (uint32_t p = 0; e == cudaSuccess && p < sizeof(KeyT); ++p) {
             e = launch_resident<long_rows_count_kernel<KeyT>, kLongThreads, 0>(num_rows * tpr, sm_count, stream, plan, p, in, out, alt,
@@ -3216,6 +3472,105 @@ cudaError_t launch_long_rows(const void* keys_in, void* keys_out, uint32_t* indi
         long_rows_copy_home_kernel<KeyT><<<capped_grid(n, 512, static_cast<uint64_t>(sm_count) * 4), 512, 0, stream>>>(
             plan, in, alt, out, alt_idx, indices, n, row_len);
         return cudaGetLastError();
+    });
+}
+
+// =====================================================================================================
+// Long segments (osb200_sort_long_segments): the segment sort's binning and classes for segments of up to long_min - 1 keys,
+// and the long-row passes over the tiles of the longer ones (DESIGN §4.17).  The tiles of segment j of the long list are
+// tfirst[j] .. tfirst[j + 1] - 1 and its counts start at 256 * tfirst[j]; each kernel finds a tile's or chunk's segment
+// by a search over the prefixes (LongSegGeo).  The list's order comes from atomics; it moves where a segment's counts are,
+// never where its keys go.
+// =====================================================================================================
+template <typename KeyT>
+__global__ void __launch_bounds__(256)
+long_segment_bin_kernel(const unsigned long long* __restrict__ off, uint64_t num_segments, uint64_t n, uint32_t max_len,
+                        uint32_t* __restrict__ list, unsigned long long* __restrict__ counts, const KeyT* keys_in, KeyT* keys_out,
+                        uint32_t* idx_out, uint32_t long_min, uint32_t* __restrict__ long_list, uint64_t long_cap)
+{
+    segment_bin_body<KeyT, false, true>(off, num_segments, n, max_len, list, counts, keys_in, keys_out, idx_out, kRowWarpMaxLen,
+                                        long_min, long_list, long_cap);
+}
+
+LongSegLayout long_segments_layout(uint64_t n, uint32_t long_min)
+{
+    auto whole = [](uint64_t words) { return (words + 3) / 4 * 4; };  // every array 16-byte aligned
+    LongSegLayout l;
+    l.list_cap = n / long_min;
+    l.tile_cap = (n + kLongRowTile - 1) / kLongRowTile + l.list_cap;
+    l.chunk_cap = (l.tile_cap * kRadix + kLongChunk - 1) / kLongChunk + l.list_cap;
+    l.csum = whole(l.tile_cap * kRadix);
+    l.list = l.csum + whole(l.chunk_cap);
+    l.tfirst = l.list + whole(l.list_cap);
+    l.cfirst = l.tfirst + whole(l.list_cap + 1);
+    l.words = l.cfirst + whole(l.list_cap + 1);
+    return l;
+}
+
+cudaError_t launch_long_segments(const void* keys_in, void* keys_out, uint32_t* indices, void* alt_keys, uint32_t* alt_idx, uint64_t n,
+                                 const unsigned long long* off, uint64_t num_segments, uint32_t max_len, uint32_t long_min,
+                                 int key_bytes, const KeyCodec* codec_in, int rank_mode, bool allow_skip, unsigned long long* ghist,
+                                 unsigned long long* gbase, SortPlan* plan, uint32_t* list, unsigned long long* counts,
+                                 uint32_t* scratch, int sm_count, cudaStream_t stream)
+{
+    if (num_segments == 0 || max_len < long_min || long_min < 2) return cudaErrorInvalidValue;
+    const LongSegLayout l = long_segments_layout(n, long_min);
+    uint32_t* cnt = scratch;
+    uint32_t* csum = max_len > kLongChunk / kRadix * kLongRowTile ? scratch + l.csum : nullptr;  // some segment has 2+ chunks
+    uint32_t* llist = scratch + l.list;
+    const LongSegGeo geo{off, llist, scratch + l.tfirst, scratch + l.cfirst, counts};
+    const KeyCodec codec = codec_in ? *codec_in : KeyCodec();
+    KeyCodec enc = codec;
+    enc.flags &= kCodecEncodeOnLoad;
+    cudaError_t e = cudaMemsetAsync(counts, 0, kLongSegCounts * sizeof(unsigned long long), stream);
+    if (e != cudaSuccess) return e;
+    return with_key_type(LongRowKeys{}, key_bytes, [&](auto kt) {
+        using KeyT = decltype(kt);
+        const KeyT* in = static_cast<const KeyT*>(keys_in);
+        KeyT* out = static_cast<KeyT*>(keys_out);
+        KeyT* alt = static_cast<KeyT*>(alt_keys);
+        long_segment_bin_kernel<KeyT><<<capped_grid(num_segments, 256, static_cast<uint64_t>(sm_count) * 8), 256, 0, stream>>>(
+            off, num_segments, n, max_len, list, counts, in, out, indices, long_min, llist, l.list_cap);
+        cudaError_t e = cudaGetLastError();
+        // the classes first: their lists live in the alternate keys, which the long passes overwrite
+        if (e == cudaSuccess && long_min > 2)
+            e = launch_segment_classes(keys_in, keys_out, indices, off, num_segments, long_min - 1, key_bytes, codec, rank_mode, sm_count,
+                                       list, counts, stream);
+        if (e == cudaSuccess) {
+            long_segments_map_kernel<<<1, kLongThreads, 0, stream>>>(off, llist, scratch + l.tfirst, scratch + l.cfirst, counts, l.list_cap,
+                                                                     l.tile_cap, l.chunk_cap);
+            e = cudaGetLastError();
+        }
+        // the plan over all n keys, as for the long rows
+        if (e == cudaSuccess)
+            e = launch_long_plan(in, n, key_bytes, codec_in ? &enc : nullptr, allow_skip, ghist, gbase, plan, sm_count, stream);
+        const unsigned scan_grid = capped_grid(l.chunk_cap, 1, static_cast<uint64_t>(sm_count) * 4);
+        for (uint32_t p = 0; e == cudaSuccess && p < sizeof(KeyT); ++p) {
+            e = launch_resident<long_segments_count_kernel<KeyT>, kLongThreads, 0>(l.tile_cap, sm_count, stream, plan, p, in,
+                                                                                   static_cast<const KeyT*>(out), static_cast<const KeyT*>(alt),
+                                                                                   geo, cnt, codec);
+            if (e == cudaSuccess && csum) {
+                long_segments_chunk_sum_kernel<<<scan_grid, kLongThreads, 0, stream>>>(plan, p, cnt, csum, geo);
+                long_segments_chunk_scan_kernel<<<capped_grid(l.list_cap, 1, static_cast<uint64_t>(sm_count) * 4), kLongThreads, 0, stream>>>(
+                    plan, p, csum, geo);
+            }
+            if (e == cudaSuccess) {
+                long_segments_scan_kernel<<<scan_grid, kLongThreads, 0, stream>>>(plan, p, cnt, csum, geo);
+                e = cudaGetLastError();
+            }
+            if (e == cudaSuccess) e = with_rank_mode(rank_mode, [&](auto rm) {
+                auto go = [&](auto ind) {
+                    constexpr bool I = decltype(ind)::value;
+                    return launch_resident<long_segments_scatter_kernel<KeyT, decltype(rm)::value, I>, kLongThreads, sizeof(LongRowsSmem<KeyT, I>)>(
+                        l.tile_cap, sm_count, stream, plan, p, in, out, alt, indices, alt_idx, geo, static_cast<const uint32_t*>(cnt), codec);
+                };
+                return indices ? go(std::true_type{}) : go(std::false_type{});
+            });
+        }
+        if (e != cudaSuccess) return e;
+        return launch_resident<long_segments_copy_home_kernel<KeyT>, kLongThreads, 0>(l.tile_cap, sm_count, stream, plan, in,
+                                                                                      static_cast<const KeyT*>(alt), out,
+                                                                                      static_cast<const uint32_t*>(alt_idx), indices, geo);
     });
 }
 
@@ -3670,6 +4025,13 @@ cudaError_t configure_kernels()
         if (m == cudaSuccess) m = set_smem(long_rows_scatter_kernel<KeyT, kRankBallot, false>, sizeof(LongRowsSmem<KeyT, false>));
         if (m == cudaSuccess) m = set_smem(long_rows_scatter_kernel<KeyT, kRankAtomic, true>, sizeof(LongRowsSmem<KeyT, true>));
         return m != cudaSuccess ? m : set_smem(long_rows_scatter_kernel<KeyT, kRankBallot, true>, sizeof(LongRowsSmem<KeyT, true>));
+    });
+    if (e == cudaSuccess) e = for_each_type(LongRowKeys{}, [](auto k) {
+        using KeyT = decltype(k);
+        cudaError_t m = set_smem(long_segments_scatter_kernel<KeyT, kRankAtomic, false>, sizeof(LongRowsSmem<KeyT, false>));
+        if (m == cudaSuccess) m = set_smem(long_segments_scatter_kernel<KeyT, kRankBallot, false>, sizeof(LongRowsSmem<KeyT, false>));
+        if (m == cudaSuccess) m = set_smem(long_segments_scatter_kernel<KeyT, kRankAtomic, true>, sizeof(LongRowsSmem<KeyT, true>));
+        return m != cudaSuccess ? m : set_smem(long_segments_scatter_kernel<KeyT, kRankBallot, true>, sizeof(LongRowsSmem<KeyT, true>));
     });
     return e;
 }

@@ -144,6 +144,24 @@ cudaError_t launch_long_rows(const void* keys_in, void* keys_out, uint32_t* indi
                              bool allow_skip, unsigned long long* ghist, unsigned long long* gbase, SortPlan* plan,
                              uint32_t* scratch, int sm_count, cudaStream_t stream);
 
+// Long segments (osb200_sort_long_segments): launch_sort_segments for segments of 2 to long_min - 1 keys, and the long
+// rows' passes for segments of long_min to max_len keys (long_min >= 2), whose tiles of kLongRowTile keys never straddle
+// segments; nothing outside [0, n)'s valid segments of at most max_len keys is written.  Enqueues the binning (the class
+// lists in `list`, num_segments u32), the class kernels, a one-CTA tile map of the long list, the GlobalHistogram over all
+// n keys into ghist (zeroed by the caller) and the scan that writes `plan`, per digit place a count, a scan of each long
+// segment's tile counts and a scatter, then the copy home of the long segments.  counts: 7 u64, cleared here.  alt_keys:
+// n keys of key_bytes (it may hold `list`: the class kernels run before the passes); alt_idx: n u32 when indices is not
+// null; scratch: long_segments_layout(n, long_min).words u32, 16-byte aligned.  The codec as for launch_row_sort.
+// The layout bounds every listed set of disjoint segments of long_min or more keys among n: at most list_cap = n / long_min
+// of them, with at most tile_cap tiles and chunk_cap scan chunks.
+struct LongSegLayout { uint64_t list_cap, tile_cap, chunk_cap, csum, list, tfirst, cfirst, words; };  // offsets in u32 words
+LongSegLayout long_segments_layout(uint64_t n, uint32_t long_min);
+cudaError_t launch_long_segments(const void* keys_in, void* keys_out, uint32_t* indices, void* alt_keys, uint32_t* alt_idx, uint64_t n,
+                                 const unsigned long long* off, uint64_t num_segments, uint32_t max_len, uint32_t long_min,
+                                 int key_bytes, const KeyCodec* codec, int rank_mode, bool allow_skip, unsigned long long* ghist,
+                                 unsigned long long* gbase, SortPlan* plan, uint32_t* list, unsigned long long* counts,
+                                 uint32_t* scratch, int sm_count, cudaStream_t stream);
+
 // Segment sort by offsets (osb200_sort_segments): segment s = [off[s], off[s + 1]) of keys_in, sorted stable into the same
 // positions of keys_out (== keys_in: in place); indices (may be null) receives every output key's position within its segment.
 // A binning kernel puts every segment of 2 to max_len keys that lies inside [0, n) into a class by its length -- one warp

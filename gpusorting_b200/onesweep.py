@@ -306,6 +306,23 @@ class OneSweepSorter:
                    x.numel(), offsets.data_ptr(), segs, int(max_segment_len), kb, kt, 1 if descending else 0, stream=stream)
         return (out, idx) if return_indices else out
 
+    def sort_long_segments(self, x: torch.Tensor, offsets: torch.Tensor, key_type: str, descending: bool = False,
+                           return_indices: bool = True, inplace: bool = False, max_segment_len: Optional[int] = None,
+                           stream=None):
+        """sort_segments for segments of any length (osb200_sort_long_segments): the same arguments, shapes and results, with
+        max_segment_len any uint32 (None: the longest segment, read with one device->host read).  Up to 16,384 (8,192 for
+        8-byte dtypes) it is sort_segments' own launch on any sorter.  Above that the longer segments use this sorter's
+        workspace: x.numel() may be at most max_n, the sorter's key_bytes must be at least x's element size, and
+        return_indices=True needs value_bytes == 4 -- a (4, 4) sorter for 2- and 4-byte dtypes, a (8, 4) one for any."""
+        kb, kt = self._ragged_keys(x, key_type, offsets)
+        segs = max(offsets.numel() - 1, 0)
+        if max_segment_len is None:
+            max_segment_len = max(int((offsets[1:] - offsets[:-1]).max().item()), 0) if segs else 0
+        out, idx = _new_outputs(stream, x, x.shape, return_indices, x if inplace else None)
+        self._call(lib.osb200_sort_long_segments, x.data_ptr(), out.data_ptr(), idx.data_ptr() if idx is not None else None,
+                   x.numel(), offsets.data_ptr(), segs, int(max_segment_len), kb, kt, 1 if descending else 0, stream=stream)
+        return (out, idx) if return_indices else out
+
     # -- segment top-k: row top-k for ragged rows given by offsets -----------------------------------------------------------
     def topk_segments(self, x: torch.Tensor, offsets: torch.Tensor, k: int, key_type: str, largest: bool = True,
                       sorted: bool = True, stream=None):
@@ -558,6 +575,24 @@ def sort_segments(x: torch.Tensor, offsets: torch.Tensor, descending: bool = Fal
     (the call keeps one uint32 per segment in the sorter's workspace); see there for max_segment_len and what is written."""
     s = _module_sorter(x, "x", 4, max(offsets.numel() - 1, 1), stream, _ROW_KEY_TYPES)
     return s.sort_segments(x, offsets, _ROW_KEY_TYPES[x.dtype], descending, return_indices, False, max_segment_len, stream)
+
+
+def sort_long_segments(x: torch.Tensor, offsets: torch.Tensor, descending: bool = False, return_indices: bool = True,
+                       max_segment_len: Optional[int] = None, stream=None):
+    """sort_segments for segments of any length: (values, int32 positions within the segment), or values alone, for a
+    contiguous 1-D CUDA tensor of one of sort_rows' ten dtypes.  With max_segment_len above sort_segments' limit (None: the
+    longest segment, one device->host read) it runs on the stream's cached (4, 4) sorter, or its (8, 4) sorter for 8-byte
+    dtypes, grown to max(x.numel(), number of segments); otherwise on the (4, 4) one grown to the number of segments, as in
+    sort_segments."""
+    segs = max(offsets.numel() - 1, 0) if isinstance(offsets, torch.Tensor) else 0
+    if max_segment_len is None and segs:
+        max_segment_len = max(int((offsets[1:] - offsets[:-1]).max().item()), 0)
+    kb = x.element_size() if isinstance(x, torch.Tensor) else 4
+    if (max_segment_len or 0) > _ROW_CAPACITY.get(kb, 16384):
+        s = _module_sorter(x, "x", 8 if kb == 8 else 4, max(x.numel(), segs), stream, _ROW_KEY_TYPES)
+    else:
+        s = _module_sorter(x, "x", 4, max(segs, 1), stream, _ROW_KEY_TYPES)
+    return s.sort_long_segments(x, offsets, _ROW_KEY_TYPES[x.dtype], descending, return_indices, False, max_segment_len, stream)
 
 
 def topk_segments(x: torch.Tensor, offsets: torch.Tensor, k: int, largest: bool = True, sorted: bool = True, stream=None):

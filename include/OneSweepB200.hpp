@@ -122,6 +122,16 @@ class OneSweepSorterB200 {
                                    key_bytes, key_type, descending ? 1 : 0, stream),
               "osb200_sort_segments");
     }
+    // SortSegments for any max_segment_len: segments above SortSegments' limit use this handle's workspace (n <= max_n, a key
+    // width of at least key_bytes, and value_bytes 4 with indices)
+    void SortLongSegments(const void* d_keys_in, void* d_keys_out, uint32_t* d_indices, uint64_t n, const uint64_t* d_segment_offsets,
+                          uint64_t num_segments, uint32_t max_segment_len, int key_bytes, int key_type, bool descending,
+                          void* stream = nullptr)
+    {
+        check(osb200_sort_long_segments(h_, d_keys_in, d_keys_out, d_indices, n, d_segment_offsets, num_segments, max_segment_len,
+                                        key_bytes, key_type, descending ? 1 : 0, stream),
+              "osb200_sort_long_segments");
+    }
     // every segment [offsets[i], offsets[i+1]) sorted ascending and stable in place, one thread block per segment
     // (reference: SplitSort, SegSort/SplitSort/SplitSort.cuh:702-938); d_values may be null; max_segment_len <= 16,384
     void SegmentedSort(uint32_t* d_keys, uint32_t* d_values, const uint64_t* d_segment_offsets, uint64_t num_segments,

@@ -225,6 +225,35 @@ OSB200_API int osb200_sort_segments(osb200_handle h, const void* d_keys_in, void
                                     const uint64_t* d_segment_offsets, uint64_t num_segments, uint32_t max_segment_len,
                                     int key_bytes, int key_type, int descending, void* stream);
 
+/* Segments of any length: osb200_sort_segments with max_segment_len any uint32, the same arguments and the same semantics for
+ * every segment -- stable in both directions, uint32 positions within the segment, in place when d_keys_out == d_keys_in,
+ * natural alignment only.  Nothing outside segments is written; segments whose offsets decrease or pass n, and segments
+ * longer than max_segment_len, are not written.  Segments that overlap (offsets that go back) have no defined result, as in
+ * osb200_sort_segments; if overlapping long segments hold more tiles than the workspace bound below, the call leaves every
+ * long segment untouched and still returns OSB200_OK.  The argument errors of osb200_sort_segments come first, in the same
+ * order.
+ * max_segment_len <= 16,384 (8,192 for 8-byte keys): osb200_sort_segments' own launch, on any handle, with its workspace rule.
+ * Above that, segments longer than the limit take the long path, which uses the handle's workspace and allocates nothing.
+ * It needs:
+ *   - n <= max_n and num_segments <= min(max_n, 2^32), else OSB200_ERR_SIZE;
+ *   - a handle key width of at least key_bytes, else OSB200_ERR_INVALID_ARG;
+ *   - value_bytes == 4 when d_indices is given, else OSB200_ERR_INVALID_ARG;
+ *   - room in the handle's reductions for the tile counts of the worst case, segments of limit + 1 keys: 1 KiB per tile of
+ *     8,192 keys, ceil(n / 8,192) + floor(n / (limit + 1)) tiles, and the tile map.  The bound depends on n and key_bytes
+ *     only, never on the offsets, and a handle of the right shape with max_n >= max(n, num_segments) always has the room;
+ *     else OSB200_ERR_SIZE.
+ * The binning kernel of osb200_sort_segments lists the long segments apart; the shorter ones are sorted by its class kernels.
+ * A one-CTA kernel maps the long list to tiles of 8,192 keys that never straddle segments, and the long rows' passes
+ * (osb200_sort_long_rows) sort them, each tile finding its segment by a search over the map: a GlobalHistogram over all n
+ * keys decides which digit places are skipped (info "last_executed_passes" reads this call's plan), then per executed place a
+ * count, a scan of each segment's tile counts and a stable scatter, and a copy home within the long segments only.  The long
+ * path writes the handle's alternate key buffer and payloads, control block and compact reductions.  Asynchronous, no host
+ * synchronisation, graph-capturable; one call in flight per handle.  Option "debug_long_rows" = 1 (a test hook) sends
+ * segments of 2 .. 16,384 (8,192) keys to the long path too, with its workspace rules (bounded then by n / 2 segments). */
+OSB200_API int osb200_sort_long_segments(osb200_handle h, const void* d_keys_in, void* d_keys_out, uint32_t* d_indices, uint64_t n,
+                                         const uint64_t* d_segment_offsets, uint64_t num_segments, uint32_t max_segment_len,
+                                         int key_bytes, int key_type, int descending, void* stream);
+
 /* Row top-k: the k smallest (largest = 0) or largest (largest = 1) keys of every row and their positions, the shape of
  * torch.topk(x, k, dim=-1, largest, sorted).  Row r of d_keys_in is elements [r*row_len, (r+1)*row_len); its result is
  * [r*k, (r+1)*k) of d_values_out and d_indices (uint32 positions within the row, required).
@@ -355,7 +384,8 @@ OSB200_API int osb200_init_random_u32(uint32_t* d_keys, uint32_t* d_payload, uin
  *                    osb200_topk_rows honours it too: its rows of at most 256 keys are then radix-selected one per block
  *   "debug_long_rows"  test hook of osb200_sort_long_rows: 1 = rows of 2 .. 16,384 keys (8,192 for 8-byte keys) take the long
  *                    path too, with its workspace rules (short rows have a tile each, so many of them may need more room
- *                    than max_n gives: OSB200_ERR_SIZE), to compare it with osb200_sort_rows; 0 (default) = osb200_sort_rows' launch
+ *                    than max_n gives: OSB200_ERR_SIZE), to compare it with osb200_sort_rows; 0 (default) = osb200_sort_rows' launch.
+ *                    osb200_sort_long_segments honours it too: its segments of 2 .. 16,384 (8,192) keys then take the long path
  *   "debug_topk_capacity"  test hook of osb200_topk_rows: N > 0 keeps at most N candidates of a row in shared memory (instead
  *                    of 16,384, or 8,192 for 8-byte keys), so that short rows exercise the passes that read global memory
  *                    and the switch to shared memory; 0 (default) = the full capacity
