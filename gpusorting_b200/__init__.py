@@ -23,6 +23,7 @@ from .onesweep import (  # noqa: F401
     sort_rows,
     sort_segments,
     topk,
+    topk_long_rows,
     topk_segments,
 )
 

@@ -24,7 +24,7 @@
 
 namespace {
 
-constexpr int kVersion = 1011;  // 1002: device plan, bit ranges, forward-progress fallback, hot passes, segmented sort; 1003: argsort;
+constexpr int kVersion = 1012;  // 1002: device plan, bit ranges, forward-progress fallback, hot passes, segmented sort; 1003: argsort;
                                 // 1004: 16-bit keys (osb200_sort_keys16, osb200_sort_pairs16, osb200_argsort16);
                                 // 1005: row sort (osb200_sort_rows);
                                 // 1006: 64-bit keys with uint32 payloads and their argsort (osb200_create_pairs64);
@@ -32,7 +32,8 @@ constexpr int kVersion = 1011;  // 1002: device plan, bit ranges, forward-progre
                                 // 1008: row top-k (osb200_topk_rows);
                                 // 1009: segment top-k (osb200_topk_segments);
                                 // 1010: rows of any length (osb200_sort_long_rows);
-                                // 1011: segments of any length (osb200_sort_long_segments)
+                                // 1011: segments of any length (osb200_sort_long_segments);
+                                // 1012: row top-k of long rows and any k (osb200_topk_long_rows)
 constexpr int kMaxPlaces = 8;
 
 inline int cuda_status(cudaError_t e) { return e == cudaSuccess ? OSB200_OK : OSB200_ERR_CUDA - static_cast<int>(e); }
@@ -837,9 +838,11 @@ int osb200_sort_long_segments(osb200_handle h, const void* d_keys_in, void* d_ke
                               key_type, descending, stream, true);
 }
 
-// Row top-k: at most two launches, no workspace -- like the row sort, any handle will do.
-int osb200_topk_rows(osb200_handle h, const void* d_keys_in, void* d_values_out, uint32_t* d_indices, uint64_t num_rows,
-                     uint32_t row_len, uint32_t k, int key_bytes, int key_type, int largest, int sorted, void* stream)
+// Row top-k: at most two launches, no workspace -- like the row sort, any handle will do.  long_rows (osb200_topk_long_rows):
+// any k, and the split path for the calls of the path rule (the header), on the handle's alternate buffers, reductions and,
+// for the sort of k > C keys per row, control block.
+static int topk_rows_impl(osb200_sorter* h, const void* d_keys_in, void* d_values_out, uint32_t* d_indices, uint64_t num_rows,
+                          uint32_t row_len, uint32_t k, int key_bytes, int key_type, int largest, int sorted, void* stream, bool long_rows)
 {
     if (check_handle(h) != OSB200_OK) return OSB200_ERR_INVALID_ARG;
     osb::KeyCodec c;
@@ -856,11 +859,42 @@ int osb200_topk_rows(osb200_handle h, const void* d_keys_in, void* d_values_out,
                                {d_indices, ib, 4, true, true}};
     st = check_arrays(arrays, num_rows <= UINT64_MAX / row_len && n <= UINT64_MAX / 8, false);
     if (st != OSB200_OK) return st;
-    if (k > osb::row_sort_capacity(key_bytes)) return OSB200_ERR_SIZE;
-    OSB_TRY(osb::launch_topk_rows(d_keys_in, d_values_out, d_indices, num_rows, row_len, k, key_bytes, codec, sorted != 0,
-                                  h->debug_topk_capacity, h->cfg.rank_mode, h->debug_rows_block, h->sm_count,
-                                  static_cast<cudaStream_t>(stream)));
+    const uint32_t cap = osb::row_sort_capacity(key_bytes);
+    if (!long_rows && k > cap) return OSB200_ERR_SIZE;
+    // the path rule of the header: below 8 tiles per row one CTA per row was faster on the H100 (rows of 32,000 keys)
+    const bool split = long_rows && (h->debug_long_rows ? row_len >= 2
+                                                        : k > cap || (row_len > 8 * osb::kLongRowTile && num_rows < static_cast<uint64_t>(h->sm_count)));
+    cudaStream_t q = static_cast<cudaStream_t>(stream);
+    if (!split) {
+        OSB_TRY(osb::launch_topk_rows(d_keys_in, d_values_out, d_indices, num_rows, row_len, k, key_bytes, codec, sorted != 0,
+                                      h->debug_topk_capacity, h->cfg.rank_mode, h->debug_rows_block, h->sm_count, q));
+        return OSB200_OK;
+    }
+    // the split path's workspace: row state, totals and tile bases in the reductions, the tile counts and then the stopped
+    // rows' candidates in the alternate buffers; the sort of k > C keys per row takes the long rows' workspace over m keys
+    if (h->key_bytes < key_bytes || h->value_bytes != 4) return OSB200_ERR_INVALID_ARG;
+    const osb::TopkLongLayout l = osb::topk_long_layout(num_rows, row_len);
+    const bool long_sort = sorted && k > cap;
+    if (n > h->max_n || l.words * sizeof(uint32_t) > h->agg16_bytes || l.cnt_words > h->max_n ||
+        (long_sort && osb::long_rows_scratch_bytes(num_rows, k) > h->agg16_bytes))
+        return OSB200_ERR_SIZE;
+    if (long_sort) OSB_TRY(cudaMemsetAsync(h->control, 0, ControlLayout::zeroed_bytes, q));
+    OSB_TRY(osb::launch_topk_long_rows(d_keys_in, d_values_out, d_indices, h->alt_keys, h->alt_vals, num_rows, row_len, k, key_bytes,
+                                       codec, sorted != 0, h->debug_topk_capacity, h->cfg.rank_mode, h->short_circuit, h->ghist(),
+                                       h->gbase(), h->plan(), reinterpret_cast<uint32_t*>(h->agg16), h->sm_count, q));
     return OSB200_OK;
+}
+
+int osb200_topk_rows(osb200_handle h, const void* d_keys_in, void* d_values_out, uint32_t* d_indices, uint64_t num_rows,
+                     uint32_t row_len, uint32_t k, int key_bytes, int key_type, int largest, int sorted, void* stream)
+{
+    return topk_rows_impl(h, d_keys_in, d_values_out, d_indices, num_rows, row_len, k, key_bytes, key_type, largest, sorted, stream, false);
+}
+
+int osb200_topk_long_rows(osb200_handle h, const void* d_keys_in, void* d_values_out, uint32_t* d_indices, uint64_t num_rows,
+                          uint32_t row_len, uint32_t k, int key_bytes, int key_type, int largest, int sorted, void* stream)
+{
+    return topk_rows_impl(h, d_keys_in, d_values_out, d_indices, num_rows, row_len, k, key_bytes, key_type, largest, sorted, stream, true);
 }
 
 // Segment top-k: row top-k for ragged segments, with the workspace of check_segment_workspace.

@@ -3225,7 +3225,8 @@ struct LongRowsSmem {
     uint32_t wtot[kRadix / 32];
 };
 
-template <typename KeyT, int RANK_MODE, bool INDICES, typename Geo>
+// GIVEN (topk_long_sort_scatter_kernel): the first executed pass loads the indices given in idx_out instead of making them.
+template <typename KeyT, int RANK_MODE, bool INDICES, typename Geo, bool GIVEN = false>
 __device__ __forceinline__ void long_scatter_body(const Geo& geo, const SortPlan* __restrict__ plan, uint32_t place, const KeyT* keys_in,
                                                   KeyT* keys_out, KeyT* alt, uint32_t* idx_out, uint32_t* alt_idx,
                                                   const uint32_t* __restrict__ base, KeyCodec codec)
@@ -3266,7 +3267,7 @@ __device__ __forceinline__ void long_scatter_body(const Geo& geo, const SortPlan
             KeyT k = j < len ? src[row_lo + t0 + j] : static_cast<KeyT>(0);
             if (enc) k = codec_encode<KeyT>(k, ca, cb, cd);
             key[i] = j < len ? k : static_cast<KeyT>(~static_cast<KeyT>(0));
-            if constexpr (INDICES) val[i] = ps.first ? t0 + j : j < len ? src_idx[row_lo + t0 + j] : 0u;
+            if constexpr (INDICES) val[i] = ps.first && !GIVEN ? t0 + j : j < len ? src_idx[row_lo + t0 + j] : 0u;
         }
         // a warp's chunks of 32 keys that lie wholly behind the tile are neither counted nor ranked (as in segment_sort_body)
         const uint32_t live_chunks = len > warp_lo ? (len - warp_lo + 31) / 32 : 0u;
@@ -3342,6 +3343,33 @@ long_rows_copy_home_kernel(const SortPlan* __restrict__ plan, const KeyT* keys_i
     for (uint64_t i = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += stride) {
         if (keys) __stcs(keys_out + i, __ldcs(src + i));
         if (idx_out) __stcs(idx_out + i, ex ? __ldcs(alt_idx + i) : static_cast<uint32_t>(i % row_len));
+    }
+}
+
+
+// osb200_topk_long_rows' sort of k > C selected keys per row, in place: the long rows' passes with the positions as payloads
+template <typename KeyT, int RANK_MODE>
+__global__ void __launch_bounds__(kLongThreads, 1)
+topk_long_sort_scatter_kernel(const SortPlan* __restrict__ plan, uint32_t place, const KeyT* keys_in, KeyT* keys_out, KeyT* alt,
+                              uint32_t* idx_out, uint32_t* alt_idx, uint64_t num_rows, uint32_t row_len, uint32_t tpr,
+                              const uint32_t* __restrict__ base, KeyCodec codec)
+{
+    long_scatter_body<KeyT, RANK_MODE, true, LongRowGeo, true>(LongRowGeo{num_rows, row_len, tpr, 0, 0}, plan, place, keys_in, keys_out, alt,
+                                                               idx_out, alt_idx, base, codec);
+}
+
+// Its copy home: an odd number of executed passes moves keys and indices from the alternate buffers; after none the sort was
+// in place already, and the given indices stay.
+template <typename KeyT>
+__global__ void __launch_bounds__(512)
+topk_long_sort_copy_home_kernel(const SortPlan* __restrict__ plan, const KeyT* __restrict__ alt, KeyT* __restrict__ keys,
+                                const uint32_t* __restrict__ alt_idx, uint32_t* __restrict__ idx, uint64_t n)
+{
+    if (!(plan->executed & 1u)) return;
+    const uint64_t stride = static_cast<uint64_t>(gridDim.x) * blockDim.x;
+    for (uint64_t i = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += stride) {
+        __stcs(keys + i, __ldcs(alt + i));
+        __stcs(idx + i, __ldcs(alt_idx + i));
     }
 }
 
@@ -3427,9 +3455,9 @@ static cudaError_t launch_long_plan(const KeyT* in, uint64_t n, int key_bytes, c
 cudaError_t launch_long_rows(const void* keys_in, void* keys_out, uint32_t* indices, void* alt_keys, uint32_t* alt_idx,
                              uint64_t num_rows, uint32_t row_len, int key_bytes, const KeyCodec* codec_in, int rank_mode,
                              bool allow_skip, unsigned long long* ghist, unsigned long long* gbase, SortPlan* plan,
-                             uint32_t* scratch, int sm_count, cudaStream_t stream)
+                             uint32_t* scratch, int sm_count, cudaStream_t stream, bool given_indices)
 {
-    if (num_rows == 0 || row_len < 2) return cudaErrorInvalidValue;
+    if (num_rows == 0 || row_len < 2 || (given_indices && !indices)) return cudaErrorInvalidValue;
     const uint64_t n = num_rows * row_len;
     const uint32_t tpr = (row_len + kLongRowTile - 1) / kLongRowTile;
     const uint64_t row_counts = static_cast<uint64_t>(tpr) * kRadix;
@@ -3465,12 +3493,19 @@ cudaError_t launch_long_rows(const void* keys_in, void* keys_out, uint32_t* indi
                         num_rows * tpr, sm_count, stream, plan, p, in, out, alt, indices, alt_idx, num_rows, row_len, tpr,
                         static_cast<const uint32_t*>(cnt), codec);
                 };
+                if (given_indices)
+                    return launch_resident<topk_long_sort_scatter_kernel<KeyT, decltype(rm)::value>, kLongThreads, sizeof(LongRowsSmem<KeyT, true>)>(
+                        num_rows * tpr, sm_count, stream, plan, p, in, out, alt, indices, alt_idx, num_rows, row_len, tpr,
+                        static_cast<const uint32_t*>(cnt), codec);
                 return indices ? go(std::true_type{}) : go(std::false_type{});
             });
         }
         if (e != cudaSuccess) return e;
-        long_rows_copy_home_kernel<KeyT><<<capped_grid(n, 512, static_cast<uint64_t>(sm_count) * 4), 512, 0, stream>>>(
-            plan, in, alt, out, alt_idx, indices, n, row_len);
+        const unsigned home_grid = capped_grid(n, 512, static_cast<uint64_t>(sm_count) * 4);
+        if (given_indices)
+            topk_long_sort_copy_home_kernel<KeyT><<<home_grid, 512, 0, stream>>>(plan, alt, out, alt_idx, indices, n);
+        else
+            long_rows_copy_home_kernel<KeyT><<<home_grid, 512, 0, stream>>>(plan, in, alt, out, alt_idx, indices, n, row_len);
         return cudaGetLastError();
     });
 }
@@ -3597,6 +3632,12 @@ cudaError_t launch_long_segments(const void* keys_in, void* keys_out, uint32_t* 
 constexpr int kTopkWarps = 16, kTopkThreads = kTopkWarps * 32;
 constexpr int kTopkE = 8;  // keys per thread and chunk: a chunk is 4,096 keys, one block barrier
 
+// osb200_topk_long_rows' state of one row on the split path: the digits chosen so far, v under the mask m (encoded keys); the
+// keys selected so far, taken (those with (x & m) < v); the candidates, cand ((x & m) == v); the last chosen digit b.  All
+// zero is a row at level 0.
+constexpr uint32_t kTopkLongActive = 0, kTopkLongResolved = 1, kTopkLongStopped = 2;
+struct TopkLongRow { unsigned long long v, m; uint32_t taken, cand, b, status; };
+
 template <typename KeyT>
 struct TopkSmem {
     static constexpr uint32_t C = SegGeomN<KeyT, 2>::K * SegGeomN<KeyT, 2>::WARPS * 32;  // row_sort_capacity
@@ -3612,11 +3653,15 @@ struct TopkSmem {
 // back of `list` (entry i at list[num_rows - 1 - i], counts[kSegCountBlockList] of them), row s = [off[s], off[s + 1]) of
 // `in`, with k' = m = min(length, k) and its result at row s * k; columns m .. k - 1 are padding (the decoded all-ones key,
 // position 0xFFFFFFFF).  A segment of at most k keys starts with `last` set: one ordered pass selects all of it.
-template <typename KeyT, bool LIST>
+// FIN (osb200_topk_long_rows' finisher, topk_long_finish_kernel): only the rows the split path stopped (TopkLongRow) are
+// selected.  Row r's candidates are `in` + r * row_len (encoded keys, row order) and pos + r * row_len (their positions);
+// they are the row's first cand keys, of which the row still needs k - taken, written from column taken.
+template <typename KeyT, bool LIST, bool FIN = false>
 __device__ __forceinline__ void topk_select_body(const KeyT* __restrict__ in, KeyT* __restrict__ out, uint32_t* __restrict__ idx_out,
                                                  uint64_t num_rows, uint32_t row_len, uint32_t k, uint32_t cap, const KeyCodec& codec,
                                                  const unsigned long long* __restrict__ off, const uint32_t* __restrict__ list,
-                                                 const unsigned long long* __restrict__ counts)
+                                                 const unsigned long long* __restrict__ counts,
+                                                 const TopkLongRow* __restrict__ rows = nullptr, const uint32_t* __restrict__ pos = nullptr)
 {
     using S = TopkSmem<KeyT>;
     using U = std::conditional_t<sizeof(KeyT) == 8, uint64_t, uint32_t>;
@@ -3628,7 +3673,7 @@ __device__ __forceinline__ void topk_select_body(const KeyT* __restrict__ in, Ke
     const uint32_t lt = lanemask_lt();
     uint32_t* wh = sm.hist + warp * kRadix;
     const KeyT ca = static_cast<KeyT>(codec.a), cb = static_cast<KeyT>(codec.b), cd = static_cast<KeyT>(codec.d);
-    const bool enc = codec.flags & kCodecEncodeOnLoad, dec = codec.flags & kCodecDecodeOnStore;
+    const bool enc = !FIN && (codec.flags & kCodecEncodeOnLoad), dec = codec.flags & kCodecDecodeOnStore;
 
     const uint64_t work = LIST ? counts[kSegCountBlockList] : num_rows;
     if (LIST && work == 0) return;
@@ -3636,12 +3681,17 @@ __device__ __forceinline__ void topk_select_body(const KeyT* __restrict__ in, Ke
     __syncthreads();
     for (uint64_t it = blockIdx.x; it < work; it += gridDim.x) {
         const uint64_t row = LIST ? list[num_rows - 1 - it] : it;
+        TopkLongRow fin{};
+        if constexpr (FIN) {
+            fin = rows[row];
+            if (fin.status != kTopkLongStopped) continue;
+        }
         const uint64_t lo = LIST ? off[row] : row * row_len;
-        const uint32_t len = LIST ? static_cast<uint32_t>(off[row + 1] - lo) : row_len;  // (LIST: binned as 257 .. 2^32 - 1)
+        const uint32_t len = LIST ? static_cast<uint32_t>(off[row + 1] - lo) : FIN ? fin.cand : row_len;  // (LIST: binned as 257 .. 2^32 - 1)
         const KeyT* src = in + lo;
-        KeyT* dst = out + row * k;
-        uint32_t* dst_idx = idx_out + row * k;
-        const uint32_t m = LIST ? min(len, k) : k;
+        KeyT* dst = out + row * k + (FIN ? fin.taken : 0u);
+        uint32_t* dst_idx = idx_out + row * k + (FIN ? fin.taken : 0u);
+        const uint32_t m = LIST ? min(len, k) : FIN ? k - fin.taken : k;
         // S_{t-1} = {x : (x & mprev) == vprev}; selected this pass: x in S_{t-1} with (x & mcur) < vcur; S_t: (x & mcur) == vcur
         U mprev = 0, vprev = 0, mcur = 0, vcur = 0;
         uint32_t need = m, cand = len, written = 0, in_smem = 0;  // in_smem: 0, or the number of candidates held there
@@ -3664,7 +3714,8 @@ __device__ __forceinline__ void topk_select_body(const KeyT* __restrict__ in, Ke
                     if (valid) v = in_smem ? sm.keys[i] : src[i];
                     if (valid && !in_smem && enc) v = codec_encode<KeyT>(v, ca, cb, cd);
                     x[e] = static_cast<U>(v);
-                    p[e] = in_smem && valid ? sm.pos[i] : static_cast<uint32_t>(i);
+                    if constexpr (FIN) p[e] = valid ? (in_smem ? sm.pos[i] : pos[lo + i]) : 0u;
+                    else p[e] = in_smem && valid ? sm.pos[i] : static_cast<uint32_t>(i);
                     sel[e] = valid && (x[e] & mprev) == vprev && (x[e] & mcur) < vcur;
                     eq[e] = valid && (x[e] & mcur) == vcur;
                     if (!last && eq[e]) atomicAdd(&wh[static_cast<uint32_t>(x[e] >> shift) & 0xffu], 1u);
@@ -3902,6 +3953,28 @@ using TopkSortShapes = TypeList<TopkSortShape<uint16_t, 1>, TopkSortShape<uint16
                                 TopkSortShape<uint32_t, 2>, TopkSortShape<uint64_t, 1>, TopkSortShape<uint64_t, 2>>;
 using TopkKeys = TypeList<uint16_t, uint32_t, uint64_t>;
 
+// `sorted` for a [num_rows, k] result of at most C columns, in place with its positions as payloads: one warp per row for
+// k <= 32 K, else the row sort's block body.
+template <typename KeyT, int R>
+static cudaError_t sort_topk_result(KeyT* out, uint32_t* indices, uint64_t num_rows, uint32_t k, const KeyCodec& codec, int sm_count,
+                                    cudaStream_t stream)
+{
+    if (k <= kRowWarpMaxLen)
+        return with_warp_k(k, [&](auto kk) {
+            constexpr int K = decltype(kk)::value;
+            return launch_resident<topk_warp_kernel<KeyT, K, R>, kRowWarps * 32, kRowWarpSmemBytes<KeyT, K, true>>(
+                (num_rows + kRowWarps - 1) / kRowWarps, sm_count, stream, out, out, indices, indices, num_rows, k, k, codec);
+        });
+    return find_type(
+        TopkSortShapes{},
+        [&](auto s) { using Sh = decltype(s); return std::is_same_v<typename Sh::Key, KeyT> && k <= Sh::T; },
+        [&](auto s) {
+            using Sh = decltype(s);
+            return launch_resident<Sh::template kernel<R>(), Sh::S::THREADS, Sh::smem>(
+                num_rows, sm_count, stream, reinterpret_cast<typename Sh::Key*>(out), indices, num_rows, k, codec);
+        });
+}
+
 cudaError_t launch_topk_rows(const void* keys_in, void* values_out, uint32_t* indices, uint64_t num_rows, uint32_t row_len,
                              uint32_t k, int key_bytes, const KeyCodec* codec_in, bool sorted, uint32_t capacity, int rank_mode,
                              bool block_only, int sm_count, cudaStream_t stream)
@@ -3928,15 +4001,7 @@ cudaError_t launch_topk_rows(const void* keys_in, void* values_out, uint32_t* in
             const cudaError_t e = launch_resident<topk_select_kernel<KeyT>, kTopkThreads, sizeof(TopkSmem<KeyT>)>(
                 num_rows, sm_count, stream, in, out, indices, num_rows, row_len, k, cap, codec);
             if (e != cudaSuccess || !sorted || k == 1) return e;
-            if (k <= kRowWarpMaxLen) return warp_rows(out, indices, k);
-            return find_type(
-                TopkSortShapes{},
-                [&](auto s) { using Sh = decltype(s); return std::is_same_v<typename Sh::Key, KeyT> && k <= Sh::T; },
-                [&](auto s) {
-                    using Sh = decltype(s);
-                    return launch_resident<Sh::template kernel<R>(), Sh::S::THREADS, Sh::smem>(
-                        num_rows, sm_count, stream, static_cast<typename Sh::Key*>(values_out), indices, num_rows, k, codec);
-                });
+            return sort_topk_result<KeyT, R>(out, indices, num_rows, k, codec, sm_count, stream);
         });
     });
 }
@@ -3988,6 +4053,310 @@ cudaError_t launch_topk_segments(const void* keys_in, void* values_out, uint32_t
     });
 }
 
+// =====================================================================================================
+// Row top-k of long rows (osb200_topk_long_rows, DESIGN §4.18): the split path.  An MSD radix select per row over the long
+// rows' tiles (LongRowGeo: 8,192 keys, none straddling rows), every kernel grid-striding over all rows' tiles (or rows) on
+// the resident CTAs; no tile waits on another, and each kernel returns at once when it has no work.
+//   * level t = 0 .. D - 1: topk_long_count_kernel counts digit t of every tile's candidates of an active row into the
+//     tile's 256 counts (cnt) and adds them to the row's totals (tot); first it adds the tile's keys below the previous
+//     level's chosen digit to its selected count.  topk_long_pick_kernel picks per row the digit holding the need-th
+//     candidate, as topk_select_body does; the row is resolved when its candidates are exactly the keys it needs or after
+//     the last digit, stopped when they are at most cap.
+//   * topk_long_tiles_kernel: the last level's fold, and each tile's candidate count.
+//   * bases: the exclusive scan of each row's [selected of its tiles, candidates of its tiles] with the long rows' scan
+//     kernels (a zeroed SortPlan: no place skipped), so the candidates' bases come out offset by the row's selected total.
+//   * topk_long_compact_kernel: the ordered compaction of every tile, in row order -- selected keys to their columns, the
+//     first `need` candidates of a resolved row after them, every candidate of a stopped row (at most cap) with its
+//     position to the row's own range of the alternate buffers.
+//   * topk_long_finish_kernel: topk_select_body (FIN) over the stopped rows' candidates, one CTA per row.
+// =====================================================================================================
+template <typename KeyT>
+__global__ void __launch_bounds__(kLongThreads)
+topk_long_count_kernel(const KeyT* __restrict__ in, uint64_t num_rows, uint32_t row_len, uint32_t tpr, uint32_t k, uint32_t level,
+                       const TopkLongRow* __restrict__ rows, uint32_t* __restrict__ tot, uint32_t* cnt, uint32_t* __restrict__ sc,
+                       KeyCodec codec)
+{
+    if (k == row_len) return;  // every row is resolved before level 0
+    using U = std::conditional_t<sizeof(KeyT) == 8, uint64_t, uint32_t>;
+    const uint32_t shift = 8u * (static_cast<uint32_t>(sizeof(KeyT)) - 1u - level);
+    const KeyT ca = static_cast<KeyT>(codec.a), cb = static_cast<KeyT>(codec.b), cd = static_cast<KeyT>(codec.d);
+    const bool enc = codec.flags & kCodecEncodeOnLoad;
+    // bank-private columns, as in long_count_body
+    __shared__ uint32_t s_hist[kRadix * 32];
+    __shared__ uint32_t s_sel;
+    uint32_t* s_col = s_hist + (threadIdx.x & 31);
+    const LongRowGeo geo{num_rows, row_len, tpr, 0, 0};
+    const uint64_t tiles = geo.tiles();
+    for (uint64_t g = blockIdx.x; g < tiles; g += gridDim.x) {
+        const auto x = geo.tile(g);
+        const TopkLongRow st = rows[x.r];
+        if (st.status != kTopkLongActive) continue;
+        for (int i = threadIdx.x; i < kRadix * 32; i += kLongThreads) s_hist[i] = 0;
+        if (threadIdx.x == 0) s_sel = 0;
+        __syncthreads();
+        // the previous level's counts below its chosen digit are selected keys
+        if (level > 0 && threadIdx.x < st.b) atomicAdd(&s_sel, cnt[g * kRadix + threadIdx.x]);
+        const U m = static_cast<U>(st.m), v = static_cast<U>(st.v);
+        const KeyT* tile = in + x.lo + x.t0;
+        KeyT key[kLongK];
+#pragma unroll
+        for (int i = 0; i < kLongK; ++i) {
+            const uint32_t j = threadIdx.x + i * kLongThreads;
+            key[i] = j < x.len ? tile[j] : static_cast<KeyT>(0);
+        }
+#pragma unroll
+        for (int i = 0; i < kLongK; ++i) {
+            if (threadIdx.x + i * kLongThreads >= x.len) break;
+            const U e = static_cast<U>(enc ? codec_encode<KeyT>(key[i], ca, cb, cd) : key[i]);
+            if ((e & m) == v) atomicAdd(&s_col[digit_of(e, shift) * 32], 1u);
+        }
+        __syncthreads();
+        if (threadIdx.x < kRadix) {
+            uint32_t sum = 0;
+#pragma unroll 8
+            for (int c = 0; c < 32; ++c) sum += s_hist[threadIdx.x * 32 + ((c + threadIdx.x) & 31)];
+            cnt[g * kRadix + threadIdx.x] = sum;
+            if (sum) atomicAdd(&tot[x.r * kRadix + threadIdx.x], sum);
+        }
+        if (threadIdx.x == 0 && level > 0) sc[x.r * 2 * tpr + x.t] += s_sel;
+        __syncthreads();  // the fold has read s_hist
+    }
+}
+
+template <typename KeyT>
+__global__ void __launch_bounds__(kRadix)
+topk_long_pick_kernel(uint64_t num_rows, uint32_t row_len, uint32_t k, uint32_t level, uint32_t cap, TopkLongRow* __restrict__ rows,
+                      uint32_t* __restrict__ tot)
+{
+    if (k == row_len) return;
+    constexpr uint32_t D = sizeof(KeyT);
+    const uint32_t shift = 8u * (D - 1u - level);
+    __shared__ uint32_t s_wtot[kRadix / 32];
+    for (uint64_t r = blockIdx.x; r < num_rows; r += gridDim.x) {
+        const TopkLongRow st = rows[r];
+        if (st.status != kTopkLongActive) continue;
+        const uint32_t c = tot[r * kRadix + threadIdx.x];
+        tot[r * kRadix + threadIdx.x] = 0;  // for the next level
+        const uint32_t excl = block_excl_scan_256<kRadix>(c, s_wtot);
+        const uint32_t need = k - st.taken;
+        if (c && excl < need && need <= excl + c) {
+            TopkLongRow nx = st;
+            nx.v |= static_cast<unsigned long long>(threadIdx.x) << shift;
+            nx.m |= 0xffull << shift;
+            nx.taken += excl;
+            nx.cand = c;
+            nx.b = threadIdx.x;
+            nx.status = c == need - excl || level + 1 == D ? kTopkLongResolved : c <= cap ? kTopkLongStopped : kTopkLongActive;
+            rows[r] = nx;
+        }
+        __syncthreads();  // s_wtot is reused by the next row
+    }
+}
+
+// The last level's fold: each tile's selected count gains its keys below the row's last chosen digit, and its candidate
+// count is its count of that digit (k == row_len: no level ran, every key is a candidate).
+__global__ void __launch_bounds__(kRadix)
+topk_long_tiles_kernel(uint64_t num_rows, uint32_t row_len, uint32_t tpr, uint32_t k, const TopkLongRow* __restrict__ rows,
+                       const uint32_t* __restrict__ cnt, uint32_t* __restrict__ sc)
+{
+    __shared__ uint32_t s_sel;
+    const LongRowGeo geo{num_rows, row_len, tpr, 0, 0};
+    const uint64_t tiles = geo.tiles();
+    for (uint64_t g = blockIdx.x; g < tiles; g += gridDim.x) {
+        const auto x = geo.tile(g);
+        uint32_t* s = sc + x.r * 2 * tpr;
+        if (k == row_len) {
+            if (threadIdx.x == 0) { s[x.t] = 0; s[tpr + x.t] = x.len; }
+            continue;
+        }
+        const uint32_t b = rows[x.r].b;
+        if (threadIdx.x == 0) s_sel = 0;
+        __syncthreads();
+        const uint32_t c = cnt[g * kRadix + threadIdx.x];
+        if (threadIdx.x < b && c) atomicAdd(&s_sel, c);
+        if (threadIdx.x == b) s[tpr + x.t] = c;
+        __syncthreads();
+        if (threadIdx.x == 0) s[x.t] += s_sel;
+        __syncthreads();  // s_sel is reused by the next tile
+    }
+}
+
+// The ordered compaction of every tile (two chunks of 4,096 keys, each ranked by per-warp ballots and a scan of the
+// chunk's packed (e, warp) counts in row order, as in topk_select_body), from the tile's bases in sc.
+template <typename KeyT>
+__global__ void __launch_bounds__(kTopkThreads)
+topk_long_compact_kernel(const KeyT* __restrict__ in, KeyT* __restrict__ out, uint32_t* __restrict__ idx_out, uint64_t num_rows,
+                         uint32_t row_len, uint32_t tpr, uint32_t k, const TopkLongRow* __restrict__ rows,
+                         const uint32_t* __restrict__ sc, KeyT* __restrict__ buf, uint32_t* __restrict__ buf_pos, KeyCodec codec)
+{
+    using U = std::conditional_t<sizeof(KeyT) == 8, uint64_t, uint32_t>;
+    constexpr uint32_t CHUNK = kTopkE * kTopkThreads;
+    __shared__ uint32_t s_cnt[2][kTopkE * kTopkWarps];  // per chunk (double-buffered): selected | candidates << 16
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const uint32_t lt = lanemask_lt();
+    const KeyT ca = static_cast<KeyT>(codec.a), cb = static_cast<KeyT>(codec.b), cd = static_cast<KeyT>(codec.d);
+    const bool enc = codec.flags & kCodecEncodeOnLoad, dec = codec.flags & kCodecDecodeOnStore;
+    const LongRowGeo geo{num_rows, row_len, tpr, 0, 0};
+    const uint64_t tiles = geo.tiles();
+    uint32_t parity = 0;
+    for (uint64_t g = blockIdx.x; g < tiles; g += gridDim.x) {
+        const auto x = geo.tile(g);
+        TopkLongRow st{};
+        st.status = kTopkLongResolved;
+        if (k != row_len) st = rows[x.r];
+        const uint32_t* s = sc + x.r * 2 * tpr;
+        const uint32_t need = k - st.taken;
+        const bool stopped = st.status == kTopkLongStopped;
+        uint32_t sel_run = s[x.t], eq_run = s[tpr + x.t] - st.taken;
+        const U m = static_cast<U>(st.m), v = static_cast<U>(st.v);
+        const KeyT* src = in + x.lo + x.t0;
+        KeyT* dst = out + x.r * k;
+        uint32_t* dst_idx = idx_out + x.r * k;
+        for (uint32_t c0 = 0; c0 < x.len; c0 += CHUNK, parity ^= 1u) {
+            U xv[kTopkE];
+            bool sel[kTopkE], eq[kTopkE];
+#pragma unroll
+            for (int e = 0; e < kTopkE; ++e) {
+                const uint32_t i = c0 + static_cast<uint32_t>(e * kTopkThreads + tid);
+                const bool valid = i < x.len;
+                KeyT kv = valid ? src[i] : static_cast<KeyT>(0);
+                xv[e] = static_cast<U>(enc ? codec_encode<KeyT>(kv, ca, cb, cd) : kv);
+                sel[e] = valid && (xv[e] & m) < v;
+                eq[e] = valid && (xv[e] & m) == v;
+            }
+            uint32_t bsel[kTopkE], beq[kTopkE];
+            uint32_t* cnt = s_cnt[parity];
+#pragma unroll
+            for (int e = 0; e < kTopkE; ++e) {
+                bsel[e] = __ballot_sync(0xffffffffu, sel[e]);
+                beq[e] = __ballot_sync(0xffffffffu, eq[e]);
+                if (lane == 0) cnt[e * kTopkWarps + warp] = __popc(bsel[e]) | (__popc(beq[e]) << 16);
+            }
+            __syncthreads();
+            const uint4 c4 = reinterpret_cast<const uint4*>(cnt)[lane];
+            const uint32_t s4 = c4.x + c4.y + c4.z + c4.w;
+            uint32_t incl = s4;
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+                const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o);
+                if (lane >= o) incl += t;
+            }
+            const uint32_t total = __shfl_sync(0xffffffffu, incl, 31);
+            const uint32_t sub = warp & 3;
+            const uint32_t mine = incl - s4 + (sub > 0 ? c4.x : 0u) + (sub > 1 ? c4.y : 0u) + (sub > 2 ? c4.z : 0u);
+#pragma unroll
+            for (int e = 0; e < kTopkE; ++e) {
+                const uint32_t pre = __shfl_sync(0xffffffffu, mine, 4 * e + (warp >> 2));
+                const uint32_t p = x.t0 + c0 + static_cast<uint32_t>(e * kTopkThreads + tid);
+                if (sel[e] || (eq[e] && !stopped)) {
+                    const uint32_t s_before = sel_run + (pre & 0xffffu) + __popc(bsel[e] & lt);
+                    const uint32_t e_before = eq_run + (pre >> 16) + __popc(beq[e] & lt);
+                    if (sel[e] || e_before < need) {
+                        const uint32_t o = sel[e] ? s_before : st.taken + e_before;
+                        KeyT kv = static_cast<KeyT>(xv[e]);
+                        if (dec) kv = codec_decode<KeyT>(kv, ca, cb, cd);
+                        dst[o] = kv;
+                        dst_idx[o] = p;
+                    }
+                } else if (eq[e]) {
+                    const uint32_t e_before = eq_run + (pre >> 16) + __popc(beq[e] & lt);
+                    buf[x.lo + e_before] = static_cast<KeyT>(xv[e]);
+                    buf_pos[x.lo + e_before] = p;
+                }
+            }
+            sel_run += total & 0xffffu;
+            eq_run += total >> 16;
+        }
+    }
+}
+
+template <typename KeyT>
+__global__ void __launch_bounds__(kTopkThreads, 1)
+topk_long_finish_kernel(const KeyT* __restrict__ buf, KeyT* __restrict__ out, uint32_t* __restrict__ idx_out, uint64_t num_rows,
+                        uint32_t row_len, uint32_t k, uint32_t cap, KeyCodec codec, const TopkLongRow* __restrict__ rows,
+                        const uint32_t* __restrict__ buf_pos)
+{
+    topk_select_body<KeyT, false, true>(buf, out, idx_out, num_rows, row_len, k, cap, codec, nullptr, nullptr, nullptr, rows, buf_pos);
+}
+
+TopkLongLayout topk_long_layout(uint64_t num_rows, uint32_t row_len)
+{
+    static_assert(sizeof(SortPlan) <= 16 * sizeof(uint32_t) && sizeof(TopkLongRow) == 8 * sizeof(uint32_t), "the layout's words");
+    auto whole = [](uint64_t words) { return (words + 3) / 4 * 4; };
+    TopkLongLayout l;
+    l.tpr = static_cast<uint32_t>((static_cast<uint64_t>(row_len) + kLongRowTile - 1) / kLongRowTile);
+    l.cpr = static_cast<uint32_t>((2ull * l.tpr + kLongChunk - 1) / kLongChunk);
+    l.rows = 16;
+    l.tot = l.rows + num_rows * 8;
+    l.sc = l.tot + num_rows * kRadix;
+    l.zeroed = whole(l.sc + num_rows * 2 * l.tpr);
+    l.words = l.zeroed + (l.cpr > 1 ? whole(num_rows * l.cpr) : 0);
+    l.cnt_words = num_rows * l.tpr * kRadix;
+    return l;
+}
+
+cudaError_t launch_topk_long_rows(const void* keys_in, void* values_out, uint32_t* indices, void* alt_keys, uint32_t* alt_idx,
+                                  uint64_t num_rows, uint32_t row_len, uint32_t k, int key_bytes, const KeyCodec* codec_in, bool sorted,
+                                  uint32_t capacity, int rank_mode, bool allow_skip, unsigned long long* ghist, unsigned long long* gbase,
+                                  SortPlan* plan, uint32_t* scratch, int sm_count, cudaStream_t stream)
+{
+    if (num_rows == 0 || row_len < 2 || k == 0 || k > row_len) return cudaErrorInvalidValue;
+    const TopkLongLayout l = topk_long_layout(num_rows, row_len);
+    const uint32_t C = row_sort_capacity(key_bytes);
+    const uint32_t cap = capacity && capacity < C ? capacity : C;
+    const KeyCodec codec = codec_in ? *codec_in : KeyCodec();
+    cudaError_t e = cudaMemsetAsync(scratch, 0, l.zeroed * sizeof(uint32_t), stream);
+    if (e != cudaSuccess) return e;
+    const SortPlan* none_skipped = reinterpret_cast<const SortPlan*>(scratch);
+    TopkLongRow* rows = reinterpret_cast<TopkLongRow*>(scratch + l.rows);
+    uint32_t* tot = scratch + l.tot;
+    uint32_t* sc = scratch + l.sc;
+    uint32_t* csum = l.cpr > 1 ? scratch + l.zeroed : nullptr;
+    uint32_t* cnt = alt_idx;  // free until the compaction writes the candidates' positions there
+    const uint64_t tiles = num_rows * l.tpr;
+    return with_key_type(TopkKeys{}, key_bytes, [&](auto kt) {
+        using KeyT = decltype(kt);
+        const KeyT* in = static_cast<const KeyT*>(keys_in);
+        KeyT* out = static_cast<KeyT*>(values_out);
+        KeyT* buf = static_cast<KeyT*>(alt_keys);
+        cudaError_t le = cudaSuccess;
+        for (uint32_t t = 0; le == cudaSuccess && t < sizeof(KeyT); ++t) {
+            le = launch_resident<topk_long_count_kernel<KeyT>, kLongThreads, 0>(tiles, sm_count, stream, in, num_rows, row_len, l.tpr, k, t,
+                                                                                static_cast<const TopkLongRow*>(rows), tot, cnt, sc, codec);
+            if (le == cudaSuccess)
+                le = launch_resident<topk_long_pick_kernel<KeyT>, kRadix, 0>(num_rows, sm_count, stream, num_rows, row_len, k, t, cap, rows, tot);
+        }
+        if (le == cudaSuccess)
+            le = launch_resident<topk_long_tiles_kernel, kRadix, 0>(tiles, sm_count, stream, num_rows, row_len, l.tpr, k,
+                                                                    static_cast<const TopkLongRow*>(rows), static_cast<const uint32_t*>(cnt), sc);
+        if (le != cudaSuccess) return le;
+        // the bases: per row, the exclusive scan of its 2 tpr counts [selected of each tile, candidates of each tile]
+        const uint64_t row_counts = 2ull * l.tpr;
+        const unsigned scan_grid = capped_grid(num_rows * l.cpr, 1, static_cast<uint64_t>(sm_count) * 4);
+        if (csum) {
+            long_rows_chunk_sum_kernel<<<scan_grid, kLongThreads, 0, stream>>>(none_skipped, 0, sc, csum, num_rows, row_counts, l.cpr);
+            long_rows_chunk_scan_kernel<<<capped_grid(num_rows, 1, static_cast<uint64_t>(sm_count) * 4), kLongThreads, 0, stream>>>(
+                none_skipped, 0, csum, num_rows, l.cpr);
+        }
+        long_rows_scan_kernel<<<scan_grid, kLongThreads, 0, stream>>>(none_skipped, 0, sc, csum, num_rows, row_counts, l.cpr);
+        if ((le = cudaGetLastError()) != cudaSuccess) return le;
+        le = launch_resident<topk_long_compact_kernel<KeyT>, kTopkThreads, 0>(tiles, sm_count, stream, in, out, indices, num_rows, row_len,
+                                                                             l.tpr, k, static_cast<const TopkLongRow*>(rows),
+                                                                             static_cast<const uint32_t*>(sc), buf, alt_idx, codec);
+        if (le == cudaSuccess)
+            le = launch_resident<topk_long_finish_kernel<KeyT>, kTopkThreads, sizeof(TopkSmem<KeyT>)>(
+                num_rows, sm_count, stream, static_cast<const KeyT*>(buf), out, indices, num_rows, row_len, k, cap, codec,
+                static_cast<const TopkLongRow*>(rows), static_cast<const uint32_t*>(alt_idx));
+        if (le != cudaSuccess || !sorted || k == 1) return le;
+        if (k <= C)
+            return with_rank_mode(rank_mode, [&](auto r) { return sort_topk_result<KeyT, decltype(r)::value>(out, indices, num_rows, k, codec, sm_count, stream); });
+        // k > C: the long rows' passes over the [num_rows, k] result, in place, loading the positions as payloads (the
+        // control block's histogram was cleared by the caller)
+        return launch_long_rows(out, out, indices, alt_keys, alt_idx, num_rows, k, key_bytes, codec_in, rank_mode, allow_skip, ghist, gbase,
+                                plan, scratch, sm_count, stream, true);
+    });
+}
+
 cudaError_t configure_kernels()
 {
     cudaError_t e = for_each_type(HistKeys{}, [](auto k) {
@@ -4032,6 +4401,12 @@ cudaError_t configure_kernels()
         if (m == cudaSuccess) m = set_smem(long_segments_scatter_kernel<KeyT, kRankBallot, false>, sizeof(LongRowsSmem<KeyT, false>));
         if (m == cudaSuccess) m = set_smem(long_segments_scatter_kernel<KeyT, kRankAtomic, true>, sizeof(LongRowsSmem<KeyT, true>));
         return m != cudaSuccess ? m : set_smem(long_segments_scatter_kernel<KeyT, kRankBallot, true>, sizeof(LongRowsSmem<KeyT, true>));
+    });
+    if (e == cudaSuccess) e = for_each_type(TopkKeys{}, [](auto k) {
+        using KeyT = decltype(k);
+        cudaError_t m = set_smem(topk_long_finish_kernel<KeyT>, sizeof(TopkSmem<KeyT>));
+        if (m == cudaSuccess) m = set_smem(topk_long_sort_scatter_kernel<KeyT, kRankAtomic>, sizeof(LongRowsSmem<KeyT, true>));
+        return m != cudaSuccess ? m : set_smem(topk_long_sort_scatter_kernel<KeyT, kRankBallot>, sizeof(LongRowsSmem<KeyT, true>));
     });
     return e;
 }

@@ -136,13 +136,14 @@ cudaError_t launch_row_sort(const void* keys_in, void* keys_out, uint32_t* indic
 // row_len keys into ghist (zeroed by the caller), the scan that writes `plan` (gbase is written too, and not used), per digit
 // place a count, a scan of each row's tile counts and a scatter, then the copy home.  alt_keys: n keys of key_bytes;
 // alt_idx: n u32 when indices is not null; scratch: long_rows_scratch_bytes(num_rows, row_len) bytes, 16-byte aligned, which
-// the call overwrites before it reads them.  The codec as for launch_row_sort.
+// the call overwrites before it reads them.  The codec as for launch_row_sort.  given_indices (osb200_topk_long_rows' sort, in
+// place): the first pass loads the payloads in indices instead of making positions, and when no pass executes they stay.
 constexpr uint32_t kLongRowTile = 8192;
 uint64_t long_rows_scratch_bytes(uint64_t num_rows, uint32_t row_len);
 cudaError_t launch_long_rows(const void* keys_in, void* keys_out, uint32_t* indices, void* alt_keys, uint32_t* alt_idx,
                              uint64_t num_rows, uint32_t row_len, int key_bytes, const KeyCodec* codec, int rank_mode,
                              bool allow_skip, unsigned long long* ghist, unsigned long long* gbase, SortPlan* plan,
-                             uint32_t* scratch, int sm_count, cudaStream_t stream);
+                             uint32_t* scratch, int sm_count, cudaStream_t stream, bool given_indices = false);
 
 // Long segments (osb200_sort_long_segments): launch_sort_segments for segments of 2 to long_min - 1 keys, and the long
 // rows' passes for segments of long_min to max_len keys (long_min >= 2), whose tiles of kLongRowTile keys never straddle
@@ -197,6 +198,20 @@ cudaError_t launch_topk_segments(const void* keys_in, void* values_out, uint32_t
                                  uint64_t num_segments, uint32_t k, int key_bytes, const KeyCodec* codec, bool sorted,
                                  uint32_t capacity, int rank_mode, bool block_only, int sm_count, uint32_t* list,
                                  unsigned long long* counts, cudaStream_t stream);
+
+// Row top-k of long rows, the split path of osb200_topk_long_rows: launch_topk_rows' results for any k in 1 .. row_len and
+// row_len >= 2, each row's tiles of kLongRowTile keys spread over the GPU (an MSD radix select per row, DESIGN §4.18).  Rows
+// whose candidates fall to `capacity` or fewer (0: row_sort_capacity(key_bytes)) are finished one per CTA in shared memory.
+// Workspace: scratch, topk_long_layout(num_rows, row_len).words u32 (16-byte aligned; its first `zeroed` words are cleared
+// here) and, when sorted and k > row_sort_capacity(key_bytes), at least long_rows_scratch_bytes(num_rows, k) bytes; alt_keys:
+// n keys of key_bytes; alt_idx: n u32, at least cnt_words of them.  sorted with k > row_sort_capacity(key_bytes) runs
+// launch_long_rows on the result, which needs ghist zeroed by the caller.  The codec as for launch_row_sort.
+struct TopkLongLayout { uint64_t rows, tot, sc, zeroed, words, cnt_words; uint32_t tpr, cpr; };  // offsets in u32 words
+TopkLongLayout topk_long_layout(uint64_t num_rows, uint32_t row_len);
+cudaError_t launch_topk_long_rows(const void* keys_in, void* values_out, uint32_t* indices, void* alt_keys, uint32_t* alt_idx,
+                                  uint64_t num_rows, uint32_t row_len, uint32_t k, int key_bytes, const KeyCodec* codec, bool sorted,
+                                  uint32_t capacity, int rank_mode, bool allow_skip, unsigned long long* ghist, unsigned long long* gbase,
+                                  SortPlan* plan, uint32_t* scratch, int sm_count, cudaStream_t stream);
 
 // Validate (reference: Validate, UtilityKernels.cuh:403-429): err_count += #(keys[i] > keys[i+1]).
 cudaError_t launch_validate(const void* keys, uint64_t n, int key_bytes, unsigned long long* err_count, int sm_count,

@@ -282,6 +282,22 @@ class OneSweepSorter:
                    1 if largest else 0, 1 if sorted else 0, stream=stream)
         return out, idx
 
+    def topk_long_rows(self, x: torch.Tensor, k: int, key_type: str, largest: bool = True, sorted: bool = True, stream=None):
+        """topk_rows for any k up to the row length and rows of any length (osb200_topk_long_rows): the same arguments, shapes
+        and results.  k above 16,384 (8,192 for 8-byte dtypes), and fewer rows than the GPU has SMs of more than 65,536 keys,
+        split their rows across thread blocks on this sorter's workspace; every other call is topk_rows' own launch on any
+        sorter.  The split path needs: x.numel() may be at most max_n, the sorter's key_bytes must be at least x's element size and its
+        value_bytes 4 -- a (4, 4) sorter for 2- and 4-byte dtypes, a (8, 4) one for any."""
+        kb, kt = self._ragged_keys(x, key_type)
+        k = int(k)
+        row_len = x.shape[-1]
+        num_rows = x.numel() // row_len if row_len else 0
+        shape = tuple(x.shape[:-1]) + (k,)
+        out, idx = _new_outputs(stream, x, shape)
+        self._call(lib.osb200_topk_long_rows, x.data_ptr(), out.data_ptr(), idx.data_ptr(), num_rows, row_len, k, kb, kt,
+                   1 if largest else 0, 1 if sorted else 0, stream=stream)
+        return out, idx
+
     # -- segment sort: ragged rows given by offsets -------------------------------------------------------------------------
     def sort_segments(self, x: torch.Tensor, offsets: torch.Tensor, key_type: str, descending: bool = False,
                       return_indices: bool = True, inplace: bool = False, max_segment_len: Optional[int] = None, stream=None):
@@ -542,6 +558,8 @@ def sort_rows(x: torch.Tensor, descending: bool = False, return_indices: bool = 
 
 # the longest row sort_rows takes, by element size: sort_long_rows needs a sorter's workspace only above it
 _ROW_CAPACITY = {2: 16384, 4: 16384, 8: 8192}
+# the long paths' tile: topk_long_rows splits only longer rows across thread blocks
+_LONG_ROW_TILE = 8192
 
 
 def sort_long_rows(x: torch.Tensor, descending: bool = False, return_indices: bool = True, stream=None):
@@ -565,6 +583,21 @@ def topk(x: torch.Tensor, k: int, largest: bool = True, sorted: bool = True, str
     (the top-k needs no workspace)."""
     s = _module_sorter(x, "x", 4, 1, stream, _ROW_KEY_TYPES)
     return s.topk_rows(x, k, _ROW_KEY_TYPES[x.dtype], largest, sorted, stream)
+
+
+def topk_long_rows(x: torch.Tensor, k: int, largest: bool = True, sorted: bool = True, stream=None):
+    """topk for any k up to the row length and rows of any length: ``torch.topk(x, k, dim=-1, largest, sorted)`` for a
+    contiguous CUDA tensor of one of sort_rows' ten dtypes, returning (values, int32 positions within the row), ties taken in
+    input order.  Rows longer than 8,192 keys run on the stream's cached (4, 4) sorter, the one argsort uses, or its (8, 4)
+    sorter for 8-byte dtypes, grown to x.numel(); shorter rows (which never take the split path) on the (4, 4) one as in
+    topk."""
+    kb = x.element_size() if isinstance(x, torch.Tensor) else 4
+    row_len = x.shape[-1] if isinstance(x, torch.Tensor) and x.dim() else 0
+    if row_len > _LONG_ROW_TILE:
+        s = _module_sorter(x, "x", 8 if kb == 8 else 4, x.numel(), stream, _ROW_KEY_TYPES)
+    else:
+        s = _module_sorter(x, "x", 4, 1, stream, _ROW_KEY_TYPES)
+    return s.topk_long_rows(x, k, _ROW_KEY_TYPES[x.dtype], largest, sorted, stream)
 
 
 def sort_segments(x: torch.Tensor, offsets: torch.Tensor, descending: bool = False, return_indices: bool = True,

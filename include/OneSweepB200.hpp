@@ -101,6 +101,16 @@ class OneSweepSorterB200 {
                                sorted ? 1 : 0, stream),
               "osb200_topk_rows");
     }
+    // TopkRows for any k <= row_len and rows of any length: k above TopkRows' limit, or fewer rows than SMs of more than 65,536
+    // keys, are split across thread blocks on this handle's workspace (num_rows * row_len <= max_n, a key width of at least
+    // key_bytes, value_bytes 4)
+    void TopkLongRows(const void* d_keys_in, void* d_values_out, uint32_t* d_indices, uint64_t num_rows, uint32_t row_len, uint32_t k,
+                      int key_bytes, int key_type, bool largest, bool sorted, void* stream = nullptr)
+    {
+        check(osb200_topk_long_rows(h_, d_keys_in, d_values_out, d_indices, num_rows, row_len, k, key_bytes, key_type,
+                                    largest ? 1 : 0, sorted ? 1 : 0, stream),
+              "osb200_topk_long_rows");
+    }
     // the first m = min(length, k) keys of every segment [offsets[s], offsets[s+1]) in its stable sort (ascending, or descending
     // for largest) and their positions within the segment, into row s of [num_segments, k] outputs; columns m .. k-1 are
     // padding (position 0xFFFFFFFF, the key that sorts last); segments whose offsets decrease or pass n are all padding;

@@ -305,6 +305,35 @@ OSB200_API int osb200_topk_segments(osb200_handle h, const void* d_keys_in, void
                                     const uint64_t* d_segment_offsets, uint64_t num_segments, uint32_t k, int key_bytes,
                                     int key_type, int largest, int sorted, void* stream);
 
+/* Row top-k of long rows and any k: osb200_topk_rows with the same arguments, the same argument errors (in the same order) and
+ * the same results, bit for bit, wherever that call accepts them -- the first k columns of the row's stable sort, ties at the
+ * lowest positions, uint32 positions within the row; sorted = 0 writes the same pairs in an unspecified order.  It also takes
+ * any k with 1 <= k <= row_len and rows of up to 2^32 - 1 keys.
+ * Path rule, with C = 16,384 (8,192 for 8-byte keys), T = 8,192 and S the device's SM count:
+ *   - the split path, which spreads each row's tiles of T keys over the GPU, when k > C, or when row_len > 8 T (65,536 keys)
+ *     and num_rows < S (some SM would have no row);
+ *   - every other call: osb200_topk_rows' own launch, on any handle and with no workspace.  (Measured on an H100: with one
+ *     CTA per SM busy, or rows of 32,000 keys, that launch is the faster one.)
+ * The split path uses the handle's workspace and allocates nothing.  It needs:
+ *   - a handle key width of at least key_bytes and value_bytes == 4 -- a (4, 4) handle for 2- and 4-byte keys, a (8, 4) one
+ *     for any -- else OSB200_ERR_INVALID_ARG;
+ *   - num_rows * row_len <= max_n, else OSB200_ERR_SIZE;
+ *   - room in the reductions for 1 KiB + 32 B per row and 8 B per tile, and in the alternate payloads for 1 KiB per tile; a
+ *     handle of that shape with max_n >= num_rows * row_len always has it outside the test hook; else OSB200_ERR_SIZE, checked
+ *     before anything is enqueued.  The bound depends on num_rows, row_len and key_bytes only.
+ * It writes the handle's alternate keys and payloads, its compact reductions and (sorted = 1 with k > C) its control block.
+ * It is an MSD radix select per row over tiles that never straddle rows: per digit place a count of every tile's candidates
+ * and a pick of each row's digit, until a row's candidates are exactly the keys it needs or at most C of them are left; a
+ * scan of the tiles' counts, one ordered compaction of the keys in row order, then the stopped rows' candidates finished one
+ * per thread block in shared memory.  sorted = 1 then sorts the [num_rows, k] result in place (for k > C with the passes of
+ * osb200_sort_long_rows).  No tile waits on another.  One memset (two with k > C and sorted) and a fixed sequence of launches:
+ * asynchronous, no host synchronisation, graph-capturable; one call in flight per handle.  The test hooks
+ * "debug_topk_capacity" (the candidate count at which a row stops) and "debug_long_rows" (every row of 2 or more keys takes
+ * the split path, with its workspace rules) apply. */
+OSB200_API int osb200_topk_long_rows(osb200_handle h, const void* d_keys_in, void* d_values_out, uint32_t* d_indices,
+                                     uint64_t num_rows, uint32_t row_len, uint32_t k, int key_bytes, int key_type,
+                                     int largest, int sorted, void* stream);
+
 /* Sort on a bit range [begin_bit, end_bit) of the (unsigned) key only, CUB-style: keys that agree on those bits keep their
  * input order (stable).  ceil((end_bit-begin_bit)/8) digit passes instead of key_bytes; the last digit may be narrower
  * than 8 bits; an odd pass count is handled inside (the result is always returned in the caller's buffers).  d_values may
@@ -385,10 +414,12 @@ OSB200_API int osb200_init_random_u32(uint32_t* d_keys, uint32_t* d_payload, uin
  *   "debug_long_rows"  test hook of osb200_sort_long_rows: 1 = rows of 2 .. 16,384 keys (8,192 for 8-byte keys) take the long
  *                    path too, with its workspace rules (short rows have a tile each, so many of them may need more room
  *                    than max_n gives: OSB200_ERR_SIZE), to compare it with osb200_sort_rows; 0 (default) = osb200_sort_rows' launch.
- *                    osb200_sort_long_segments honours it too: its segments of 2 .. 16,384 (8,192) keys then take the long path
+ *                    osb200_sort_long_segments honours it too: its segments of 2 .. 16,384 (8,192) keys then take the long path,
+ *                    and osb200_topk_long_rows: its rows of 2 or more keys then take the split path
  *   "debug_topk_capacity"  test hook of osb200_topk_rows: N > 0 keeps at most N candidates of a row in shared memory (instead
  *                    of 16,384, or 8,192 for 8-byte keys), so that short rows exercise the passes that read global memory
- *                    and the switch to shared memory; 0 (default) = the full capacity
+ *                    and the switch to shared memory; 0 (default) = the full capacity.  osb200_topk_long_rows' split path
+ *                    stops a row at N candidates
  *   "debug_epoch"    test hook of the descriptor epochs: sets the handle's epoch counter (0 .. 2^24 - 1; info "epoch"), so
  *                    that the next passes cross the wrap-around (which clears every descriptor) or reuse the epochs of a
  *                    captured sort
