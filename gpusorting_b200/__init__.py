@@ -17,7 +17,12 @@ from .onesweep import (  # noqa: F401
     argsort,
     argsort16,
     init_random,
+    kthvalue,
+    median,
+    quantile,
     release_cached_sorters,
+    select_rows,
+    select_workspace_words,
     sort_long_rows,
     sort_long_segments,
     sort_rows,

@@ -24,7 +24,7 @@
 
 namespace {
 
-constexpr int kVersion = 1012;  // 1002: device plan, bit ranges, forward-progress fallback, hot passes, segmented sort; 1003: argsort;
+constexpr int kVersion = 1013;  // 1002: device plan, bit ranges, forward-progress fallback, hot passes, segmented sort; 1003: argsort;
                                 // 1004: 16-bit keys (osb200_sort_keys16, osb200_sort_pairs16, osb200_argsort16);
                                 // 1005: row sort (osb200_sort_rows);
                                 // 1006: 64-bit keys with uint32 payloads and their argsort (osb200_create_pairs64);
@@ -33,7 +33,8 @@ constexpr int kVersion = 1012;  // 1002: device plan, bit ranges, forward-progre
                                 // 1009: segment top-k (osb200_topk_segments);
                                 // 1010: rows of any length (osb200_sort_long_rows);
                                 // 1011: segments of any length (osb200_sort_long_segments);
-                                // 1012: row top-k of long rows and any k (osb200_topk_long_rows)
+                                // 1012: row top-k of long rows and any k (osb200_topk_long_rows);
+                                // 1013: row select at given ranks (osb200_select_rows)
 constexpr int kMaxPlaces = 8;
 
 inline int cuda_status(cudaError_t e) { return e == cudaSuccess ? OSB200_OK : OSB200_ERR_CUDA - static_cast<int>(e); }
@@ -895,6 +896,55 @@ int osb200_topk_long_rows(osb200_handle h, const void* d_keys_in, void* d_values
                           uint32_t row_len, uint32_t k, int key_bytes, int key_type, int largest, int sorted, void* stream)
 {
     return topk_rows_impl(h, d_keys_in, d_values_out, d_indices, num_rows, row_len, k, key_bytes, key_type, largest, sorted, stream, true);
+}
+
+// Row select: the checks of the row top-k, then the rank list; rows of at most row_sort_capacity keys take the row sort's
+// kernels on any handle, longer ones (and with the test hook debug_long_rows every row of two or more keys) the split path,
+// whose workspace -- select_layout(...).words u32 -- lives in the handle's alternate keys.
+int osb200_select_rows(osb200_handle h, const void* d_keys_in, void* d_values_out, uint32_t* d_indices, uint64_t num_rows,
+                       uint32_t row_len, const uint32_t* h_ranks, uint32_t num_ranks, int key_bytes, int key_type, void* stream)
+{
+    if (check_handle(h) != OSB200_OK) return OSB200_ERR_INVALID_ARG;
+    osb::KeyCodec c;
+    const osb::KeyCodec* codec = nullptr;
+    int st = codec_for(key_bytes, key_type, 0, kRaggedCodecFlags, &c, &codec);
+    if (st != OSB200_OK) return st;
+    if (num_rows == 0) return OSB200_OK;
+    const uint64_t n = num_rows * row_len, m = num_rows * num_ranks;
+    const uint64_t kb = n * static_cast<uint64_t>(key_bytes), ob = m * static_cast<uint64_t>(key_bytes), ib = m * sizeof(uint32_t);
+    // the outputs have another shape than the input: no in-place form
+    const ArrayArg arrays[] = {{d_keys_in, kb, key_bytes, true, false}, {d_values_out, ob, key_bytes, true, true},
+                               {d_indices, ib, 4, false, true}};
+    st = check_arrays(arrays, (row_len == 0 || num_rows <= UINT64_MAX / row_len) && n <= UINT64_MAX / 8 &&
+                                  (num_ranks == 0 || num_rows <= UINT64_MAX / 8 / num_ranks), false);
+    if (st != OSB200_OK) return st;
+    // the rank list: 1 .. 16 ranks, strictly increasing, each below row_len
+    if (!h_ranks || num_ranks == 0 || num_ranks > osb::kMaxSelectRanks) return OSB200_ERR_INVALID_ARG;
+    osb::SelectRanks ranks{};
+    ranks.count = num_ranks;
+    for (uint32_t i = 0; i < num_ranks; ++i) {
+        if (h_ranks[i] >= row_len || (i > 0 && h_ranks[i] <= h_ranks[i - 1])) return OSB200_ERR_INVALID_ARG;
+        ranks.r[i] = h_ranks[i];
+    }
+    cudaStream_t q = static_cast<cudaStream_t>(stream);
+    if (row_len == 1) {  // (rank 0 of every row)
+        OSB_TRY(cudaMemcpyAsync(d_values_out, d_keys_in, kb, cudaMemcpyDeviceToDevice, q));
+        if (d_indices) OSB_TRY(cudaMemsetAsync(d_indices, 0, ib, q));
+        return OSB200_OK;
+    }
+    const bool split = h->debug_long_rows || row_len > osb::row_sort_capacity(key_bytes);
+    if (!split) {
+        OSB_TRY(osb::launch_select_rows(d_keys_in, d_values_out, d_indices, num_rows, row_len, ranks, key_bytes, codec, h->cfg.rank_mode,
+                                        h->debug_rows_block, h->sm_count, q));
+        return OSB200_OK;
+    }
+    // the split path's bound (the header): a handle with max_n >= n always meets it for rows longer than row_sort_capacity
+    const uint64_t alt_words = h->alt_key_slots * static_cast<uint64_t>(h->key_bytes) / sizeof(uint32_t);
+    if (num_rows > alt_words || osb::select_layout(num_rows, row_len, num_ranks, d_indices != nullptr).words > alt_words)
+        return OSB200_ERR_SIZE;
+    OSB_TRY(osb::launch_select_long_rows(d_keys_in, d_values_out, d_indices, num_rows, row_len, ranks, key_bytes, codec,
+                                         static_cast<uint32_t*>(h->alt_keys), h->sm_count, q));
+    return OSB200_OK;
 }
 
 // Segment top-k: row top-k for ragged segments, with the workspace of check_segment_workspace.

@@ -2267,6 +2267,15 @@ struct SegSmem {
     uint32_t wtot[kRadix / 32];
 };
 
+// ranks.r[i] (0 for i >= kMaxSelectRanks), read with constant indices only, so the ranks stay in the launch parameters
+__device__ __forceinline__ uint32_t select_rank_of(const SelectRanks& ranks, uint32_t i)
+{
+    uint32_t r = 0;
+#pragma unroll
+    for (uint32_t j = 0; j < kMaxSelectRanks; ++j) r = i == j ? ranks.r[j] : r;
+    return r;
+}
+
 // osb200_sort_segments' class counts (see segment_bin_kernel)
 enum SegCount : int { kSegCountWarp = 0, kSegCountBlock1 = 1, kSegCountBlock2 = 2, kSegCountBlockList = 3, kSegCounts = 4 };
 // osb200_sort_long_segments' counts after them: the long list's length, then its tiles and scan chunks (see launch_long_segments)
@@ -2286,17 +2295,21 @@ enum LongSegCount : int { kSegCountLong = 4, kSegCountLongTiles = 5, kSegCountLo
 // [seg_off[s], seg_off[s + 1]) is one the radix select wrote: inside [0, sel_n), longer than sel_min and shorter than 2^32
 // keys (the binning kernel's test).  (Not its block list: with the list and its device-side count the 16,384-key
 // instantiations spill; the row count is a kernel parameter, as for ROWS.)
+// COLS (with ROWS; osb200_select_rows, select_rows_block_kernel): only the sorted row's columns ranks->r[0 .. count - 1] are
+// stored, to [s * count, (s + 1) * count) of keys and vals.
 // max_len: the caller's max_segment_len (<= T); longer segments are left as they are.
-template <typename KeyT, bool PAIRS, int K, int WARPS, int RANK_MODE, bool INDICES, bool ROWS, bool LIST, bool ROW_SEL = false>
+template <typename KeyT, bool PAIRS, int K, int WARPS, int RANK_MODE, bool INDICES, bool ROWS, bool LIST, bool ROW_SEL = false,
+          bool COLS = false>
 __device__ __forceinline__ void segment_sort_body(KeyT* keys, uint32_t* vals, const unsigned long long* __restrict__ seg_off,
                                                   uint64_t num_segments, uint64_t single_n, uint32_t max_len, uint32_t begin_bit,
                                                   uint32_t places, uint32_t last_bits, const KeyCodec& codec,
                                                   const KeyT* __restrict__ keys_in, const uint32_t* __restrict__ seg_list,
                                                   const unsigned long long* __restrict__ seg_counts, uint64_t sel_n = 0,
-                                                  uint32_t sel_min = 0)
+                                                  uint32_t sel_min = 0, const SelectRanks* ranks = nullptr)
 {
     static_assert(!(ROWS && LIST), "one addressing mode");
     static_assert(!ROW_SEL || ROWS, "a selection of rows");
+    static_assert(!COLS || (ROWS && !ROW_SEL), "the columns of rows");
     static_assert(!INDICES || PAIRS, "the indices are the payloads");
     using S = SegSmem<KeyT, PAIRS, K, WARPS>;
     constexpr int THREADS = S::THREADS;
@@ -2385,6 +2398,16 @@ __device__ __forceinline__ void segment_sort_body(KeyT* keys, uint32_t* vals, co
                     if constexpr (PAIRS) val[i] = sm.sorted_val[warp_off + i * 32];
                 }
             }
+        }
+        if constexpr (COLS) {  // the last pass ended with a block barrier: the sorted row is in sm.sorted
+            const uint32_t rk = select_rank_of(*ranks, static_cast<uint32_t>(tid));
+            if (static_cast<uint32_t>(tid) < ranks->count) {
+                KeyT k = sm.sorted[rk];
+                if (dec) k = codec_decode<KeyT>(k, ca, cb, cd);
+                keys[seg * ranks->count + tid] = k;
+                if constexpr (PAIRS) vals[seg * ranks->count + tid] = sm.sorted_val[rk];
+            }
+            continue;
         }
         // the padding sits behind the `len` real keys
         for (uint32_t idx = tid; idx < len; idx += THREADS) {
@@ -2589,13 +2612,16 @@ __device__ __forceinline__ WarpSortCtx<KeyT> warp_sort_ctx(uint32_t* hist, const
 // they are the positions in the run.  (A compile-time flag, so that the other kernels' instantiations compile as before.)
 // PAD (with TOPK; osb200_topk_segments, whose keep may pass len): the stored columns at or past len are padding, the decoded
 // all-ones key that the padding carries through the sort and the position 0xFFFFFFFF.
-template <typename KeyT, int K, int RANK_MODE, bool INDICES, bool TOPK = false, bool PAD = false>
+// COLS (osb200_select_rows, select_rows_warp_kernel; not with TOPK): only the sorted run's columns ranks->r[0 .. count - 1] are
+// stored, at [obase, obase + count) of out and (with INDICES) idx_out.
+template <typename KeyT, int K, int RANK_MODE, bool INDICES, bool TOPK = false, bool PAD = false, bool COLS = false>
 __device__ __forceinline__ void warp_sort_run(RowWarpSmem<KeyT, K, INDICES>& sm, const WarpSortCtx<KeyT>& x, const KeyT* in, KeyT* out,
                                               uint32_t* idx_out, uint64_t base, uint32_t len, const uint32_t* idx_in = nullptr,
-                                              uint64_t obase = 0, uint32_t keep = 0)
+                                              uint64_t obase = 0, uint32_t keep = 0, const SelectRanks* ranks = nullptr)
 {
     static_assert(!TOPK || INDICES, "top-k stores positions");
     static_assert(!PAD || TOPK, "padding is a top-k store");
+    static_assert(!(COLS && TOPK), "one store");
     const int lane = x.lane;
     uint4* h4 = x.h4;
     const uint32_t lt = x.lt;
@@ -2654,6 +2680,25 @@ __device__ __forceinline__ void warp_sort_run(RowWarpSmem<KeyT, K, INDICES>& sm,
             if constexpr (INDICES) val[i] = sm.idx[i * 32 + lane];
         }
         __syncwarp();
+    }
+    if constexpr (COLS) {
+        // the registers hold the sorted run in tile order (the staging area does not when no pass moved a key): through
+        // the staging area to the lanes that store a column
+#pragma unroll
+        for (int i = 0; i < K; ++i) {
+            sm.keys[i * 32 + lane] = key[i];
+            if constexpr (INDICES) sm.idx[i * 32 + lane] = val[i];
+        }
+        __syncwarp();
+        const uint32_t rk = select_rank_of(*ranks, static_cast<uint32_t>(lane));
+        if (static_cast<uint32_t>(lane) < ranks->count) {
+            KeyT k = sm.keys[rk];
+            if (dec) k = codec_decode<KeyT>(k, ca, cb, cd);
+            out[obase + lane] = k;
+            if constexpr (INDICES) idx_out[obase + lane] = sm.idx[rk];
+        }
+        __syncwarp();  // the next run's passes overwrite the staging area
+        return;
     }
 #pragma unroll
     for (int i = 0; i < K; ++i) {
@@ -4357,6 +4402,389 @@ cudaError_t launch_topk_long_rows(const void* keys_in, void* values_out, uint32_
     });
 }
 
+// =====================================================================================================
+// Row select (osb200_select_rows, DESIGN §4.19): columns r_0 < .. < r_{R-1} (R <= 16) of every row's ascending stable sort,
+// and their positions within the row.
+//
+// Rows of at most row_sort_capacity keys: the row sort's kernels (warp_sort_run, segment_sort_body's ROWS mode) with the
+// COLS store, which writes only the R columns.
+//
+// Longer rows (and, with the test hook, every row of two or more keys), the split path: a multi-rank MSD radix select over the
+// long rows' tiles (LongRowGeo), no tile waiting on another.  Every (row, rank) has a state (SelectState): the prefix v of
+// its key's top t digits (encoded) and `taken`, the keys of the row below v's range.  Level t = 0 .. D - 1:
+//   * select_count_kernel: the ranks of a row whose prefixes are equal form a group (contiguous, the ranks increasing; one
+//     group at level 0).  Each key of a tile matches at most one group's prefix and is counted once, by digit t, into that
+//     group's 256 bins; the tile adds them to the row's totals of the group's first rank.
+//   * select_pick_kernel: per group, each rank takes the bucket holding its (r - taken)-th candidate, extends its prefix and
+//     adds the candidates below the bucket to taken; the totals are cleared for the next level.  After the last level v is
+//     the key itself, and the pick writes the values.
+// Positions: select_eq_count_kernel counts per tile the keys equal to each rank's key, the long rows' scan kernels scan each
+// row's [rank][tile] counts, and select_locate_kernel finds occurrence r - taken in the one tile whose range holds it.
+// =====================================================================================================
+template <typename KeyT, int K, int RANK_MODE, bool INDICES>
+__global__ void __launch_bounds__(kRowWarps * 32)
+select_rows_warp_kernel(const KeyT* in, KeyT* out, uint32_t* __restrict__ idx_out, uint64_t num_rows, uint32_t row_len, KeyCodec codec,
+                        SelectRanks ranks)
+{
+    using W = RowWarpSmem<KeyT, K, INDICES>;
+    extern __shared__ __align__(16) unsigned char s_raw[];
+    const int warp = threadIdx.x >> 5;
+    W& sm = reinterpret_cast<W*>(s_raw)[warp];
+    const WarpSortCtx<KeyT> x = warp_sort_ctx<KeyT>(sm.hist, codec);
+    for (uint64_t row = static_cast<uint64_t>(blockIdx.x) * kRowWarps + warp; row < num_rows;
+         row += static_cast<uint64_t>(gridDim.x) * kRowWarps)
+        warp_sort_run<KeyT, K, RANK_MODE, INDICES, false, false, true>(sm, x, in, out, idx_out, row * row_len, row_len, nullptr,
+                                                                      row * ranks.count, 0u, &ranks);
+}
+
+template <typename KeyT, int K, int WARPS, int RANK_MODE, bool INDICES>
+__global__ void __launch_bounds__(WARPS * 32, 1)
+select_rows_block_kernel(const KeyT* __restrict__ in, KeyT* out, uint32_t* idx_out, uint64_t num_rows, uint32_t row_len, KeyCodec codec,
+                         SelectRanks ranks)
+{
+    segment_sort_body<KeyT, INDICES, K, WARPS, RANK_MODE, INDICES, true, false, false, true>(
+        out, idx_out, nullptr, num_rows, row_len, row_len, 0u, sizeof(KeyT), 8u, codec, in, nullptr, nullptr, 0, 0u, &ranks);
+}
+
+// the block path's geometries: 2,048 keys, and the row sort's capacity
+template <typename KeyT, int SIZE, bool INDICES>
+struct SelectShape {
+    using Key = KeyT;
+    static constexpr bool indices = INDICES, has_hot = false;
+    using G = SegGeomN<KeyT, SIZE>;
+    using S = SegSmem<KeyT, INDICES, G::K, G::WARPS>;
+    static constexpr uint32_t T = S::T;
+    static constexpr size_t smem = sizeof(S);
+    template <int RANK_MODE, bool HOT = false>
+    static constexpr auto kernel() { return select_rows_block_kernel<KeyT, G::K, G::WARPS, RANK_MODE, INDICES>; }
+};
+using SelectShapes = TypeList<
+    SelectShape<uint16_t, 1, false>, SelectShape<uint16_t, 2, false>, SelectShape<uint16_t, 1, true>, SelectShape<uint16_t, 2, true>,
+    SelectShape<uint32_t, 1, false>, SelectShape<uint32_t, 2, false>, SelectShape<uint32_t, 1, true>, SelectShape<uint32_t, 2, true>,
+    SelectShape<uint64_t, 1, false>, SelectShape<uint64_t, 2, false>, SelectShape<uint64_t, 1, true>, SelectShape<uint64_t, 2, true>>;
+
+cudaError_t launch_select_rows(const void* keys_in, void* values_out, uint32_t* indices, uint64_t num_rows, uint32_t row_len,
+                               const SelectRanks& ranks, int key_bytes, const KeyCodec* codec_in, int rank_mode, bool block_only,
+                               int sm_count, cudaStream_t stream)
+{
+    if (num_rows == 0 || row_len < 2 || row_len > row_sort_capacity(key_bytes) || ranks.count == 0 || ranks.count > kMaxSelectRanks)
+        return cudaErrorInvalidValue;
+    const KeyCodec codec = codec_in ? *codec_in : KeyCodec();
+    return with_rank_mode(rank_mode, [&](auto r) {
+        constexpr int R = decltype(r)::value;
+        if (row_len <= kRowWarpMaxLen && !block_only)
+            return with_key_type(TopkKeys{}, key_bytes, [&](auto k) {
+                using KeyT = decltype(k);
+                return with_warp_k(row_len, [&](auto kk) {
+                    constexpr int K = decltype(kk)::value;
+                    auto go = [&](auto ind) {
+                        constexpr bool I = decltype(ind)::value;
+                        return launch_resident<select_rows_warp_kernel<KeyT, K, R, I>, kRowWarps * 32, kRowWarpSmemBytes<KeyT, K, I>>(
+                            (num_rows + kRowWarps - 1) / kRowWarps, sm_count, stream, static_cast<const KeyT*>(keys_in),
+                            static_cast<KeyT*>(values_out), indices, num_rows, row_len, codec, ranks);
+                    };
+                    return indices ? go(std::true_type{}) : go(std::false_type{});
+                });
+            });
+        return find_type(
+            SelectShapes{},
+            [&](auto s) {
+                using S = decltype(s);
+                return key_bytes == static_cast<int>(sizeof(typename S::Key)) && S::indices == (indices != nullptr) && row_len <= S::T;
+            },
+            [&](auto s) {
+                using S = decltype(s);
+                using KeyT = typename S::Key;
+                return launch_resident<S::template kernel<R>(), S::S::THREADS, S::smem>(
+                    num_rows, sm_count, stream, static_cast<const KeyT*>(keys_in), static_cast<KeyT*>(values_out), indices, num_rows,
+                    row_len, codec, ranks);
+            });
+    });
+}
+
+// One (row, rank) of the split path: the prefix v (encoded; the top t digits at level t, the key after the last level) and
+// the row's keys below v's range.  All zero is level 0.
+struct SelectState { unsigned long long v; uint32_t taken, pad; };
+
+// The groups of row r's ranks, by one warp (the caller's warp 0): s_v[g] the prefix of group g (ascending), s_first[g] its
+// first rank, s_gi[i] rank i's group, *s_ng the number of groups.
+template <typename U>
+__device__ __forceinline__ void select_groups(const SelectState* __restrict__ rs, uint32_t nr, U* s_v, uint32_t* s_first,
+                                              uint32_t* s_gi, uint32_t* s_ng)
+{
+    const uint32_t i = threadIdx.x;
+    const U v = i < nr ? static_cast<U>(rs[i].v) : static_cast<U>(0);
+    const U prev = __shfl_up_sync(0xffffffffu, v, 1);
+    const bool first = i < nr && (i == 0 || v != prev);
+    const uint32_t b = __ballot_sync(0xffffffffu, first);
+    const uint32_t gi = __popc(b & lanemask_lt()) + (first ? 0u : 0xffffffffu);  // the last group starting at or before i
+    if (first) { s_v[gi] = v; s_first[gi] = i; }
+    if (i < nr) s_gi[i] = gi;
+    if (i == 0) *s_ng = __popc(b);
+}
+
+// The group whose prefix p is, among the ng ascending prefixes s_v; ng when there is none.
+template <typename U>
+__device__ __forceinline__ uint32_t select_group_of(U p, const U* s_v, uint32_t ng)
+{
+    uint32_t g = 0;
+#pragma unroll
+    for (uint32_t step = kMaxSelectRanks / 2; step; step >>= 1)
+        if (g + step < ng && s_v[g + step] <= p) g += step;
+    return s_v[g] == p ? g : ng;
+}
+
+template <typename KeyT>
+__global__ void __launch_bounds__(kLongThreads)
+select_count_kernel(const KeyT* __restrict__ in, uint64_t num_rows, uint32_t row_len, uint32_t tpr, uint32_t nr, uint32_t level,
+                    const SelectState* __restrict__ st, uint32_t* __restrict__ tot, KeyCodec codec)
+{
+    using U = std::conditional_t<sizeof(KeyT) == 8, uint64_t, uint32_t>;
+    constexpr uint32_t D = sizeof(KeyT);
+    const uint32_t shift = 8u * (D - 1u - level);
+    const U m = level ? static_cast<U>(~static_cast<U>(0) << (8u * (D - level))) : static_cast<U>(0);
+    const KeyT ca = static_cast<KeyT>(codec.a), cb = static_cast<KeyT>(codec.b), cd = static_cast<KeyT>(codec.d);
+    const bool enc = codec.flags & kCodecEncodeOnLoad;
+    // a bin's counts in 2^lc bank-private columns, as in long_count_body (32 columns for one group, the skewed rows' case);
+    // G groups take 32 / G columns or more, at most 8,192 counters
+    __shared__ uint32_t s_hist[kRadix * 32];
+    __shared__ U s_v[kMaxSelectRanks];
+    __shared__ uint32_t s_first[kMaxSelectRanks], s_gi[kMaxSelectRanks], s_ng;
+    const uint32_t lane = threadIdx.x & 31;
+    const LongRowGeo geo{num_rows, row_len, tpr, 0, 0};
+    const uint64_t tiles = geo.tiles();
+    for (uint64_t g = blockIdx.x; g < tiles; g += gridDim.x) {
+        const auto x = geo.tile(g);
+        if (threadIdx.x < 32) select_groups<U>(st + x.r * nr, nr, s_v, s_first, s_gi, &s_ng);
+        __syncthreads();
+        const uint32_t ng = s_ng;
+        const uint32_t lc = ng <= 1 ? 5u : ng <= 2 ? 4u : ng <= 4 ? 3u : ng <= 8 ? 2u : 1u, cm = (1u << lc) - 1u;
+        for (uint32_t i = threadIdx.x; i < (ng * kRadix << lc); i += kLongThreads) s_hist[i] = 0;
+        __syncthreads();
+        const KeyT* tile = in + x.lo + x.t0;
+        KeyT key[kLongK];
+#pragma unroll
+        for (int i = 0; i < kLongK; ++i) {
+            const uint32_t j = threadIdx.x + i * kLongThreads;
+            key[i] = j < x.len ? tile[j] : static_cast<KeyT>(0);
+        }
+        const U v0 = s_v[0];
+#pragma unroll
+        for (int i = 0; i < kLongK; ++i) {
+            if (threadIdx.x + i * kLongThreads >= x.len) break;
+            const U e = static_cast<U>(enc ? codec_encode<KeyT>(key[i], ca, cb, cd) : key[i]);
+            const U p = e & m;
+            const uint32_t gi = ng == 1 ? (p == v0 ? 0u : 1u) : select_group_of<U>(p, s_v, ng);
+            if (gi < ng) atomicAdd(&s_hist[((gi * kRadix + digit_of(e, shift)) << lc) + (lane & cm)], 1u);
+        }
+        __syncthreads();
+        for (uint32_t b = threadIdx.x; b < ng * kRadix; b += kLongThreads) {
+            uint32_t sum = 0;
+            for (uint32_t c = 0; c <= cm; ++c) sum += s_hist[(b << lc) + ((c + b) & cm)];
+            if (sum) atomicAdd(&tot[(x.r * nr + s_first[b / kRadix]) * kRadix + (b % kRadix)], sum);
+        }
+        __syncthreads();  // the fold has read s_hist and the groups
+    }
+}
+
+template <typename KeyT>
+__global__ void __launch_bounds__(kRadix)
+select_pick_kernel(uint64_t num_rows, uint32_t level, SelectState* __restrict__ st, uint32_t* __restrict__ tot, KeyT* __restrict__ out,
+                   SelectRanks ranks, KeyCodec codec)
+{
+    constexpr uint32_t D = sizeof(KeyT);
+    const uint32_t shift = 8u * (D - 1u - level), nr = ranks.count;
+    const bool last = level + 1 == D, dec = codec.flags & kCodecDecodeOnStore;
+    const KeyT ca = static_cast<KeyT>(codec.a), cb = static_cast<KeyT>(codec.b), cd = static_cast<KeyT>(codec.d);
+    __shared__ unsigned long long s_v[kMaxSelectRanks];
+    __shared__ uint32_t s_taken[kMaxSelectRanks], s_need[kMaxSelectRanks], s_wtot[kRadix / 32];
+    const uint32_t rk = select_rank_of(ranks, threadIdx.x);
+    for (uint64_t r = blockIdx.x; r < num_rows; r += gridDim.x) {
+        SelectState* rs = st + r * nr;
+        if (threadIdx.x < nr) {
+            const SelectState s = rs[threadIdx.x];
+            s_v[threadIdx.x] = s.v;
+            s_taken[threadIdx.x] = s.taken;
+            s_need[threadIdx.x] = rk - s.taken;
+        }
+        __syncthreads();
+        for (uint32_t i = 0; i < nr;) {  // group [i, j)
+            uint32_t j = i + 1;
+            while (j < nr && s_v[j] == s_v[i]) ++j;
+            uint32_t* t = tot + (r * nr + i) * kRadix;
+            const uint32_t c = t[threadIdx.x];
+            t[threadIdx.x] = 0;  // for the next level
+            const uint32_t excl = block_excl_scan_256<kRadix>(c, s_wtot);
+            for (uint32_t q = i; q < j; ++q) {
+                const uint32_t need = s_need[q];
+                if (excl <= need && need < excl + c) {  // (c > 0)
+                    SelectState ns;
+                    ns.v = s_v[q] | static_cast<unsigned long long>(threadIdx.x) << shift;
+                    ns.taken = s_taken[q] + excl;
+                    ns.pad = 0;
+                    rs[q] = ns;
+                    if (last) {
+                        KeyT k = static_cast<KeyT>(ns.v);
+                        if (dec) k = codec_decode<KeyT>(k, ca, cb, cd);
+                        out[r * nr + q] = k;
+                    }
+                }
+            }
+            __syncthreads();  // s_wtot is reused by the next group, s_v etc. by the next row
+            i = j;
+        }
+    }
+}
+
+// Per tile, the keys equal to each rank's key (its group's), into cnt[row][rank][tile]; a warp adds the lanes of one group at once.
+template <typename KeyT>
+__global__ void __launch_bounds__(kLongThreads)
+select_eq_count_kernel(const KeyT* __restrict__ in, uint64_t num_rows, uint32_t row_len, uint32_t tpr, uint32_t nr,
+                       const SelectState* __restrict__ st, uint32_t* __restrict__ cnt, KeyCodec codec)
+{
+    using U = std::conditional_t<sizeof(KeyT) == 8, uint64_t, uint32_t>;
+    const KeyT ca = static_cast<KeyT>(codec.a), cb = static_cast<KeyT>(codec.b), cd = static_cast<KeyT>(codec.d);
+    const bool enc = codec.flags & kCodecEncodeOnLoad;
+    __shared__ U s_v[kMaxSelectRanks];
+    __shared__ uint32_t s_first[kMaxSelectRanks], s_gi[kMaxSelectRanks], s_ng, s_c[kMaxSelectRanks];
+    const uint32_t lane = threadIdx.x & 31;
+    const LongRowGeo geo{num_rows, row_len, tpr, 0, 0};
+    const uint64_t tiles = geo.tiles();
+    for (uint64_t g = blockIdx.x; g < tiles; g += gridDim.x) {
+        const auto x = geo.tile(g);
+        if (threadIdx.x < 32) select_groups<U>(st + x.r * nr, nr, s_v, s_first, s_gi, &s_ng);
+        if (threadIdx.x < kMaxSelectRanks) s_c[threadIdx.x] = 0;
+        __syncthreads();
+        const uint32_t ng = s_ng;
+        const KeyT* tile = in + x.lo + x.t0;
+        KeyT key[kLongK];
+#pragma unroll
+        for (int i = 0; i < kLongK; ++i) {
+            const uint32_t j = threadIdx.x + i * kLongThreads;
+            key[i] = j < x.len ? tile[j] : static_cast<KeyT>(0);
+        }
+#pragma unroll
+        for (int i = 0; i < kLongK; ++i) {
+            const bool valid = threadIdx.x + i * kLongThreads < x.len;
+            const U e = static_cast<U>(enc ? codec_encode<KeyT>(key[i], ca, cb, cd) : key[i]);
+            const uint32_t gi = valid ? select_group_of<U>(e, s_v, ng) : ng;
+            const uint32_t peers = __match_any_sync(0xffffffffu, gi);
+            if (gi < ng && lane == static_cast<uint32_t>(__ffs(peers) - 1)) atomicAdd(&s_c[gi], static_cast<uint32_t>(__popc(peers)));
+        }
+        __syncthreads();
+        if (threadIdx.x < nr) cnt[(x.r * nr + threadIdx.x) * tpr + x.t] = s_c[s_gi[threadIdx.x]];
+        __syncthreads();  // s_c and the groups are reused by the next tile
+    }
+}
+
+// For every (row, rank) whose occurrence o = r - taken of its key lies in this tile by the scanned counts: the position of the
+// tile's (o - tile prefix)-th key equal to it, in tile order (per-warp ballots and a scan of the warp counts, chunk by chunk).
+template <typename KeyT>
+__global__ void __launch_bounds__(kLongThreads)
+select_locate_kernel(const KeyT* __restrict__ in, uint32_t* __restrict__ idx_out, uint64_t num_rows, uint32_t row_len, uint32_t tpr,
+                     const SelectState* __restrict__ st, const uint32_t* __restrict__ cnt, SelectRanks ranks, KeyCodec codec)
+{
+    using U = std::conditional_t<sizeof(KeyT) == 8, uint64_t, uint32_t>;
+    const KeyT ca = static_cast<KeyT>(codec.a), cb = static_cast<KeyT>(codec.b), cd = static_cast<KeyT>(codec.d);
+    const bool enc = codec.flags & kCodecEncodeOnLoad;
+    __shared__ uint32_t s_w[kLongWarps];
+    const uint32_t nr = ranks.count, lane = threadIdx.x & 31, warp = threadIdx.x >> 5, lt = lanemask_lt();
+    const LongRowGeo geo{num_rows, row_len, tpr, 0, 0};
+    const uint64_t tiles = geo.tiles();
+    for (uint64_t g = blockIdx.x; g < tiles; g += gridDim.x) {
+        const auto x = geo.tile(g);
+        const KeyT* tile = in + x.lo + x.t0;
+        for (uint32_t i = 0; i < nr; ++i) {
+            const uint32_t* s = cnt + (x.r * nr + i) * tpr;  // the scan ran over the row's ranks one after another
+            const uint32_t b0 = s[0], lo = s[x.t] - b0, hi = x.t + 1 < tpr ? s[x.t + 1] - b0 : 0xffffffffu;
+            const SelectState ss = st[x.r * nr + i];
+            const uint32_t o = select_rank_of(ranks, i) - ss.taken;
+            if (o < lo || o >= hi) continue;
+            const U v = static_cast<U>(ss.v);
+            const uint32_t want = o - lo;
+            uint32_t run = 0;
+            for (uint32_t c0 = 0; c0 < x.len; c0 += kLongThreads) {
+                const uint32_t j = c0 + threadIdx.x;
+                KeyT k = j < x.len ? tile[j] : static_cast<KeyT>(0);
+                const bool eq = j < x.len && static_cast<U>(enc ? codec_encode<KeyT>(k, ca, cb, cd) : k) == v;
+                const uint32_t b = __ballot_sync(0xffffffffu, eq);
+                if (lane == 0) s_w[warp] = __popc(b);
+                __syncthreads();
+                uint32_t pre = 0, total = 0;
+#pragma unroll
+                for (int w = 0; w < kLongWarps; ++w) { const uint32_t y = s_w[w]; pre += static_cast<uint32_t>(w) < warp ? y : 0u; total += y; }
+                __syncthreads();  // s_w is reused by the next chunk
+                if (eq && run + pre + __popc(b & lt) == want) idx_out[x.r * nr + i] = x.t0 + j;
+                run += total;
+                if (run > want) break;
+            }
+        }
+    }
+}
+
+SelectLayout select_layout(uint64_t num_rows, uint32_t row_len, uint32_t num_ranks, bool positions)
+{
+    static_assert(sizeof(SortPlan) <= 16 * sizeof(uint32_t) && sizeof(SelectState) == 4 * sizeof(uint32_t), "the layout's words");
+    auto whole = [](uint64_t words) { return (words + 3) / 4 * 4; };
+    SelectLayout l;
+    l.tpr = static_cast<uint32_t>((static_cast<uint64_t>(row_len) + kLongRowTile - 1) / kLongRowTile);
+    l.cpr = static_cast<uint32_t>((static_cast<uint64_t>(num_ranks) * l.tpr + kLongChunk - 1) / kLongChunk);
+    l.st = 16;  // words 0 .. 15: a zeroed SortPlan, with which the long rows' scan kernels skip nothing
+    l.tot = l.st + num_rows * num_ranks * 4;
+    l.zeroed = whole(l.tot + num_rows * num_ranks * kRadix);
+    l.cnt = l.zeroed;
+    l.csum = positions ? whole(l.cnt + num_rows * num_ranks * l.tpr) : l.cnt;
+    l.words = positions && l.cpr > 1 ? whole(l.csum + num_rows * l.cpr) : l.csum;
+    return l;
+}
+
+cudaError_t launch_select_long_rows(const void* keys_in, void* values_out, uint32_t* indices, uint64_t num_rows, uint32_t row_len,
+                                    const SelectRanks& ranks, int key_bytes, const KeyCodec* codec_in, uint32_t* scratch, int sm_count,
+                                    cudaStream_t stream)
+{
+    if (num_rows == 0 || row_len < 2 || ranks.count == 0 || ranks.count > kMaxSelectRanks) return cudaErrorInvalidValue;
+    const uint32_t nr = ranks.count;
+    const SelectLayout l = select_layout(num_rows, row_len, nr, indices != nullptr);
+    const KeyCodec codec = codec_in ? *codec_in : KeyCodec();
+    cudaError_t e = cudaMemsetAsync(scratch, 0, l.zeroed * sizeof(uint32_t), stream);
+    if (e != cudaSuccess) return e;
+    const SortPlan* none_skipped = reinterpret_cast<const SortPlan*>(scratch);
+    SelectState* st = reinterpret_cast<SelectState*>(scratch + l.st);
+    uint32_t* tot = scratch + l.tot;
+    uint32_t* cnt = scratch + l.cnt;
+    uint32_t* csum = l.cpr > 1 ? scratch + l.csum : nullptr;
+    const uint64_t tiles = num_rows * l.tpr;
+    return with_key_type(TopkKeys{}, key_bytes, [&](auto kt) {
+        using KeyT = decltype(kt);
+        const KeyT* in = static_cast<const KeyT*>(keys_in);
+        cudaError_t le = cudaSuccess;
+        for (uint32_t t = 0; le == cudaSuccess && t < sizeof(KeyT); ++t) {
+            le = launch_resident<select_count_kernel<KeyT>, kLongThreads, 0>(tiles, sm_count, stream, in, num_rows, row_len, l.tpr, nr, t,
+                                                                             static_cast<const SelectState*>(st), tot, codec);
+            if (le == cudaSuccess)
+                le = launch_resident<select_pick_kernel<KeyT>, kRadix, 0>(num_rows, sm_count, stream, num_rows, t, st, tot,
+                                                                          static_cast<KeyT*>(values_out), ranks, codec);
+        }
+        if (le != cudaSuccess || !indices) return le;
+        le = launch_resident<select_eq_count_kernel<KeyT>, kLongThreads, 0>(tiles, sm_count, stream, in, num_rows, row_len, l.tpr, nr,
+                                                                            static_cast<const SelectState*>(st), cnt, codec);
+        if (le != cudaSuccess) return le;
+        // per row, the exclusive scan of its nr * tpr counts [rank][tile]
+        const uint64_t row_counts = static_cast<uint64_t>(nr) * l.tpr;
+        const unsigned scan_grid = capped_grid(num_rows * l.cpr, 1, static_cast<uint64_t>(sm_count) * 4);
+        if (csum) {
+            long_rows_chunk_sum_kernel<<<scan_grid, kLongThreads, 0, stream>>>(none_skipped, 0, cnt, csum, num_rows, row_counts, l.cpr);
+            long_rows_chunk_scan_kernel<<<capped_grid(num_rows, 1, static_cast<uint64_t>(sm_count) * 4), kLongThreads, 0, stream>>>(
+                none_skipped, 0, csum, num_rows, l.cpr);
+        }
+        long_rows_scan_kernel<<<scan_grid, kLongThreads, 0, stream>>>(none_skipped, 0, cnt, csum, num_rows, row_counts, l.cpr);
+        if ((le = cudaGetLastError()) != cudaSuccess) return le;
+        return launch_resident<select_locate_kernel<KeyT>, kLongThreads, 0>(tiles, sm_count, stream, in, indices, num_rows, row_len, l.tpr,
+                                                                            static_cast<const SelectState*>(st),
+                                                                            static_cast<const uint32_t*>(cnt), ranks, codec);
+    });
+}
+
 cudaError_t configure_kernels()
 {
     cudaError_t e = for_each_type(HistKeys{}, [](auto k) {
@@ -4408,6 +4836,7 @@ cudaError_t configure_kernels()
         if (m == cudaSuccess) m = set_smem(topk_long_sort_scatter_kernel<KeyT, kRankAtomic>, sizeof(LongRowsSmem<KeyT, true>));
         return m != cudaSuccess ? m : set_smem(topk_long_sort_scatter_kernel<KeyT, kRankBallot>, sizeof(LongRowsSmem<KeyT, true>));
     });
+    if (e == cudaSuccess) e = for_each_type(SelectShapes{}, shape);
     return e;
 }
 

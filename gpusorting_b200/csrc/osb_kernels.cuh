@@ -213,6 +213,26 @@ cudaError_t launch_topk_long_rows(const void* keys_in, void* values_out, uint32_
                                   uint32_t capacity, int rank_mode, bool allow_skip, unsigned long long* ghist, unsigned long long* gbase,
                                   SortPlan* plan, uint32_t* scratch, int sm_count, cudaStream_t stream);
 
+// Row select (osb200_select_rows): columns ranks.r[0 .. count - 1] (strictly increasing, each below row_len) of every row's
+// ascending stable sort into [r * count, (r + 1) * count) of values_out, and their positions within the row into the same
+// entries of indices (may be null).  The ranks travel in the launch parameters.
+constexpr uint32_t kMaxSelectRanks = 16;
+struct SelectRanks { uint32_t r[kMaxSelectRanks]; uint32_t count; };
+// Rows of 2 .. row_sort_capacity(key_bytes) keys: launch_row_sort's kernels (one warp per row up to kRowWarpMaxLen keys, else
+// one CTA per row, always with block_only), each storing only the selected columns.  No workspace.  The codec as for
+// launch_row_sort.
+cudaError_t launch_select_rows(const void* keys_in, void* values_out, uint32_t* indices, uint64_t num_rows, uint32_t row_len,
+                               const SelectRanks& ranks, int key_bytes, const KeyCodec* codec, int rank_mode, bool block_only,
+                               int sm_count, cudaStream_t stream);
+// The split path (rows of 2 or more keys, DESIGN §4.19): a multi-rank MSD radix select per row over the long rows' tiles, then,
+// with indices, a count of each selected key per tile, the long rows' scan of those counts and a locate kernel.  Workspace:
+// scratch, select_layout(...).words u32, 16-byte aligned (its first `zeroed` words are cleared here).
+struct SelectLayout { uint64_t st, tot, zeroed, cnt, csum, words; uint32_t tpr, cpr; };  // offsets in u32 words
+SelectLayout select_layout(uint64_t num_rows, uint32_t row_len, uint32_t num_ranks, bool positions);
+cudaError_t launch_select_long_rows(const void* keys_in, void* values_out, uint32_t* indices, uint64_t num_rows, uint32_t row_len,
+                                    const SelectRanks& ranks, int key_bytes, const KeyCodec* codec, uint32_t* scratch, int sm_count,
+                                    cudaStream_t stream);
+
 // Validate (reference: Validate, UtilityKernels.cuh:403-429): err_count += #(keys[i] > keys[i+1]).
 cudaError_t launch_validate(const void* keys, uint64_t n, int key_bytes, unsigned long long* err_count, int sm_count,
                             cudaStream_t stream);

@@ -13,6 +13,7 @@ libonesweep_b200.so.
 from __future__ import annotations
 
 import ctypes
+import math
 from typing import Optional
 
 import numpy as np
@@ -297,6 +298,29 @@ class OneSweepSorter:
         self._call(lib.osb200_topk_long_rows, x.data_ptr(), out.data_ptr(), idx.data_ptr(), num_rows, row_len, k, kb, kt,
                    1 if largest else 0, 1 if sorted else 0, stream=stream)
         return out, idx
+
+    # -- row select: given columns of every row's ascending stable sort ---------------------------------------------------
+    def select_rows(self, x: torch.Tensor, ranks, key_type: str, return_indices: bool = True, stream=None):
+        """Columns `ranks` of every row's ascending stable sort along the last dimension of `x`, and their positions within
+        the row (osb200_select_rows).  `x` and key_type as in sort_rows; `ranks` a sequence of 1 to 16 strictly increasing
+        ints below the row length, shared by every row.  Among equal keys a rank picks by position: the values are bit for
+        bit those of ``sort_rows(x)[..., ranks]``.
+
+        Returns (values, indices) shaped ``x.shape[:-1] + (len(ranks),)``, indices as torch.int32, or values alone with
+        return_indices=False, allocated with torch.empty on the stream.  Rows of at most 16,384 keys (8,192 for 8-byte dtypes)
+        need no workspace; longer rows use this sorter's alternate keys, for a bound that depends on the number of rows, the
+        row length and len(ranks) only (see select_workspace_words)."""
+        kb, kt = self._ragged_keys(x, key_type)
+        ranks = [int(r) for r in ranks]
+        if any(not 0 <= r <= 0xFFFFFFFF for r in ranks):
+            raise ValueError(f"ranks must lie in [0, 2^32), got {ranks}")
+        row_len = x.shape[-1]
+        num_rows = math.prod(x.shape[:-1])
+        arr = (ctypes.c_uint32 * max(len(ranks), 1))(*ranks)
+        out, idx = _new_outputs(stream, x, tuple(x.shape[:-1]) + (len(ranks),), return_indices)
+        self._call(lib.osb200_select_rows, x.data_ptr(), out.data_ptr(), idx.data_ptr() if idx is not None else None, num_rows,
+                   row_len, arr, len(ranks), kb, kt, stream=stream)
+        return (out, idx) if return_indices else out
 
     # -- segment sort: ragged rows given by offsets -------------------------------------------------------------------------
     def sort_segments(self, x: torch.Tensor, offsets: torch.Tensor, key_type: str, descending: bool = False,
@@ -598,6 +622,148 @@ def topk_long_rows(x: torch.Tensor, k: int, largest: bool = True, sorted: bool =
     else:
         s = _module_sorter(x, "x", 4, 1, stream, _ROW_KEY_TYPES)
     return s.topk_long_rows(x, k, _ROW_KEY_TYPES[x.dtype], largest, sorted, stream)
+
+
+def select_workspace_words(num_rows: int, row_len: int, num_ranks: int, indices: bool = True) -> int:
+    """The 32-bit words of a sorter's alternate keys that select_rows' split path (rows above sort_rows' limit) needs -- the
+    bound of osb200_select_rows in include/onesweep_b200.h: per rank a 4-word state and 256 totals, and with indices one count
+    per rank and tile of 8,192 keys plus the scan's chunk sums.  A (4, 4) sorter with max_n >= this many has the room."""
+    def round4(w):
+        return (w + 3) // 4 * 4
+    tiles = (row_len + _LONG_ROW_TILE - 1) // _LONG_ROW_TILE
+    words = round4(16 + num_rows * num_ranks * (4 + 256))
+    if indices:
+        words += round4(num_rows * num_ranks * tiles)
+        chunks = (num_ranks * tiles + 4095) // 4096
+        if chunks > 1:
+            words += round4(num_rows * chunks)
+    return words
+
+
+def _select_sorter(x: torch.Tensor, rows: torch.Tensor, num_ranks: int, stream) -> OneSweepSorter:
+    """The stream's cached (4, 4) sorter for select_rows on `rows` (a view of x), grown only when the split path's bound does
+    not fit it -- never to x.numel()."""
+    row_len = rows.shape[-1]
+    if row_len > _ROW_CAPACITY.get(rows.element_size(), 16384):
+        need = select_workspace_words(math.prod(rows.shape[:-1]), row_len, num_ranks)
+        return _module_sorter(x, "x", 4, need, stream, _ROW_KEY_TYPES)
+    return _module_sorter(x, "x", 4, 1, stream, _ROW_KEY_TYPES)
+
+
+def _select_view(x: torch.Tensor, dim):
+    """x as rows: dim None flattens it into one row of at most 2^32 - 1 keys, dim -1 (or x.dim() - 1) keeps its rows; any
+    other dim raises ValueError."""
+    if not isinstance(x, torch.Tensor):
+        raise TypeError("x must be a CUDA tensor")
+    if dim is None:
+        if x.numel() > 0xFFFFFFFF:
+            raise ValueError(f"dim=None takes at most 2^32 - 1 elements, got {x.numel()}")
+        return x.reshape(1, x.numel())
+    if dim not in (-1, max(x.dim(), 1) - 1):
+        raise ValueError(f"only the last dimension (dim=-1) or dim=None can be reduced, got dim={dim}")
+    return x if x.dim() else x.reshape(1)
+
+
+def _reduced_shape(x: torch.Tensor, dim, keepdim: bool):
+    if dim is None:
+        return (1,) * x.dim() if keepdim else ()
+    shape = tuple(x.shape[:-1])
+    return shape + (1,) if keepdim and x.dim() else shape
+
+
+def select_rows(x: torch.Tensor, ranks, dim=-1, return_indices: bool = True, stream=None):
+    """Columns `ranks` (1 to 16 strictly increasing ints) of the ascending stable sort of every row of a contiguous CUDA tensor
+    of one of sort_rows' ten dtypes: (values, int32 positions within the row) shaped ``rows.shape[:-1] + (len(ranks),)``, or
+    values alone.  dim=-1 selects along the last dimension, dim=None in the flattened tensor (one row).  The key type follows
+    the dtype.  OneSweepSorter.select_rows on the stream's cached (4, 4) sorter, grown only when rows above sort_rows' limit
+    need more room than it has (select_workspace_words)."""
+    rows = _select_view(x, dim)
+    ranks = list(ranks)
+    s = _select_sorter(x, rows, len(ranks), stream)
+    return s.select_rows(rows, ranks, _ROW_KEY_TYPES[x.dtype], return_indices, stream)
+
+
+def kthvalue(x: torch.Tensor, k: int, dim=-1, keepdim: bool = False, stream=None):
+    """``torch.kthvalue(x, k, dim, keepdim)`` for a contiguous CUDA tensor of one of sort_rows' ten dtypes: the k-th smallest
+    key (k 1-based) of every row and its int32 position, column k - 1 of the row's ascending stable sort -- of equal keys the
+    one at the (k - taken)-th position among them.  dim is -1 (or the last dimension) or None (the flattened tensor).  Keys
+    follow this library's total order: floats by their bits (-0.0 before +0.0, NaNs of either sign at the matching end)."""
+    rows = _select_view(x, dim)
+    k = int(k)
+    if not 1 <= k <= rows.shape[-1]:
+        raise ValueError(f"k={k} is outside 1 .. {rows.shape[-1]}")
+    v, i = select_rows(rows, [k - 1], -1, True, stream)
+    shape = _reduced_shape(x, dim, keepdim)
+    return v.view(shape), i.view(shape)
+
+
+def median(x: torch.Tensor, dim=None, keepdim: bool = False, stream=None):
+    """``torch.median``: the lower median, rank (L - 1) // 2 of the ascending stable sort of rows of L keys.  dim=None returns
+    the median of the flattened tensor as a 0-dim tensor; dim=-1 returns (values, int32 indices) of every row, as kthvalue."""
+    rows = _select_view(x, dim)
+    L = rows.shape[-1]
+    if L == 0:
+        raise ValueError("median of an empty row")
+    if dim is None:
+        return select_rows(rows, [(L - 1) // 2], -1, False, stream).view(())
+    return kthvalue(x, (L - 1) // 2 + 1, dim, keepdim, stream)
+
+
+_INTERPOLATIONS = ("linear", "lower", "higher", "midpoint", "nearest")
+
+
+def quantile(x: torch.Tensor, q, dim=None, keepdim: bool = False, interpolation: str = "linear", stream=None):
+    """``torch.quantile(x, q, dim, keepdim, interpolation)`` for a contiguous float32 or float64 CUDA tensor, bit for bit on
+    inputs without -0.0 (torch's sort does not order the two zeros): rows with a NaN give NaN, as in torch.  q is a float, a
+    sequence or a CPU tensor of values in [0, 1] (a CUDA q is refused: the ranks are needed on the host).  The ranks are ATen's,
+    q * (L - 1) in x's dtype, then floor / ceil / round per mode; the distinct ranks, plus 0 and L - 1 (in this library's order
+    a NaN sorts to one end, so they find NaN rows without another read), are selected 16 per call, and torch.lerp finishes the
+    [rows, q] result.  Unlike torch.quantile it takes rows above 2^24 keys.  dim is None (the flattened tensor) or -1."""
+    if not (isinstance(x, torch.Tensor) and x.dtype in (torch.float32, torch.float64)):
+        raise TypeError("quantile() takes float32 or float64 tensors")
+    if interpolation not in _INTERPOLATIONS:
+        raise ValueError(f"interpolation must be one of {_INTERPOLATIONS}, got {interpolation!r}")
+    if isinstance(q, torch.Tensor) and q.is_cuda:
+        raise ValueError("q must be a float, a sequence or a CPU tensor: the ranks are computed on the host")
+    qt = torch.as_tensor(q, dtype=x.dtype, device="cpu")
+    if qt.dim() > 1:
+        raise ValueError("q must be a scalar or a 1-D tensor")
+    if not bool(((qt >= 0) & (qt <= 1)).all()):
+        raise ValueError("q values must lie in [0, 1]")
+    rows = _select_view(x, dim)
+    L = rows.shape[-1]
+    if L == 0:
+        raise ValueError("quantile() input rows must be non-empty")
+    num_rows = math.prod(rows.shape[:-1])
+    qv = qt.reshape(-1)
+    pos = qv * (L - 1)  # ATen's ranks, in x's dtype
+    if interpolation == "lower":
+        pos = pos.floor()
+    elif interpolation == "higher":
+        pos = pos.ceil()
+    elif interpolation == "nearest":
+        pos = pos.round()
+    below = pos.to(torch.int64).clamp_(0, L - 1)
+    above = pos.ceil().to(torch.int64).clamp_(0, L - 1)
+    lerp = interpolation in ("linear", "midpoint")
+    wanted = sorted(set(below.tolist()) | (set(above.tolist()) if lerp else set()) | {0, L - 1})
+    flat = rows.reshape(num_rows, L)
+    parts = [select_rows(flat, wanted[c:c + 16], -1, False, stream) for c in range(0, len(wanted), 16)]
+    with torch.cuda.stream(stream):
+        vals = parts[0] if len(parts) == 1 else torch.cat(parts, dim=-1)
+        col = {r: j for j, r in enumerate(wanted)}
+        dev = x.device
+        res = vals[:, torch.tensor([col[r] for r in below.tolist()], device=dev)]
+        if lerp:
+            w = torch.full_like(qv, 0.5) if interpolation == "midpoint" else pos - below.to(x.dtype)
+            hi = vals[:, torch.tensor([col[r] for r in above.tolist()], device=dev)]
+            res = torch.lerp(res, hi, w.to(dev).expand_as(res))
+        nan_row = vals[:, col[0]].isnan() | vals[:, col[L - 1]].isnan()
+        res = torch.where(nan_row[:, None], torch.full_like(res, float("nan")), res)
+        shape = _reduced_shape(x, dim, keepdim)
+        if qt.dim() == 0:
+            return res.reshape(shape)
+        return res.t().reshape((qv.numel(),) + shape)
 
 
 def sort_segments(x: torch.Tensor, offsets: torch.Tensor, descending: bool = False, return_indices: bool = True,

@@ -111,6 +111,17 @@ class OneSweepSorterB200 {
                                     largest ? 1 : 0, sorted ? 1 : 0, stream),
               "osb200_topk_long_rows");
     }
+    // columns h_ranks[0 .. num_ranks) (host array, 1 to 16 strictly increasing ranks below row_len) of every row's ascending
+    // stable sort into [r*num_ranks, (r+1)*num_ranks) of d_values_out, and their positions within the row into d_indices (may be
+    // null); rows above 16,384 keys (8,192 for 8-byte keys) use this handle's alternate keys for a bound that depends on
+    // num_rows, row_len and num_ranks only
+    void SelectRows(const void* d_keys_in, void* d_values_out, uint32_t* d_indices, uint64_t num_rows, uint32_t row_len,
+                    const uint32_t* h_ranks, uint32_t num_ranks, int key_bytes, int key_type, void* stream = nullptr)
+    {
+        check(osb200_select_rows(h_, d_keys_in, d_values_out, d_indices, num_rows, row_len, h_ranks, num_ranks, key_bytes, key_type,
+                                 stream),
+              "osb200_select_rows");
+    }
     // the first m = min(length, k) keys of every segment [offsets[s], offsets[s+1]) in its stable sort (ascending, or descending
     // for largest) and their positions within the segment, into row s of [num_segments, k] outputs; columns m .. k-1 are
     // padding (position 0xFFFFFFFF, the key that sorts last); segments whose offsets decrease or pass n are all padding;

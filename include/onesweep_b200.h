@@ -334,6 +334,45 @@ OSB200_API int osb200_topk_long_rows(osb200_handle h, const void* d_keys_in, voi
                                      uint64_t num_rows, uint32_t row_len, uint32_t k, int key_bytes, int key_type,
                                      int largest, int sorted, void* stream);
 
+/* Row select: the keys at given ranks of every row, and where they are (kthvalue, median, quantile).  Row r of d_keys_in is
+ * elements [r * row_len, (r + 1) * row_len); key_bytes, key_type, their codec and the natural alignment are those of
+ * osb200_sort_rows (all ten key types).  h_ranks is a HOST array of num_ranks ranks shared by every row: 1 <= num_ranks <= 16,
+ * strictly increasing, each below row_len.  Its values travel in the launch parameters, so a captured graph replays with the
+ * ranks of the capture (as with row_len).
+ * Output: [num_rows, num_ranks] arrays.  d_values_out[r * num_ranks + i] is column h_ranks[i] of the row's ASCENDING stable
+ * sort -- bit for bit what osb200_sort_long_rows(descending = 0) writes there -- and d_indices[r * num_ranks + i] (d_indices
+ * may be NULL: values only) that column's uint32 position within the row, so among equal keys a rank picks by position.
+ * Ascending only: the j-th largest is rank row_len - 1 - j, which with ties is NOT column j of the descending stable sort
+ * (that one takes the lowest position among equal keys, rank row_len - 1 - j the highest ones first).
+ * Errors, in the order of the other row calls: a null handle, or a bad key_bytes / key_type pair (OSB200_ERR_INVALID_ARG);
+ * then num_rows == 0 is a no-op; then a null input or output, a misaligned pointer, sizes that overflow 64 bits, or any
+ * overlap among the three arrays (no in-place form); then a bad rank list (h_ranks NULL, num_ranks 0 or above 16, not
+ * strictly increasing, a rank >= row_len).  All OSB200_ERR_INVALID_ARG.  row_len == 1 writes the key and position 0.
+ * Path rule, with C = 16,384 (8,192 for 8-byte keys):
+ *   - row_len <= C: the row sort's own kernels (one warp per row up to 256 keys, else one thread block per row) sort each
+ *     row in shared memory and store only the requested columns.  No workspace: any handle will do.
+ *   - row_len > C: the split path, a multi-rank MSD radix select over each row's tiles of 8,192 keys spread over the GPU
+ *     (DESIGN 4.19).  Per digit level one count of every tile (each key counted at most once, by the group of ranks sharing
+ *     its prefix) and one pick per row; with d_indices a count of the selected keys per tile, a scan of those counts and a
+ *     locate in the one tile that holds each answer.  No tile waits on another.  It reads every key key_bytes times for
+ *     values only, key_bytes + 1 times with positions, plus the tiles that hold an answer.
+ *   - the test hook "debug_long_rows" sends every row of 2 or more keys to the split path.
+ * The split path stores no keys and allocates nothing.  Its workspace lives in the handle's alternate keys (the reductions,
+ * payloads and control block are not touched); in 32-bit words, with R = num_ranks, T = ceil(row_len / 8192) and
+ * round4(x) = x rounded up to a multiple of 4:
+ *     W = round4(16 + num_rows * R * 260)                                   [plan words, per rank a 4-word state and 256 totals]
+ *       + (d_indices ? round4(num_rows * R * T) : 0)                        [per tile one count per rank]
+ *       + (d_indices && R * T > 4096 ? round4(num_rows * ceil(R * T / 4096)) : 0)   [the scan's chunk sums]
+ * and it needs W * 4 <= the alternate keys' bytes (at least max_n * the handle's key width), else OSB200_ERR_SIZE, decided
+ * before anything is enqueued.  The bound depends on num_rows, row_len, num_ranks and d_indices only: the split path does
+ * not need num_rows * row_len <= max_n, a key width or payloads.  A handle with max_n >= num_rows * row_len always has the
+ * room outside the test hook: its alternate keys hold at least 4 * row_len >= 32,772 bytes per row, against at most about
+ * 16.7 KB + 64 * T bytes per row of W.
+ * Asynchronous, no host synchronisation, graph-capturable; one call in flight per handle. */
+OSB200_API int osb200_select_rows(osb200_handle h, const void* d_keys_in, void* d_values_out, uint32_t* d_indices,
+                                  uint64_t num_rows, uint32_t row_len, const uint32_t* h_ranks, uint32_t num_ranks, int key_bytes,
+                                  int key_type, void* stream);
+
 /* Sort on a bit range [begin_bit, end_bit) of the (unsigned) key only, CUB-style: keys that agree on those bits keep their
  * input order (stable).  ceil((end_bit-begin_bit)/8) digit passes instead of key_bytes; the last digit may be narrower
  * than 8 bits; an odd pass count is handled inside (the result is always returned in the caller's buffers).  d_values may
@@ -415,7 +454,8 @@ OSB200_API int osb200_init_random_u32(uint32_t* d_keys, uint32_t* d_payload, uin
  *                    path too, with its workspace rules (short rows have a tile each, so many of them may need more room
  *                    than max_n gives: OSB200_ERR_SIZE), to compare it with osb200_sort_rows; 0 (default) = osb200_sort_rows' launch.
  *                    osb200_sort_long_segments honours it too: its segments of 2 .. 16,384 (8,192) keys then take the long path,
- *                    and osb200_topk_long_rows: its rows of 2 or more keys then take the split path
+ *                    and osb200_topk_long_rows: its rows of 2 or more keys then take the split path, and osb200_select_rows
+ *                    likewise
  *   "debug_topk_capacity"  test hook of osb200_topk_rows: N > 0 keeps at most N candidates of a row in shared memory (instead
  *                    of 16,384, or 8,192 for 8-byte keys), so that short rows exercise the passes that read global memory
  *                    and the switch to shared memory; 0 (default) = the full capacity.  osb200_topk_long_rows' split path
