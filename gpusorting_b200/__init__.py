@@ -19,9 +19,13 @@ from .onesweep import (  # noqa: F401
     init_random,
     kthvalue,
     median,
+    median_segments,
     quantile,
+    quantile_segments,
     release_cached_sorters,
     select_rows,
+    select_segments,
+    select_segments_workspace,
     select_workspace_words,
     sort_long_rows,
     sort_long_segments,

@@ -45,6 +45,9 @@ SIGNATURES = {
                                  c_vp]),
     "osb200_select_rows": (c_int, [c_vp, c_vp, c_vp, c_vp, c_u64, ctypes.c_uint32, ctypes.POINTER(c_u32), ctypes.c_uint32, c_int, c_int,
                                    c_vp]),
+    "osb200_select_segments": (c_int, [c_vp, c_vp, c_vp, c_vp, c_u64, c_vp, c_u64, ctypes.c_uint32, c_vp, ctypes.c_uint32, c_int,
+                                       c_int, c_vp]),
+    "osb200_select_segments_workspace_words": (c_u64, [c_u64, c_u64, ctypes.c_uint32, c_int, c_int]),
     "osb200_topk_segments": (c_int, [c_vp, c_vp, c_vp, c_vp, c_u64, c_vp, c_u64, ctypes.c_uint32, c_int, c_int, c_int, c_int,
                                      c_vp]),
     "osb200_sort_bits": (c_int, [c_vp, c_vp, c_vp, c_u64, c_int, c_int, c_vp]),

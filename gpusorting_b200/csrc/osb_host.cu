@@ -24,7 +24,7 @@
 
 namespace {
 
-constexpr int kVersion = 1013;  // 1002: device plan, bit ranges, forward-progress fallback, hot passes, segmented sort; 1003: argsort;
+constexpr int kVersion = 1014;  // 1002: device plan, bit ranges, forward-progress fallback, hot passes, segmented sort; 1003: argsort;
                                 // 1004: 16-bit keys (osb200_sort_keys16, osb200_sort_pairs16, osb200_argsort16);
                                 // 1005: row sort (osb200_sort_rows);
                                 // 1006: 64-bit keys with uint32 payloads and their argsort (osb200_create_pairs64);
@@ -34,7 +34,8 @@ constexpr int kVersion = 1013;  // 1002: device plan, bit ranges, forward-progre
                                 // 1010: rows of any length (osb200_sort_long_rows);
                                 // 1011: segments of any length (osb200_sort_long_segments);
                                 // 1012: row top-k of long rows and any k (osb200_topk_long_rows);
-                                // 1013: row select at given ranks (osb200_select_rows)
+                                // 1013: row select at given ranks (osb200_select_rows);
+                                // 1014: segment select at per-segment ranks (osb200_select_segments)
 constexpr int kMaxPlaces = 8;
 
 inline int cuda_status(cudaError_t e) { return e == cudaSuccess ? OSB200_OK : OSB200_ERR_CUDA - static_cast<int>(e); }
@@ -977,6 +978,65 @@ int osb200_topk_segments(osb200_handle h, const void* d_keys_in, void* d_values_
                                       h->debug_rows_block, h->sm_count, static_cast<uint32_t*>(h->alt_keys), h->err(),
                                       static_cast<cudaStream_t>(stream)));
     return OSB200_OK;
+}
+
+// Segment select: the checks of the segment top-k, then the rank array and count; segments of at most row_sort_capacity keys
+// take the class kernels with the workspace of check_segment_workspace, longer ones (with the test hook debug_long_rows every
+// segment of two or more keys) the split path over the long list, whose workspace -- select_segments_layout(...).words u32,
+// bounded from n, num_segments, num_ranks, the key width and d_indices only -- lives in the handle's alternate payloads.
+int osb200_select_segments(osb200_handle h, const void* d_keys_in, void* d_values_out, uint32_t* d_indices, uint64_t n,
+                           const uint64_t* d_segment_offsets, uint64_t num_segments, uint32_t max_segment_len, const uint32_t* d_ranks,
+                           uint32_t num_ranks, int key_bytes, int key_type, void* stream)
+{
+    if (check_handle(h) != OSB200_OK) return OSB200_ERR_INVALID_ARG;
+    osb::KeyCodec c;
+    const osb::KeyCodec* codec = nullptr;
+    int st = codec_for(key_bytes, key_type, 0, kRaggedCodecFlags, &c, &codec);
+    if (st != OSB200_OK) return st;
+    // (n == 0 is not a no-op: every row is then padding)
+    if (num_segments == 0) return OSB200_OK;
+    const uint64_t m = num_segments * num_ranks;
+    const uint64_t kb = n * static_cast<uint64_t>(key_bytes), ob = m * static_cast<uint64_t>(key_bytes), ib = m * sizeof(uint32_t),
+                   fb = (num_segments + 1) * sizeof(uint64_t);
+    // the outputs have another shape than the input: no in-place form
+    const ArrayArg arrays[] = {{d_keys_in, kb, key_bytes, n != 0, false}, {d_values_out, ob, key_bytes, true, true},
+                               {d_indices, ib, 4, false, true}, {d_segment_offsets, fb, 8, true, false}, {d_ranks, ib, 4, true, false}};
+    st = check_arrays(arrays, n <= UINT64_MAX / 8 && num_segments <= UINT64_MAX / 8 - 1 &&
+                                  (num_ranks == 0 || num_segments <= UINT64_MAX / 8 / num_ranks), false);
+    if (st != OSB200_OK) return st;
+    // the arrays the call only reads may not overlap either
+    const uintptr_t pk = reinterpret_cast<uintptr_t>(d_keys_in), pf = reinterpret_cast<uintptr_t>(d_segment_offsets),
+                    pr = reinterpret_cast<uintptr_t>(d_ranks);
+    if ((d_keys_in && (overlaps(pk, kb, pf, fb) || overlaps(pk, kb, pr, ib))) || overlaps(pf, fb, pr, ib)) return OSB200_ERR_INVALID_ARG;
+    if (num_ranks == 0 || num_ranks > osb::kMaxSelectRanks) return OSB200_ERR_INVALID_ARG;
+    if ((st = check_segment_workspace(h, num_segments)) != OSB200_OK) return st;
+    const uint32_t cap = osb::row_sort_capacity(key_bytes);
+    const uint32_t long_min = h->debug_long_rows ? 2u : cap + 1;
+    // no valid segment is longer than n: the path rule and the kernels see max_segment_len clamped to it, so a loose bound on
+    // a small input never takes the long path (whose long list would have no room for any segment)
+    const uint32_t max_len = n < max_segment_len ? static_cast<uint32_t>(n) : max_segment_len;
+    uint32_t* scratch = nullptr;
+    if (max_len >= long_min) {
+        // the split path's bound (the header): a handle with payloads and max_n >= max(n, num_segments) always meets it
+        // outside the test hook
+        if (h->value_bytes != 4) return OSB200_ERR_INVALID_ARG;
+        const osb::SelectSegLayout l = osb::select_segments_layout(n, num_segments, long_min, num_ranks, d_indices != nullptr);
+        if (l.words > h->max_n || l.tile_cap > UINT32_MAX || l.chunk_cap > UINT32_MAX) return OSB200_ERR_SIZE;
+        scratch = h->alt_vals;
+    }
+    OSB_TRY(osb::launch_select_segments(d_keys_in, d_values_out, d_indices, n, reinterpret_cast<const unsigned long long*>(d_segment_offsets),
+                                        num_segments, max_len, d_ranks, num_ranks, key_bytes, codec, h->cfg.rank_mode,
+                                        h->debug_rows_block, scratch ? long_min : 0u, h->sm_count, static_cast<uint32_t*>(h->alt_keys),
+                                        h->err(), scratch, static_cast<cudaStream_t>(stream)));
+    return OSB200_OK;
+}
+
+uint64_t osb200_select_segments_workspace_words(uint64_t n, uint64_t num_segments, uint32_t num_ranks, int key_bytes, int indices)
+{
+    if ((key_bytes != 2 && key_bytes != 4 && key_bytes != 8) || num_ranks == 0 || num_ranks > osb::kMaxSelectRanks) return 0;
+    const uint32_t long_min = osb::row_sort_capacity(key_bytes) + 1;
+    if (n < long_min || num_segments == 0) return 0;  // the long path cannot run
+    return osb::select_segments_layout(n, num_segments, long_min, num_ranks, indices != 0).words;
 }
 
 int osb200_sort_host_keys_u32(osb200_handle h, uint32_t* h_keys, uint64_t n)

@@ -2276,6 +2276,36 @@ __device__ __forceinline__ uint32_t select_rank_of(const SelectRanks& ranks, uin
     return r;
 }
 
+// osb200_select_segments' ranks of one segment, by one whole warp, lane i < nr holding rank i in r: how many of them take part
+// -- the ranks below the segment's length len, a prefix since they do not decrease -- or 0 when they decrease anywhere (the
+// whole row is then padding).
+__device__ __forceinline__ uint32_t select_ranks_active(uint32_t r, uint32_t nr, unsigned long long len)
+{
+    const uint32_t lane = threadIdx.x & 31;
+    const uint32_t prev = __shfl_up_sync(0xffffffffu, r, 1);
+    if (__any_sync(0xffffffffu, lane > 0 && lane < nr && r < prev)) return 0;
+    return static_cast<uint32_t>(__popc(__ballot_sync(0xffffffffu, lane < nr && r < len)));
+}
+
+// The RCOLS store (osb200_select_segments' warp and block classes), by one whole warp over a sorted run of len keys in shared
+// memory (encoded, positions in sorted_idx): lane i < nr stores column ranks[i] to obase + i of out and idx_out, or padding --
+// the decoded all-ones key and the position 0xFFFFFFFF -- for a rank that takes no part (select_ranks_active).
+template <typename KeyT, bool INDICES>
+__device__ __forceinline__ void select_store_ranks(const KeyT* sorted, const uint32_t* sorted_idx, uint32_t len,
+                                                   const uint32_t* __restrict__ ranks, uint32_t nr, KeyT* out, uint32_t* idx_out,
+                                                   uint64_t obase, bool dec, KeyT ca, KeyT cb, KeyT cd)
+{
+    const uint32_t lane = threadIdx.x & 31;
+    const uint32_t r = lane < nr ? ranks[lane] : 0xffffffffu;
+    const uint32_t na = select_ranks_active(r, nr, len);
+    if (lane < nr) {
+        KeyT k = lane < na ? sorted[r] : static_cast<KeyT>(~static_cast<KeyT>(0));
+        if (dec) k = codec_decode<KeyT>(k, ca, cb, cd);
+        out[obase + lane] = k;
+        if constexpr (INDICES) idx_out[obase + lane] = lane < na ? sorted_idx[r] : 0xFFFFFFFFu;
+    }
+}
+
 // osb200_sort_segments' class counts (see segment_bin_kernel)
 enum SegCount : int { kSegCountWarp = 0, kSegCountBlock1 = 1, kSegCountBlock2 = 2, kSegCountBlockList = 3, kSegCounts = 4 };
 // osb200_sort_long_segments' counts after them: the long list's length, then its tiles and scan chunks (see launch_long_segments)
@@ -2297,17 +2327,21 @@ enum LongSegCount : int { kSegCountLong = 4, kSegCountLongTiles = 5, kSegCountLo
 // instantiations spill; the row count is a kernel parameter, as for ROWS.)
 // COLS (with ROWS; osb200_select_rows, select_rows_block_kernel): only the sorted row's columns ranks->r[0 .. count - 1] are
 // stored, to [s * count, (s + 1) * count) of keys and vals.
+// RCOLS (with LIST; osb200_select_segments, select_segment_block_kernel): only the sorted segment's columns
+// seg_ranks[s * nr .. s * nr + nr) are stored, to [s * nr, (s + 1) * nr) of keys and vals (select_store_ranks, by warp 0).
 // max_len: the caller's max_segment_len (<= T); longer segments are left as they are.
 template <typename KeyT, bool PAIRS, int K, int WARPS, int RANK_MODE, bool INDICES, bool ROWS, bool LIST, bool ROW_SEL = false,
-          bool COLS = false>
+          bool COLS = false, bool RCOLS = false>
 __device__ __forceinline__ void segment_sort_body(KeyT* keys, uint32_t* vals, const unsigned long long* __restrict__ seg_off,
                                                   uint64_t num_segments, uint64_t single_n, uint32_t max_len, uint32_t begin_bit,
                                                   uint32_t places, uint32_t last_bits, const KeyCodec& codec,
                                                   const KeyT* __restrict__ keys_in, const uint32_t* __restrict__ seg_list,
                                                   const unsigned long long* __restrict__ seg_counts, uint64_t sel_n = 0,
-                                                  uint32_t sel_min = 0, const SelectRanks* ranks = nullptr)
+                                                  uint32_t sel_min = 0, const SelectRanks* ranks = nullptr,
+                                                  const uint32_t* __restrict__ seg_ranks = nullptr, uint32_t nr = 0)
 {
     static_assert(!(ROWS && LIST), "one addressing mode");
+    static_assert(!RCOLS || LIST, "the columns of listed segments");
     static_assert(!ROW_SEL || ROWS, "a selection of rows");
     static_assert(!COLS || (ROWS && !ROW_SEL), "the columns of rows");
     static_assert(!INDICES || PAIRS, "the indices are the payloads");
@@ -2407,6 +2441,12 @@ __device__ __forceinline__ void segment_sort_body(KeyT* keys, uint32_t* vals, co
                 keys[seg * ranks->count + tid] = k;
                 if constexpr (PAIRS) vals[seg * ranks->count + tid] = sm.sorted_val[rk];
             }
+            continue;
+        }
+        if constexpr (RCOLS) {  // (as COLS)
+            if (warp == 0)
+                select_store_ranks<KeyT, PAIRS>(sm.sorted, sm.sorted_val, len, seg_ranks + seg * nr, nr, keys, vals, seg * nr, dec, ca,
+                                                cb, cd);
             continue;
         }
         // the padding sits behind the `len` real keys
@@ -2614,14 +2654,19 @@ __device__ __forceinline__ WarpSortCtx<KeyT> warp_sort_ctx(uint32_t* hist, const
 // all-ones key that the padding carries through the sort and the position 0xFFFFFFFF.
 // COLS (osb200_select_rows, select_rows_warp_kernel; not with TOPK): only the sorted run's columns ranks->r[0 .. count - 1] are
 // stored, at [obase, obase + count) of out and (with INDICES) idx_out.
-template <typename KeyT, int K, int RANK_MODE, bool INDICES, bool TOPK = false, bool PAD = false, bool COLS = false>
+// RCOLS (osb200_select_segments, select_segment_warp_kernel; not with TOPK or COLS): only the sorted run's columns
+// seg_ranks[0 .. nr) are stored, at [obase, obase + nr), by select_store_ranks.
+template <typename KeyT, int K, int RANK_MODE, bool INDICES, bool TOPK = false, bool PAD = false, bool COLS = false,
+          bool RCOLS = false>
 __device__ __forceinline__ void warp_sort_run(RowWarpSmem<KeyT, K, INDICES>& sm, const WarpSortCtx<KeyT>& x, const KeyT* in, KeyT* out,
                                               uint32_t* idx_out, uint64_t base, uint32_t len, const uint32_t* idx_in = nullptr,
-                                              uint64_t obase = 0, uint32_t keep = 0, const SelectRanks* ranks = nullptr)
+                                              uint64_t obase = 0, uint32_t keep = 0, const SelectRanks* ranks = nullptr,
+                                              const uint32_t* seg_ranks = nullptr, uint32_t nr = 0)
 {
     static_assert(!TOPK || INDICES, "top-k stores positions");
     static_assert(!PAD || TOPK, "padding is a top-k store");
     static_assert(!(COLS && TOPK), "one store");
+    static_assert(!(RCOLS && (TOPK || COLS)), "one store");
     const int lane = x.lane;
     uint4* h4 = x.h4;
     const uint32_t lt = x.lt;
@@ -2698,6 +2743,17 @@ __device__ __forceinline__ void warp_sort_run(RowWarpSmem<KeyT, K, INDICES>& sm,
             if constexpr (INDICES) idx_out[obase + lane] = sm.idx[rk];
         }
         __syncwarp();  // the next run's passes overwrite the staging area
+        return;
+    }
+    if constexpr (RCOLS) {  // (as COLS)
+#pragma unroll
+        for (int i = 0; i < K; ++i) {
+            sm.keys[i * 32 + lane] = key[i];
+            if constexpr (INDICES) sm.idx[i * 32 + lane] = val[i];
+        }
+        __syncwarp();
+        select_store_ranks<KeyT, INDICES>(sm.keys, sm.idx, len, seg_ranks, nr, out, idx_out, obase, dec, ca, cb, cd);
+        __syncwarp();
         return;
     }
 #pragma unroll
@@ -2788,8 +2844,11 @@ cudaError_t launch_row_sort(const void* keys_in, void* keys_out, uint32_t* indic
 // LONG (osb200_sort_long_segments, long_segment_bin_kernel): segments of long_min to max_len keys go to the long list
 // instead (ids in arrival order, at most long_cap of them; counts[kSegCountLong] counts them all), the shorter ones to the
 // classes as above.
+// SEL (osb200_select_segments, select_segment_bin_kernel): every segment is listed, as with TOPK.  Segments of 2 to max_len
+// keys inside [0, n) go to the block classes by length (with LONG those of long_min or more to the long list) unless they
+// have at most warp_max keys; all others -- fewer than two keys, empty, and invalid ones -- to the warp list.
 // =====================================================================================================
-template <typename KeyT, bool TOPK, bool LONG = false>
+template <typename KeyT, bool TOPK, bool LONG = false, bool SEL = false>
 __device__ __forceinline__ void segment_bin_body(const unsigned long long* __restrict__ off, uint64_t num_segments, uint64_t n,
                                                  uint32_t max_len, uint32_t* __restrict__ list,
                                                  unsigned long long* __restrict__ counts, const KeyT* keys_in, KeyT* keys_out,
@@ -2805,6 +2864,13 @@ __device__ __forceinline__ void segment_bin_body(const unsigned long long* __res
         if (TOPK && s < num_segments) {
             const unsigned long long lo = off[s], hi = off[s + 1];
             cls = lo <= hi && hi <= n && hi - lo > warp_max && hi - lo <= 0xFFFFFFFFull ? 1 : 0;
+        } else if (SEL && s < num_segments) {
+            const unsigned long long lo = off[s], hi = off[s + 1], len = hi - lo;
+            cls = !(lo <= hi && hi <= n && len <= max_len) || len < 2 ? 0
+                  : LONG && len >= long_min                          ? 3
+                  : len <= warp_max                                  ? 0
+                  : len <= kSegBlock1Max                             ? 1
+                                                                     : 2;
         } else if (s < num_segments) {
             const unsigned long long lo = off[s], hi = off[s + 1];
             if (lo <= hi && hi <= n && hi - lo <= max_len) {
@@ -3058,7 +3124,7 @@ struct LongSegGeo {
     const uint32_t* tfirst;
     const uint32_t* cfirst;
     const unsigned long long* counts;
-    struct Tile { uint64_t cb, lo; uint32_t t, t0, len, tpr; };
+    struct Tile { uint64_t cb, lo; uint32_t t, t0, len, tpr; uint64_t r; };  // r: the list entry (osb200_select_segments)
     struct Chunk { uint64_t base, c0, row_counts; };
     struct Group { uint64_t first; uint32_t count; };
     __device__ __forceinline__ uint32_t listed() const { return static_cast<uint32_t>(counts[kSegCountLong]); }
@@ -3070,7 +3136,7 @@ struct LongSegGeo {
         const uint32_t seg_len = static_cast<uint32_t>(off[s + 1] - lo);
         const uint32_t t = static_cast<uint32_t>(g - f), t0 = t * kLongRowTile;
         const uint32_t len = seg_len - t0 < kLongRowTile ? seg_len - t0 : kLongRowTile;
-        return {static_cast<uint64_t>(f) * kRadix, lo, t, t0, len, tfirst[j + 1] - f};
+        return {static_cast<uint64_t>(f) * kRadix, lo, t, t0, len, tfirst[j + 1] - f, j};
     }
     template <typename D>
     __device__ __forceinline__ uint64_t cnt_index(const Tile& x, D d) const { return x.cb + static_cast<uint64_t>(d) * x.tpr + x.t; }
@@ -4534,10 +4600,50 @@ __device__ __forceinline__ uint32_t select_group_of(U p, const U* s_v, uint32_t 
     return s_v[g] == p ? g : ng;
 }
 
-template <typename KeyT>
-__global__ void __launch_bounds__(kLongThreads)
-select_count_kernel(const KeyT* __restrict__ in, uint64_t num_rows, uint32_t row_len, uint32_t tpr, uint32_t nr, uint32_t level,
-                    const SelectState* __restrict__ st, uint32_t* __restrict__ tot, KeyCodec codec)
+// The split path's bodies are templated on where the rows are (Geo): LongRowGeo, osb200_select_rows' rows with the ranks
+// of the launch parameters, or LongSegGeo, osb200_select_segments' long list (DESIGN §4.20), whose entry j is segment list[j]
+// with the ranks seg_ranks[list[j] * nr ..] in device memory.  A state, its totals and its tile counts are indexed by row or
+// list entry.  A segment's ranks at or past its length, or all of them when they decrease, take no part: only the first
+// `active` ranks are grouped, counted, picked and located, and the pick's last level pads the others.
+__device__ __forceinline__ uint32_t select_active(const LongRowGeo&, uint64_t, uint32_t nr, const uint32_t*, uint32_t* = nullptr)
+{
+    return nr;
+}
+// (one whole warp; lane i < nr gets rank i in *rk)
+__device__ __forceinline__ uint32_t select_active(const LongSegGeo& geo, uint64_t j, uint32_t nr, const uint32_t* __restrict__ seg_ranks,
+                                                  uint32_t* rk = nullptr)
+{
+    const uint32_t lane = threadIdx.x & 31, s = geo.list[j];
+    const uint32_t r = lane < nr ? seg_ranks[static_cast<uint64_t>(s) * nr + lane] : 0xffffffffu;
+    if (rk) *rk = r;
+    return select_ranks_active(r, nr, geo.off[s + 1] - geo.off[s]);
+}
+// the rows of the pick: num_rows, or the listed segments
+__device__ __forceinline__ uint64_t select_rows_of(const LongRowGeo&, uint64_t num_rows) { return num_rows; }
+__device__ __forceinline__ uint64_t select_rows_of(const LongSegGeo& geo, uint64_t) { return geo.listed(); }
+// where row r's columns go in the [rows or segments, nr] outputs
+__device__ __forceinline__ uint64_t select_obase(const LongRowGeo&, uint64_t r, uint32_t nr) { return r * nr; }
+__device__ __forceinline__ uint64_t select_obase(const LongSegGeo& geo, uint64_t j, uint32_t nr)
+{
+    return static_cast<uint64_t>(geo.list[j]) * nr;
+}
+// where the equal-key counts of rank i of a tile's row start (tile t's is t further): [row][rank][tile], or per list entry
+// [rank][tile] from nr * its first tile
+__device__ __forceinline__ uint64_t select_cnt_base(const LongRowGeo& geo, const LongRowGeo::Tile& x, uint32_t nr, uint32_t i)
+{
+    return (x.r * nr + i) * geo.tpr;
+}
+__device__ __forceinline__ uint64_t select_cnt_base(const LongSegGeo&, const LongSegGeo::Tile& x, uint32_t nr, uint32_t i)
+{
+    return x.cb / kRadix * nr + static_cast<uint64_t>(i) * x.tpr;
+}
+__device__ __forceinline__ uint32_t select_tpr(const LongRowGeo& geo, const LongRowGeo::Tile&) { return geo.tpr; }
+__device__ __forceinline__ uint32_t select_tpr(const LongSegGeo&, const LongSegGeo::Tile& x) { return x.tpr; }
+
+template <typename KeyT, typename Geo>
+__device__ __forceinline__ void select_count_body(const Geo& geo, const KeyT* __restrict__ in, uint32_t nr, uint32_t level,
+                                                  const SelectState* __restrict__ st, uint32_t* __restrict__ tot, const KeyCodec& codec,
+                                                  const uint32_t* __restrict__ seg_ranks)
 {
     using U = std::conditional_t<sizeof(KeyT) == 8, uint64_t, uint32_t>;
     constexpr uint32_t D = sizeof(KeyT);
@@ -4551,11 +4657,10 @@ select_count_kernel(const KeyT* __restrict__ in, uint64_t num_rows, uint32_t row
     __shared__ U s_v[kMaxSelectRanks];
     __shared__ uint32_t s_first[kMaxSelectRanks], s_gi[kMaxSelectRanks], s_ng;
     const uint32_t lane = threadIdx.x & 31;
-    const LongRowGeo geo{num_rows, row_len, tpr, 0, 0};
     const uint64_t tiles = geo.tiles();
     for (uint64_t g = blockIdx.x; g < tiles; g += gridDim.x) {
         const auto x = geo.tile(g);
-        if (threadIdx.x < 32) select_groups<U>(st + x.r * nr, nr, s_v, s_first, s_gi, &s_ng);
+        if (threadIdx.x < 32) select_groups<U>(st + x.r * nr, select_active(geo, x.r, nr, seg_ranks), s_v, s_first, s_gi, &s_ng);
         __syncthreads();
         const uint32_t ng = s_ng;
         const uint32_t lc = ng <= 1 ? 5u : ng <= 2 ? 4u : ng <= 4 ? 3u : ng <= 8 ? 2u : 1u, cm = (1u << lc) - 1u;
@@ -4588,19 +4693,46 @@ select_count_kernel(const KeyT* __restrict__ in, uint64_t num_rows, uint32_t row
 }
 
 template <typename KeyT>
-__global__ void __launch_bounds__(kRadix)
-select_pick_kernel(uint64_t num_rows, uint32_t level, SelectState* __restrict__ st, uint32_t* __restrict__ tot, KeyT* __restrict__ out,
-                   SelectRanks ranks, KeyCodec codec)
+__global__ void __launch_bounds__(kLongThreads)
+select_count_kernel(const KeyT* __restrict__ in, uint64_t num_rows, uint32_t row_len, uint32_t tpr, uint32_t nr, uint32_t level,
+                    const SelectState* __restrict__ st, uint32_t* __restrict__ tot, KeyCodec codec)
 {
+    select_count_body<KeyT>(LongRowGeo{num_rows, row_len, tpr, 0, 0}, in, nr, level, st, tot, codec, nullptr);
+}
+
+template <typename KeyT>
+__global__ void __launch_bounds__(kLongThreads)
+select_segments_count_kernel(const KeyT* __restrict__ in, LongSegGeo geo, const uint32_t* __restrict__ seg_ranks, uint32_t nr,
+                             uint32_t level, const SelectState* __restrict__ st, uint32_t* __restrict__ tot, KeyCodec codec)
+{
+    select_count_body<KeyT>(geo, in, nr, level, st, tot, codec, seg_ranks);
+}
+
+// rows: num_rows, with the ranks of `ranks`; long segments: the listed ones, with their own ranks (seg_ranks), and after the
+// last level the columns that take no part are padded (idx_out: their positions, may be null)
+template <typename KeyT, typename Geo>
+__device__ __forceinline__ void select_pick_body(const Geo& geo, uint64_t num_rows, uint32_t nr, uint32_t level, SelectState* __restrict__ st,
+                                                 uint32_t* __restrict__ tot, KeyT* __restrict__ out, const SelectRanks* ranks,
+                                                 const KeyCodec& codec, const uint32_t* __restrict__ seg_ranks, uint32_t* idx_out)
+{
+    constexpr bool SEG = std::is_same_v<Geo, LongSegGeo>;
     constexpr uint32_t D = sizeof(KeyT);
-    const uint32_t shift = 8u * (D - 1u - level), nr = ranks.count;
+    const uint32_t shift = 8u * (D - 1u - level);
     const bool last = level + 1 == D, dec = codec.flags & kCodecDecodeOnStore;
     const KeyT ca = static_cast<KeyT>(codec.a), cb = static_cast<KeyT>(codec.b), cd = static_cast<KeyT>(codec.d);
     __shared__ unsigned long long s_v[kMaxSelectRanks];
-    __shared__ uint32_t s_taken[kMaxSelectRanks], s_need[kMaxSelectRanks], s_wtot[kRadix / 32];
-    const uint32_t rk = select_rank_of(ranks, threadIdx.x);
-    for (uint64_t r = blockIdx.x; r < num_rows; r += gridDim.x) {
+    __shared__ uint32_t s_taken[kMaxSelectRanks], s_need[kMaxSelectRanks], s_wtot[kRadix / 32], s_na;
+    uint32_t rk = SEG ? 0u : select_rank_of(*ranks, threadIdx.x);
+    const uint64_t rows = select_rows_of(geo, num_rows);
+    for (uint64_t r = blockIdx.x; r < rows; r += gridDim.x) {
         SelectState* rs = st + r * nr;
+        uint32_t na = nr;
+        if constexpr (SEG) {
+            if (threadIdx.x < 32) {
+                const uint32_t a = select_active(geo, r, nr, seg_ranks, &rk);
+                if (threadIdx.x == 0) s_na = a;
+            }
+        }
         if (threadIdx.x < nr) {
             const SelectState s = rs[threadIdx.x];
             s_v[threadIdx.x] = s.v;
@@ -4608,9 +4740,11 @@ select_pick_kernel(uint64_t num_rows, uint32_t level, SelectState* __restrict__ 
             s_need[threadIdx.x] = rk - s.taken;
         }
         __syncthreads();
-        for (uint32_t i = 0; i < nr;) {  // group [i, j)
+        if constexpr (SEG) na = s_na;
+        const uint64_t ob = select_obase(geo, r, nr);
+        for (uint32_t i = 0; i < na;) {  // group [i, j)
             uint32_t j = i + 1;
-            while (j < nr && s_v[j] == s_v[i]) ++j;
+            while (j < na && s_v[j] == s_v[i]) ++j;
             uint32_t* t = tot + (r * nr + i) * kRadix;
             const uint32_t c = t[threadIdx.x];
             t[threadIdx.x] = 0;  // for the next level
@@ -4626,21 +4760,47 @@ select_pick_kernel(uint64_t num_rows, uint32_t level, SelectState* __restrict__ 
                     if (last) {
                         KeyT k = static_cast<KeyT>(ns.v);
                         if (dec) k = codec_decode<KeyT>(k, ca, cb, cd);
-                        out[r * nr + q] = k;
+                        out[ob + q] = k;
                     }
                 }
             }
             __syncthreads();  // s_wtot is reused by the next group, s_v etc. by the next row
             i = j;
         }
+        if constexpr (SEG) {
+            if (last && threadIdx.x >= na && threadIdx.x < nr) {
+                const KeyT ones = static_cast<KeyT>(~static_cast<KeyT>(0));
+                out[ob + threadIdx.x] = dec ? codec_decode<KeyT>(ones, ca, cb, cd) : ones;
+                if (idx_out) idx_out[ob + threadIdx.x] = 0xFFFFFFFFu;
+            }
+            __syncthreads();  // s_na and s_v are rewritten for the next entry even when it had no group
+        }
     }
 }
 
-// Per tile, the keys equal to each rank's key (its group's), into cnt[row][rank][tile]; a warp adds the lanes of one group at once.
 template <typename KeyT>
-__global__ void __launch_bounds__(kLongThreads)
-select_eq_count_kernel(const KeyT* __restrict__ in, uint64_t num_rows, uint32_t row_len, uint32_t tpr, uint32_t nr,
-                       const SelectState* __restrict__ st, uint32_t* __restrict__ cnt, KeyCodec codec)
+__global__ void __launch_bounds__(kRadix)
+select_pick_kernel(uint64_t num_rows, uint32_t level, SelectState* __restrict__ st, uint32_t* __restrict__ tot, KeyT* __restrict__ out,
+                   SelectRanks ranks, KeyCodec codec)
+{
+    select_pick_body<KeyT>(LongRowGeo{num_rows, 0, 0, 0, 0}, num_rows, ranks.count, level, st, tot, out, &ranks, codec, nullptr, nullptr);
+}
+
+template <typename KeyT>
+__global__ void __launch_bounds__(kRadix)
+select_segments_pick_kernel(LongSegGeo geo, const uint32_t* __restrict__ seg_ranks, uint32_t nr, uint32_t level,
+                            SelectState* __restrict__ st, uint32_t* __restrict__ tot, KeyT* __restrict__ out, uint32_t* idx_out,
+                            KeyCodec codec)
+{
+    select_pick_body<KeyT>(geo, 0, nr, level, st, tot, out, nullptr, codec, seg_ranks, idx_out);
+}
+
+// Per tile, the keys equal to each rank's key (its group's), into the tile's count of the rank (select_cnt_index); a warp adds
+// the lanes of one group at once.
+template <typename KeyT, typename Geo>
+__device__ __forceinline__ void select_eq_count_body(const Geo& geo, const KeyT* __restrict__ in, uint32_t nr,
+                                                     const SelectState* __restrict__ st, uint32_t* __restrict__ cnt, const KeyCodec& codec,
+                                                     const uint32_t* __restrict__ seg_ranks)
 {
     using U = std::conditional_t<sizeof(KeyT) == 8, uint64_t, uint32_t>;
     const KeyT ca = static_cast<KeyT>(codec.a), cb = static_cast<KeyT>(codec.b), cd = static_cast<KeyT>(codec.d);
@@ -4648,11 +4808,14 @@ select_eq_count_kernel(const KeyT* __restrict__ in, uint64_t num_rows, uint32_t 
     __shared__ U s_v[kMaxSelectRanks];
     __shared__ uint32_t s_first[kMaxSelectRanks], s_gi[kMaxSelectRanks], s_ng, s_c[kMaxSelectRanks];
     const uint32_t lane = threadIdx.x & 31;
-    const LongRowGeo geo{num_rows, row_len, tpr, 0, 0};
     const uint64_t tiles = geo.tiles();
     for (uint64_t g = blockIdx.x; g < tiles; g += gridDim.x) {
         const auto x = geo.tile(g);
-        if (threadIdx.x < 32) select_groups<U>(st + x.r * nr, nr, s_v, s_first, s_gi, &s_ng);
+        uint32_t na = nr;  // (warp 0's, which writes the counts)
+        if (threadIdx.x < 32) {
+            na = select_active(geo, x.r, nr, seg_ranks);
+            select_groups<U>(st + x.r * nr, na, s_v, s_first, s_gi, &s_ng);
+        }
         if (threadIdx.x < kMaxSelectRanks) s_c[threadIdx.x] = 0;
         __syncthreads();
         const uint32_t ng = s_ng;
@@ -4672,33 +4835,61 @@ select_eq_count_kernel(const KeyT* __restrict__ in, uint64_t num_rows, uint32_t 
             if (gi < ng && lane == static_cast<uint32_t>(__ffs(peers) - 1)) atomicAdd(&s_c[gi], static_cast<uint32_t>(__popc(peers)));
         }
         __syncthreads();
-        if (threadIdx.x < nr) cnt[(x.r * nr + threadIdx.x) * tpr + x.t] = s_c[s_gi[threadIdx.x]];
+        if (threadIdx.x < na) cnt[select_cnt_base(geo, x, nr, threadIdx.x) + x.t] = s_c[s_gi[threadIdx.x]];
         __syncthreads();  // s_c and the groups are reused by the next tile
     }
 }
 
-// For every (row, rank) whose occurrence o = r - taken of its key lies in this tile by the scanned counts: the position of the
-// tile's (o - tile prefix)-th key equal to it, in tile order (per-warp ballots and a scan of the warp counts, chunk by chunk).
 template <typename KeyT>
 __global__ void __launch_bounds__(kLongThreads)
-select_locate_kernel(const KeyT* __restrict__ in, uint32_t* __restrict__ idx_out, uint64_t num_rows, uint32_t row_len, uint32_t tpr,
-                     const SelectState* __restrict__ st, const uint32_t* __restrict__ cnt, SelectRanks ranks, KeyCodec codec)
+select_eq_count_kernel(const KeyT* __restrict__ in, uint64_t num_rows, uint32_t row_len, uint32_t tpr, uint32_t nr,
+                       const SelectState* __restrict__ st, uint32_t* __restrict__ cnt, KeyCodec codec)
 {
+    select_eq_count_body<KeyT>(LongRowGeo{num_rows, row_len, tpr, 0, 0}, in, nr, st, cnt, codec, nullptr);
+}
+
+template <typename KeyT>
+__global__ void __launch_bounds__(kLongThreads)
+select_segments_eq_count_kernel(const KeyT* __restrict__ in, LongSegGeo geo, const uint32_t* __restrict__ seg_ranks, uint32_t nr,
+                                const SelectState* __restrict__ st, uint32_t* __restrict__ cnt, KeyCodec codec)
+{
+    select_eq_count_body<KeyT>(geo, in, nr, st, cnt, codec, seg_ranks);
+}
+
+// For every (row, rank) whose occurrence o = r - taken of its key lies in this tile by the scanned counts: the position of the
+// tile's (o - tile prefix)-th key equal to it, in tile order (per-warp ballots and a scan of the warp counts, chunk by chunk).
+template <typename KeyT, typename Geo>
+__device__ __forceinline__ void select_locate_body(const Geo& geo, const KeyT* __restrict__ in, uint32_t* __restrict__ idx_out, uint32_t nr,
+                                                   const SelectState* __restrict__ st, const uint32_t* __restrict__ cnt,
+                                                   const SelectRanks* ranks, const KeyCodec& codec, const uint32_t* __restrict__ seg_ranks)
+{
+    constexpr bool SEG = std::is_same_v<Geo, LongSegGeo>;
     using U = std::conditional_t<sizeof(KeyT) == 8, uint64_t, uint32_t>;
     const KeyT ca = static_cast<KeyT>(codec.a), cb = static_cast<KeyT>(codec.b), cd = static_cast<KeyT>(codec.d);
     const bool enc = codec.flags & kCodecEncodeOnLoad;
-    __shared__ uint32_t s_w[kLongWarps];
-    const uint32_t nr = ranks.count, lane = threadIdx.x & 31, warp = threadIdx.x >> 5, lt = lanemask_lt();
-    const LongRowGeo geo{num_rows, row_len, tpr, 0, 0};
+    __shared__ uint32_t s_w[kLongWarps], s_na;
+    const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5, lt = lanemask_lt();
     const uint64_t tiles = geo.tiles();
     for (uint64_t g = blockIdx.x; g < tiles; g += gridDim.x) {
         const auto x = geo.tile(g);
         const KeyT* tile = in + x.lo + x.t0;
-        for (uint32_t i = 0; i < nr; ++i) {
-            const uint32_t* s = cnt + (x.r * nr + i) * tpr;  // the scan ran over the row's ranks one after another
+        const uint32_t tpr = select_tpr(geo, x);
+        uint32_t na = nr;
+        if constexpr (SEG) {
+            if (threadIdx.x < 32) {
+                const uint32_t a = select_active(geo, x.r, nr, seg_ranks);
+                if (threadIdx.x == 0) s_na = a;
+            }
+            __syncthreads();
+            na = s_na;
+        }
+        for (uint32_t i = 0; i < na; ++i) {
+            const uint32_t* s = cnt + select_cnt_base(geo, x, nr, i);  // the scan ran over the row's ranks one after another
             const uint32_t b0 = s[0], lo = s[x.t] - b0, hi = x.t + 1 < tpr ? s[x.t + 1] - b0 : 0xffffffffu;
             const SelectState ss = st[x.r * nr + i];
-            const uint32_t o = select_rank_of(ranks, i) - ss.taken;
+            uint32_t o;
+            if constexpr (SEG) o = seg_ranks[select_obase(geo, x.r, nr) + i] - ss.taken;
+            else o = select_rank_of(*ranks, i) - ss.taken;
             if (o < lo || o >= hi) continue;
             const U v = static_cast<U>(ss.v);
             const uint32_t want = o - lo;
@@ -4714,12 +4905,30 @@ select_locate_kernel(const KeyT* __restrict__ in, uint32_t* __restrict__ idx_out
 #pragma unroll
                 for (int w = 0; w < kLongWarps; ++w) { const uint32_t y = s_w[w]; pre += static_cast<uint32_t>(w) < warp ? y : 0u; total += y; }
                 __syncthreads();  // s_w is reused by the next chunk
-                if (eq && run + pre + __popc(b & lt) == want) idx_out[x.r * nr + i] = x.t0 + j;
+                if (eq && run + pre + __popc(b & lt) == want) idx_out[select_obase(geo, x.r, nr) + i] = x.t0 + j;
                 run += total;
                 if (run > want) break;
             }
         }
+        if constexpr (SEG) __syncthreads();  // s_na is rewritten for the next tile
     }
+}
+
+template <typename KeyT>
+__global__ void __launch_bounds__(kLongThreads)
+select_locate_kernel(const KeyT* __restrict__ in, uint32_t* __restrict__ idx_out, uint64_t num_rows, uint32_t row_len, uint32_t tpr,
+                     const SelectState* __restrict__ st, const uint32_t* __restrict__ cnt, SelectRanks ranks, KeyCodec codec)
+{
+    select_locate_body<KeyT>(LongRowGeo{num_rows, row_len, tpr, 0, 0}, in, idx_out, ranks.count, st, cnt, &ranks, codec, nullptr);
+}
+
+template <typename KeyT>
+__global__ void __launch_bounds__(kLongThreads)
+select_segments_locate_kernel(const KeyT* __restrict__ in, uint32_t* __restrict__ idx_out, LongSegGeo geo,
+                              const uint32_t* __restrict__ seg_ranks, uint32_t nr, const SelectState* __restrict__ st,
+                              const uint32_t* __restrict__ cnt, KeyCodec codec)
+{
+    select_locate_body<KeyT>(geo, in, idx_out, nr, st, cnt, nullptr, codec, seg_ranks);
 }
 
 SelectLayout select_layout(uint64_t num_rows, uint32_t row_len, uint32_t num_ranks, bool positions)
@@ -4785,6 +4994,279 @@ cudaError_t launch_select_long_rows(const void* keys_in, void* values_out, uint3
     });
 }
 
+// =====================================================================================================
+// Segment select (osb200_select_segments, DESIGN §4.20): the row select for ragged segments given by offsets, each with its
+// own ranks seg_ranks[s * nr .. s * nr + nr) (device memory, non-decreasing).  Segment s's result is row s of [num_segments,
+// nr] outputs; a column whose rank takes no part (select_ranks_active: at or past the length, or the row's ranks decrease),
+// and every column of an empty or invalid segment, is padding.
+//   * select_segment_bin_kernel (segment_bin_body, SEL) lists every segment: up to warp_max keys (or fewer than two), and the
+//     empty and invalid ones, on the warp list; with LONG segments of long_min or more keys on the long list; the others on
+//     the block list, by the segment sort's two block classes.
+//   * select_segment_warp_kernel (warp_sort_run, RCOLS) and select_segment_block_kernel (segment_sort_body, LIST and RCOLS)
+//     sort each segment in shared memory and store only its columns.
+//   * the long list: long_segments_map_kernel's tile map, then the split path's bodies over it (LongSegGeo), and with
+//     positions the long segments' scan bodies over each entry's [rank][tile] counts (SelectSegScanGeo).  Should the map
+//     not fit its bounds (only offsets that make valid segments overlap can do that), select_segment_unmapped_kernel pads
+//     every long segment instead.
+// =====================================================================================================
+__global__ void __launch_bounds__(256)
+select_segment_bin_kernel(const unsigned long long* __restrict__ off, uint64_t num_segments, uint64_t n, uint32_t max_len,
+                          uint32_t warp_max, uint32_t* __restrict__ list, unsigned long long* __restrict__ counts)
+{
+    segment_bin_body<uint32_t, false, false, true>(off, num_segments, n, max_len, list, counts, nullptr, nullptr, nullptr, warp_max);
+}
+
+__global__ void __launch_bounds__(256)
+select_long_segment_bin_kernel(const unsigned long long* __restrict__ off, uint64_t num_segments, uint64_t n, uint32_t max_len,
+                               uint32_t warp_max, uint32_t* __restrict__ list, unsigned long long* __restrict__ counts,
+                               uint32_t long_min, uint32_t* __restrict__ long_list, uint64_t long_cap)
+{
+    segment_bin_body<uint32_t, false, true, true>(off, num_segments, n, max_len, list, counts, nullptr, nullptr, nullptr, warp_max,
+                                                  long_min, long_list, long_cap);
+}
+
+template <typename KeyT, int RANK_MODE, bool INDICES>
+__global__ void __launch_bounds__(kRowWarps * 32)
+select_segment_warp_kernel(const KeyT* in, KeyT* out, uint32_t* __restrict__ idx_out, uint64_t n, uint32_t max_len,
+                           const unsigned long long* __restrict__ off, const uint32_t* __restrict__ list,
+                           const unsigned long long* __restrict__ counts, const uint32_t* __restrict__ seg_ranks, uint32_t nr,
+                           KeyCodec codec)
+{
+    extern __shared__ __align__(16) unsigned char s_raw[];
+    const int warp = threadIdx.x >> 5;
+    unsigned char* wsm = s_raw + warp * sizeof(RowWarpSmem<KeyT, 8, INDICES>);  // every K's layout starts with the same hist
+    const WarpSortCtx<KeyT> x = warp_sort_ctx<KeyT>(reinterpret_cast<uint32_t*>(wsm), codec);
+    const uint64_t count = counts[kSegCountWarp];
+    for (uint64_t i = static_cast<uint64_t>(blockIdx.x) * kRowWarps + warp; i < count; i += static_cast<uint64_t>(gridDim.x) * kRowWarps) {
+        const uint32_t s = list[i];
+        const unsigned long long lo = off[s], hi = off[s + 1];
+        // offsets that decrease, pass n or exceed max_len: the binning kernel listed it here as empty
+        const uint32_t len = lo <= hi && hi <= n && hi - lo <= max_len && hi - lo <= kRowWarpMaxLen ? static_cast<uint32_t>(hi - lo) : 0u;
+        const uint64_t obase = static_cast<uint64_t>(s) * nr;
+        const uint32_t* rk = seg_ranks + obase;
+        if (len <= 32)
+            warp_sort_run<KeyT, 1, RANK_MODE, INDICES, false, false, false, true>(*reinterpret_cast<RowWarpSmem<KeyT, 1, INDICES>*>(wsm), x,
+                                                                                  in, out, idx_out, lo, len, nullptr, obase, 0u, nullptr, rk, nr);
+        else if (len <= 64)
+            warp_sort_run<KeyT, 2, RANK_MODE, INDICES, false, false, false, true>(*reinterpret_cast<RowWarpSmem<KeyT, 2, INDICES>*>(wsm), x,
+                                                                                  in, out, idx_out, lo, len, nullptr, obase, 0u, nullptr, rk, nr);
+        else if (len <= 128)
+            warp_sort_run<KeyT, 4, RANK_MODE, INDICES, false, false, false, true>(*reinterpret_cast<RowWarpSmem<KeyT, 4, INDICES>*>(wsm), x,
+                                                                                  in, out, idx_out, lo, len, nullptr, obase, 0u, nullptr, rk, nr);
+        else
+            warp_sort_run<KeyT, 8, RANK_MODE, INDICES, false, false, false, true>(*reinterpret_cast<RowWarpSmem<KeyT, 8, INDICES>*>(wsm), x,
+                                                                                  in, out, idx_out, lo, len, nullptr, obase, 0u, nullptr, rk, nr);
+    }
+}
+
+template <typename KeyT, int K, int WARPS, int RANK_MODE, bool INDICES>
+__global__ void __launch_bounds__(WARPS * 32, 1)
+select_segment_block_kernel(const KeyT* __restrict__ in, KeyT* out, uint32_t* idx_out, const unsigned long long* __restrict__ off,
+                            uint64_t num_segments, uint32_t max_len, KeyCodec codec, const uint32_t* __restrict__ list,
+                            const unsigned long long* __restrict__ counts, const uint32_t* __restrict__ seg_ranks, uint32_t nr)
+{
+    segment_sort_body<KeyT, INDICES, K, WARPS, RANK_MODE, INDICES, false, true, false, false, true>(
+        out, idx_out, off, num_segments, 0, max_len, 0u, sizeof(KeyT), 8u, codec, in, list, counts, 0, 0u, nullptr, seg_ranks, nr);
+}
+
+// the block classes' geometries: 2,048 keys, and the row sort's capacity
+template <typename KeyT, int SIZE, bool INDICES>
+struct SelectSegShape {
+    using Key = KeyT;
+    static constexpr bool indices = INDICES, has_hot = false;
+    using G = SegGeomN<KeyT, SIZE>;
+    using S = SegSmem<KeyT, INDICES, G::K, G::WARPS>;
+    static constexpr uint32_t T = S::T;
+    static constexpr size_t smem = sizeof(S);
+    template <int RANK_MODE, bool HOT = false>
+    static constexpr auto kernel() { return select_segment_block_kernel<KeyT, G::K, G::WARPS, RANK_MODE, INDICES>; }
+};
+using SelectSegShapes = TypeList<
+    SelectSegShape<uint16_t, 1, false>, SelectSegShape<uint16_t, 2, false>, SelectSegShape<uint16_t, 1, true>, SelectSegShape<uint16_t, 2, true>,
+    SelectSegShape<uint32_t, 1, false>, SelectSegShape<uint32_t, 2, false>, SelectSegShape<uint32_t, 1, true>, SelectSegShape<uint32_t, 2, true>,
+    SelectSegShape<uint64_t, 1, false>, SelectSegShape<uint64_t, 2, false>, SelectSegShape<uint64_t, 1, true>, SelectSegShape<uint64_t, 2, true>>;
+
+// The long segments' equal-key counts for the scan bodies: entry j's nr * tiles counts [rank][tile] from nr * tfirst[j], cut
+// into chunks of 16 tiles' counts per rank -- as many as long_segments_map_kernel gives the entry (ceil(tiles / 16), from
+// cfirst[j]), so its chunk map serves here too.
+struct SelectSegScanGeo {
+    LongSegGeo seg;
+    uint32_t nr;
+    using Chunk = LongSegGeo::Chunk;
+    using Group = LongSegGeo::Group;
+    __device__ __forceinline__ uint64_t chunks() const { return seg.chunks(); }
+    __device__ __forceinline__ Chunk chunk(uint64_t g) const
+    {
+        const uint32_t j = cta_find(seg.cfirst, seg.listed(), g), f = seg.tfirst[j];
+        const uint64_t w = static_cast<uint64_t>(kLongChunk / kRadix) * nr, c0 = (g - seg.cfirst[j]) * w;
+        const uint64_t rc = static_cast<uint64_t>(seg.tfirst[j + 1] - f) * nr;
+        return {static_cast<uint64_t>(f) * nr + c0, 0, rc - c0 < w ? rc - c0 : w};
+    }
+    __device__ __forceinline__ uint64_t groups() const { return seg.groups(); }
+    __device__ __forceinline__ Group group(uint64_t j) const { return seg.group(j); }
+};
+static_assert(kLongChunk % kRadix == 0, "a chunk of the tile map is whole tiles");
+
+__global__ void __launch_bounds__(kLongThreads)
+select_segments_chunk_sum_kernel(const SortPlan* __restrict__ plan, uint32_t* cnt, uint32_t* __restrict__ csum, SelectSegScanGeo geo)
+{
+    long_chunk_sum_body(geo, plan, 0u, cnt, csum);
+}
+
+__global__ void __launch_bounds__(kLongThreads)
+select_segments_chunk_scan_kernel(const SortPlan* __restrict__ plan, uint32_t* csum, SelectSegScanGeo geo)
+{
+    long_chunk_scan_body(geo, plan, 0u, csum);
+}
+
+__global__ void __launch_bounds__(kLongThreads)
+select_segments_scan_kernel(const SortPlan* __restrict__ plan, uint32_t* cnt, const uint32_t* __restrict__ csum, SelectSegScanGeo geo)
+{
+    long_scan_body(geo, plan, 0u, cnt, csum);
+}
+
+// When the tile map did not fit (counts[kSegCountLong] == 0), every segment the binning kernel sent to the long list is padding.
+template <typename KeyT>
+__global__ void __launch_bounds__(256)
+select_segment_unmapped_kernel(const unsigned long long* __restrict__ off, uint64_t num_segments, uint64_t n, uint32_t max_len,
+                               uint32_t long_min, const unsigned long long* __restrict__ counts, KeyT* out, uint32_t* idx_out,
+                               uint32_t nr, KeyCodec codec)
+{
+    if (counts[kSegCountLong] != 0) return;
+    const KeyT ones = static_cast<KeyT>(~static_cast<KeyT>(0));
+    const KeyT pad = codec.flags & kCodecDecodeOnStore
+                         ? codec_decode<KeyT>(ones, static_cast<KeyT>(codec.a), static_cast<KeyT>(codec.b), static_cast<KeyT>(codec.d))
+                         : ones;
+    for (uint64_t s = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x; s < num_segments;
+         s += static_cast<uint64_t>(gridDim.x) * blockDim.x) {
+        const unsigned long long lo = off[s], hi = off[s + 1];
+        if (!(lo <= hi && hi <= n && hi - lo <= max_len && hi - lo >= long_min)) continue;
+        for (uint32_t i = 0; i < nr; ++i) {
+            out[s * nr + i] = pad;
+            if (idx_out) idx_out[s * nr + i] = 0xFFFFFFFFu;
+        }
+    }
+}
+
+SelectSegLayout select_segments_layout(uint64_t n, uint64_t num_segments, uint32_t long_min, uint32_t num_ranks, bool positions)
+{
+    auto whole = [](uint64_t words) { return (words + 3) / 4 * 4; };  // every array 16-byte aligned
+    SelectSegLayout l;
+    l.list_cap = n / long_min < num_segments ? n / long_min : num_segments;
+    l.tile_cap = (n + kLongRowTile - 1) / kLongRowTile + l.list_cap;
+    l.chunk_cap = (l.tile_cap * kRadix + kLongChunk - 1) / kLongChunk + l.list_cap;
+    l.st = 16;  // words 0 .. 15: a zeroed SortPlan, with which the scan bodies skip nothing
+    l.tot = l.st + l.list_cap * num_ranks * 4;
+    l.zeroed = whole(l.tot + l.list_cap * num_ranks * kRadix);
+    l.list = l.zeroed;
+    l.tfirst = l.list + whole(l.list_cap);
+    l.cfirst = l.tfirst + whole(l.list_cap + 1);
+    l.cnt = l.cfirst + whole(l.list_cap + 1);
+    l.csum = positions ? l.cnt + whole(l.tile_cap * num_ranks) : l.cnt;
+    l.words = positions ? l.csum + whole(l.chunk_cap) : l.csum;
+    return l;
+}
+
+cudaError_t launch_select_segments(const void* keys_in, void* values_out, uint32_t* indices, uint64_t n, const unsigned long long* off,
+                                   uint64_t num_segments, uint32_t max_len, const uint32_t* seg_ranks, uint32_t nr, int key_bytes,
+                                   const KeyCodec* codec_in, int rank_mode, bool block_only, uint32_t long_min, int sm_count,
+                                   uint32_t* list, unsigned long long* counts, uint32_t* scratch, cudaStream_t stream)
+{
+    if (num_segments == 0 || nr == 0 || nr > kMaxSelectRanks || (long_min && (long_min < 2 || !scratch))) return cudaErrorInvalidValue;
+    if (!long_min && max_len > row_sort_capacity(key_bytes)) return cudaErrorInvalidValue;
+    const bool lng = long_min && max_len >= long_min && n >= long_min;  // (then the long list has room for one segment or more)
+    const KeyCodec codec = codec_in ? *codec_in : KeyCodec();
+    const SelectSegLayout l = select_segments_layout(n, num_segments, lng ? long_min : 1u, nr, indices != nullptr);
+    cudaError_t e = cudaMemsetAsync(counts, 0, (lng ? kLongSegCounts : kSegCounts) * sizeof(unsigned long long), stream);
+    if (e == cudaSuccess && lng) e = cudaMemsetAsync(scratch, 0, l.zeroed * sizeof(uint32_t), stream);
+    if (e != cudaSuccess) return e;
+    const uint32_t warp_max = block_only ? 0u : kRowWarpMaxLen;
+    const unsigned bin_grid = capped_grid(num_segments, 256, static_cast<uint64_t>(sm_count) * 8);
+    if (lng)
+        select_long_segment_bin_kernel<<<bin_grid, 256, 0, stream>>>(off, num_segments, n, max_len, warp_max, list, counts, long_min,
+                                                                     scratch + l.list, l.list_cap);
+    else
+        select_segment_bin_kernel<<<bin_grid, 256, 0, stream>>>(off, num_segments, n, max_len, warp_max, list, counts);
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    // the classes: every segment the long list does not take
+    const uint32_t class_max = lng ? long_min - 1 : max_len;
+    e = with_key_type(TopkKeys{}, key_bytes, [&](auto kt) {
+        using KeyT = decltype(kt);
+        return with_rank_mode(rank_mode, [&](auto r) {
+            constexpr int R = decltype(r)::value;
+            auto go = [&](auto ind) {  // each warp's staging area is sized for 8 keys per lane
+                constexpr bool I = decltype(ind)::value;
+                return launch_resident<select_segment_warp_kernel<KeyT, R, I>, kRowWarps * 32, kRowWarpSmemBytes<KeyT, 8, I>>(
+                    kAllResident, sm_count, stream, static_cast<const KeyT*>(keys_in), static_cast<KeyT*>(values_out), indices, n,
+                    max_len, off, list, counts, seg_ranks, nr, codec);
+            };
+            return indices ? go(std::true_type{}) : go(std::false_type{});
+        });
+    });
+    for (int cls = 1; e == cudaSuccess && cls <= 2; ++cls) {
+        if (class_max < 2 || class_max <= (cls == 1 ? warp_max : kSegBlock1Max)) break;
+        e = find_type(
+            SelectSegShapes{},
+            [&](auto s) {
+                using S = decltype(s);
+                return key_bytes == static_cast<int>(sizeof(typename S::Key)) && S::indices == (indices != nullptr) &&
+                       (S::T == kSegBlock1Max) == (cls == 1);
+            },
+            [&](auto s) {
+                using S = decltype(s);
+                using KeyT = typename S::Key;
+                return with_rank_mode(rank_mode, [&](auto r) {
+                    return launch_resident<S::template kernel<decltype(r)::value>(), S::S::THREADS, S::smem>(
+                        kAllResident, sm_count, stream, static_cast<const KeyT*>(keys_in), static_cast<KeyT*>(values_out), indices,
+                        off, num_segments, class_max, codec, list, counts, seg_ranks, nr);
+                });
+            });
+    }
+    if (e != cudaSuccess || !lng) return e;
+    // the long list: its tile map, then the split path over its tiles
+    const SortPlan* none_skipped = reinterpret_cast<const SortPlan*>(scratch);
+    SelectState* st = reinterpret_cast<SelectState*>(scratch + l.st);
+    uint32_t* tot = scratch + l.tot;
+    uint32_t* cnt = scratch + l.cnt;
+    uint32_t* csum = max_len > kLongChunk / kRadix * kLongRowTile ? scratch + l.csum : nullptr;  // some segment has 2+ chunks
+    const LongSegGeo geo{off, scratch + l.list, scratch + l.tfirst, scratch + l.cfirst, counts};
+    long_segments_map_kernel<<<1, kLongThreads, 0, stream>>>(off, scratch + l.list, scratch + l.tfirst, scratch + l.cfirst, counts,
+                                                             l.list_cap, l.tile_cap, l.chunk_cap);
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    return with_key_type(TopkKeys{}, key_bytes, [&](auto kt) {
+        using KeyT = decltype(kt);
+        const KeyT* in = static_cast<const KeyT*>(keys_in);
+        KeyT* out = static_cast<KeyT*>(values_out);
+        select_segment_unmapped_kernel<KeyT><<<bin_grid, 256, 0, stream>>>(off, num_segments, n, max_len, long_min, counts, out, indices, nr,
+                                                                          codec);
+        cudaError_t le = cudaGetLastError();
+        for (uint32_t t = 0; le == cudaSuccess && t < sizeof(KeyT); ++t) {
+            le = launch_resident<select_segments_count_kernel<KeyT>, kLongThreads, 0>(l.tile_cap, sm_count, stream, in, geo, seg_ranks, nr,
+                                                                                      t, static_cast<const SelectState*>(st), tot, codec);
+            if (le == cudaSuccess)
+                le = launch_resident<select_segments_pick_kernel<KeyT>, kRadix, 0>(l.list_cap, sm_count, stream, geo, seg_ranks, nr, t, st,
+                                                                                   tot, out, indices, codec);
+        }
+        if (le != cudaSuccess || !indices) return le;
+        le = launch_resident<select_segments_eq_count_kernel<KeyT>, kLongThreads, 0>(l.tile_cap, sm_count, stream, in, geo, seg_ranks, nr,
+                                                                                     static_cast<const SelectState*>(st), cnt, codec);
+        if (le != cudaSuccess) return le;
+        // per list entry, the exclusive scan of its nr * tiles counts [rank][tile]
+        const SelectSegScanGeo sg{geo, nr};
+        const unsigned scan_grid = capped_grid(l.chunk_cap, 1, static_cast<uint64_t>(sm_count) * 4);
+        if (csum) {
+            select_segments_chunk_sum_kernel<<<scan_grid, kLongThreads, 0, stream>>>(none_skipped, cnt, csum, sg);
+            select_segments_chunk_scan_kernel<<<capped_grid(l.list_cap, 1, static_cast<uint64_t>(sm_count) * 4), kLongThreads, 0, stream>>>(
+                none_skipped, csum, sg);
+        }
+        select_segments_scan_kernel<<<scan_grid, kLongThreads, 0, stream>>>(none_skipped, cnt, csum, sg);
+        if ((le = cudaGetLastError()) != cudaSuccess) return le;
+        return launch_resident<select_segments_locate_kernel<KeyT>, kLongThreads, 0>(l.tile_cap, sm_count, stream, in, indices, geo,
+                                                                                     seg_ranks, nr, static_cast<const SelectState*>(st),
+                                                                                     static_cast<const uint32_t*>(cnt), codec);
+    });
+}
+
 cudaError_t configure_kernels()
 {
     cudaError_t e = for_each_type(HistKeys{}, [](auto k) {
@@ -4837,6 +5319,7 @@ cudaError_t configure_kernels()
         return m != cudaSuccess ? m : set_smem(topk_long_sort_scatter_kernel<KeyT, kRankBallot>, sizeof(LongRowsSmem<KeyT, true>));
     });
     if (e == cudaSuccess) e = for_each_type(SelectShapes{}, shape);
+    if (e == cudaSuccess) e = for_each_type(SelectSegShapes{}, shape);
     return e;
 }
 

@@ -233,6 +233,20 @@ cudaError_t launch_select_long_rows(const void* keys_in, void* values_out, uint3
                                     const SelectRanks& ranks, int key_bytes, const KeyCodec* codec, uint32_t* scratch, int sm_count,
                                     cudaStream_t stream);
 
+// Segment select (osb200_select_segments): columns seg_ranks[s * nr .. s * nr + nr) (device memory; 1 <= nr <= kMaxSelectRanks)
+// of every segment's ascending stable sort into row s of [num_segments, nr] values_out and indices (may be null); a rank at
+// or past the segment's length, every rank of a row whose ranks decrease, and every column of an empty or invalid segment
+// (offsets that decrease or pass n, longer than max_len) is padding: the decoded all-ones key and position 0xFFFFFFFF.
+// long_min == 0: max_len <= row_sort_capacity(key_bytes), the warp and block classes only.  Otherwise segments of long_min to
+// max_len keys take the split path over the long list's tiles (DESIGN §4.20), with scratch: select_segments_layout(...).words
+// u32, 16-byte aligned (its first `zeroed` words are cleared here).  list: num_segments u32; counts: 7 u64, cleared here.
+struct SelectSegLayout { uint64_t list_cap, tile_cap, chunk_cap, st, tot, zeroed, list, tfirst, cfirst, cnt, csum, words; };  // u32 words
+SelectSegLayout select_segments_layout(uint64_t n, uint64_t num_segments, uint32_t long_min, uint32_t num_ranks, bool positions);
+cudaError_t launch_select_segments(const void* keys_in, void* values_out, uint32_t* indices, uint64_t n, const unsigned long long* off,
+                                   uint64_t num_segments, uint32_t max_len, const uint32_t* seg_ranks, uint32_t nr, int key_bytes,
+                                   const KeyCodec* codec, int rank_mode, bool block_only, uint32_t long_min, int sm_count,
+                                   uint32_t* list, unsigned long long* counts, uint32_t* scratch, cudaStream_t stream);
+
 // Validate (reference: Validate, UtilityKernels.cuh:403-429): err_count += #(keys[i] > keys[i+1]).
 cudaError_t launch_validate(const void* keys, uint64_t n, int key_bytes, unsigned long long* err_count, int sm_count,
                             cudaStream_t stream);

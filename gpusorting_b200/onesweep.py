@@ -322,6 +322,33 @@ class OneSweepSorter:
                    row_len, arr, len(ranks), kb, kt, stream=stream)
         return (out, idx) if return_indices else out
 
+    # -- segment select: given columns of every segment's ascending stable sort ---------------------------------------------
+    def select_segments(self, x: torch.Tensor, offsets: torch.Tensor, ranks, key_type: str, return_indices: bool = True,
+                        max_segment_len: Optional[int] = None, stream=None):
+        """Columns `ranks` of every segment [offsets[s], offsets[s+1])'s ascending stable sort, and their positions within the
+        segment (osb200_select_segments).  `x`, `offsets` and key_type as in sort_segments.  `ranks` is either a CUDA integer
+        tensor [num_segments, R] of each segment's own ranks, non-decreasing per row (values outside [0, 2^32) become ranks
+        that take no part), or a sequence of R ints shared by every segment; 1 <= R <= 16.  The values are bit for bit those
+        of ``sort_long_segments(x)`` at ``offsets[s] + rank``.  A column whose rank is at or past the segment's length, every
+        column of a row whose ranks decrease, and every column of a segment whose offsets decrease, pass x.numel() or exceed
+        max_segment_len is padding: index -1 and the maximum of an integer dtype or the NaN 0x7F..F.
+
+        Returns (values, indices) of shape [num_segments, R], indices as torch.int32, or values alone with
+        return_indices=False, allocated with torch.empty on the stream.  max_segment_len None reads the longest segment with
+        one device->host read; pass it when capturing a CUDA graph.  Up to 16,384 (8,192 for 8-byte dtypes) the call needs one
+        uint32 per segment of workspace; above that it also uses this sorter's alternate payloads (value_bytes == 4), for a
+        bound that depends on x.numel(), num_segments and R only (see select_segments_workspace)."""
+        kb, kt = self._ragged_keys(x, key_type, offsets)
+        segs = max(offsets.numel() - 1, 0)
+        rk = _segment_ranks(ranks, segs, x.device, stream)
+        if max_segment_len is None:
+            max_segment_len = max(int((offsets[1:] - offsets[:-1]).max().item()), 0) if segs else 0
+        out, idx = _new_outputs(stream, x, (segs, rk.shape[1]), return_indices)
+        self._call(lib.osb200_select_segments, x.data_ptr() if x.numel() else None, out.data_ptr(),
+                   idx.data_ptr() if idx is not None else None, x.numel(), offsets.data_ptr(), segs,
+                   min(int(max_segment_len), 0xFFFFFFFF), rk.data_ptr(), rk.shape[1], kb, kt, stream=stream)
+        return (out, idx) if return_indices else out
+
     # -- segment sort: ragged rows given by offsets -------------------------------------------------------------------------
     def sort_segments(self, x: torch.Tensor, offsets: torch.Tensor, key_type: str, descending: bool = False,
                       return_indices: bool = True, inplace: bool = False, max_segment_len: Optional[int] = None, stream=None):
@@ -764,6 +791,154 @@ def quantile(x: torch.Tensor, q, dim=None, keepdim: bool = False, interpolation:
         if qt.dim() == 0:
             return res.reshape(shape)
         return res.t().reshape((qv.numel(),) + shape)
+
+
+def _segment_ranks(ranks, segs: int, device, stream) -> torch.Tensor:
+    """select_segments' ranks as a contiguous int32 [segs, R] tensor on `device` whose bits are the uint32 ranks: a CUDA
+    integer tensor [segs, R] (values outside [0, 2^32) become 0xFFFFFFFF, a rank that takes no part), or a sequence of R
+    ints shared by every segment."""
+    if isinstance(ranks, torch.Tensor):
+        if not ranks.is_cuda:
+            raise TypeError("ranks must be a CUDA tensor [num_segments, R] or a sequence of ints; a CPU tensor is refused")
+        if ranks.dtype.is_floating_point or ranks.dtype == torch.bool or ranks.dim() != 2 or ranks.shape[0] != segs:
+            raise TypeError(f"ranks must be an integer CUDA tensor of shape [{segs}, R]")
+        if ranks.device != device:
+            raise ValueError(f"ranks live on {ranks.device}, x on {device}")
+        if not 1 <= ranks.shape[1] <= 16:
+            raise ValueError(f"1 to 16 ranks per segment, got {ranks.shape[1]}")
+        if ranks.dtype in (torch.int32, torch.uint32) and ranks.is_contiguous():
+            return ranks
+        with torch.cuda.stream(stream):
+            r = ranks.to(torch.int64)
+            r = torch.where((r >= 0) & (r <= 0xFFFFFFFF), r, 0xFFFFFFFF)
+            return (r - ((r >> 31) << 32)).to(torch.int32).contiguous()  # the uint32 bits as int32
+    ranks = [int(r) for r in ranks]
+    if not 1 <= len(ranks) <= 16:
+        raise ValueError(f"1 to 16 ranks, got {len(ranks)}")
+    if any(not 0 <= r <= 0xFFFFFFFF for r in ranks):
+        raise ValueError(f"ranks must lie in [0, 2^32), got {ranks}")
+    row = np.array(ranks, dtype=np.uint32).view(np.int32)
+    with torch.cuda.stream(stream):
+        return torch.from_numpy(row).to(device).expand(max(segs, 1), len(ranks))[:segs].contiguous()
+
+
+def select_segments_workspace(n: int, num_segments: int, num_ranks: int, key_bytes: int = 4, indices: bool = True) -> int:
+    """The 32-bit words of a sorter's alternate payloads that select_segments needs when max_segment_len exceeds sort_segments'
+    limit -- the bound of osb200_select_segments in include/onesweep_b200.h: per long segment and rank a 4-word state and 256
+    totals, the long list and its tile map, and with indices one count per rank and tile of 8,192 keys plus the scan's chunk
+    sums; 0 where the long path cannot run (n at most 16,384, or 8,192 for 8-byte keys).  This is the library's
+    osb200_select_segments_workspace_words.  A (4, 4) sorter with max_n >= max(this, num_segments) has the room."""
+    def round4(w):
+        return (w + 3) // 4 * 4
+    long_min = _ROW_CAPACITY.get(key_bytes, 16384) + 1
+    if n < long_min or num_segments == 0:
+        return 0  # max_segment_len is clamped to n: no segment can take the long path
+    listed = min(n // long_min, num_segments)
+    tiles = (n + _LONG_ROW_TILE - 1) // _LONG_ROW_TILE + listed
+    words = round4(16 + listed * num_ranks * (4 + 256)) + round4(listed) + 2 * round4(listed + 1)
+    if indices:
+        words += round4(tiles * num_ranks) + round4((tiles + 15) // 16 + listed)
+    return words
+
+
+def _segment_args(x, offsets, max_segment_len):
+    """(number of segments, max_segment_len) of a module segment call; None reads the longest segment (one device->host read)"""
+    if not (isinstance(offsets, torch.Tensor) and offsets.is_cuda):
+        raise TypeError("offsets must be a CUDA tensor")
+    segs = max(offsets.numel() - 1, 0)
+    if max_segment_len is None:
+        max_segment_len = max(int((offsets[1:] - offsets[:-1]).max().item()), 0) if segs else 0
+    return segs, int(max_segment_len)
+
+
+def select_segments(x: torch.Tensor, offsets: torch.Tensor, ranks, return_indices: bool = True, max_segment_len: Optional[int] = None,
+                    stream=None):
+    """Columns `ranks` of the ascending stable sort of every segment [offsets[s], offsets[s+1]) of a contiguous 1-D CUDA tensor
+    of one of sort_rows' ten dtypes: (values, int32 positions within the segment) of shape [num_segments, R], or values alone;
+    see OneSweepSorter.select_segments for `ranks` and the padding.  The key type follows the dtype.  Runs on the stream's
+    cached (4, 4) sorter, grown to the number of segments, and with max_segment_len above sort_segments' limit only to
+    select_segments_workspace's bound -- never to x.numel()."""
+    segs, max_len = _segment_args(x, offsets, max_segment_len)
+    if isinstance(ranks, torch.Tensor):
+        if not ranks.is_cuda:
+            raise TypeError("ranks must be a CUDA tensor [num_segments, R] or a sequence of ints; a CPU tensor is refused")
+    else:
+        ranks = [int(r) for r in ranks]  # (read once: a generator would be consumed here)
+    num_ranks = ranks.shape[-1] if isinstance(ranks, torch.Tensor) else len(ranks)
+    kb = x.element_size() if isinstance(x, torch.Tensor) else 4
+    need = max(segs, 1)
+    if max_len > _ROW_CAPACITY.get(kb, 16384):
+        need = max(need, select_segments_workspace(x.numel(), segs, num_ranks, kb, return_indices))
+    s = _module_sorter(x, "x", 4, need, stream, _ROW_KEY_TYPES)
+    return s.select_segments(x, offsets, ranks, _ROW_KEY_TYPES[x.dtype], return_indices, max_len, stream)
+
+
+def median_segments(x: torch.Tensor, offsets: torch.Tensor, max_segment_len: Optional[int] = None, stream=None):
+    """The lower median of every segment, rank (L - 1) // 2 of its ascending stable sort: (values, int32 positions within the
+    segment) of shape [num_segments]; an empty segment is padding (see OneSweepSorter.select_segments).  The ranks are
+    computed on the device from the offsets."""
+    segs, max_len = _segment_args(x, offsets, max_segment_len)
+    with torch.cuda.stream(stream):
+        lengths = offsets[1:] - offsets[:-1]
+        ranks = torch.where(lengths > 0, (lengths - 1) // 2, -1)[:, None]
+    v, i = select_segments(x, offsets, ranks, True, max_len, stream)
+    return v.view(segs), i.view(segs)
+
+
+def quantile_segments(x: torch.Tensor, offsets: torch.Tensor, q, interpolation: str = "linear", max_segment_len: Optional[int] = None,
+                      stream=None):
+    """``torch.quantile(x[offsets[s]:offsets[s+1]], q, interpolation=...)`` of every segment of a contiguous 1-D float32 or
+    float64 CUDA tensor: [Q, num_segments], or [num_segments] for a scalar q, bit for bit on inputs without -0.0 or NaN.
+    Segments with a NaN give NaN, as in torch, but the canonical NaN rather than the NaN bits torch returns; empty segments
+    give NaN.  Past 2^24 keys (float32), which torch.quantile refuses, q * (L - 1) may round past L - 1: the rank is clamped
+    to L - 1.  q is a float, a sequence or a CPU tensor of values in [0, 1].
+    ATen's ranks are computed on the device from the lengths -- q * (L - 1) in x's dtype, then floor / ceil / round per
+    mode -- with ranks 0 and L - 1 added (a NaN sorts to one end, so they find NaN segments without another read); each
+    segment's ranks are sorted on the device and selected 16 per call, and torch.lerp finishes.  With max_segment_len given
+    nothing waits for the device."""
+    if not (isinstance(x, torch.Tensor) and x.dtype in (torch.float32, torch.float64)):
+        raise TypeError("quantile_segments() takes float32 or float64 tensors")
+    if interpolation not in _INTERPOLATIONS:
+        raise ValueError(f"interpolation must be one of {_INTERPOLATIONS}, got {interpolation!r}")
+    if isinstance(q, torch.Tensor) and q.is_cuda:
+        raise ValueError("q must be a float, a sequence or a CPU tensor")
+    qt = torch.as_tensor(q, dtype=x.dtype, device="cpu")
+    if qt.dim() > 1:
+        raise ValueError("q must be a scalar or a 1-D tensor")
+    if not bool(((qt >= 0) & (qt <= 1)).all()):
+        raise ValueError("q values must lie in [0, 1]")
+    segs, max_len = _segment_args(x, offsets, max_segment_len)
+    nq = qt.numel()
+    lerp = interpolation in ("linear", "midpoint")
+    with torch.cuda.stream(stream):
+        qv = qt.reshape(-1).to(x.device)
+        lengths = offsets[1:] - offsets[:-1]
+        last = (lengths - 1).clamp_(min=0)
+        lastf = last.to(x.dtype)[:, None]
+        pos = torch.minimum(qv[None, :] * lastf, lastf)  # ATen's ranks, in x's dtype (clamped: they can round past L - 1)
+        if interpolation == "lower":
+            pos = pos.floor()
+        elif interpolation == "higher":
+            pos = pos.ceil()
+        elif interpolation == "nearest":
+            pos = pos.round()
+        below = pos.to(torch.int64)
+        above = pos.ceil().to(torch.int64)
+        cols = [below, above] if lerp else [below]
+        wanted = torch.cat(cols + [torch.zeros_like(last)[:, None], last[:, None]], dim=1)  # [S, M]
+        ranks, perm = torch.sort(wanted, dim=1)
+    parts = [select_segments(x, offsets, ranks[:, c:c + 16], False, max_len, stream) for c in range(0, ranks.shape[1], 16)]
+    with torch.cuda.stream(stream):
+        vals = parts[0] if len(parts) == 1 else torch.cat(parts, dim=1)
+        vals = torch.empty_like(vals).scatter_(1, perm, vals)  # back to the order of `wanted`
+        res = vals[:, :nq]
+        if lerp:
+            w = torch.full_like(pos, 0.5) if interpolation == "midpoint" else pos - below.to(x.dtype)
+            res = torch.lerp(res, vals[:, nq:2 * nq], w)
+        m = vals.shape[1]
+        bad = vals[:, m - 2].isnan() | vals[:, m - 1].isnan() | (lengths <= 0)
+        res = torch.where(bad[:, None], torch.full_like(res, float("nan")), res)
+        return res[:, 0] if qt.dim() == 0 else res.t().contiguous()
 
 
 def sort_segments(x: torch.Tensor, offsets: torch.Tensor, descending: bool = False, return_indices: bool = True,

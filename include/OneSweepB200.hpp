@@ -122,6 +122,19 @@ class OneSweepSorterB200 {
                                  stream),
               "osb200_select_rows");
     }
+    // columns d_ranks[s*num_ranks .. (s+1)*num_ranks) (device array, 1 to 16 non-decreasing ranks per segment) of every segment
+    // [offsets[s], offsets[s+1])'s ascending stable sort into row s of [num_segments, num_ranks] outputs, and their positions
+    // within the segment into d_indices (may be null); ranks at or past the length, rows whose ranks decrease and invalid
+    // segments are padding (position 0xFFFFFFFF); max_segment_len above 16,384 (8,192 for 8-byte keys) uses this handle's
+    // alternate payloads for a bound that depends on n, num_segments and num_ranks only
+    void SelectSegments(const void* d_keys_in, void* d_values_out, uint32_t* d_indices, uint64_t n, const uint64_t* d_segment_offsets,
+                        uint64_t num_segments, uint32_t max_segment_len, const uint32_t* d_ranks, uint32_t num_ranks, int key_bytes,
+                        int key_type, void* stream = nullptr)
+    {
+        check(osb200_select_segments(h_, d_keys_in, d_values_out, d_indices, n, d_segment_offsets, num_segments, max_segment_len, d_ranks,
+                                     num_ranks, key_bytes, key_type, stream),
+              "osb200_select_segments");
+    }
     // the first m = min(length, k) keys of every segment [offsets[s], offsets[s+1]) in its stable sort (ascending, or descending
     // for largest) and their positions within the segment, into row s of [num_segments, k] outputs; columns m .. k-1 are
     // padding (position 0xFFFFFFFF, the key that sorts last); segments whose offsets decrease or pass n are all padding;

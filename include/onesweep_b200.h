@@ -373,6 +373,55 @@ OSB200_API int osb200_select_rows(osb200_handle h, const void* d_keys_in, void* 
                                   uint64_t num_rows, uint32_t row_len, const uint32_t* h_ranks, uint32_t num_ranks, int key_bytes,
                                   int key_type, void* stream);
 
+/* Segment select: the keys at given ranks of every ragged segment, and where they are (segment median and quantile).  Segment
+ * s is [d_segment_offsets[s], d_segment_offsets[s + 1]) of d_keys_in, as in osb200_sort_segments; key_bytes, key_type, their
+ * codec and the natural alignment are those of osb200_select_rows (all ten key types).  d_ranks is a DEVICE array
+ * [num_segments, num_ranks], row-major, 1 <= num_ranks <= 16: row s holds segment s's own ranks, non-decreasing (duplicates
+ * are allowed).  Being in device memory, a captured graph replays with the ranks the buffer holds at replay time (unlike
+ * osb200_select_rows, whose ranks are frozen into the graph), as with the keys and offsets.
+ * Output: [num_segments, num_ranks] arrays.  d_values_out[s * num_ranks + i] is column d_ranks[s * num_ranks + i] of segment
+ * s's ASCENDING stable sort -- bit for bit what osb200_sort_long_segments(descending = 0) writes at offset[s] + rank -- and
+ * d_indices[s * num_ranks + i] (d_indices may be NULL: values only) that key's uint32 position within the segment.  Every
+ * output element is written.  A column is padding -- position 0xFFFFFFFF and the decode of the all-ones radix image
+ * (UINT_MAX, INT_MAX or the NaN 0x7F..F), as osb200_topk_segments with largest = 0 pads -- when its rank is at or past the
+ * segment's length (so an empty segment is all padding), when the segment's offsets decrease or pass n, when the segment
+ * is longer than max_segment_len, and, for the whole row, when the row's ranks decrease anywhere.  None of these faults;
+ * nothing outside [0, n) of the keys is read, nothing outside [0, num_segments * num_ranks) of the outputs written.
+ * Errors, in the order of osb200_topk_segments: a null handle, or a bad key_bytes / key_type pair (OSB200_ERR_INVALID_ARG);
+ * then num_segments == 0 is a no-op; then a null output, offsets or ranks array, null keys with n > 0, a misaligned pointer,
+ * sizes that overflow 64 bits, or any overlap among keys, offsets, ranks and the two outputs (OSB200_ERR_INVALID_ARG); then
+ * num_ranks 0 or above 16 (OSB200_ERR_INVALID_ARG); then num_segments above max_n or 2^32 (OSB200_ERR_SIZE).
+ * Path rule, with C = 16,384 (8,192 for 8-byte keys):
+ *   - max_segment_len <= C: osb200_topk_segments' workspace only (one uint32 per segment), so any handle with max_n >=
+ *     num_segments will do.  A binning kernel lists every segment: 0 to 256 keys and the empty and invalid ones go to one
+ *     warp each, longer ones to one thread block each (2,048- or C-key geometry); each sorts its segment in shared memory
+ *     and stores only the requested columns.
+ *   - max_segment_len > C: segments longer than C go to a long list, and the row select's split path (osb200_select_rows)
+ *     runs over the long list's tiles of 8,192 keys spread over the GPU (DESIGN 4.20); the shorter ones as above.
+ *   - the test hooks "debug_rows_block" (segments of 2 .. 256 keys take the block class) and "debug_long_rows" (every
+ *     segment of 2 or more keys takes the split path, with the workspace below for long_min = 2) apply.
+ * The split path stores no keys and allocates nothing.  Its workspace lives in the handle's alternate payloads (so it needs
+ * value_bytes == 4, else OSB200_ERR_INVALID_ARG); in 32-bit words, with R = num_ranks, long_min = C + 1,
+ * L = min(floor(n / long_min), num_segments), T = ceil(n / 8192) + L and round4(x) = x rounded up to a multiple of 4:
+ *     W = round4(16 + L * R * 260)                           [plan words, per long segment and rank a 4-word state and 256 totals]
+ *       + round4(L) + 2 * round4(L + 1)                      [the long list and its tile map]
+ *       + (d_indices ? round4(T * R) + round4(ceil(T / 16) + L) : 0)   [per tile one count per rank, the scan's chunk sums]
+ * and it needs W <= max_n, else OSB200_ERR_SIZE, decided before anything is enqueued.  No valid segment is longer than n,
+ * so the call clamps max_segment_len to n before the path rule: with n <= C the split path never runs, whatever
+ * max_segment_len says, and needs no room (W = 0).  The bound depends on n, num_segments, num_ranks, the key width and
+ * d_indices only, never on the offsets.  A handle with value_bytes == 4 and max_n >= max(n, num_segments) always has the
+ * room outside the test hook: W is at most about 0.52 words per key.  osb200_select_segments_workspace_words returns W
+ * (0 where the split path cannot run) without a device.
+ * Asynchronous, no host synchronisation, graph-capturable; one call in flight per handle. */
+OSB200_API int osb200_select_segments(osb200_handle h, const void* d_keys_in, void* d_values_out, uint32_t* d_indices, uint64_t n,
+                                      const uint64_t* d_segment_offsets, uint64_t num_segments, uint32_t max_segment_len,
+                                      const uint32_t* d_ranks, uint32_t num_ranks, int key_bytes, int key_type, void* stream);
+/* W above, in 32-bit words, for a call of n keys in num_segments segments with num_ranks ranks (1 .. 16) of key_bytes (2, 4 or
+ * 8) keys, with indices (nonzero) or values only; 0 when n <= C or num_segments == 0 (the split path cannot run) or the
+ * arguments are out of range.  Host only: needs no handle and no device. */
+OSB200_API uint64_t osb200_select_segments_workspace_words(uint64_t n, uint64_t num_segments, uint32_t num_ranks, int key_bytes,
+                                                           int indices);
+
 /* Sort on a bit range [begin_bit, end_bit) of the (unsigned) key only, CUB-style: keys that agree on those bits keep their
  * input order (stable).  ceil((end_bit-begin_bit)/8) digit passes instead of key_bytes; the last digit may be narrower
  * than 8 bits; an odd pass count is handled inside (the result is always returned in the caller's buffers).  d_values may
@@ -455,7 +504,7 @@ OSB200_API int osb200_init_random_u32(uint32_t* d_keys, uint32_t* d_payload, uin
  *                    than max_n gives: OSB200_ERR_SIZE), to compare it with osb200_sort_rows; 0 (default) = osb200_sort_rows' launch.
  *                    osb200_sort_long_segments honours it too: its segments of 2 .. 16,384 (8,192) keys then take the long path,
  *                    and osb200_topk_long_rows: its rows of 2 or more keys then take the split path, and osb200_select_rows
- *                    likewise
+ *                    and osb200_select_segments likewise
  *   "debug_topk_capacity"  test hook of osb200_topk_rows: N > 0 keeps at most N candidates of a row in shared memory (instead
  *                    of 16,384, or 8,192 for 8-byte keys), so that short rows exercise the passes that read global memory
  *                    and the switch to shared memory; 0 (default) = the full capacity.  osb200_topk_long_rows' split path
