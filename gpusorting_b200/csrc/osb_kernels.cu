@@ -3150,9 +3150,11 @@ struct LongSegGeo {
     __device__ __forceinline__ Group group(uint64_t j) const { return {cfirst[j], cfirst[j + 1] - cfirst[j]}; }
 };
 
+// The kernels of the long paths take their Geo by value: one kernel per stage serves the rows and the segments.
 template <typename KeyT, typename Geo>
-__device__ __forceinline__ void long_count_body(const Geo& geo, const SortPlan* __restrict__ plan, uint32_t place, const KeyT* keys_in,
-                                                const KeyT* keys_out, const KeyT* alt, uint32_t* __restrict__ cnt, KeyCodec codec)
+__global__ void __launch_bounds__(kLongThreads)
+long_count_kernel(const SortPlan* __restrict__ plan, uint32_t place, const KeyT* keys_in, const KeyT* keys_out, const KeyT* alt, Geo geo,
+                  uint32_t* __restrict__ cnt, KeyCodec codec)
 {
     const LongPass ps = long_pass(plan, place);
     if (ps.skip) return;
@@ -3193,22 +3195,6 @@ __device__ __forceinline__ void long_count_body(const Geo& geo, const SortPlan* 
     }
 }
 
-template <typename KeyT>
-__global__ void __launch_bounds__(kLongThreads)
-long_rows_count_kernel(const SortPlan* __restrict__ plan, uint32_t place, const KeyT* keys_in, const KeyT* keys_out, const KeyT* alt,
-                       uint64_t num_rows, uint32_t row_len, uint32_t tpr, uint32_t* __restrict__ cnt, KeyCodec codec)
-{
-    long_count_body<KeyT>(LongRowGeo{num_rows, row_len, tpr, 0, 0}, plan, place, keys_in, keys_out, alt, cnt, codec);
-}
-
-template <typename KeyT>
-__global__ void __launch_bounds__(kLongThreads)
-long_segments_count_kernel(const SortPlan* __restrict__ plan, uint32_t place, const KeyT* keys_in, const KeyT* keys_out, const KeyT* alt,
-                           LongSegGeo geo, uint32_t* __restrict__ cnt, KeyCodec codec)
-{
-    long_count_body<KeyT>(geo, plan, place, keys_in, keys_out, alt, cnt, codec);
-}
-
 // The m <= kLongChunk counts at p, thread i holding counts 8i .. 8i+7: their sum (to every thread), and with SCAN their
 // exclusive prefix plus carry written back in place.  All kLongThreads threads call it.
 template <bool SCAN>
@@ -3245,8 +3231,8 @@ __device__ __forceinline__ uint32_t long_chunk(uint32_t* p, uint32_t m, uint32_t
 // Chunk g covers counts [c0, min(c0 + kLongChunk, row_counts)) of its row's or segment's row_counts = 256 * tiles:
 // csum[g] = their sum.
 template <typename Geo>
-__device__ __forceinline__ void long_chunk_sum_body(const Geo& geo, const SortPlan* __restrict__ plan, uint32_t place, uint32_t* cnt,
-                                                    uint32_t* __restrict__ csum)
+__global__ void __launch_bounds__(kLongThreads)
+long_chunk_sum_kernel(const SortPlan* __restrict__ plan, uint32_t place, uint32_t* cnt, uint32_t* __restrict__ csum, Geo geo)
 {
     if (long_pass(plan, place).skip) return;
     __shared__ uint32_t s_w[kLongWarps];
@@ -3258,22 +3244,10 @@ __device__ __forceinline__ void long_chunk_sum_body(const Geo& geo, const SortPl
     }
 }
 
-__global__ void __launch_bounds__(kLongThreads)
-long_rows_chunk_sum_kernel(const SortPlan* __restrict__ plan, uint32_t place, uint32_t* cnt, uint32_t* __restrict__ csum,
-                           uint64_t num_rows, uint64_t row_counts, uint32_t cpr)
-{
-    long_chunk_sum_body(LongRowGeo{num_rows, 0, 0, row_counts, cpr}, plan, place, cnt, csum);
-}
-
-__global__ void __launch_bounds__(kLongThreads)
-long_segments_chunk_sum_kernel(const SortPlan* __restrict__ plan, uint32_t place, uint32_t* cnt, uint32_t* __restrict__ csum, LongSegGeo geo)
-{
-    long_chunk_sum_body(geo, plan, place, cnt, csum);
-}
-
 // The exclusive scan of each row's or segment's chunk sums, in place; one CTA per row or segment at a time.
 template <typename Geo>
-__device__ __forceinline__ void long_chunk_scan_body(const Geo& geo, const SortPlan* __restrict__ plan, uint32_t place, uint32_t* csum)
+__global__ void __launch_bounds__(kLongThreads)
+long_chunk_scan_kernel(const SortPlan* __restrict__ plan, uint32_t place, uint32_t* csum, Geo geo)
 {
     if (long_pass(plan, place).skip) return;
     __shared__ uint32_t s_w[kLongWarps];
@@ -3285,23 +3259,11 @@ __device__ __forceinline__ void long_chunk_scan_body(const Geo& geo, const SortP
     }
 }
 
-__global__ void __launch_bounds__(kLongThreads)
-long_rows_chunk_scan_kernel(const SortPlan* __restrict__ plan, uint32_t place, uint32_t* csum, uint64_t num_rows, uint32_t cpr)
-{
-    long_chunk_scan_body(LongRowGeo{num_rows, 0, 0, 0, cpr}, plan, place, csum);
-}
-
-__global__ void __launch_bounds__(kLongThreads)
-long_segments_chunk_scan_kernel(const SortPlan* __restrict__ plan, uint32_t place, uint32_t* csum, LongSegGeo geo)
-{
-    long_chunk_scan_body(geo, plan, place, csum);
-}
-
 // Every chunk's counts become their exclusive prefix within the row or segment: the chunk's own scan plus its chunk prefix
 // (csum null: every row or segment is one chunk).
 template <typename Geo>
-__device__ __forceinline__ void long_scan_body(const Geo& geo, const SortPlan* __restrict__ plan, uint32_t place, uint32_t* cnt,
-                                               const uint32_t* __restrict__ csum)
+__global__ void __launch_bounds__(kLongThreads)
+long_scan_kernel(const SortPlan* __restrict__ plan, uint32_t place, uint32_t* cnt, const uint32_t* __restrict__ csum, Geo geo)
 {
     if (long_pass(plan, place).skip) return;
     __shared__ uint32_t s_w[kLongWarps];
@@ -3312,18 +3274,20 @@ __device__ __forceinline__ void long_scan_body(const Geo& geo, const SortPlan* _
     }
 }
 
-__global__ void __launch_bounds__(kLongThreads)
-long_rows_scan_kernel(const SortPlan* __restrict__ plan, uint32_t place, uint32_t* cnt, const uint32_t* __restrict__ csum,
-                      uint64_t num_rows, uint64_t row_counts, uint32_t cpr)
+// The three scan kernels of one place over geo's counts (with csum: the chunk sums and their scan first); chunk_bound and
+// group_bound bound geo.chunks() and geo.groups() on the host and size the grids.
+template <typename Geo>
+static cudaError_t launch_long_scan(const Geo& geo, const SortPlan* plan, uint32_t place, uint32_t* cnt, uint32_t* csum,
+                                    uint64_t chunk_bound, uint64_t group_bound, int sm_count, cudaStream_t stream)
 {
-    long_scan_body(LongRowGeo{num_rows, 0, 0, row_counts, cpr}, plan, place, cnt, csum);
-}
-
-__global__ void __launch_bounds__(kLongThreads)
-long_segments_scan_kernel(const SortPlan* __restrict__ plan, uint32_t place, uint32_t* cnt, const uint32_t* __restrict__ csum,
-                          LongSegGeo geo)
-{
-    long_scan_body(geo, plan, place, cnt, csum);
+    const uint64_t cap = static_cast<uint64_t>(sm_count) * 4;
+    const unsigned grid = capped_grid(chunk_bound, 1, cap);
+    if (csum) {
+        long_chunk_sum_kernel<<<grid, kLongThreads, 0, stream>>>(plan, place, cnt, csum, geo);
+        long_chunk_scan_kernel<<<capped_grid(group_bound, 1, cap), kLongThreads, 0, stream>>>(plan, place, csum, geo);
+    }
+    long_scan_kernel<<<grid, kLongThreads, 0, stream>>>(plan, place, cnt, static_cast<const uint32_t*>(csum), geo);
+    return cudaGetLastError();
 }
 
 template <typename KeyT, bool INDICES>
@@ -3336,12 +3300,15 @@ struct LongRowsSmem {
     uint32_t wtot[kRadix / 32];
 };
 
-// GIVEN (topk_long_sort_scatter_kernel): the first executed pass loads the indices given in idx_out instead of making them.
+// GIVEN (osb200_topk_long_rows' sort of k > C selected keys, in place): the first executed pass loads the indices given in
+// idx_out instead of making them.
+// (Two resident CTAs per SM are stated for 16- and 32-bit keys only: with indices they spill at 64 registers.)
 template <typename KeyT, int RANK_MODE, bool INDICES, typename Geo, bool GIVEN = false>
-__device__ __forceinline__ void long_scatter_body(const Geo& geo, const SortPlan* __restrict__ plan, uint32_t place, const KeyT* keys_in,
-                                                  KeyT* keys_out, KeyT* alt, uint32_t* idx_out, uint32_t* alt_idx,
-                                                  const uint32_t* __restrict__ base, KeyCodec codec)
+__global__ void __launch_bounds__(kLongThreads, sizeof(KeyT) == 8 || INDICES ? 1 : 2)
+long_scatter_kernel(const SortPlan* __restrict__ plan, uint32_t place, const KeyT* keys_in, KeyT* keys_out, KeyT* alt, uint32_t* idx_out,
+                    uint32_t* alt_idx, Geo geo, const uint32_t* __restrict__ base, KeyCodec codec)
 {
+    static_assert(INDICES || !GIVEN, "given indices are loaded as payloads");
     const LongPass ps = long_pass(plan, place);
     if (ps.skip) return;
     const KeyT* src = ps.first ? keys_in : ps.from_alt ? alt : keys_out;
@@ -3420,23 +3387,30 @@ __device__ __forceinline__ void long_scatter_body(const Geo& geo, const SortPlan
     }
 }
 
-// (Two resident CTAs per SM are stated for 16- and 32-bit keys only: with indices they spill at 64 registers.)
-template <typename KeyT, int RANK_MODE, bool INDICES>
-__global__ void __launch_bounds__(kLongThreads, sizeof(KeyT) == 8 || INDICES ? 1 : 2)
-long_rows_scatter_kernel(const SortPlan* __restrict__ plan, uint32_t place, const KeyT* keys_in, KeyT* keys_out, KeyT* alt,
-                         uint32_t* idx_out, uint32_t* alt_idx, uint64_t num_rows, uint32_t row_len, uint32_t tpr,
-                         const uint32_t* __restrict__ base, KeyCodec codec)
+// The executed places of a long sort over geo's tiles (tile_bound of them at most): per place the count, the scan and the
+// scatter; indices null, made by the first executed pass, or with GIVEN loaded from indices.
+template <typename KeyT, bool GIVEN, typename Geo>
+static cudaError_t launch_long_places(const Geo& geo, uint64_t tile_bound, uint64_t chunk_bound, uint64_t group_bound, const SortPlan* plan,
+                                      const KeyT* in, KeyT* out, KeyT* alt, uint32_t* indices, uint32_t* alt_idx, uint32_t* cnt,
+                                      uint32_t* csum, const KeyCodec& codec, int rank_mode, int sm_count, cudaStream_t stream)
 {
-    long_scatter_body<KeyT, RANK_MODE, INDICES>(LongRowGeo{num_rows, row_len, tpr, 0, 0}, plan, place, keys_in, keys_out, alt, idx_out,
-                                                alt_idx, base, codec);
-}
-
-template <typename KeyT, int RANK_MODE, bool INDICES>
-__global__ void __launch_bounds__(kLongThreads, sizeof(KeyT) == 8 || INDICES ? 1 : 2)
-long_segments_scatter_kernel(const SortPlan* __restrict__ plan, uint32_t place, const KeyT* keys_in, KeyT* keys_out, KeyT* alt,
-                             uint32_t* idx_out, uint32_t* alt_idx, LongSegGeo geo, const uint32_t* __restrict__ base, KeyCodec codec)
-{
-    long_scatter_body<KeyT, RANK_MODE, INDICES>(geo, plan, place, keys_in, keys_out, alt, idx_out, alt_idx, base, codec);
+    cudaError_t e = cudaSuccess;
+    for (uint32_t p = 0; e == cudaSuccess && p < sizeof(KeyT); ++p) {
+        e = launch_resident<long_count_kernel<KeyT, Geo>, kLongThreads, 0>(tile_bound, sm_count, stream, plan, p, in,
+                                                                           static_cast<const KeyT*>(out), static_cast<const KeyT*>(alt),
+                                                                           geo, cnt, codec);
+        if (e == cudaSuccess) e = launch_long_scan(geo, plan, p, cnt, csum, chunk_bound, group_bound, sm_count, stream);
+        if (e == cudaSuccess) e = with_rank_mode(rank_mode, [&](auto rm) {
+            auto go = [&](auto ind) {
+                constexpr bool I = decltype(ind)::value;
+                return launch_resident<long_scatter_kernel<KeyT, decltype(rm)::value, I, Geo, GIVEN>, kLongThreads, sizeof(LongRowsSmem<KeyT, I>)>(
+                    tile_bound, sm_count, stream, plan, p, in, out, alt, indices, alt_idx, geo, static_cast<const uint32_t*>(cnt), codec);
+            };
+            if constexpr (GIVEN) return go(std::true_type{});
+            else return indices ? go(std::true_type{}) : go(std::false_type{});
+        });
+    }
+    return e;
 }
 
 // Odd executed passes: keys and indices from the alternate buffers.  None: keys_in is its own stable sort -- its keys (not
@@ -3457,20 +3431,9 @@ long_rows_copy_home_kernel(const SortPlan* __restrict__ plan, const KeyT* keys_i
     }
 }
 
-
-// osb200_topk_long_rows' sort of k > C selected keys per row, in place: the long rows' passes with the positions as payloads
-template <typename KeyT, int RANK_MODE>
-__global__ void __launch_bounds__(kLongThreads, 1)
-topk_long_sort_scatter_kernel(const SortPlan* __restrict__ plan, uint32_t place, const KeyT* keys_in, KeyT* keys_out, KeyT* alt,
-                              uint32_t* idx_out, uint32_t* alt_idx, uint64_t num_rows, uint32_t row_len, uint32_t tpr,
-                              const uint32_t* __restrict__ base, KeyCodec codec)
-{
-    long_scatter_body<KeyT, RANK_MODE, true, LongRowGeo, true>(LongRowGeo{num_rows, row_len, tpr, 0, 0}, plan, place, keys_in, keys_out, alt,
-                                                               idx_out, alt_idx, base, codec);
-}
-
-// Its copy home: an odd number of executed passes moves keys and indices from the alternate buffers; after none the sort was
-// in place already, and the given indices stay.
+// osb200_topk_long_rows' sort of k > C selected keys per row, in place (launch_long_rows with given indices), has its own copy
+// home: an odd number of executed passes moves keys and indices from the alternate buffers; after none the sort was in place
+// already, and the given indices stay.
 template <typename KeyT>
 __global__ void __launch_bounds__(512)
 topk_long_sort_copy_home_kernel(const SortPlan* __restrict__ plan, const KeyT* __restrict__ alt, KeyT* __restrict__ keys,
@@ -3545,7 +3508,7 @@ long_segments_map_kernel(const unsigned long long* __restrict__ off, const uint3
     }
 }
 
-using LongRowKeys = TypeList<uint16_t, uint32_t, uint64_t>;
+using LongKeys = TypeList<uint16_t, uint32_t, uint64_t>;  // the long paths, the row and segment top-k and the selects
 
 // The long paths' plan over keys[0, n): the keys before the first 16-byte boundary of a naturally aligned input (at most
 // 7, and never more than n) by the one-warp head kernel, the rest by the GlobalHistogram, which reads 16-byte vectors;
@@ -3575,42 +3538,20 @@ cudaError_t launch_long_rows(const void* keys_in, void* keys_out, uint32_t* indi
     const uint32_t cpr = static_cast<uint32_t>((row_counts + kLongChunk - 1) / kLongChunk);
     uint32_t* cnt = scratch;
     uint32_t* csum = cpr > 1 ? scratch + (num_rows * row_counts + 3) / 4 * 4 : nullptr;
+    const LongRowGeo geo{num_rows, row_len, tpr, row_counts, cpr};
     const KeyCodec codec = codec_in ? *codec_in : KeyCodec();
     KeyCodec enc = codec;
     enc.flags &= kCodecEncodeOnLoad;
-    return with_key_type(LongRowKeys{}, key_bytes, [&](auto kt) {
+    return with_key_type(LongKeys{}, key_bytes, [&](auto kt) {
         using KeyT = decltype(kt);
         const KeyT* in = static_cast<const KeyT*>(keys_in);
         KeyT* out = static_cast<KeyT*>(keys_out);
         KeyT* alt = static_cast<KeyT*>(alt_keys);
         cudaError_t e = launch_long_plan(in, n, key_bytes, codec_in ? &enc : nullptr, allow_skip, ghist, gbase, plan, sm_count, stream);
-        const unsigned scan_grid = capped_grid(num_rows * cpr, 1, static_cast<uint64_t>(sm_count) * 4);
-        for (uint32_t p = 0; e == cudaSuccess && p < sizeof(KeyT); ++p) {
-            e = launch_resident<long_rows_count_kernel<KeyT>, kLongThreads, 0>(num_rows * tpr, sm_count, stream, plan, p, in, out, alt,
-                                                                               num_rows, row_len, tpr, cnt, codec);
-            if (e == cudaSuccess && csum) {
-                long_rows_chunk_sum_kernel<<<scan_grid, kLongThreads, 0, stream>>>(plan, p, cnt, csum, num_rows, row_counts, cpr);
-                long_rows_chunk_scan_kernel<<<capped_grid(num_rows, 1, static_cast<uint64_t>(sm_count) * 4), kLongThreads, 0, stream>>>(
-                    plan, p, csum, num_rows, cpr);
-            }
-            if (e == cudaSuccess) {
-                long_rows_scan_kernel<<<scan_grid, kLongThreads, 0, stream>>>(plan, p, cnt, csum, num_rows, row_counts, cpr);
-                e = cudaGetLastError();
-            }
-            if (e == cudaSuccess) e = with_rank_mode(rank_mode, [&](auto rm) {
-                auto go = [&](auto ind) {
-                    constexpr bool I = decltype(ind)::value;
-                    return launch_resident<long_rows_scatter_kernel<KeyT, decltype(rm)::value, I>, kLongThreads, sizeof(LongRowsSmem<KeyT, I>)>(
-                        num_rows * tpr, sm_count, stream, plan, p, in, out, alt, indices, alt_idx, num_rows, row_len, tpr,
-                        static_cast<const uint32_t*>(cnt), codec);
-                };
-                if (given_indices)
-                    return launch_resident<topk_long_sort_scatter_kernel<KeyT, decltype(rm)::value>, kLongThreads, sizeof(LongRowsSmem<KeyT, true>)>(
-                        num_rows * tpr, sm_count, stream, plan, p, in, out, alt, indices, alt_idx, num_rows, row_len, tpr,
-                        static_cast<const uint32_t*>(cnt), codec);
-                return indices ? go(std::true_type{}) : go(std::false_type{});
-            });
-        }
+        if (e == cudaSuccess)
+            e = (given_indices ? launch_long_places<KeyT, true, LongRowGeo> : launch_long_places<KeyT, false, LongRowGeo>)(
+                geo, num_rows * tpr, num_rows * cpr, num_rows, plan, in, out, alt, indices, alt_idx, cnt, csum, codec, rank_mode, sm_count,
+                stream);
         if (e != cudaSuccess) return e;
         const unsigned home_grid = capped_grid(n, 512, static_cast<uint64_t>(sm_count) * 4);
         if (given_indices)
@@ -3670,7 +3611,7 @@ cudaError_t launch_long_segments(const void* keys_in, void* keys_out, uint32_t* 
     enc.flags &= kCodecEncodeOnLoad;
     cudaError_t e = cudaMemsetAsync(counts, 0, kLongSegCounts * sizeof(unsigned long long), stream);
     if (e != cudaSuccess) return e;
-    return with_key_type(LongRowKeys{}, key_bytes, [&](auto kt) {
+    return with_key_type(LongKeys{}, key_bytes, [&](auto kt) {
         using KeyT = decltype(kt);
         const KeyT* in = static_cast<const KeyT*>(keys_in);
         KeyT* out = static_cast<KeyT*>(keys_out);
@@ -3690,29 +3631,9 @@ cudaError_t launch_long_segments(const void* keys_in, void* keys_out, uint32_t* 
         // the plan over all n keys, as for the long rows
         if (e == cudaSuccess)
             e = launch_long_plan(in, n, key_bytes, codec_in ? &enc : nullptr, allow_skip, ghist, gbase, plan, sm_count, stream);
-        const unsigned scan_grid = capped_grid(l.chunk_cap, 1, static_cast<uint64_t>(sm_count) * 4);
-        for (uint32_t p = 0; e == cudaSuccess && p < sizeof(KeyT); ++p) {
-            e = launch_resident<long_segments_count_kernel<KeyT>, kLongThreads, 0>(l.tile_cap, sm_count, stream, plan, p, in,
-                                                                                   static_cast<const KeyT*>(out), static_cast<const KeyT*>(alt),
-                                                                                   geo, cnt, codec);
-            if (e == cudaSuccess && csum) {
-                long_segments_chunk_sum_kernel<<<scan_grid, kLongThreads, 0, stream>>>(plan, p, cnt, csum, geo);
-                long_segments_chunk_scan_kernel<<<capped_grid(l.list_cap, 1, static_cast<uint64_t>(sm_count) * 4), kLongThreads, 0, stream>>>(
-                    plan, p, csum, geo);
-            }
-            if (e == cudaSuccess) {
-                long_segments_scan_kernel<<<scan_grid, kLongThreads, 0, stream>>>(plan, p, cnt, csum, geo);
-                e = cudaGetLastError();
-            }
-            if (e == cudaSuccess) e = with_rank_mode(rank_mode, [&](auto rm) {
-                auto go = [&](auto ind) {
-                    constexpr bool I = decltype(ind)::value;
-                    return launch_resident<long_segments_scatter_kernel<KeyT, decltype(rm)::value, I>, kLongThreads, sizeof(LongRowsSmem<KeyT, I>)>(
-                        l.tile_cap, sm_count, stream, plan, p, in, out, alt, indices, alt_idx, geo, static_cast<const uint32_t*>(cnt), codec);
-                };
-                return indices ? go(std::true_type{}) : go(std::false_type{});
-            });
-        }
+        if (e == cudaSuccess)
+            e = launch_long_places<KeyT, false>(geo, l.tile_cap, l.chunk_cap, l.list_cap, plan, in, out, alt, indices, alt_idx, cnt, csum, codec,
+                                                rank_mode, sm_count, stream);
         if (e != cudaSuccess) return e;
         return launch_resident<long_segments_copy_home_kernel<KeyT>, kLongThreads, 0>(l.tile_cap, sm_count, stream, plan, in,
                                                                                       static_cast<const KeyT*>(alt), out,
@@ -4062,7 +3983,6 @@ struct TopkSortShape {
 };
 using TopkSortShapes = TypeList<TopkSortShape<uint16_t, 1>, TopkSortShape<uint16_t, 2>, TopkSortShape<uint32_t, 1>,
                                 TopkSortShape<uint32_t, 2>, TopkSortShape<uint64_t, 1>, TopkSortShape<uint64_t, 2>>;
-using TopkKeys = TypeList<uint16_t, uint32_t, uint64_t>;
 
 // `sorted` for a [num_rows, k] result of at most C columns, in place with its positions as payloads: one warp per row for
 // k <= 32 K, else the row sort's block body.
@@ -4094,7 +4014,7 @@ cudaError_t launch_topk_rows(const void* keys_in, void* values_out, uint32_t* in
     if (k > row_len || k > row_sort_capacity(key_bytes)) return cudaErrorInvalidValue;
     const uint32_t cap = capacity && capacity < row_sort_capacity(key_bytes) ? capacity : row_sort_capacity(key_bytes);
     const KeyCodec codec = codec_in ? *codec_in : KeyCodec();
-    return with_key_type(TopkKeys{}, key_bytes, [&](auto kt) {
+    return with_key_type(LongKeys{}, key_bytes, [&](auto kt) {
         using KeyT = decltype(kt);
         const KeyT* in = static_cast<const KeyT*>(keys_in);
         KeyT* out = static_cast<KeyT*>(values_out);
@@ -4132,7 +4052,7 @@ cudaError_t launch_topk_segments(const void* keys_in, void* values_out, uint32_t
     topk_segment_bin_kernel<<<capped_grid(num_segments, 256, static_cast<uint64_t>(sm_count) * 8), 256, 0, stream>>>(
         off, num_segments, n, warp_max, list, counts);
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    return with_key_type(TopkKeys{}, key_bytes, [&](auto kt) {
+    return with_key_type(LongKeys{}, key_bytes, [&](auto kt) {
         using KeyT = decltype(kt);
         const KeyT* in = static_cast<const KeyT*>(keys_in);
         KeyT* out = static_cast<KeyT*>(values_out);
@@ -4192,7 +4112,7 @@ topk_long_count_kernel(const KeyT* __restrict__ in, uint64_t num_rows, uint32_t 
     const uint32_t shift = 8u * (static_cast<uint32_t>(sizeof(KeyT)) - 1u - level);
     const KeyT ca = static_cast<KeyT>(codec.a), cb = static_cast<KeyT>(codec.b), cd = static_cast<KeyT>(codec.d);
     const bool enc = codec.flags & kCodecEncodeOnLoad;
-    // bank-private columns, as in long_count_body
+    // bank-private columns, as in long_count_kernel
     __shared__ uint32_t s_hist[kRadix * 32];
     __shared__ uint32_t s_sel;
     uint32_t* s_col = s_hist + (threadIdx.x & 31);
@@ -4425,7 +4345,7 @@ cudaError_t launch_topk_long_rows(const void* keys_in, void* values_out, uint32_
     uint32_t* csum = l.cpr > 1 ? scratch + l.zeroed : nullptr;
     uint32_t* cnt = alt_idx;  // free until the compaction writes the candidates' positions there
     const uint64_t tiles = num_rows * l.tpr;
-    return with_key_type(TopkKeys{}, key_bytes, [&](auto kt) {
+    return with_key_type(LongKeys{}, key_bytes, [&](auto kt) {
         using KeyT = decltype(kt);
         const KeyT* in = static_cast<const KeyT*>(keys_in);
         KeyT* out = static_cast<KeyT*>(values_out);
@@ -4442,15 +4362,9 @@ cudaError_t launch_topk_long_rows(const void* keys_in, void* values_out, uint32_
                                                                     static_cast<const TopkLongRow*>(rows), static_cast<const uint32_t*>(cnt), sc);
         if (le != cudaSuccess) return le;
         // the bases: per row, the exclusive scan of its 2 tpr counts [selected of each tile, candidates of each tile]
-        const uint64_t row_counts = 2ull * l.tpr;
-        const unsigned scan_grid = capped_grid(num_rows * l.cpr, 1, static_cast<uint64_t>(sm_count) * 4);
-        if (csum) {
-            long_rows_chunk_sum_kernel<<<scan_grid, kLongThreads, 0, stream>>>(none_skipped, 0, sc, csum, num_rows, row_counts, l.cpr);
-            long_rows_chunk_scan_kernel<<<capped_grid(num_rows, 1, static_cast<uint64_t>(sm_count) * 4), kLongThreads, 0, stream>>>(
-                none_skipped, 0, csum, num_rows, l.cpr);
-        }
-        long_rows_scan_kernel<<<scan_grid, kLongThreads, 0, stream>>>(none_skipped, 0, sc, csum, num_rows, row_counts, l.cpr);
-        if ((le = cudaGetLastError()) != cudaSuccess) return le;
+        le = launch_long_scan(LongRowGeo{num_rows, row_len, l.tpr, 2ull * l.tpr, l.cpr}, none_skipped, 0, sc, csum, num_rows * l.cpr, num_rows,
+                              sm_count, stream);
+        if (le != cudaSuccess) return le;
         le = launch_resident<topk_long_compact_kernel<KeyT>, kTopkThreads, 0>(tiles, sm_count, stream, in, out, indices, num_rows, row_len,
                                                                              l.tpr, k, static_cast<const TopkLongRow*>(rows),
                                                                              static_cast<const uint32_t*>(sc), buf, alt_idx, codec);
@@ -4539,7 +4453,7 @@ cudaError_t launch_select_rows(const void* keys_in, void* values_out, uint32_t* 
     return with_rank_mode(rank_mode, [&](auto r) {
         constexpr int R = decltype(r)::value;
         if (row_len <= kRowWarpMaxLen && !block_only)
-            return with_key_type(TopkKeys{}, key_bytes, [&](auto k) {
+            return with_key_type(LongKeys{}, key_bytes, [&](auto k) {
                 using KeyT = decltype(k);
                 return with_warp_k(row_len, [&](auto kk) {
                     constexpr int K = decltype(kk)::value;
@@ -4600,7 +4514,7 @@ __device__ __forceinline__ uint32_t select_group_of(U p, const U* s_v, uint32_t 
     return s_v[g] == p ? g : ng;
 }
 
-// The split path's bodies are templated on where the rows are (Geo): LongRowGeo, osb200_select_rows' rows with the ranks
+// The split path's kernels are templated on where the rows are (Geo): LongRowGeo, osb200_select_rows' rows with the ranks
 // of the launch parameters, or LongSegGeo, osb200_select_segments' long list (DESIGN §4.20), whose entry j is segment list[j]
 // with the ranks seg_ranks[list[j] * nr ..] in device memory.  A state, its totals and its tile counts are indexed by row or
 // list entry.  A segment's ranks at or past its length, or all of them when they decrease, take no part: only the first
@@ -4618,9 +4532,9 @@ __device__ __forceinline__ uint32_t select_active(const LongSegGeo& geo, uint64_
     if (rk) *rk = r;
     return select_ranks_active(r, nr, geo.off[s + 1] - geo.off[s]);
 }
-// the rows of the pick: num_rows, or the listed segments
-__device__ __forceinline__ uint64_t select_rows_of(const LongRowGeo&, uint64_t num_rows) { return num_rows; }
-__device__ __forceinline__ uint64_t select_rows_of(const LongSegGeo& geo, uint64_t) { return geo.listed(); }
+// the rows of the pick: the rows, or the listed segments
+__device__ __forceinline__ uint64_t select_rows_of(const LongRowGeo& geo) { return geo.num_rows; }
+__device__ __forceinline__ uint64_t select_rows_of(const LongSegGeo& geo) { return geo.listed(); }
 // where row r's columns go in the [rows or segments, nr] outputs
 __device__ __forceinline__ uint64_t select_obase(const LongRowGeo&, uint64_t r, uint32_t nr) { return r * nr; }
 __device__ __forceinline__ uint64_t select_obase(const LongSegGeo& geo, uint64_t j, uint32_t nr)
@@ -4641,9 +4555,9 @@ __device__ __forceinline__ uint32_t select_tpr(const LongRowGeo& geo, const Long
 __device__ __forceinline__ uint32_t select_tpr(const LongSegGeo&, const LongSegGeo::Tile& x) { return x.tpr; }
 
 template <typename KeyT, typename Geo>
-__device__ __forceinline__ void select_count_body(const Geo& geo, const KeyT* __restrict__ in, uint32_t nr, uint32_t level,
-                                                  const SelectState* __restrict__ st, uint32_t* __restrict__ tot, const KeyCodec& codec,
-                                                  const uint32_t* __restrict__ seg_ranks)
+__global__ void __launch_bounds__(kLongThreads)
+select_count_kernel(const KeyT* __restrict__ in, Geo geo, const uint32_t* __restrict__ seg_ranks, uint32_t nr, uint32_t level,
+                    const SelectState* __restrict__ st, uint32_t* __restrict__ tot, KeyCodec codec)
 {
     using U = std::conditional_t<sizeof(KeyT) == 8, uint64_t, uint32_t>;
     constexpr uint32_t D = sizeof(KeyT);
@@ -4651,7 +4565,7 @@ __device__ __forceinline__ void select_count_body(const Geo& geo, const KeyT* __
     const U m = level ? static_cast<U>(~static_cast<U>(0) << (8u * (D - level))) : static_cast<U>(0);
     const KeyT ca = static_cast<KeyT>(codec.a), cb = static_cast<KeyT>(codec.b), cd = static_cast<KeyT>(codec.d);
     const bool enc = codec.flags & kCodecEncodeOnLoad;
-    // a bin's counts in 2^lc bank-private columns, as in long_count_body (32 columns for one group, the skewed rows' case);
+    // a bin's counts in 2^lc bank-private columns, as in long_count_kernel (32 columns for one group, the skewed rows' case);
     // G groups take 32 / G columns or more, at most 8,192 counters
     __shared__ uint32_t s_hist[kRadix * 32];
     __shared__ U s_v[kMaxSelectRanks];
@@ -4692,28 +4606,12 @@ __device__ __forceinline__ void select_count_body(const Geo& geo, const KeyT* __
     }
 }
 
-template <typename KeyT>
-__global__ void __launch_bounds__(kLongThreads)
-select_count_kernel(const KeyT* __restrict__ in, uint64_t num_rows, uint32_t row_len, uint32_t tpr, uint32_t nr, uint32_t level,
-                    const SelectState* __restrict__ st, uint32_t* __restrict__ tot, KeyCodec codec)
-{
-    select_count_body<KeyT>(LongRowGeo{num_rows, row_len, tpr, 0, 0}, in, nr, level, st, tot, codec, nullptr);
-}
-
-template <typename KeyT>
-__global__ void __launch_bounds__(kLongThreads)
-select_segments_count_kernel(const KeyT* __restrict__ in, LongSegGeo geo, const uint32_t* __restrict__ seg_ranks, uint32_t nr,
-                             uint32_t level, const SelectState* __restrict__ st, uint32_t* __restrict__ tot, KeyCodec codec)
-{
-    select_count_body<KeyT>(geo, in, nr, level, st, tot, codec, seg_ranks);
-}
-
-// rows: num_rows, with the ranks of `ranks`; long segments: the listed ones, with their own ranks (seg_ranks), and after the
-// last level the columns that take no part are padded (idx_out: their positions, may be null)
+// rows: with the ranks of `ranks`; long segments: the listed ones, with their own ranks (seg_ranks), and after the last level
+// the columns that take no part are padded (idx_out: their positions, may be null)
 template <typename KeyT, typename Geo>
-__device__ __forceinline__ void select_pick_body(const Geo& geo, uint64_t num_rows, uint32_t nr, uint32_t level, SelectState* __restrict__ st,
-                                                 uint32_t* __restrict__ tot, KeyT* __restrict__ out, const SelectRanks* ranks,
-                                                 const KeyCodec& codec, const uint32_t* __restrict__ seg_ranks, uint32_t* idx_out)
+__global__ void __launch_bounds__(kRadix)
+select_pick_kernel(Geo geo, const uint32_t* __restrict__ seg_ranks, uint32_t nr, uint32_t level, SelectState* __restrict__ st,
+                   uint32_t* __restrict__ tot, KeyT* __restrict__ out, uint32_t* idx_out, SelectRanks ranks, KeyCodec codec)
 {
     constexpr bool SEG = std::is_same_v<Geo, LongSegGeo>;
     constexpr uint32_t D = sizeof(KeyT);
@@ -4722,8 +4620,8 @@ __device__ __forceinline__ void select_pick_body(const Geo& geo, uint64_t num_ro
     const KeyT ca = static_cast<KeyT>(codec.a), cb = static_cast<KeyT>(codec.b), cd = static_cast<KeyT>(codec.d);
     __shared__ unsigned long long s_v[kMaxSelectRanks];
     __shared__ uint32_t s_taken[kMaxSelectRanks], s_need[kMaxSelectRanks], s_wtot[kRadix / 32], s_na;
-    uint32_t rk = SEG ? 0u : select_rank_of(*ranks, threadIdx.x);
-    const uint64_t rows = select_rows_of(geo, num_rows);
+    uint32_t rk = SEG ? 0u : select_rank_of(ranks, threadIdx.x);
+    const uint64_t rows = select_rows_of(geo);
     for (uint64_t r = blockIdx.x; r < rows; r += gridDim.x) {
         SelectState* rs = st + r * nr;
         uint32_t na = nr;
@@ -4778,29 +4676,12 @@ __device__ __forceinline__ void select_pick_body(const Geo& geo, uint64_t num_ro
     }
 }
 
-template <typename KeyT>
-__global__ void __launch_bounds__(kRadix)
-select_pick_kernel(uint64_t num_rows, uint32_t level, SelectState* __restrict__ st, uint32_t* __restrict__ tot, KeyT* __restrict__ out,
-                   SelectRanks ranks, KeyCodec codec)
-{
-    select_pick_body<KeyT>(LongRowGeo{num_rows, 0, 0, 0, 0}, num_rows, ranks.count, level, st, tot, out, &ranks, codec, nullptr, nullptr);
-}
-
-template <typename KeyT>
-__global__ void __launch_bounds__(kRadix)
-select_segments_pick_kernel(LongSegGeo geo, const uint32_t* __restrict__ seg_ranks, uint32_t nr, uint32_t level,
-                            SelectState* __restrict__ st, uint32_t* __restrict__ tot, KeyT* __restrict__ out, uint32_t* idx_out,
-                            KeyCodec codec)
-{
-    select_pick_body<KeyT>(geo, 0, nr, level, st, tot, out, nullptr, codec, seg_ranks, idx_out);
-}
-
 // Per tile, the keys equal to each rank's key (its group's), into the tile's count of the rank (select_cnt_index); a warp adds
 // the lanes of one group at once.
 template <typename KeyT, typename Geo>
-__device__ __forceinline__ void select_eq_count_body(const Geo& geo, const KeyT* __restrict__ in, uint32_t nr,
-                                                     const SelectState* __restrict__ st, uint32_t* __restrict__ cnt, const KeyCodec& codec,
-                                                     const uint32_t* __restrict__ seg_ranks)
+__global__ void __launch_bounds__(kLongThreads)
+select_eq_count_kernel(const KeyT* __restrict__ in, Geo geo, const uint32_t* __restrict__ seg_ranks, uint32_t nr,
+                       const SelectState* __restrict__ st, uint32_t* __restrict__ cnt, KeyCodec codec)
 {
     using U = std::conditional_t<sizeof(KeyT) == 8, uint64_t, uint32_t>;
     const KeyT ca = static_cast<KeyT>(codec.a), cb = static_cast<KeyT>(codec.b), cd = static_cast<KeyT>(codec.d);
@@ -4840,28 +4721,12 @@ __device__ __forceinline__ void select_eq_count_body(const Geo& geo, const KeyT*
     }
 }
 
-template <typename KeyT>
-__global__ void __launch_bounds__(kLongThreads)
-select_eq_count_kernel(const KeyT* __restrict__ in, uint64_t num_rows, uint32_t row_len, uint32_t tpr, uint32_t nr,
-                       const SelectState* __restrict__ st, uint32_t* __restrict__ cnt, KeyCodec codec)
-{
-    select_eq_count_body<KeyT>(LongRowGeo{num_rows, row_len, tpr, 0, 0}, in, nr, st, cnt, codec, nullptr);
-}
-
-template <typename KeyT>
-__global__ void __launch_bounds__(kLongThreads)
-select_segments_eq_count_kernel(const KeyT* __restrict__ in, LongSegGeo geo, const uint32_t* __restrict__ seg_ranks, uint32_t nr,
-                                const SelectState* __restrict__ st, uint32_t* __restrict__ cnt, KeyCodec codec)
-{
-    select_eq_count_body<KeyT>(geo, in, nr, st, cnt, codec, seg_ranks);
-}
-
 // For every (row, rank) whose occurrence o = r - taken of its key lies in this tile by the scanned counts: the position of the
 // tile's (o - tile prefix)-th key equal to it, in tile order (per-warp ballots and a scan of the warp counts, chunk by chunk).
 template <typename KeyT, typename Geo>
-__device__ __forceinline__ void select_locate_body(const Geo& geo, const KeyT* __restrict__ in, uint32_t* __restrict__ idx_out, uint32_t nr,
-                                                   const SelectState* __restrict__ st, const uint32_t* __restrict__ cnt,
-                                                   const SelectRanks* ranks, const KeyCodec& codec, const uint32_t* __restrict__ seg_ranks)
+__global__ void __launch_bounds__(kLongThreads)
+select_locate_kernel(const KeyT* __restrict__ in, uint32_t* __restrict__ idx_out, Geo geo, const uint32_t* __restrict__ seg_ranks,
+                     uint32_t nr, const SelectState* __restrict__ st, const uint32_t* __restrict__ cnt, SelectRanks ranks, KeyCodec codec)
 {
     constexpr bool SEG = std::is_same_v<Geo, LongSegGeo>;
     using U = std::conditional_t<sizeof(KeyT) == 8, uint64_t, uint32_t>;
@@ -4889,7 +4754,7 @@ __device__ __forceinline__ void select_locate_body(const Geo& geo, const KeyT* _
             const SelectState ss = st[x.r * nr + i];
             uint32_t o;
             if constexpr (SEG) o = seg_ranks[select_obase(geo, x.r, nr) + i] - ss.taken;
-            else o = select_rank_of(*ranks, i) - ss.taken;
+            else o = select_rank_of(ranks, i) - ss.taken;
             if (o < lo || o >= hi) continue;
             const U v = static_cast<U>(ss.v);
             const uint32_t want = o - lo;
@@ -4912,23 +4777,6 @@ __device__ __forceinline__ void select_locate_body(const Geo& geo, const KeyT* _
         }
         if constexpr (SEG) __syncthreads();  // s_na is rewritten for the next tile
     }
-}
-
-template <typename KeyT>
-__global__ void __launch_bounds__(kLongThreads)
-select_locate_kernel(const KeyT* __restrict__ in, uint32_t* __restrict__ idx_out, uint64_t num_rows, uint32_t row_len, uint32_t tpr,
-                     const SelectState* __restrict__ st, const uint32_t* __restrict__ cnt, SelectRanks ranks, KeyCodec codec)
-{
-    select_locate_body<KeyT>(LongRowGeo{num_rows, row_len, tpr, 0, 0}, in, idx_out, ranks.count, st, cnt, &ranks, codec, nullptr);
-}
-
-template <typename KeyT>
-__global__ void __launch_bounds__(kLongThreads)
-select_segments_locate_kernel(const KeyT* __restrict__ in, uint32_t* __restrict__ idx_out, LongSegGeo geo,
-                              const uint32_t* __restrict__ seg_ranks, uint32_t nr, const SelectState* __restrict__ st,
-                              const uint32_t* __restrict__ cnt, KeyCodec codec)
-{
-    select_locate_body<KeyT>(geo, in, idx_out, nr, st, cnt, nullptr, codec, seg_ranks);
 }
 
 SelectLayout select_layout(uint64_t num_rows, uint32_t row_len, uint32_t num_ranks, bool positions)
@@ -4963,34 +4811,28 @@ cudaError_t launch_select_long_rows(const void* keys_in, void* values_out, uint3
     uint32_t* cnt = scratch + l.cnt;
     uint32_t* csum = l.cpr > 1 ? scratch + l.csum : nullptr;
     const uint64_t tiles = num_rows * l.tpr;
-    return with_key_type(TopkKeys{}, key_bytes, [&](auto kt) {
+    const LongRowGeo geo{num_rows, row_len, l.tpr, static_cast<uint64_t>(nr) * l.tpr, l.cpr};  // its chunks: the counts [rank][tile]
+    const uint32_t* no_seg_ranks = nullptr;
+    return with_key_type(LongKeys{}, key_bytes, [&](auto kt) {
         using KeyT = decltype(kt);
         const KeyT* in = static_cast<const KeyT*>(keys_in);
         cudaError_t le = cudaSuccess;
         for (uint32_t t = 0; le == cudaSuccess && t < sizeof(KeyT); ++t) {
-            le = launch_resident<select_count_kernel<KeyT>, kLongThreads, 0>(tiles, sm_count, stream, in, num_rows, row_len, l.tpr, nr, t,
-                                                                             static_cast<const SelectState*>(st), tot, codec);
+            le = launch_resident<select_count_kernel<KeyT, LongRowGeo>, kLongThreads, 0>(tiles, sm_count, stream, in, geo, no_seg_ranks, nr, t,
+                                                                                         static_cast<const SelectState*>(st), tot, codec);
             if (le == cudaSuccess)
-                le = launch_resident<select_pick_kernel<KeyT>, kRadix, 0>(num_rows, sm_count, stream, num_rows, t, st, tot,
-                                                                          static_cast<KeyT*>(values_out), ranks, codec);
+                le = launch_resident<select_pick_kernel<KeyT, LongRowGeo>, kRadix, 0>(num_rows, sm_count, stream, geo, no_seg_ranks, nr, t, st,
+                                                                                      tot, static_cast<KeyT*>(values_out), nullptr, ranks, codec);
         }
         if (le != cudaSuccess || !indices) return le;
-        le = launch_resident<select_eq_count_kernel<KeyT>, kLongThreads, 0>(tiles, sm_count, stream, in, num_rows, row_len, l.tpr, nr,
-                                                                            static_cast<const SelectState*>(st), cnt, codec);
-        if (le != cudaSuccess) return le;
+        le = launch_resident<select_eq_count_kernel<KeyT, LongRowGeo>, kLongThreads, 0>(tiles, sm_count, stream, in, geo, no_seg_ranks, nr,
+                                                                                        static_cast<const SelectState*>(st), cnt, codec);
         // per row, the exclusive scan of its nr * tpr counts [rank][tile]
-        const uint64_t row_counts = static_cast<uint64_t>(nr) * l.tpr;
-        const unsigned scan_grid = capped_grid(num_rows * l.cpr, 1, static_cast<uint64_t>(sm_count) * 4);
-        if (csum) {
-            long_rows_chunk_sum_kernel<<<scan_grid, kLongThreads, 0, stream>>>(none_skipped, 0, cnt, csum, num_rows, row_counts, l.cpr);
-            long_rows_chunk_scan_kernel<<<capped_grid(num_rows, 1, static_cast<uint64_t>(sm_count) * 4), kLongThreads, 0, stream>>>(
-                none_skipped, 0, csum, num_rows, l.cpr);
-        }
-        long_rows_scan_kernel<<<scan_grid, kLongThreads, 0, stream>>>(none_skipped, 0, cnt, csum, num_rows, row_counts, l.cpr);
-        if ((le = cudaGetLastError()) != cudaSuccess) return le;
-        return launch_resident<select_locate_kernel<KeyT>, kLongThreads, 0>(tiles, sm_count, stream, in, indices, num_rows, row_len, l.tpr,
-                                                                            static_cast<const SelectState*>(st),
-                                                                            static_cast<const uint32_t*>(cnt), ranks, codec);
+        if (le == cudaSuccess) le = launch_long_scan(geo, none_skipped, 0, cnt, csum, num_rows * l.cpr, num_rows, sm_count, stream);
+        if (le != cudaSuccess) return le;
+        return launch_resident<select_locate_kernel<KeyT, LongRowGeo>, kLongThreads, 0>(tiles, sm_count, stream, in, indices, geo, no_seg_ranks,
+                                                                                        nr, static_cast<const SelectState*>(st),
+                                                                                        static_cast<const uint32_t*>(cnt), ranks, codec);
     });
 }
 
@@ -5004,8 +4846,8 @@ cudaError_t launch_select_long_rows(const void* keys_in, void* values_out, uint3
 //     the block list, by the segment sort's two block classes.
 //   * select_segment_warp_kernel (warp_sort_run, RCOLS) and select_segment_block_kernel (segment_sort_body, LIST and RCOLS)
 //     sort each segment in shared memory and store only its columns.
-//   * the long list: long_segments_map_kernel's tile map, then the split path's bodies over it (LongSegGeo), and with
-//     positions the long segments' scan bodies over each entry's [rank][tile] counts (SelectSegScanGeo).  Should the map
+//   * the long list: long_segments_map_kernel's tile map, then the split path's kernels over it (LongSegGeo), and with
+//     positions the long paths' scan kernels over each entry's [rank][tile] counts (SelectSegScanGeo).  Should the map
 //     not fit its bounds (only offsets that make valid segments overlap can do that), select_segment_unmapped_kernel pads
 //     every long segment instead.
 // =====================================================================================================
@@ -5086,7 +4928,7 @@ using SelectSegShapes = TypeList<
     SelectSegShape<uint32_t, 1, false>, SelectSegShape<uint32_t, 2, false>, SelectSegShape<uint32_t, 1, true>, SelectSegShape<uint32_t, 2, true>,
     SelectSegShape<uint64_t, 1, false>, SelectSegShape<uint64_t, 2, false>, SelectSegShape<uint64_t, 1, true>, SelectSegShape<uint64_t, 2, true>>;
 
-// The long segments' equal-key counts for the scan bodies: entry j's nr * tiles counts [rank][tile] from nr * tfirst[j], cut
+// The long segments' equal-key counts for the scan kernels: entry j's nr * tiles counts [rank][tile] from nr * tfirst[j], cut
 // into chunks of 16 tiles' counts per rank -- as many as long_segments_map_kernel gives the entry (ceil(tiles / 16), from
 // cfirst[j]), so its chunk map serves here too.
 struct SelectSegScanGeo {
@@ -5106,24 +4948,6 @@ struct SelectSegScanGeo {
     __device__ __forceinline__ Group group(uint64_t j) const { return seg.group(j); }
 };
 static_assert(kLongChunk % kRadix == 0, "a chunk of the tile map is whole tiles");
-
-__global__ void __launch_bounds__(kLongThreads)
-select_segments_chunk_sum_kernel(const SortPlan* __restrict__ plan, uint32_t* cnt, uint32_t* __restrict__ csum, SelectSegScanGeo geo)
-{
-    long_chunk_sum_body(geo, plan, 0u, cnt, csum);
-}
-
-__global__ void __launch_bounds__(kLongThreads)
-select_segments_chunk_scan_kernel(const SortPlan* __restrict__ plan, uint32_t* csum, SelectSegScanGeo geo)
-{
-    long_chunk_scan_body(geo, plan, 0u, csum);
-}
-
-__global__ void __launch_bounds__(kLongThreads)
-select_segments_scan_kernel(const SortPlan* __restrict__ plan, uint32_t* cnt, const uint32_t* __restrict__ csum, SelectSegScanGeo geo)
-{
-    long_scan_body(geo, plan, 0u, cnt, csum);
-}
 
 // When the tile map did not fit (counts[kSegCountLong] == 0), every segment the binning kernel sent to the long list is padding.
 template <typename KeyT>
@@ -5155,7 +4979,7 @@ SelectSegLayout select_segments_layout(uint64_t n, uint64_t num_segments, uint32
     l.list_cap = n / long_min < num_segments ? n / long_min : num_segments;
     l.tile_cap = (n + kLongRowTile - 1) / kLongRowTile + l.list_cap;
     l.chunk_cap = (l.tile_cap * kRadix + kLongChunk - 1) / kLongChunk + l.list_cap;
-    l.st = 16;  // words 0 .. 15: a zeroed SortPlan, with which the scan bodies skip nothing
+    l.st = 16;  // words 0 .. 15: a zeroed SortPlan, with which the scan kernels skip nothing
     l.tot = l.st + l.list_cap * num_ranks * 4;
     l.zeroed = whole(l.tot + l.list_cap * num_ranks * kRadix);
     l.list = l.zeroed;
@@ -5190,7 +5014,7 @@ cudaError_t launch_select_segments(const void* keys_in, void* values_out, uint32
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
     // the classes: every segment the long list does not take
     const uint32_t class_max = lng ? long_min - 1 : max_len;
-    e = with_key_type(TopkKeys{}, key_bytes, [&](auto kt) {
+    e = with_key_type(LongKeys{}, key_bytes, [&](auto kt) {
         using KeyT = decltype(kt);
         return with_rank_mode(rank_mode, [&](auto r) {
             constexpr int R = decltype(r)::value;
@@ -5233,7 +5057,7 @@ cudaError_t launch_select_segments(const void* keys_in, void* values_out, uint32
     long_segments_map_kernel<<<1, kLongThreads, 0, stream>>>(off, scratch + l.list, scratch + l.tfirst, scratch + l.cfirst, counts,
                                                              l.list_cap, l.tile_cap, l.chunk_cap);
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    return with_key_type(TopkKeys{}, key_bytes, [&](auto kt) {
+    return with_key_type(LongKeys{}, key_bytes, [&](auto kt) {
         using KeyT = decltype(kt);
         const KeyT* in = static_cast<const KeyT*>(keys_in);
         KeyT* out = static_cast<KeyT*>(values_out);
@@ -5241,29 +5065,23 @@ cudaError_t launch_select_segments(const void* keys_in, void* values_out, uint32
                                                                           codec);
         cudaError_t le = cudaGetLastError();
         for (uint32_t t = 0; le == cudaSuccess && t < sizeof(KeyT); ++t) {
-            le = launch_resident<select_segments_count_kernel<KeyT>, kLongThreads, 0>(l.tile_cap, sm_count, stream, in, geo, seg_ranks, nr,
-                                                                                      t, static_cast<const SelectState*>(st), tot, codec);
+            le = launch_resident<select_count_kernel<KeyT, LongSegGeo>, kLongThreads, 0>(l.tile_cap, sm_count, stream, in, geo, seg_ranks, nr,
+                                                                                         t, static_cast<const SelectState*>(st), tot, codec);
             if (le == cudaSuccess)
-                le = launch_resident<select_segments_pick_kernel<KeyT>, kRadix, 0>(l.list_cap, sm_count, stream, geo, seg_ranks, nr, t, st,
-                                                                                   tot, out, indices, codec);
+                le = launch_resident<select_pick_kernel<KeyT, LongSegGeo>, kRadix, 0>(l.list_cap, sm_count, stream, geo, seg_ranks, nr, t, st,
+                                                                                      tot, out, indices, SelectRanks{}, codec);
         }
         if (le != cudaSuccess || !indices) return le;
-        le = launch_resident<select_segments_eq_count_kernel<KeyT>, kLongThreads, 0>(l.tile_cap, sm_count, stream, in, geo, seg_ranks, nr,
-                                                                                     static_cast<const SelectState*>(st), cnt, codec);
-        if (le != cudaSuccess) return le;
+        le = launch_resident<select_eq_count_kernel<KeyT, LongSegGeo>, kLongThreads, 0>(l.tile_cap, sm_count, stream, in, geo, seg_ranks, nr,
+                                                                                        static_cast<const SelectState*>(st), cnt, codec);
         // per list entry, the exclusive scan of its nr * tiles counts [rank][tile]
-        const SelectSegScanGeo sg{geo, nr};
-        const unsigned scan_grid = capped_grid(l.chunk_cap, 1, static_cast<uint64_t>(sm_count) * 4);
-        if (csum) {
-            select_segments_chunk_sum_kernel<<<scan_grid, kLongThreads, 0, stream>>>(none_skipped, cnt, csum, sg);
-            select_segments_chunk_scan_kernel<<<capped_grid(l.list_cap, 1, static_cast<uint64_t>(sm_count) * 4), kLongThreads, 0, stream>>>(
-                none_skipped, csum, sg);
-        }
-        select_segments_scan_kernel<<<scan_grid, kLongThreads, 0, stream>>>(none_skipped, cnt, csum, sg);
-        if ((le = cudaGetLastError()) != cudaSuccess) return le;
-        return launch_resident<select_segments_locate_kernel<KeyT>, kLongThreads, 0>(l.tile_cap, sm_count, stream, in, indices, geo,
-                                                                                     seg_ranks, nr, static_cast<const SelectState*>(st),
-                                                                                     static_cast<const uint32_t*>(cnt), codec);
+        if (le == cudaSuccess)
+            le = launch_long_scan(SelectSegScanGeo{geo, nr}, none_skipped, 0, cnt, csum, l.chunk_cap, l.list_cap, sm_count, stream);
+        if (le != cudaSuccess) return le;
+        return launch_resident<select_locate_kernel<KeyT, LongSegGeo>, kLongThreads, 0>(l.tile_cap, sm_count, stream, in, indices, geo,
+                                                                                        seg_ranks, nr, static_cast<const SelectState*>(st),
+                                                                                        static_cast<const uint32_t*>(cnt), SelectRanks{},
+                                                                                        codec);
     });
 }
 
@@ -5286,7 +5104,7 @@ cudaError_t configure_kernels()
     if (e == cudaSuccess) e = for_each_type(RowShapes{}, shape);
     if (e == cudaSuccess) e = for_each_type(ListShapes{}, shape);
     if (e == cudaSuccess) e = for_each_type(TopkSortShapes{}, shape);
-    if (e == cudaSuccess) e = for_each_type(TopkKeys{}, [](auto k) {
+    if (e == cudaSuccess) e = for_each_type(LongKeys{}, [](auto k) {
         using KeyT = decltype(k);
         const cudaError_t m = set_smem(topk_select_kernel<KeyT>, sizeof(TopkSmem<KeyT>));
         return m != cudaSuccess ? m : set_smem(topk_segment_select_kernel<KeyT>, sizeof(TopkSmem<KeyT>));
@@ -5298,25 +5116,20 @@ cudaError_t configure_kernels()
     });
     if (e == cudaSuccess) e = set_smem(fused_kernel<kRankAtomic>(), FusedShape::smem);
     if (e == cudaSuccess) e = set_smem(fused_kernel<kRankBallot>(), FusedShape::smem);
-    if (e == cudaSuccess) e = for_each_type(LongRowKeys{}, [](auto k) {
+    if (e == cudaSuccess) e = for_each_type(LongKeys{}, [](auto k) {
         using KeyT = decltype(k);
-        cudaError_t m = set_smem(long_rows_scatter_kernel<KeyT, kRankAtomic, false>, sizeof(LongRowsSmem<KeyT, false>));
-        if (m == cudaSuccess) m = set_smem(long_rows_scatter_kernel<KeyT, kRankBallot, false>, sizeof(LongRowsSmem<KeyT, false>));
-        if (m == cudaSuccess) m = set_smem(long_rows_scatter_kernel<KeyT, kRankAtomic, true>, sizeof(LongRowsSmem<KeyT, true>));
-        return m != cudaSuccess ? m : set_smem(long_rows_scatter_kernel<KeyT, kRankBallot, true>, sizeof(LongRowsSmem<KeyT, true>));
-    });
-    if (e == cudaSuccess) e = for_each_type(LongRowKeys{}, [](auto k) {
-        using KeyT = decltype(k);
-        cudaError_t m = set_smem(long_segments_scatter_kernel<KeyT, kRankAtomic, false>, sizeof(LongRowsSmem<KeyT, false>));
-        if (m == cudaSuccess) m = set_smem(long_segments_scatter_kernel<KeyT, kRankBallot, false>, sizeof(LongRowsSmem<KeyT, false>));
-        if (m == cudaSuccess) m = set_smem(long_segments_scatter_kernel<KeyT, kRankAtomic, true>, sizeof(LongRowsSmem<KeyT, true>));
-        return m != cudaSuccess ? m : set_smem(long_segments_scatter_kernel<KeyT, kRankBallot, true>, sizeof(LongRowsSmem<KeyT, true>));
-    });
-    if (e == cudaSuccess) e = for_each_type(TopkKeys{}, [](auto k) {
-        using KeyT = decltype(k);
-        cudaError_t m = set_smem(topk_long_finish_kernel<KeyT>, sizeof(TopkSmem<KeyT>));
-        if (m == cudaSuccess) m = set_smem(topk_long_sort_scatter_kernel<KeyT, kRankAtomic>, sizeof(LongRowsSmem<KeyT, true>));
-        return m != cudaSuccess ? m : set_smem(topk_long_sort_scatter_kernel<KeyT, kRankBallot>, sizeof(LongRowsSmem<KeyT, true>));
+        constexpr size_t keys = sizeof(LongRowsSmem<KeyT, false>), idx = sizeof(LongRowsSmem<KeyT, true>);
+        // the long scatter over the rows and the segments, and the rows' with given indices
+        cudaError_t m = for_each_type(TypeList<LongRowGeo, LongSegGeo>{}, [](auto g) {
+            using Geo = decltype(g);
+            cudaError_t r = set_smem(long_scatter_kernel<KeyT, kRankAtomic, false, Geo>, keys);
+            if (r == cudaSuccess) r = set_smem(long_scatter_kernel<KeyT, kRankBallot, false, Geo>, keys);
+            if (r == cudaSuccess) r = set_smem(long_scatter_kernel<KeyT, kRankAtomic, true, Geo>, idx);
+            return r != cudaSuccess ? r : set_smem(long_scatter_kernel<KeyT, kRankBallot, true, Geo>, idx);
+        });
+        if (m == cudaSuccess) m = set_smem(long_scatter_kernel<KeyT, kRankAtomic, true, LongRowGeo, true>, idx);
+        if (m == cudaSuccess) m = set_smem(long_scatter_kernel<KeyT, kRankBallot, true, LongRowGeo, true>, idx);
+        return m != cudaSuccess ? m : set_smem(topk_long_finish_kernel<KeyT>, sizeof(TopkSmem<KeyT>));
     });
     if (e == cudaSuccess) e = for_each_type(SelectShapes{}, shape);
     if (e == cudaSuccess) e = for_each_type(SelectSegShapes{}, shape);

@@ -1,7 +1,7 @@
-"""A numpy restatement of the row select's split path (osb200_select_rows; select_count_kernel, select_pick_kernel,
-select_eq_count_kernel, select_locate_kernel), over one row's radix images (unsigned keys whose ascending order is the
-library's order), and of the workspace bound the header states.  tests/test_select_plan_cpu.py checks it against a stable
-argsort.
+"""A numpy restatement of the row select's split path (osb200_select_rows; the LongRowGeo instantiations of
+select_count_kernel, select_pick_kernel, select_eq_count_kernel and select_locate_kernel), over one row's radix images
+(unsigned keys whose ascending order is the library's order), and of the workspace bound the header states.
+tests/test_select_plan_cpu.py checks it against a stable argsort.
 
 Every rank r_i has a state: the prefix v_i of its key's top t digits and taken_i, the keys below v_i's range.  At level t the
 ranks whose prefixes are equal form a group (contiguous, the ranks increasing); each key matches at most one group's prefix

@@ -7,11 +7,14 @@ import re
 
 from tests.test_ptxas_spills import _report, parse_report
 
-# long_rows_scatter_kernel<KeyT, RANK_MODE, INDICES>
-SCATTER = re.compile(r"_ZN3osb24long_rows_scatter_kernelI([tjm])Li(\d+)ELb([01])EE")
-# long_rows_count_kernel<KeyT>, long_rows_copy_home_kernel<KeyT>, long_rows_head_hist_kernel<KeyT>
-PER_KEY = re.compile(r"_ZN3osb\d+long_rows_(count|copy_home|head_hist)_kernelI([tjm])EE")
-SCAN = re.compile(r"_ZN3osb\d+long_rows_(chunk_sum|chunk_scan|scan)_kernelE")
+# long_scatter_kernel<KeyT, RANK_MODE, INDICES, LongRowGeo, false>
+SCATTER = re.compile(r"_ZN3osb19long_scatter_kernelI([tjm])Li(\d+)ELb([01])ENS_10LongRowGeoELb0EEE")
+# long_count_kernel<KeyT, LongRowGeo>
+COUNT = re.compile(r"_ZN3osb17long_count_kernelI([tjm])NS_10LongRowGeoEEE")
+# long_rows_copy_home_kernel<KeyT>, long_rows_head_hist_kernel<KeyT>
+PER_KEY = re.compile(r"_ZN3osb\d+long_rows_(copy_home|head_hist)_kernelI([tjm])EE")
+# long_{chunk_sum,chunk_scan,scan}_kernel<LongRowGeo>
+SCAN = re.compile(r"_ZN3osb\d+long_(chunk_sum|chunk_scan|scan)_kernelINS_10LongRowGeoEEE")
 WIDTH = {"t": "u16", "j": "u32", "m": "u64"}
 RANK_ATOMIC = 0
 
@@ -23,6 +26,9 @@ def guarded_long_rows(report):
         m = SCATTER.match(name)
         if m and int(m.group(2)) == RANK_ATOMIC:
             out[f"scatter/{WIDTH[m.group(1)]}/" + ("indices" if m.group(3) == "1" else "keys")] = (st, ld)
+        m = COUNT.match(name)
+        if m:
+            out[f"count/{WIDTH[m.group(1)]}"] = (st, ld)
         m = PER_KEY.match(name)
         if m:
             out[f"{m.group(1)}/{WIDTH[m.group(2)]}"] = (st, ld)
@@ -33,13 +39,13 @@ def guarded_long_rows(report):
 
 
 def test_the_regex_reads_the_long_row_kernels_mangling():
-    text = ("ptxas info    : Function properties for _ZN3osb24long_rows_scatter_kernelImLi0ELb1EEEvPKNS_8SortPlanEjPKT_PS4_S7_PjS8_mjjPKjNS_8KeyCodecE\n"
+    text = ("ptxas info    : Function properties for _ZN3osb19long_scatter_kernelImLi0ELb1ENS_10LongRowGeoELb0EEEvPKNS_8SortPlanEjPKT_PS5_S8_PjS9_T2_PKjNS_8KeyCodecE\n"
             "    0 bytes stack frame, 4 bytes spill stores, 8 bytes spill loads\n"
-            "ptxas info    : Function properties for _ZN3osb24long_rows_scatter_kernelImLi1ELb1EEEvPKNS_8SortPlanEjPKT_PS4_S7_PjS8_mjjPKjNS_8KeyCodecE\n"
+            "ptxas info    : Function properties for _ZN3osb19long_scatter_kernelImLi1ELb1ENS_10LongRowGeoELb0EEEvPKNS_8SortPlanEjPKT_PS5_S8_PjS9_T2_PKjNS_8KeyCodecE\n"
             "    0 bytes stack frame, 4 bytes spill stores, 8 bytes spill loads\n"
-            "ptxas info    : Function properties for _ZN3osb22long_rows_count_kernelItEEvPKNS_8SortPlanEjPKT_S6_S6_mjjPjNS_8KeyCodecE\n"
+            "ptxas info    : Function properties for _ZN3osb17long_count_kernelItNS_10LongRowGeoEEEvPKNS_8SortPlanEjPKT_S7_S7_T0_PjNS_8KeyCodecE\n"
             "    0 bytes stack frame, 0 bytes spill stores, 0 bytes spill loads\n"
-            "ptxas info    : Function properties for _ZN3osb21long_rows_scan_kernelEPKNS_8SortPlanEjPjPKjmmj\n"
+            "ptxas info    : Function properties for _ZN3osb16long_scan_kernelINS_10LongRowGeoEEEvPKNS_8SortPlanEjPjPKjT_\n"
             "    0 bytes stack frame, 0 bytes spill stores, 0 bytes spill loads\n")
     assert guarded_long_rows(parse_report(text)) == {"scatter/u64/indices": (4, 8), "count/u16": (0, 0), "scan": (0, 0)}
 

@@ -7,11 +7,15 @@ import re
 
 from tests.test_ptxas_spills import _report, parse_report
 
-# long_segments_scatter_kernel<KeyT, RANK_MODE, INDICES>
-SCATTER = re.compile(r"_ZN3osb28long_segments_scatter_kernelI([tjm])Li(\d+)ELb([01])EE")
-# long_segments_count_kernel<KeyT>, long_segments_copy_home_kernel<KeyT>, long_segment_bin_kernel<KeyT>
-PER_KEY = re.compile(r"_ZN3osb\d+long_(segments_count|segments_copy_home|segment_bin)_kernelI([tjm])EE")
-SCAN = re.compile(r"_ZN3osb\d+long_segments_(chunk_sum|chunk_scan|scan|map)_kernelE")
+# long_scatter_kernel<KeyT, RANK_MODE, INDICES, LongSegGeo, false>
+SCATTER = re.compile(r"_ZN3osb19long_scatter_kernelI([tjm])Li(\d+)ELb([01])ENS_10LongSegGeoELb0EEE")
+# long_count_kernel<KeyT, LongSegGeo>
+COUNT = re.compile(r"_ZN3osb17long_count_kernelI([tjm])NS_10LongSegGeoEEE")
+# long_segments_copy_home_kernel<KeyT>, long_segment_bin_kernel<KeyT>
+PER_KEY = re.compile(r"_ZN3osb\d+long_(segments_copy_home|segment_bin)_kernelI([tjm])EE")
+# long_{chunk_sum,chunk_scan,scan}_kernel<LongSegGeo>, long_segments_map_kernel
+SCAN = re.compile(r"_ZN3osb\d+long_(chunk_sum|chunk_scan|scan)_kernelINS_10LongSegGeoEEE")
+MAP = re.compile(r"_ZN3osb24long_segments_map_kernelE")
 WIDTH = {"t": "u16", "j": "u32", "m": "u64"}
 RANK_ATOMIC = 0
 
@@ -23,21 +27,26 @@ def guarded_long_segments(report):
         m = SCATTER.match(name)
         if m and int(m.group(2)) == RANK_ATOMIC:
             out[f"scatter/{WIDTH[m.group(1)]}/" + ("indices" if m.group(3) == "1" else "keys")] = (st, ld)
+        m = COUNT.match(name)
+        if m:
+            out[f"count/{WIDTH[m.group(1)]}"] = (st, ld)
         m = PER_KEY.match(name)
         if m:
             out[f"{m.group(1).replace('segments_', '')}/{WIDTH[m.group(2)]}"] = (st, ld)
         m = SCAN.match(name)
         if m:
             out[m.group(1)] = (st, ld)
+        if MAP.match(name):
+            out["map"] = (st, ld)
     return out
 
 
 def test_the_regex_reads_the_long_segment_kernels_mangling():
-    text = ("ptxas info    : Function properties for _ZN3osb28long_segments_scatter_kernelImLi0ELb1EEEvPKNS_8SortPlanEjPKT_PS4_S7_PjS8_NS_10LongSegGeoEPKjNS_8KeyCodecE\n"
+    text = ("ptxas info    : Function properties for _ZN3osb19long_scatter_kernelImLi0ELb1ENS_10LongSegGeoELb0EEEvPKNS_8SortPlanEjPKT_PS5_S8_PjS9_T2_PKjNS_8KeyCodecE\n"
             "    0 bytes stack frame, 4 bytes spill stores, 8 bytes spill loads\n"
-            "ptxas info    : Function properties for _ZN3osb28long_segments_scatter_kernelImLi1ELb1EEEvPKNS_8SortPlanEjPKT_PS4_S7_PjS8_NS_10LongSegGeoEPKjNS_8KeyCodecE\n"
+            "ptxas info    : Function properties for _ZN3osb19long_scatter_kernelImLi1ELb1ENS_10LongSegGeoELb0EEEvPKNS_8SortPlanEjPKT_PS5_S8_PjS9_T2_PKjNS_8KeyCodecE\n"
             "    0 bytes stack frame, 4 bytes spill stores, 8 bytes spill loads\n"
-            "ptxas info    : Function properties for _ZN3osb26long_segments_count_kernelItEEvPKNS_8SortPlanEjPKT_S6_S6_NS_10LongSegGeoEPjNS_8KeyCodecE\n"
+            "ptxas info    : Function properties for _ZN3osb17long_count_kernelItNS_10LongSegGeoEEEvPKNS_8SortPlanEjPKT_S7_S7_T0_PjNS_8KeyCodecE\n"
             "    0 bytes stack frame, 0 bytes spill stores, 0 bytes spill loads\n"
             "ptxas info    : Function properties for _ZN3osb23long_segment_bin_kernelIjEEvPKymmjPjPyPKT_PS5_S3_jS3_m\n"
             "    0 bytes stack frame, 0 bytes spill stores, 0 bytes spill loads\n"

@@ -10,7 +10,8 @@ from tests.test_ptxas_spills import _report, parse_report
 # select_rows_warp_kernel<KeyT, K, RANK_MODE, INDICES>, select_rows_block_kernel<KeyT, K, WARPS, RANK_MODE, INDICES>
 WARP = re.compile(r"_ZN3osb\d+select_rows_warp_kernelI([tjm])Li(\d+)ELi(\d+)ELb([01])EE")
 BLOCK = re.compile(r"_ZN3osb\d+select_rows_block_kernelI([tjm])Li(\d+)ELi(\d+)ELi(\d+)ELb([01])EE")
-SPLIT = re.compile(r"_ZN3osb\d+select_(count|pick|eq_count|locate)_kernelI([tjm])EE")
+# select_{count,pick,eq_count,locate}_kernel<KeyT, LongRowGeo>
+SPLIT = re.compile(r"_ZN3osb\d+select_(count|pick|eq_count|locate)_kernelI([tjm])NS_10LongRowGeoEEE")
 WIDTH = {"t": "u16", "j": "u32", "m": "u64"}
 
 
@@ -35,7 +36,7 @@ def test_the_regex_reads_the_select_kernels_mangling():
             "    0 bytes stack frame, 4 bytes spill stores, 8 bytes spill loads\n"
             "ptxas info    : Function properties for _ZN3osb23select_rows_warp_kernelItLi8ELi0ELb0EEEvPKT_PS1_PjmjNS_8KeyCodecENS_11SelectRanksE\n"
             "    0 bytes stack frame, 0 bytes spill stores, 0 bytes spill loads\n"
-            "ptxas info    : Function properties for _ZN3osb22select_eq_count_kernelImEEvPKT_mjjjPKNS_11SelectStateEPjNS_8KeyCodecE\n"
+            "ptxas info    : Function properties for _ZN3osb22select_eq_count_kernelImNS_10LongRowGeoEEEvPKT_T0_PKjjPKNS_11SelectStateEPjNS_8KeyCodecE\n"
             "    0 bytes stack frame, 0 bytes spill stores, 0 bytes spill loads\n")
     assert guarded_select_rows(parse_report(text)) == {"block/u32/K32/rank1/idx1": (4, 8), "warp/u16/K8/rank0/idx0": (0, 0),
                                                        "eq_count/u64": (0, 0)}

@@ -7,8 +7,8 @@ import re
 
 from tests.test_ptxas_spills import _report, parse_report
 
-# topk_long_sort_scatter_kernel<KeyT, RANK_MODE>
-SCATTER = re.compile(r"_ZN3osb\d+topk_long_sort_scatter_kernelI([tjm])Li(\d+)EE")
+# the in-place sort's scatter: long_scatter_kernel<KeyT, RANK_MODE, true, LongRowGeo, GIVEN = true>
+SCATTER = re.compile(r"_ZN3osb19long_scatter_kernelI([tjm])Li(\d+)ELb1ENS_10LongRowGeoELb1EEE")
 # topk_long_{count,pick,compact,finish,sort_copy_home}_kernel<KeyT>
 PER_KEY = re.compile(r"_ZN3osb\d+topk_long_(count|pick|compact|finish|sort_copy_home)_kernelI([tjm])EE")
 TILES = re.compile(r"_ZN3osb\d+topk_long_tiles_kernelE")
@@ -31,7 +31,7 @@ def guarded_topk_long_rows(report):
 
 
 def test_the_regex_reads_the_split_path_kernels_mangling():
-    text = ("ptxas info    : Function properties for _ZN3osb29topk_long_sort_scatter_kernelImLi1EEEvPKNS_8SortPlanEjPKT_PS4_S7_PjS8_mjjPKjNS_8KeyCodecE\n"
+    text = ("ptxas info    : Function properties for _ZN3osb19long_scatter_kernelImLi1ELb1ENS_10LongRowGeoELb1EEEvPKNS_8SortPlanEjPKT_PS5_S8_PjS9_T2_PKjNS_8KeyCodecE\n"
             "    0 bytes stack frame, 4 bytes spill stores, 8 bytes spill loads\n"
             "ptxas info    : Function properties for _ZN3osb22topk_long_count_kernelItEEvPKT_mjjjjPKNS_11TopkLongRowEPjS7_S7_NS_8KeyCodecE\n"
             "    0 bytes stack frame, 0 bytes spill stores, 0 bytes spill loads\n"
